@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- 416x416 images/sec of the YOLOv2 hot path on B200 (BASELINE.json metric).
+"""bench.py -- 416x416 images/sec of the YOLOv2 hot path on one GPU (H100; BASELINE.json metric).
 
 Workload (BASELINE.json configs[1], "C2"): Darknet-19 416x416 batch-32 inference + anchor decode +
 class softmax + threshold filter + NMS + per-class expansion, synthetic images, random-init
 weights.  One "step" = one batch of 32 images through the whole chain.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W]            # B200 arm (prints ONE JSON line)
+    python bench.py [--gpus N] [--steps K] [--warmup W]            # GPU arm (prints ONE JSON line)
     python bench.py --impl reference [--steps K] [--warmup W]      # the reference's CPU implementation of the same chain
 
 N > 1: launched by torch.distributed.run, one rank per GPU; the inference path shards by image with no
@@ -14,7 +14,7 @@ data-path collective (replicas), so scaling is "weak" and `value` is the whole-j
 exchange step (the NCCL gradient all-reduce).
 
 Numbers in the JSON line:
-  value      images/s, inputs resident in HBM (4 rotating input batches = 265 MB > 126 MB L2), CUDA-graph
+  value      images/s, inputs resident in HBM (4 rotating input batches = 265 MB > 50 MB L2), CUDA-graph
              replay of the kernel chain, 2 batches in flight, CUDA events on the launching stream, max over ranks.
   one_lane   the same with ONE batch in flight (what a latency-bound caller sees); the per-kernel figures below are
              fractions of THIS step time.
@@ -22,9 +22,10 @@ Numbers in the JSON line:
              batch and D2H of the detection arrays inside the timed region (double-buffered).
   strict     the same chain with precision='strict' (split fp16 operands; the mode whose head feature is inside the
              reference's 1e-3 contract) -- its cost next to the default 'fast' mode's measured error.
-  roofline   tensor-core roofline of the dominant kernel family (the tcgen05 implicit-GEMM conv, 22 launches/step):
+  roofline   tensor-core roofline of the dominant kernel family (the wgmma implicit-GEMM conv, 22 launches/step):
              algorithmic FLOPs of those launches / (their share of the step's kernel time x the one-lane step time), against
-             MEASURED_PEAKS.json bf16_tflops (the BURST figure: the timed region is tens of milliseconds).
+             MEASURED_PEAKS.json bf16_tflops when that file exists, else the H100 SXM data sheet's dense fp16 rate (989 TFLOP/s,
+             a denominator, not a reached figure).
   train      BASELINE configs[2]: 416x416 batch-64 training step per GPU (train-mode fwd, region loss, bwd, Adam), with the
              gradient all-reduce when N > 1 (plus the same step with the exchange switched off = exposed communication).
   train_ddp  N > 1, BASELINE configs[3]: 16 images per GPU, sizes cycling {320, 416, 608}.
@@ -48,7 +49,7 @@ for _p in (PKG, ROOT):
         sys.path.insert(0, _p)
 
 GFLOP_PER_IMAGE_416 = 29.360334848          # SURVEY 8d: sum 2*Cin*Cout*k^2*H*W over the 23 convs
-GFLOP_LAYER0_416 = 0.299040768              # layers1.0 (direct CUDA-core kernel, not tcgen05)
+GFLOP_LAYER0_416 = 0.299040768              # layers1.0 (its own tensor-core kernel, not the implicit-GEMM family)
 METRIC = '416x416 images/sec'
 
 
@@ -68,9 +69,10 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         # the timed regions here last tens of milliseconds at full clocks: the BURST figure is the honest denominator
-        return dict(tflops=float(d.get('bf16_tflops', 1700.0)), tflops_sustained=float(d.get('bf16_tflops_sustained', 1460.0)),
-                    hbm=float(d.get('hbm_gbs', 6650.0)), source='MEASURED_PEAKS.json (bf16_tflops, burst)')
-    return dict(tflops=1700.0, tflops_sustained=1460.0, hbm=6650.0, source='fallback (B200_PROFILING.md)')
+        return dict(tflops=float(d.get('bf16_tflops', 989.0)), tflops_sustained=float(d.get('bf16_tflops_sustained', 989.0)),
+                    hbm=float(d.get('hbm_gbs', 3350.0)), source='MEASURED_PEAKS.json (bf16_tflops, burst)')
+    # NVIDIA's H100 SXM data sheet (dense fp16, 700 W card): a denominator, not a figure this code reaches
+    return dict(tflops=989.0, tflops_sustained=989.0, hbm=3350.0, source='H100 SXM data sheet (dense fp16 989 TFLOP/s, HBM3 3.35 TB/s)')
 
 
 def committed_traffic():
@@ -160,21 +162,21 @@ class ClockSampler(object):
 
 
 # ------------------------------------------------------------------------------------------------
-# reference arm / cpu baseline: the oracle port on the host cores
+# reference arm / cpu baseline: the reference (or the oracle port) on the host cores
 # ------------------------------------------------------------------------------------------------
 def make_cpu_chain():
-    """The CPU implementation of the C2 chain: the UNMODIFIED reference staged under baseline/_ref (kind 'reference') when present,
+    """The CPU implementation of the C2 chain: the reference built into oracle/_ref by build() (kind 'reference') when present,
     else the oracle port (kind 'port').  Returns (chain(x) -> (feature, detections), kind, image generator)."""
     import torch
     from oracle import yolo2_oracle as O      # seeded input / weight generators (and the port when the reference is not staged)
     sd = O.make_state_dict(0)
     anchors = O.anchors_yolo_voc()
     try:
-        from baseline import ref_runner
+        from oracle import ref_runner
         if ref_runner.available():
             return ref_runner.build_chain(sd, anchors), 'reference', O.synth_images
     except Exception as ex:
-        sys.stderr.write('bench.py: staged reference unusable (%s); timing the oracle port\n' % ex)
+        sys.stderr.write('bench.py: built reference unusable (%s); timing the oracle port\n' % ex)
 
     def chain(x):
         with torch.no_grad():
@@ -221,7 +223,7 @@ def cpu_measure(batch, steps, warmup, budget_s, keep_features=0):
     if keep_features:
         n = min(keep_features, sample)
         feats = (x[:n].clone(), feature[:n].clone())
-    what = "the reference's own modules (baseline/_ref)" if kind == 'reference' else 'oracle port of the reference'
+    what = "the reference's own modules (oracle/_ref)" if kind == 'reference' else 'oracle port of the reference'
     return (sample * steps / dt, cores, '%d steps x %d images (of the %d-image batch), fp32, %s, torch %d threads' % (steps, sample, batch, what, cores),
             dt / steps * 1e3, kind, feats)
 
@@ -238,7 +240,7 @@ def run_reference(args):
                 ms_per_step=ms, higher_is_better=True, scaling='weak', vs_baseline=None, dtype='f32', data='synthetic',
                 config=dict(workload='Darknet-19 416x416 batch-%d inference + decode + softmax + filter + NMS (BASELINE configs[1])' % args.batch,
                             global_batch=args.batch,
-                            note=('CPU: the unmodified reference (model.yolo2.Darknet + model.Inference + detect.postprocess from baseline/_ref), torch fp32'
+                            note=('CPU: the unmodified reference (model.yolo2.Darknet + model.Inference + detect.postprocess built into oracle/_ref), torch fp32'
                                   if kind == 'reference' else 'CPU: oracle port of the reference algorithm (torch fp32)') + ', bounded sample per step'),
                 cpu_baseline=dict(value=value, unit='images/s', cores=cores, kind=kind, sample=sample),
                 e2e=dict(value=value, unit='images/s', h2d_bytes_per_step=0, d2h_bytes_per_step=0), gpu_launches=0)
@@ -246,7 +248,7 @@ def run_reference(args):
 
 
 def cpu_leg_subprocess(batch, budget_s, keep_features):
-    """cpu_baseline of the B200 arm: the CPU path in a child process (the reference's packages are called `model` / `utils` like
+    """cpu_baseline of the GPU arm: the CPU path in a child process (the reference's packages are called `model` / `utils` like
     this repository's own, so the two cannot share an interpreter).  Returns (cpu_baseline dict, (images, features) or None)."""
     import tempfile
     import numpy as np
@@ -272,7 +274,7 @@ def cpu_leg_subprocess(batch, budget_s, keep_features):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------
 def build_model(device):
     import torch
@@ -295,7 +297,7 @@ def build_model(device):
 
 
 def profile_layers(pipe, steps):
-    """Instrumented eager pass: CUDA events around every tcgen05 conv launch (a long spin kernel in
+    """Instrumented eager pass: CUDA events around every implicit-GEMM conv launch (a long spin kernel in
     front of each step lets the host run ahead so the events bracket back-to-back kernels)."""
     import torch
     from b200 import ops
@@ -365,6 +367,33 @@ def profile_layers(pipe, steps):
     return dict(layers=layers, others=others, conv_ms=conv_ms, conv_flops=conv_flops, eager_step_ms=step_ms, kernels_ms=kernels_ms, launches=per_step)
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, out):
+    """What the timed path handed its caller in its last step (head feature, decoded boxes, class probabilities and the detection
+    arrays of every image) as DIR/<name>.npy: fp32 arrays as float32, integer arrays as float64 (exact).  The inputs and weights
+    are seeded, so two builds run with the same arguments can be compared array by array (~11 MB at batch 32, 416x416).  Past
+    DUMP_LIMIT_BYTES in all, every array is cut to the same fixed, seeded sample of whole images (the images' arrays stay intact)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {}
+    for name, t in sorted(out.items()):
+        a = t.detach().cpu()
+        arrays[name] = (a.float() if a.is_floating_point() else a.double()).numpy()
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        batch = next(iter(arrays.values())).shape[0]
+        keep = max(1, batch * DUMP_LIMIT_BYTES // total)
+        images = np.sort(np.random.RandomState(0).choice(batch, keep, replace=False))
+        arrays = {k: a[images] for k, a in arrays.items()}
+        arrays['sampled_images'] = images.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 def timed_steps(pipe, steps, warmup, slots, cur, barrier, world, device):
     """W warm-up + K timed graph replays rotating over the resident input slots.  Returns ms for K steps (max over ranks)."""
     import torch
@@ -431,7 +460,7 @@ def mobilenet_record(args, device, peaks):
         with torch.cuda.graph(gr):
             chain(x)
         graphs.append(gr)
-    steps = max(10, args.steps)
+    steps = args.steps
     for i in range(max(3, args.warmup)):
         graphs[i % 4].replay()
     torch.cuda.synchronize()
@@ -442,7 +471,7 @@ def mobilenet_record(args, device, peaks):
     e.record()
     torch.cuda.synchronize()
     ms = s.elapsed_time(e) / steps
-    # instrumented eager pass: pointwise (tcgen05) vs depthwise / first conv (HBM-bound) kernel time
+    # instrumented eager pass: pointwise (wgmma) vs depthwise / first conv (HBM-bound) kernel time
     recs = []
     orig_conv, orig_call = ops.conv_bn_act, ops.call
 
@@ -477,13 +506,13 @@ def mobilenet_record(args, device, peaks):
     for kind, s1, e1, fl, by in recs:
         d = agg.setdefault(kind, [0.0, 0.0, 0.0, 0])
         d[0] += s1.elapsed_time(e1) / reps; d[1] += fl / reps; d[2] += by / reps; d[3] += 1
-    out = dict(metric=METRIC, value=B / (ms / 1e3), unit='images/s', ms_per_step=ms, batch=B, gpu_launches_per_step=launches,
+    out = dict(metric=METRIC, value=B / (ms / 1e3), unit='images/s', ms_per_step=ms, steps=steps, batch=B, gpu_launches_per_step=launches,
                workload='MobileNet 416x416 batch-%d inference + decode + softmax + filter + NMS (BASELINE configs[4]), CUDA graph, 1 batch in flight' % B,
                gflop_per_image=3.959)
     if 'pw' in agg:
         t, fl, by, n = agg['pw']
         out['pointwise'] = dict(launches=n // reps, us=t * 1e3, tflops=fl / t / 1e9, frac_of_tensor_peak=fl / t / 1e9 / peaks['tflops'],
-                                alg_gbs=by / t / 1e6, note='1x1 convs + head on the tcgen05 kernel; arithmetic intensity 30-250 FLOP/B: HBM/latency-bound at batch 32')
+                                alg_gbs=by / t / 1e6, note='1x1 convs + head on the wgmma kernel; arithmetic intensity 30-250 FLOP/B: HBM/latency-bound at batch 32')
     for kind in ('dw', 'conv0'):
         if kind in agg:
             t, fl, by, n = agg[kind]
@@ -562,7 +591,7 @@ def run_b200(args):
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py: the B200 arm needs a CUDA device (there is no CPU fallback); use --impl reference for the CPU arm')
+        raise SystemExit('bench.py: the GPU arm needs a CUDA device (there is no CPU fallback); use --impl reference for the CPU arm')
     # launching thread + the pinned staging buffers it allocates live on the GPU's own NUMA node (e2e is PCIe-bound)
     affinity_before, affinity_now = hostbind.bind_to_gpu(local)
     torch.cuda.set_device(local)
@@ -594,6 +623,8 @@ def run_b200(args):
     t_wall = time.perf_counter()
     ms = timed_steps(pipe, args.steps, args.warmup, slots, cur, barrier, world, device)
     wall_ms = (time.perf_counter() - t_wall) * 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, pipe.out[(args.steps - 1) % slots])
     graph_launches = pipe.launches_per_run * args.steps
     value = world * B * args.steps / (ms / 1e3)
 
@@ -666,9 +697,9 @@ def run_b200(args):
             dist.destroy_process_group()
         return
 
-    # ---- roofline of the dominant kernel family (tcgen05 convs): share of the step from an instrumented pass x the one-lane step ----
+    # ---- roofline of the dominant kernel family (implicit-GEMM convs): share of the step from an instrumented pass x the one-lane step ----
     peaks = measured_peaks()
-    prof = profile_layers(pipe1, max(3, min(args.steps, 10)))
+    prof = profile_layers(pipe1, args.steps)
     step1_ms = ms1 / args.steps
     share = prof['conv_ms'] / prof['kernels_ms']
     conv_ms = share * step1_ms                        # conv-family time inside the timed one-lane step (sum of kernel times == step time)
@@ -678,7 +709,7 @@ def run_b200(args):
     roofline = dict(bound='tensor', achieved=achieved, peak=peaks['tflops'], unit='TFLOP/s', frac=achieved / peaks['tflops'],
                     frac_of_sustained_peak=achieved / peaks['tflops_sustained'],
                     traffic=traffic, traffic_source=traffic_source,
-                    kernel='conv_igemm_kernel x21 + conv_c32_kernel x1 (the tcgen05 implicit-GEMM conv family, 22 launches/step)', peak_source=peaks['source'],
+                    kernel='conv_igemm_kernel x21 + conv_c32_kernel x1 (the wgmma implicit-GEMM conv family, 22 launches/step)', peak_source=peaks['source'],
                     flops_per_launch=prof['conv_flops'] / prof['launches'], us_per_launch=conv_ms * 1e3 / prof['launches'],
                     share_of_step=share, step_ms=step1_ms,
                     how='share = conv CUDA-event time / all kernels\' CUDA-event time in an instrumented eager pass of this run; us_per_launch = share x one_lane.ms_per_step / 22',
@@ -702,9 +733,6 @@ def run_b200(args):
             us = rec['us_per_step'] / (prof['kernels_ms'] * 1e3) * step1_ms * 1e3
             gbs = nbytes / (us * 1e-6) / 1e9
             hbm_kernels[name] = dict(us=us, alg_bytes=nbytes, achieved_gbs=gbs, frac_of_hbm_peak=gbs / peaks['hbm'])
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-    with open(os.path.join(ROOT, 'gpurun_out', 'bench_layers.json'), 'w') as f:
-        json.dump(dict(prof, graph_step_ms=graph_step_ms, one_lane_step_ms=step1_ms, value=value), f, indent=1)
 
     mobilenet = None
     if not args.no_mobilenet:
@@ -736,7 +764,7 @@ def run_b200(args):
                 higher_is_better=True, scaling='weak', vs_baseline=None, dtype='f16', data='synthetic',
                 config=dict(workload='Darknet-19 416x416 batch-%d inference + decode + softmax + filter + NMS (BASELINE configs[1])' % B,
                             global_batch=B * world, per_gpu_batch=B, parallelism='replicas x%d (images shard, no collective)' % world,
-                            l2='inputs rotate over %d resident batches (%.0f MB > 126 MB L2); ~0.6 GB of activations streamed per step' % (slots, slots * h2d / 1e6),
+                            l2='inputs rotate over %d resident batches (%.0f MB > 50 MB L2); ~0.6 GB of activations streamed per step' % (slots, slots * h2d / 1e6),
                             cuda_graph=not args.no_graph, lanes=pipe.lanes, precision='fast', weights='random-init (kaiming) + random BN statistics',
                             host_affinity=(sorted(affinity_now)[:1] + sorted(affinity_now)[-1:] + [len(affinity_now)]) if affinity_now else None),
                 clocks=clocks, e2e=dict(value=e2e_value, unit='images/s', h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h, ms_per_step=ms_e2e / args.steps,
@@ -816,7 +844,7 @@ def run_train_records(args):
     if world > 1:
         dist.init_process_group('nccl', device_id=device)
     peaks = measured_peaks()
-    steps = max(5, min(args.steps, 20))
+    steps = args.steps
     warmup = max(3, args.warmup)
     g = torch.Generator().manual_seed(200 + rank)
     config, dnn, inference, anchors, optimizer = _train_setup(device, capturable=True)
@@ -872,7 +900,8 @@ def run_train_records(args):
     records['train'] = rec
     # ---- configs[3]: 16 images per GPU, sizes cycling {320, 416, 608} ----
     if world > 1:
-        Bs, sizes, maintain = 16, (320, 416, 608), max(4, steps // 2)
+        Bs, sizes = 16, (320, 416, 608)
+        maintain = max(1, steps // len(sizes))        # --steps timed steps in all, split evenly over the sizes
         per_size = {}
         tot_ms = tot_local = 0.0
         for size in sizes:
@@ -886,7 +915,7 @@ def run_train_records(args):
         nsteps = maintain * len(sizes)
         arena = dnn.trainer.arena
         records['train_ddp'] = dict(metric='multi-scale training images/sec', value=world * Bs * nsteps / (tot_ms / 1e3), unit='images/s', n_gpus=world,
-                                    per_gpu_batch=Bs, global_batch=Bs * world, sizes=list(sizes), steps_per_size=maintain, per_size=per_size,
+                                    per_gpu_batch=Bs, global_batch=Bs * world, sizes=list(sizes), steps_per_size=maintain, steps=nsteps, per_size=per_size,
                                     allreduce_bytes_per_step=int(arena.flat.numel() * 4), allreduce_buckets=len(arena.buckets),
                                     exposed_comm_ms=(tot_ms - tot_local) / nsteps, efficiency_vs_compute_only=tot_local / tot_ms,
                                     workload='Darknet-19 multi-scale {320,416,608} training, %d images per GPU (global batch %d), NCCL data parallel '
@@ -928,6 +957,8 @@ def main():
     ap.add_argument('--cpu-budget', type=float, default=150.0, help='reference arm: seconds of CPU work for the whole run')
     ap.add_argument('--keep-features', type=int, default=0, help=argparse.SUPPRESS)
     ap.add_argument('--features-out', default=None, help=argparse.SUPPRESS)
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='after the timed steps, write the outputs of the last timed step as DIR/<name>.npy (at most 64 MB: a seeded sample of images beyond that)')
     args = ap.parse_args()
     if args.impl == 'reference':
         # the reference moves tensors to a GPU whenever it sees one (utils/__init__.py:104-111); this arm is its CPU path

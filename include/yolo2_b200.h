@@ -1,4 +1,4 @@
-/* libyolo2_b200.so -- C ABI of the B200-native YOLOv2 hot path.
+/* libyolo2_b200.so -- C ABI of the H100-native YOLOv2 hot path.
  *
  * Drop-in boundary for the Darknet-19 detection path of ruiminshen/yolo2-pytorch.  The reference
  * has no FFI of its own (it is pure Python over torch, SURVEY.md section 8b); each entry point below
@@ -55,7 +55,7 @@ const char* yb_last_error(void);
  * time-out: out[0] = 0x0BADxxxx code, out[1] = block, out[2] = thread, out[3] = parity. */
 int yb_debug_read(int out[4]);
 /* Profiling aid (tools/conv_trace.py): when dev_buf (768 x uint64, device memory) is non-NULL, block 0 of the
- * tcgen05 conv kernels records clock64() per pipeline event: [0,256) TMA producer, [256,512) MMA issuer,
+ * wgmma conv kernels records clock64() per pipeline event: [0,256) TMA producer, [256,512) MMA issuer,
  * [512,768) epilogue.  NULL switches it off (the default). */
 int yb_conv_set_trace(void* dev_buf);
 
@@ -77,7 +77,7 @@ int yb_conv0_bn_leaky_pool_fwd(const float* x_nchw, const float* w_oihw, const f
  * transform/__init__.py) and cuts the host->device copy 4x. */
 int yb_conv0_u8_bn_leaky_pool_fwd(const unsigned char* x_nhwc_u8, const float* w_oihw, const float* scale, const float* shift,
                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream);
-/* k in {1,3}, stride 1, pad (k-1)/2 conv + per-channel scale/shift + leaky(slope) as a tcgen05
+/* k in {1,3}, stride 1, pad (k-1)/2 conv + per-channel scale/shift + leaky(slope) as a wgmma
  * implicit GEMM.  x: fp16 NHWC [B,H,W,Cin] with pixel pitch x_ld; w: fp16 [Cout][k][k][Cin];
  * y: fp16 NHWC (pixel pitch y_ld, first channel y_ch_off) or fp32 NCHW [B,Cout,H,W].
  * slope = 1 disables the activation; the head passes scale = 1, shift = bias. */
@@ -101,7 +101,7 @@ int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, cons
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);
 /* Split-precision ("strict") form of the same unit, for callers that need the reference's fp32 results to 1e-3 end to end
  * (model/yolo2.py:125-130 runs in fp32; 23 fp16-operand layers drift 1.6e-3).  The GEMM's reduction dimension is a concatenation
- * of fp16 terms accumulated in one fp32 TMEM accumulator:  A = [a_hi | a_lo | a_hi],  W = [w_hi | w_hi | w_lo]  (or the two-term
+ * of fp16 terms accumulated in one fp32 accumulator:  A = [a_hi | a_lo | a_hi],  W = [w_hi | w_hi | w_lo]  (or the two-term
  * forms [a_hi | a_lo] x [w_hi | w_hi] and [a_hi | a_hi] x [w_hi | w_lo]).
  *   x        fp16 NHWC, pixel pitch x_ld, holding a_channels channels: C (hi only) or 2C ([hi | lo] of the same pixel);
  *   w_split  fp16 [Cout][k][k][k_channels] from yb_pack_weight_split_f16 (k_channels = 2C or 3C; channel offsets >= a_channels
@@ -235,7 +235,7 @@ int yb_conv0_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw,
 int yb_conv0_wgrad_bn(const float* x_nchw, const void* z_nhwc_f16, const void* dap, long long ld_dap, int dap_off, const float* mean, const float* invstd,
                       const float* gamma, const float* beta, float slope, const double* sums, float* dw_oihw, int batch, int height, int width,
                       yb_stream_t stream);
-/* tcgen05 weight gradient: dw_krsc fp32 [Cout][k][k][Cin] (overwritten) from x fp16 NHWC [B,H,W,x_ld] and dz fp16 [B,H,W,dz_ld]. */
+/* wgmma weight gradient: dw_krsc fp32 [Cout][k][k][Cin] (overwritten) from x fp16 NHWC [B,H,W,x_ld] and dz fp16 [B,H,W,dz_ld]. */
 int yb_conv_wgrad(const void* x, const void* dz, float* dw_krsc, int batch, int height, int width, int cin, int cout, int ksize, int x_ld,
                   int dz_ld, yb_stream_t stream);
 /* fp32 [Cout][k][k][Cin] (yb_conv_wgrad's layout) -> the reference's OIHW parameter-gradient layout, multiplied by `scale`. */

@@ -438,6 +438,47 @@ def synth_images(batch, height=416, width=416, seed=0):
     return torch.rand(batch, 3, height, width, generator=g)
 
 
+def synth_feature(batch, size, seed):
+    """Head feature map [B, 125, S, S] the region-loss fixtures start from (tests/golden/make_golden_loss.py), regenerated from its seed."""
+    g = torch.Generator().manual_seed(100 + seed)
+    return torch.randn(batch, 125, size, size, generator=g) * 1.5
+
+
+# Fixture activations larger than SAMPLE_MIN_ELEMS are stored as a seeded sample of SAMPLE_FRACTION of their elements (name + '_sample'),
+# next to their full max|.| and L2 norm, so that the fixtures stay small; sample_index() regenerates which elements were kept.
+SAMPLE_MIN_ELEMS = 16384
+SAMPLE_FRACTION = 4
+
+
+def sample_index(numel, seed=0):
+    """Sorted flat indices of the stored sample of a `numel`-element fixture tensor (numpy's legacy generator: stable across machines)."""
+    return np.sort(np.random.RandomState(seed).choice(numel, numel // SAMPLE_FRACTION, replace=False))
+
+
+def store_sampled(out, name, a):
+    """Put array `a` into the fixture dict `out` under `name`, sampled when large (see SAMPLE_MIN_ELEMS)."""
+    a = np.ascontiguousarray(a)
+    if a.size <= SAMPLE_MIN_ELEMS:
+        out[name] = a
+        return
+    out[name + '_sample'] = a.reshape(-1)[sample_index(a.size)]
+    out[name + '_shape'] = np.array(a.shape)
+    out[name + '_absmax'] = np.float64(np.abs(a).max())
+
+
+def load_sampled(g, name):
+    """(flat indices or None, reference values, max|.| of the full tensor) of a fixture stored by store_sampled()."""
+    if name in g.files:
+        a = g[name]
+        return None, a, float(np.abs(a).max())
+    shape = tuple(int(v) for v in g[name + '_shape'])
+    return sample_index(int(np.prod(shape))), g[name + '_sample'], float(g[name + '_absmax'])
+
+
+def has_sampled(g, name):
+    return name in g.files or name + '_sample' in g.files
+
+
 def synth_targets(batch, height=416, width=416, slots=16, num_cls=20, seed=2):
     """G=`slots` GT slots per image, 1..slots real boxes, rest zero rows (utils/data.py:38-41);
     boxes in PIXELS (y, x), centres chosen so floor(centre*S/H) < S."""

@@ -107,8 +107,10 @@ def main():
     x64 = O.synth_images(1, 64, 64, seed=10)
     with torch.no_grad():
         f64 = dnn(x64)
-    np.savez_compressed(os.path.join(HERE, 'darknet_64.npz'), feature=f64.numpy(),
-                        **{'act_' + k: v.numpy() for k, v in outs.items()})
+    acts = {}
+    for k, v in outs.items():
+        O.store_sampled(acts, 'act_' + k, v.numpy())      # the large early layers as a seeded sample (keeps the file under 1 MB)
+    np.savez_compressed(os.path.join(HERE, 'darknet_64.npz'), feature=f64.numpy(), **acts)
 
     # ---- 2. backbone at 416x416: feature + per-layer checksums ------------------------------
     outs.clear()

@@ -33,13 +33,14 @@ MEASURED = {}
 
 
 def record(name, value):
-    """Measured parity figures of this run -> gpurun_out/parity_measured.json (copied to profiles/ when committed)."""
+    """Measured parity figures of this run -> $YB_PARITY_OUT/parity_measured.json when that directory is given."""
     import json
     MEASURED[name] = value
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    os.makedirs(os.path.join(root, 'gpurun_out'), exist_ok=True)
-    with open(os.path.join(root, 'gpurun_out', 'parity_measured.json'), 'w') as f:
-        json.dump(MEASURED, f, indent=1, sort_keys=True)
+    out = os.environ.get('YB_PARITY_OUT')
+    if out:
+        os.makedirs(out, exist_ok=True)
+        with open(os.path.join(out, 'parity_measured.json'), 'w') as f:
+            json.dump(MEASURED, f, indent=1, sort_keys=True)
 
 
 # Contract (BASELINE.json north_star): conv/BN activations within 1e-3 relative of the reference's fp32 -- asserted for
@@ -195,7 +196,7 @@ def test_decode_vs_oracle(ops, shape):
 
 
 # ------------------------------------------------------------------------------------------------
-# convolutions (tcgen05 implicit GEMM) vs the oracle arithmetic
+# convolutions (wgmma implicit GEMM) vs the oracle arithmetic
 # ------------------------------------------------------------------------------------------------
 CONV_CASES = [
     # b, h, w, cin, cout, k, flags-name
@@ -239,10 +240,10 @@ def test_conv_unit_vs_oracle(ops, case):
 
 SK_CASES = [
     # b, h, w, cin, cout, k, bn, mt   (bn 0 = library's choice); every case is forced onto the stream-K path
-    (32, 13, 13, 512, 1024, 3, 0, 0),      # layers2.x: 88 tiles over 148 CTAs, every tile cut once or twice
-    (2, 13, 13, 1024, 1024, 3, 256, 2),    # 8 tiles x 144 K-blocks: each tile is summed from ~19 CTAs
-    (8, 26, 26, 256, 512, 3, 256, 1),      # two accumulator stages: dump / collect overlap the next segment
-    (4, 52, 52, 128, 256, 3, 128, 2),
+    (32, 13, 13, 512, 1024, 3, 0, 0),      # layers2.x: every tile cut across CTAs
+    (2, 13, 13, 1024, 1024, 3, 128, 1),    # 24 tiles x 144 K-blocks: each tile is summed from ~5 CTAs
+    (8, 26, 26, 256, 512, 3, 128, 1),      # register + shared-memory accumulator: dump / collect overlap the next segment
+    (4, 52, 52, 128, 256, 3, 64, 2),
     (3, 13, 13, 1024, 512, 1, 0, 0),       # 1x1
     (5, 19, 17, 64, 72, 3, 64, 1),         # ragged rows, Cout not a multiple of the tile, BK = 64 taps
     (5, 19, 17, 96, 136, 3, 128, 1),       # BK = 32 path, two column tiles with a ragged second one
@@ -345,9 +346,9 @@ def test_conv0_u8_frames_vs_oracle(ops):
     assert rel_err(y.permute(0, 3, 1, 2), ref) <= 1e-3
 
 
-@pytest.mark.parametrize('cfg', [(128, 2), (256, 2), (256, 1), (64, 2)])
+@pytest.mark.parametrize('cfg', [(128, 1), (64, 1), (64, 2), (0, 0)])
 def test_conv_tile_shapes_agree(ops, cfg):
-    """Every CTA tile shape (BLOCK_N x M-subtiles) computes the same result as the oracle arithmetic."""
+    """Every CTA tile shape (BLOCK_N x M-subtiles; (0, 0) = the library's choice) computes the same result as the oracle arithmetic."""
     bn, mt = cfg
     gen = torch.Generator().manual_seed(bn + mt)
     cout = 64 if bn == 64 else 512
@@ -463,9 +464,11 @@ def test_darknet_64_every_layer_golden(darknet, darknet_strict, golden_dir, prec
     feature = dnn.engine.forward(x, collect=collect).clone()
     worst = 0.0
     for key, act in collect.items():
-        if 'act_' + key not in g:
+        if not O.has_sampled(g, 'act_' + key):
             continue
-        e = rel_err(act.permute(0, 3, 1, 2), torch.from_numpy(g['act_' + key]))
+        idx, ref, _ = O.load_sampled(g, 'act_' + key)
+        got = act.permute(0, 3, 1, 2).float().cpu().reshape(-1)
+        e = rel_err(got if idx is None else got[torch.from_numpy(idx)], torch.from_numpy(ref.reshape(-1)))
         worst = max(worst, e)
         assert e <= tol, '%s rel err %.3e' % (key, e)
     e = rel_err(feature, torch.from_numpy(g['feature']))
@@ -594,7 +597,7 @@ def test_region_loss_vs_executed_reference_golden(golden_dir, tag):
     b, s, slots, seed, one_hot = (int(v) for v in g[tag + '_dims'])
     anchors = O.anchors_yolo_voc()
     data = O.norm_data(O.synth_targets(b, s * 32, s * 32, slots=slots, seed=20 + seed), s * 32, s * 32, s, s)
-    f = torch.from_numpy(g[tag + '_feature']).to(DEV).requires_grad_(True)
+    f = O.synth_feature(b, s, seed).to(DEV).requires_grad_(True)
     losses, dbg = model.loss(anchors, {k: v.to(DEV) for k, v in data.items()}, dict(feature=f), 0.6, cross_entropy=not one_hot)
     sum(losses[k] * O.HPARAM_DEFAULT[k] for k in losses).backward()
     for k, v in losses.items():
@@ -1251,7 +1254,7 @@ def test_resnet_kernels_vs_torch(ops):
 
 
 def test_resnet_plugin_vs_reference_golden(golden_dir):
-    """model.resnet.resnet18 / resnet50 on the B200 kernels vs the EXECUTED reference (tests/golden/make_golden_resnet.py): stem pool and
+    """model.resnet.resnet18 / resnet50 on the CUDA kernels vs the EXECUTED reference (tests/golden/make_golden_resnet.py): stem pool and
     every block's output at 64x64, head feature at 64 and 416.  fp16 operands through 17 (resnet18) / 49 (resnet50) convs: <= 3e-3."""
     import detect
     import model

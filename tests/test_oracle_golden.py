@@ -30,8 +30,10 @@ def test_backbone_64_every_layer(golden_dir):
     with torch.no_grad():
         f = O.darknet_forward(sd, x, collect=collect)
     for key, act in collect.items():
-        ref = g['act_' + key]
-        np.testing.assert_allclose(act.numpy(), ref, rtol=0, atol=2e-5 * max(1.0, np.abs(ref).max()), err_msg=key)
+        idx, ref, absmax = O.load_sampled(g, 'act_' + key)
+        got = act.numpy().reshape(-1) if idx is None else act.numpy().reshape(-1)[idx]
+        assert abs(float(np.abs(act.numpy()).max()) - absmax) <= 2e-5 * max(1.0, absmax), key
+        np.testing.assert_allclose(got, ref.reshape(-1), rtol=0, atol=2e-5 * max(1.0, absmax), err_msg=key)
     np.testing.assert_allclose(f.numpy(), g['feature'], rtol=0, atol=2e-5 * np.abs(g['feature']).max())
 
 
@@ -230,16 +232,15 @@ def test_resize_oracle_matches_cv2_golden(golden_dir):
         out = O.resize_u8(O.synth_frame(seed, h0, w0), h, w)
         assert out.shape == (h, w, 3)
         assert hashlib.sha256(out.tobytes()).digest() == g['case%d_sha' % seed].tobytes(), seed
-    jpg = '/root/reference/image.jpg'
-    if os.path.exists(jpg):                                   # build container only: the reference's own sample image
-        import cv2
-        img = cv2.imread(jpg)
-        if hashlib.sha256(img.tobytes()).digest() == g['jpg_src_sha'].tobytes():
-            r, a, b = O.rescale_label(img, g['jpg_yx_min_in'].copy(), g['jpg_yx_max_in'].copy(), 416, 416)
-            assert hashlib.sha256(r.tobytes()).digest() == g['jpg_sha_bgr'].tobytes()
-            assert hashlib.sha256(r[..., ::-1].tobytes()).digest() == g['jpg_sha_rgb'].tobytes()
-            assert np.array_equal(a, g['jpg_yx_min']) and np.array_equal(b, g['jpg_yx_max'])
-            assert np.array_equal(r[100:132, 200:232], g['jpg_crop'])
+    # the reference's own sample image (stored as tests/golden/image.jpg)
+    import cv2
+    img = cv2.imread(os.path.join(golden_dir, 'image.jpg'))
+    assert hashlib.sha256(img.tobytes()).digest() == g['jpg_src_sha'].tobytes()
+    r, a, b = O.rescale_label(img, g['jpg_yx_min_in'].copy(), g['jpg_yx_max_in'].copy(), 416, 416)
+    assert hashlib.sha256(r.tobytes()).digest() == g['jpg_sha_bgr'].tobytes()
+    assert hashlib.sha256(r[..., ::-1].tobytes()).digest() == g['jpg_sha_rgb'].tobytes()
+    assert np.array_equal(a, g['jpg_yx_min']) and np.array_equal(b, g['jpg_yx_max'])
+    assert np.array_equal(r[100:132, 200:232], g['jpg_crop'])
 
 
 @pytest.mark.parametrize('tag', list('abcd'))
@@ -251,7 +252,7 @@ def test_region_loss_oracle_matches_executed_reference(golden_dir, tag):
     g = load(golden_dir, 'loss.npz')
     b, s, slots, seed, one_hot = (int(v) for v in g[tag + '_dims'])
     anchors = O.anchors_yolo_voc()
-    feature = torch.from_numpy(g[tag + '_feature']).clone().requires_grad_(True)
+    feature = O.synth_feature(b, s, seed).requires_grad_(True)
     pred = O.decode(feature, anchors)
     pred['feature'] = feature
     data = O.norm_data(O.synth_targets(b, s * 32, s * 32, slots=slots, seed=20 + seed), s * 32, s * 32, s, s)
@@ -329,11 +330,9 @@ def test_c1_single_image_chain_oracle_matches_executed_reference(golden_dir):
         np.testing.assert_allclose(res[0].numpy(), g['det_iou'], rtol=1e-5, atol=1e-7)
         np.testing.assert_allclose(res[1].numpy(), g['det_yx_min'], rtol=1e-5, atol=1e-5)
         np.testing.assert_allclose(res[4].numpy(), g['det_score'], rtol=1e-5, atol=1e-8)
-    # the stored network input is what the oracle's cv2-exact resize produces from the reference's sample image, if present
-    jpg = '/root/reference/image.jpg'
-    if os.path.exists(jpg):
-        import cv2
-        assert np.array_equal(O.resize_u8(cv2.imread(jpg), 416, 416)[..., ::-1], g['rgb'])
+    # the stored network input is what the oracle's cv2-exact resize produces from the reference's sample image
+    import cv2
+    assert np.array_equal(O.resize_u8(cv2.imread(os.path.join(golden_dir, 'image.jpg')), 416, 416)[..., ::-1], g['rgb'])
 
 
 def test_c2_batch32_oracle_matches_executed_reference(golden_dir):

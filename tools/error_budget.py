@@ -1,13 +1,13 @@
 """Error budget of the EVAL-mode backbone under fp16 operands, in pure CPU fp32 arithmetic with one rounding switched on at a time:
 for every unit, round only its weights (w) or only its input activation (a) to fp16 and measure the head feature against the fp32
-forward.  Result (profiles/r02_error_budget.txt): all 46 roundings contribute alike (~2e-4 relative rms each; the first two layers and
+forward.  Result: all 46 roundings contribute alike (~2e-4 relative rms each; the first two layers and
 the passthrough half of that), they add in quadrature to 1.3e-3 rms = 1.7e-3 max-norm -- there is no offending layer, so reaching the
 reference's 1e-3 contract needs ~3/4 of the roundings removed: b200.engine.STRICT_KEEP.
 
     python tools/error_budget.py
 """
-import sys, time, torch, torch.nn.functional as F
-sys.path.insert(0, '/root/repo')
+import os, sys, time, torch, torch.nn.functional as F
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import yolo2_oracle as O
 torch.set_num_threads(8)
 sd = O.make_state_dict(0)

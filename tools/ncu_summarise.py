@@ -30,7 +30,7 @@ def main(path):
     print('|---|---|---|---|---|---|---|---|---|---|---|---|')
     tot_us = tot_rd = tot_wr = 0.0
     n = 0
-    conv = [0, 0.0, 0.0]      # launches, bytes, us of the tcgen05 conv family (conv_igemm + conv_c32)
+    conv = [0, 0.0, 0.0]      # launches, bytes, us of the wgmma conv family (conv_igemm + conv_c32)
     for r in rows[start + 2:]:
         if len(r) < len(header):
             continue
@@ -53,14 +53,14 @@ def main(path):
     print()
     print('Totals over %d launches: %.1f us, DRAM read %.1f MB + write %.1f MB = %.1f MB (%.1f MB per launch).' % (n, tot_us, tot_rd, tot_wr, tot_rd + tot_wr, (tot_rd + tot_wr) / max(n, 1)))
     if conv[0]:
-        print('tcgen05 conv family (conv_igemm_kernel + conv_c32_kernel): %d launches, %.1f us = %.3f of the listed kernel time, DRAM %.1f MB per launch.'
+        print('wgmma conv family (conv_igemm_kernel + conv_c32_kernel): %d launches, %.1f us = %.3f of the listed kernel time, DRAM %.1f MB per launch.'
               % (conv[0], conv[2], conv[2] / max(tot_us, 1e-9), conv[1] / conv[0] / 1e6))
     if len(sys.argv) > 2:       # traffic.json for bench.py's roofline.traffic
         import json
         with open(sys.argv[2], 'w') as f:
             json.dump(dict(conv_family_dram_bytes_per_launch=(conv[1] / conv[0]) if conv[0] else None, conv_family_launches=conv[0],
                            conv_family_share_of_listed_time=(conv[2] / tot_us) if tot_us else None,
-                           source='%s: dram__bytes_read.sum + dram__bytes_write.sum of the tcgen05 conv launches of one B=32 inference step (ncu --set full)' % sys.argv[3]
+                           source='%s: dram__bytes_read.sum + dram__bytes_write.sum of the wgmma conv launches of one B=32 inference step (ncu --set full)' % sys.argv[3]
                            if len(sys.argv) > 3 else None), f, indent=1)
 
 

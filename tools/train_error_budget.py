@@ -4,10 +4,10 @@ a relative perturbation by ~sqrt(1 + mu^2/sigma^2) per layer (the batch mean it 
 the head feature of this untrained network moves by 3.7e-2 although every layer adds only ~1e-3 -- the reason the end-to-end training
 test (tests/test_gpu_parity.py: C3) asserts losses / statistics and the per-layer test asserts activations.
 
-    python tools/train_error_budget.py 8 416     # batch, size  ->  profiles/r02_train_error_budget.txt
+    python tools/train_error_budget.py 8 416     # batch, size
 """
-import sys, time, torch, torch.nn.functional as F
-sys.path.insert(0, '/root/repo')
+import os, sys, time, torch, torch.nn.functional as F
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import yolo2_oracle as O
 torch.set_num_threads(8)
 sd = O.make_state_dict(0)

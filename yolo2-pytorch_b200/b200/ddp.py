@@ -7,7 +7,7 @@ Replaces the reference's single-process nn.DataParallel (train.py:65-71: replica
 BatchNorm statistics stay per rank (the per-replica statistics of DataParallel); initial parameters and buffers are
 rank 0's (DataParallel replicates GPU 0's module every step).
 
-Design (B200, one process per GPU):
+Design (one process per GPU):
   * every parameter gradient lives in ONE persistent fp32 arena (`GradArena`), laid out in the order the backward chain
     produces them (head first: layers3.0 = 47 MB and layers2.6/2.7 = 38 MB each come out at the very start).  The
     weight-gradient / BatchNorm-gradient kernels write their un-scaled results straight into their arena slots

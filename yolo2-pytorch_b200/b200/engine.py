@@ -1,4 +1,4 @@
-"""Execution plan of the Darknet-19 forward pass on the B200 kernels.
+"""Execution plan of the Darknet-19 forward pass on the CUDA kernels.
 
 The plugin module (`model.yolo2.Darknet`) only holds parameters with the reference's state_dict
 names; this engine turns them into kernel operands (fp16 KRSC weights, folded BN scale/shift),
@@ -174,7 +174,7 @@ class DarknetEngine(object):
         return self._k1 + self._k2 + ['passthrough', 'layers3.0', 'layers3.1']
 
     def set_precision(self, precision, keep=None):
-        """'fast' (default): fp16 operands, one tcgen05 pass per unit; measured end-to-end drift of the head feature vs the
+        """'fast' (default): fp16 operands, one wgmma pass per unit; measured end-to-end drift of the head feature vs the
         reference's fp32 1.1e-3 .. 2.0e-3 (max|d| / max|ref|).  'strict': split-precision operands on every unit except `keep`
         (default STRICT_KEEP) -- inside the reference contract of 1e-3 at ~2.6x the tensor-core work."""
         if precision not in PRECISIONS:
@@ -229,7 +229,7 @@ class DarknetEngine(object):
         (a plan-owned buffer, overwritten by the next call with the same shape).
         `collect` (dict) receives references to every unit's fp16 NHWC output (tests)."""
         if not x.is_cuda:
-            raise RuntimeError('Darknet (B200): input must be a CUDA tensor; there is no CPU fallback')
+            raise RuntimeError('Darknet: input must be a CUDA tensor; there is no CPU fallback')
         u8 = x.dtype == torch.uint8          # raw RGB frames [B,H,W,3]: the kernel applies ToTensor's 1/255
         if u8:
             b, h, w, c = x.shape

@@ -93,7 +93,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             'libyolo2_b200.so not found at %s -- build it with `python yolo2-pytorch_b200/build.py` '
-            '(nvcc, sm_100a).  There is no CPU or PyTorch fallback for this path.' % LIB_PATH)
+            '(nvcc, sm_90a).  There is no CPU or PyTorch fallback for this path.' % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported

@@ -32,7 +32,7 @@ def conv_force_mt(mt):
 
 
 def conv_force_pair(v):
-    """0 = auto, 1 = single-CTA tiles, 2 = CTA pairs (cta_group::2)."""
+    """0 = auto, 1 = single-CTA tiles (the only form on sm_90; 2, CTA pairs, is rejected)."""
     return v << 22
 
 
@@ -49,7 +49,7 @@ def _s():
 
 def _req(t, dtype, name):
     if not (isinstance(t, torch.Tensor) and t.is_cuda):
-        raise RuntimeError('%s must be a CUDA tensor: the B200 path has no CPU fallback' % name)
+        raise RuntimeError('%s must be a CUDA tensor: the GPU path has no CPU fallback' % name)
     if t.dtype != dtype:
         raise TypeError('%s must be %s, got %s' % (name, dtype, t.dtype))
     if not t.is_contiguous():

@@ -1,12 +1,12 @@
-"""Training-mode forward and backward of the Darknet-19 backbone on the B200 kernels.
+"""Training-mode forward and backward of the Darknet-19 backbone on the CUDA kernels.
 
 What the reference gets from torch autograd over nn.Conv2d / BatchNorm2d(train) / LeakyReLU / MaxPool2d /
 reorg / cat (model/yolo2.py:49-65,125-130; train.py:344-351) is issued here as an explicit kernel chain:
 
-  forward, per unit : tcgen05 conv -> raw z (fp16 NHWC) -> batch statistics (double) -> running-stat update
+  forward, per unit : wgmma conv -> raw z (fp16 NHWC) -> batch statistics (double) -> running-stat update
                       (momentum 0.01) -> normalise + leaky (+ 2x2 max-pool) -> a
   backward, per unit: leaky/BN(/pool) backward in two passes (reduce, apply) -> dgamma, dbeta, dz (fp16)
-                      -> tcgen05 weight gradient (pixels are the reduction dim) + tcgen05 data gradient
+                      -> wgmma weight gradient (pixels are the reduction dim) + wgmma data gradient
                       (the forward kernel on dz with rotated, transposed weights)
 
 Gradients travel in fp16 multiplied by `grad_scale` (static loss scaling; parameter gradients are un-scaled in fp32).
@@ -235,11 +235,11 @@ class DarknetTrainer(object):
         self._tracked = []
         eng = self.engine
         if not x.is_cuda:
-            raise RuntimeError('Darknet (B200) training: input must be a CUDA tensor')
+            raise RuntimeError('Darknet training: input must be a CUDA tensor')
         b, _, h, w = x.shape
         x = x.contiguous().float()
         if eng.precision != 'fast':
-            raise RuntimeError("Darknet (B200) training uses fp16 operands with fp32 accumulation; precision='strict' is an inference mode "
+            raise RuntimeError("Darknet training uses fp16 operands with fp32 accumulation; precision='strict' is an inference mode "
                                "(call dnn.engine.set_precision('fast') before train())")
         self._repack(x.device)       # every step: do not trust parameter version counters (fused optimizers do not advance them)
         for u in eng.all_units()[:-1]:
@@ -509,7 +509,7 @@ class TinyTrainer(DarknetTrainer):
     def forward(self, x):
         self._tracked = []
         if not x.is_cuda:
-            raise RuntimeError('Tiny (B200) training: input must be a CUDA tensor')
+            raise RuntimeError('Tiny training: input must be a CUDA tensor')
         b, _, h, w = x.shape
         x = x.contiguous().float()
         dev = x.device
@@ -525,7 +525,7 @@ class TinyTrainer(DarknetTrainer):
         key0, u0, after0 = plan[0]
         c0 = u0.cout
         if c0 > 32 or after0 != 'pool':
-            raise RuntimeError('Tiny (B200): the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
+            raise RuntimeError('Tiny: the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
         w0 = torch.zeros(32, 3, 3, 3, dtype=torch.float32, device=dev)
         w0[:c0].copy_(u0.conv.weight.detach())
         z = self._zeros(('z0', b, h, w), (b, h, w, 32), dev)
@@ -654,7 +654,7 @@ class _TinyEngineView(object):
 
 
 class _BNUnit(object):
-    """What the BatchNorm helpers read of a unit, for layers that are not tcgen05 conv units (first conv, depthwise)."""
+    """What the BatchNorm helpers read of a unit, for layers that are not wgmma conv units (first conv, depthwise)."""
 
     def __init__(self, bn, cout):
         self.bn, self.cout = bn, cout
@@ -664,7 +664,7 @@ class _BNUnit(object):
 class MobileNetTrainer(DarknetTrainer):
     """Training-mode forward / backward of `model.mobilenet.MobileNet` (reference model/mobilenet.py:25-85): conv_bn(3, 32, stride 2), thirteen
     [depthwise 3x3 (stride 1 or 2) + BN + ReLU, pointwise 1x1 + BN + ReLU] units, a 1x1 head with bias.  Pointwise convs, their weight /
-    data gradients and the head run on the tcgen05 kernels of the Darknet path; the depthwise and first-layer kernels are HBM-bound CUDA-core
+    data gradients and the head run on the wgmma kernels of the Darknet path; the depthwise and first-layer kernels are HBM-bound CUDA-core
     kernels (csrc/mobilenet_ops.cu).  BatchNorm momentum is the PyTorch default 0.1 here (read from the modules), the activation ReLU."""
 
     def __init__(self, dnn, grad_scale=16384.0):
@@ -696,7 +696,7 @@ class MobileNetTrainer(DarknetTrainer):
     def forward(self, x):
         self._tracked = []
         if not x.is_cuda:
-            raise RuntimeError('MobileNet (B200) training: input must be a CUDA tensor')
+            raise RuntimeError('MobileNet training: input must be a CUDA tensor')
         b, _, h, w = x.shape
         x = x.contiguous().float()
         dev = x.device
@@ -705,7 +705,7 @@ class MobileNetTrainer(DarknetTrainer):
         saved.x, saved.b, saved.h, saved.w, saved.units = x, b, h, w, []
         first = self.dnn.layers[0]
         if first.conv.weight.shape[0] != 32:
-            raise ValueError('MobileNet (B200): the first layer must have 32 output channels')
+            raise ValueError('MobileNet: the first layer must have 32 output channels')
         hh, ww = h // 2, w // 2
         z = torch.empty(b, hh, ww, 32, dtype=torch.float16, device=dev)
         ops.call('yb_mb_conv0_raw_fwd', x, first.conv.weight.detach().contiguous(), z, b, h, w)
@@ -773,7 +773,7 @@ class MobileNetTrainer(DarknetTrainer):
         one, zero = self._ones(cin, dev)
         g = ops.conv_bn_act(dzh, wdh, one, zero, 1.0)
         for key, sd, sp in reversed(saved.units):
-            # pointwise unit: generic BN backward + tcgen05 weight / data gradient (state-dict names layers.N.pw.*)
+            # pointwise unit: generic BN backward + wgmma weight / data gradient (state-dict names layers.N.pw.*)
             g = self._unit_backward(key + '.pw', sp, b, grads, da=g)
             # depthwise unit
             ch = sd.u.cout

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""Build libyolo2_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libyolo2_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python yolo2-pytorch_b200/build.py [--force] [--verbose]
 
 One object per translation unit (parallel), then a shared library with the static CUDA runtime so
-it does not depend on which libcudart the hosting process (PyTorch) loaded.  The .so is
-git-ignored but travels to the GPU box with the gpurun snapshot.
+it does not depend on which libcudart the hosting process (PyTorch) loaded.  The .so and the
+objects are build products (git-ignored).
 """
 import argparse
 import concurrent.futures
@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 OUT = os.path.join(HERE, 'libyolo2_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC',
          '--expt-relaxed-constexpr', '-Xptxas', '-v']
 
 
@@ -47,7 +47,7 @@ def build(force=False, verbose=False):
     if verbose:
         for _, log in results:
             sys.stderr.write(log)
-    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-Xcompiler', '-fPIC', '-ldl']
+    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-Xcompiler', '-fPIC', '-ldl']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

@@ -1,6 +1,6 @@
 // conv0 (layers1.0): 3x3 conv, Cin = 3 -> Cout = 32, + folded BN + leaky-ReLU + 2x2 max-pool, on the
 // tensor cores.  Replaces nn.Conv2d(3,32,3,pad 1) -> BatchNorm2d -> LeakyReLU -> MaxPool2d(2)
-// (/root/reference model/yolo2.py:78-79) and doubles as the layout boundary: it reads the caller's
+// (reference model/yolo2.py:78-79) and doubles as the layout boundary: it reads the caller's
 // image batch (fp32 NCHW as the reference's ToTensor produces it, or raw uint8 NHWC frames scaled
 // by 1/255 == torchvision ToTensor) and writes the first fp16 NHWC activation.
 //
@@ -8,11 +8,11 @@
 // builds the A operand itself: a 16x32-pixel conv tile (+1 halo) is staged in shared memory once,
 // each of the 128 threads converts the 4x4x3 patch of ONE 2x2 pool window to fp16 and writes the
 // four im2col rows (K padded to 32, 64-byte rows, 64B-swizzled exactly like a TMA box would be)
-// into four 128-row M-tiles -- M-tile j holds pixel j of every window.  One thread issues
-// 4 x 2 tcgen05.mma (M=128, N=32, K=16) into four TMEM accumulators; in the epilogue thread t reads
-// lane t of all four accumulators = the four conv outputs of its window, applies scale/shift +
-// leaky, takes the max in registers and stores the pooled pixel's 32 channels as 64 contiguous
-// bytes.  Persistent CTAs (4 per SM), weights (B operand) built once per CTA.
+// into four 128-row M-tiles -- M-tile j holds pixel j of every window.  The CTA (one warpgroup)
+// issues 4 x 2 x 2 wgmma (M=64, N=32, K=16) into four register accumulators; every accumulator
+// has the same row -> thread mapping, so a thread holds the four conv outputs of each window row
+// it owns, applies scale/shift + leaky, takes the max in registers and stores the pooled pixel's
+// channels.  Persistent CTAs (2 per SM), weights (B operand) built once per CTA.
 #include "yb_common.h"
 #include "yb_ptx.cuh"
 #include <stdlib.h>
@@ -23,12 +23,8 @@ constexpr int kT0Rows = 16, kT0Cols = 32;          // conv pixels per tile (8 x 
 constexpr int kPatchRows = kT0Rows + 2, kPatchCols = kT0Cols + 2, kPatchPitch = 48;
 constexpr int kC0Out = 32;
 
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
+// CTAs per SM: each thread keeps 4 x 2 x 16 fp32 accumulators in registers
+constexpr int kC0CtasPerSm = 2;
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
@@ -50,25 +46,15 @@ struct Conv0Params {
 };
 
 template <bool kU8>
-__global__ void __launch_bounds__(128, 4) conv0_tc_kernel(const Conv0Params p) {
+__global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_tc_kernel(const Conv0Params p) {
   __shared__ __align__(1024) uint8_t a_smem[4 * 128 * 64];          // 4 M-tiles x 128 rows x 64 B (SW64)
   __shared__ __align__(1024) uint8_t b_smem[kC0Out * 64];           // 32 rows (Cout) x 64 B (SW64)
   __shared__ __align__(16) float patch[3][kPatchRows][kPatchPitch];
   __shared__ __align__(16) float sc[kC0Out], sh[kC0Out];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_slot;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t a_base = smem_u32(a_smem), b_base = smem_u32(b_smem), bar_addr = smem_u32(&bar);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t a_base = smem_u32(a_smem), b_base = smem_u32(b_smem);
 
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(smem_u32(&tmem_slot), 128);
-    tmem_relinquish();
-  }
   if (tid < kC0Out) { sc[tid] = p.scale[tid]; sh[tid] = p.shift[tid]; }
   {
     // B operand: row n = output channel, k = ci*9 + r*3 + s (the OIHW flattening), zero padded to 32
@@ -82,16 +68,11 @@ __global__ void __launch_bounds__(128, 4) conv0_tc_kernel(const Conv0Params p) {
     const uint4 pk = make_uint4(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]), pack_h2(v[4], v[5]), pack_h2(v[6], v[7]));
     *reinterpret_cast<uint4*>(b_smem + n * 64 + ((j ^ ((n >> 1) & 3)) << 4)) = pk;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   pdl_trigger();        // lets a PDL successor (the next conv) set up while this grid drains
 
-  const int wy = tid >> 4, wx = tid & 15;        // this thread's pool window inside the tile
+  const int wy = tid >> 4, wx = tid & 15;        // the pool window whose im2col rows this thread builds
   const int oh = p.height >> 1, ow = p.width >> 1;
-  uint32_t phase = 0;
-  constexpr uint32_t idesc = make_idesc_f16(128, kC0Out);
 
   constexpr int kPatchElems = 3 * kPatchRows * kPatchCols;
   constexpr int kPatchIters = (kPatchElems + 127) / 128;
@@ -174,81 +155,80 @@ __global__ void __launch_bounds__(128, 4) conv0_tc_kernel(const Conv0Params p) {
         *reinterpret_cast<uint4*>(row + ((q ^ sw) << 4)) = pk;
       }
     }
-    // generic-proxy smem writes -> visible to the tensor core (async proxy); previous tile's TMEM
-    // reads are ordered before the MMAs that overwrite the accumulators
+    // generic-proxy smem writes -> visible to the tensor core (async proxy)
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    // ---- 3. MMA: 4 accumulators x (K = 32 = 2 x 16) ----
-    if (tid == 0) {
-      tc_fence_after();
+    // ---- 3. MMA: 4 accumulators x 2 row halves x (K = 32 = 2 x 16) ----
+    float acc[4][2][16];
+    {
       const uint64_t bdesc = make_kmajor_desc<64>(b_base);
+      wgmma_fence();
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const uint64_t adesc = make_kmajor_desc<64>(a_base + j * (128 * 64));
-        umma_f16(tmem_base + j * kC0Out, adesc, bdesc, idesc, 0);
-        umma_f16(tmem_base + j * kC0Out, adesc + 2, bdesc + 2, idesc, 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t adesc = make_kmajor_desc<64>(a_base + j * (128 * 64) + h * (64 * 64));
+          wgmma_f16<kC0Out>(acc[j][h], adesc, bdesc, 0);
+          wgmma_f16<kC0Out>(acc[j][h], adesc + 2, bdesc + 2, 1);
+        }
       }
-      umma_commit(bar_addr);
+      wgmma_commit();
     }
     {
-      const int next = tile + gridDim.x;          // overlap the next tile's input fetch with MMA + epilogue
+      const int next = tile + gridDim.x;          // overlap the next tile's input fetch with the MMAs
       if (next < p.num_tiles) prefetch(next, pre);
     }
-    mbar_wait(bar_addr, phase, p.dbg, 0x500);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- 4. epilogue: scale/shift + leaky on the 4 pixels of the window, max, fp16 NHWC store ----
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    const int py = ty * (kT0Rows / 2) + wy, px = tx * (kT0Cols / 2) + wx;
-    __half* dst = p.y + ((static_cast<long long>(img) * oh + py) * ow + px) * kC0Out;
+    wgmma_wait<0>();
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint32_t v[4][8];
+    for (int j = 0; j < 4; ++j) { fence_regs(acc[j][0]); fence_regs(acc[j][1]); }
+    // ---- 4. epilogue: scale/shift + leaky on the 4 pixels of each window, max, fp16 NHWC store ----
+    // accumulator row m (= pool window m of the tile) of fragment half (h, hh), channels 8 jj + 2 (lane % 4) + {0, 1}
 #pragma unroll
-      for (int j = 0; j < 4; ++j) tmem_ld_32x32b_x8(lane_addr + j * kC0Out + g * 8, v[j]);
-      tmem_ld_wait();
-      if (p.raw) {
-        // training mode: the raw (pre-BatchNorm) conv output of the 4 pixels of this window, unpooled
+    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int yy = ty * kT0Rows + 2 * wy + (j >> 1), xx = tx * kT0Cols + 2 * wx + (j & 1);
-          *reinterpret_cast<uint4*>(p.y + ((static_cast<long long>(img) * p.height + yy) * p.width + xx) * kC0Out + g * 8) =
-              make_uint4(pack_h2(__uint_as_float(v[j][0]), __uint_as_float(v[j][1])), pack_h2(__uint_as_float(v[j][2]), __uint_as_float(v[j][3])),
-                         pack_h2(__uint_as_float(v[j][4]), __uint_as_float(v[j][5])), pack_h2(__uint_as_float(v[j][6]), __uint_as_float(v[j][7])));
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = 64 * h + 16 * warp + (lane >> 2) + 8 * hh;
+        const int my = m >> 4, mx = m & 15;
+        const int py = ty * (kT0Rows / 2) + my, px = tx * (kT0Cols / 2) + mx;
+        __half* dst = p.y + ((static_cast<long long>(img) * oh + py) * ow + px) * kC0Out;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int c = 8 * jj + 2 * (lane & 3);
+          if (p.raw) {
+            // training mode: the raw (pre-BatchNorm) conv output of the 4 pixels of this window, unpooled
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const int yy = ty * kT0Rows + 2 * my + (j >> 1), xx = tx * kT0Cols + 2 * mx + (j & 1);
+              *reinterpret_cast<uint32_t*>(p.y + ((static_cast<long long>(img) * p.height + yy) * p.width + xx) * kC0Out + c) =
+                  pack_h2(acc[j][h][4 * jj + 2 * hh], acc[j][h][4 * jj + 2 * hh + 1]);
+            }
+            continue;
+          }
+          float mm[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float s = sc[c + e], b = sh[c + e];
+            float best = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              float t = acc[j][h][4 * jj + 2 * hh + e] * s + b;
+              t = t > 0.f ? t : t * p.slope;
+              best = fmaxf(best, t);
+            }
+            mm[e] = best;
+          }
+          *reinterpret_cast<uint32_t*>(dst + c) = pack_h2(mm[0], mm[1]);
         }
-        continue;
       }
-      float m[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float s = sc[g * 8 + e], b = sh[g * 8 + e];
-        float best = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float t = __uint_as_float(v[j][e]) * s + b;
-          t = t > 0.f ? t : t * p.slope;
-          best = fmaxf(best, t);
-        }
-        m[e] = best;
-      }
-      *reinterpret_cast<uint4*>(dst + g * 8) = make_uint4(pack_h2(m[0], m[1]), pack_h2(m[2], m[3]), pack_h2(m[4], m[5]), pack_h2(m[6], m[7]));
     }
-    // The next tile's barriers (after patch staging and before its MMAs) order these TMEM reads
-    // and this tile's smem reads before anything is overwritten.
-    tc_fence_before();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
+    // The next tile's barrier (after patch staging, before its MMAs) orders this tile's smem reads before anything is
+    // overwritten.
   }
 }
 
 // ---------------------------------------------------------------------------------------------
-// Second form of the same layer: NO thread-built im2col rows.  The first form above spends its time writing four 64-byte im2col rows
-// per thread (ncu: SM 61 %, tensor pipe 6 %, DRAM 14 % -- issue-bound at 0.27 of the HBM roofline).  Here the haloed input patch is
+// Second form of the same layer: NO thread-built im2col rows.  The first form above spends most of its instruction issue writing four
+// 64-byte im2col rows per thread while the tensor core and HBM sit mostly idle.  Here the haloed input patch is
 // kept in shared memory as fp16 pixels of 4 channels (r, g, b, 0 = 8 bytes) and the tensor core reads every operand IN PLACE through
 // un-swizzled K-major descriptors: one filter ROW (3 taps x 4 channels = 12, padded to K = 16) of output pixel (y, x) is the 32
 // contiguous bytes starting at patch pixel (y + r, x); pixels two columns apart are 16 bytes apart, which is exactly the row pitch of
@@ -265,35 +245,25 @@ constexpr int kV2Copy = kV2PR * kV2Pitch;                       // 4896 B
 constexpr int kV2Pixels = kV2PR * kV2PC;                        // 612
 constexpr int kV2Iters = (kV2Pixels + 127) / 128;               // 5 pixels per thread
 
-// kRaw (training forward): the un-normalised conv output z goes out at full resolution.  Written 16 B per lane straight from the TMEM layout,
-// every store instruction touched 32 different 128-byte lines (the kernel ran at 2.2 TB/s, bound by L2 write transactions); instead the tile is
-// staged in shared memory (swizzled, conflict-free) and leaves as 512 contiguous bytes per warp instruction.  The copy-out loop hands every thread
+// kRaw (training forward): the un-normalised conv output z goes out at full resolution.  Written straight from the accumulator layout, every
+// store instruction would touch many different 128-byte lines (bound by L2 write transactions); instead the tile is staged in shared memory
+// (swizzled) and leaves as 512 contiguous bytes per warp instruction.  The copy-out loop hands every thread
 // the same 8 channels on every trip, so the BatchNorm batch statistics (sum z, sum z^2 of the fp16 values that are stored) accumulate in 16
 // registers over all of the CTA's tiles and are reduced once at the end (p.stats: double [2][32], as yb_bn_stats).
 constexpr int kV2StageBytes = kV2Rows * kV2Cols * kC0Out * 2;   // 32 KB
 
 template <bool kU8, bool kRaw>
-__global__ void __launch_bounds__(128, 4) conv0_k16_kernel(const Conv0Params p) {
+__global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv0Params p) {
   __shared__ __align__(128) uint8_t stage[kRaw ? kV2StageBytes : 16];
   __shared__ float s_stats[2 * kC0Out];
   __shared__ __align__(128) uint8_t patch_e[kV2Copy + 48];      // pixel (r, c) at (r * 18 + c) * 8: even columns 16 B aligned
   __shared__ __align__(128) uint8_t patch_o[kV2Copy + 48];      // the same pixels at + 8 B: odd columns 16 B aligned
   __shared__ __align__(128) uint8_t b_smem[3 * 1024];           // per filter row: [n / 8][k / 8][n % 8][k % 8] fp16 (32 x 16)
   __shared__ __align__(16) float sc[kC0Out], sh[kC0Out];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tmem_slot;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const uint32_t e_base = smem_u32(patch_e), o_base = smem_u32(patch_o), b_base = smem_u32(b_smem), bar_addr = smem_u32(&bar);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t e_base = smem_u32(patch_e), o_base = smem_u32(patch_o), b_base = smem_u32(b_smem);
 
-  if (tid == 0) {
-    mbar_init(bar_addr, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(smem_u32(&tmem_slot), 128);
-    tmem_relinquish();
-  }
   if (tid < kC0Out) { sc[tid] = p.scale[tid]; sh[tid] = p.shift[tid]; }
   // the bytes past the last patch pixel are read by the K-pad lanes of the last row: keep them finite
   if (tid < 12) {
@@ -313,16 +283,10 @@ __global__ void __launch_bounds__(128, 4) conv0_k16_kernel(const Conv0Params p) 
       *reinterpret_cast<uint2*>(b_smem + r * 1024 + (n >> 3) * 256 + (s4 >> 1) * 128 + (n & 7) * 16 + (s4 & 1) * 8) = pk;
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_slot;
   pdl_trigger();
 
-  const int wy = tid >> 3, wx = tid & 7;         // this thread's pool window inside the tile (its TMEM lane)
   const int oh = p.height >> 1, ow = p.width >> 1;
-  uint32_t phase = 0;
-  constexpr uint32_t idesc = make_idesc_f16(128, kC0Out);
 
   auto prefetch = [&](int t, float (&v)[kV2Iters][3]) {
     const int ptx = t % p.tiles_x;
@@ -359,6 +323,9 @@ __global__ void __launch_bounds__(128, 4) conv0_k16_kernel(const Conv0Params p) 
     const int t2 = tile / p.tiles_x;
     const int ty = t2 % p.tiles_y;
     const int img = t2 / p.tiles_y;
+    // every warp's wgmma of the previous tile has retired (each warp waited on its own part) before any thread overwrites the
+    // operands it read
+    __syncthreads();
     // ---- 1. the patch, twice (8 B per pixel each) ----
 #pragma unroll
     for (int k = 0; k < kV2Iters; ++k) {
@@ -370,68 +337,71 @@ __global__ void __launch_bounds__(128, 4) conv0_k16_kernel(const Conv0Params p) 
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    // ---- 2. MMA: accumulator (dy, dx) += sum over filter rows, operands read in place ----
-    if (tid == 0) {
-      tc_fence_after();
+    // ---- 2. MMA: accumulator (dy, dx) += sum over filter rows, operands read in place.  Accumulator rows = pool windows
+    // (8 per window row, window rows 2 patch rows apart); rows 64..127 start 8 window rows further down ----
+    float acc[4][2][16];
+    wgmma_fence();
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int dy = j >> 1, dx = j & 1;
+    for (int j = 0; j < 4; ++j) {
+      const int dy = j >> 1, dx = j & 1;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
-          const uint32_t a_addr = (dx ? o_base + 8 : e_base) + ((dy + r) * kV2PC + dx) * 8;
-          umma_f16(tmem_base + j * kC0Out, make_kmajor_desc_noswz(a_addr, 16, 2 * kV2Pitch), make_kmajor_desc_noswz(b_base + r * 1024, 128, 256), idesc,
-                   r != 0);
+          const uint32_t a_addr = (dx ? o_base + 8 : e_base) + ((dy + r) * kV2PC + dx) * 8 + h * 8 * (2 * kV2Pitch);
+          wgmma_f16<kC0Out>(acc[j][h], make_kmajor_desc_noswz(a_addr, 16, 2 * kV2Pitch), make_kmajor_desc_noswz(b_base + r * 1024, 128, 256), r != 0);
         }
       }
-      umma_commit(bar_addr);
     }
+    wgmma_commit();
     {
       const int next = tile + gridDim.x;
       if (next < p.num_tiles) prefetch(next, pre);
     }
-    mbar_wait(bar_addr, phase, p.dbg, 0x510);
-    phase ^= 1;
-    tc_fence_after();
-    // ---- 3. epilogue: as the first form, window (wy, wx) = TMEM lane ----
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-    const int py = ty * (kV2Rows / 2) + wy, px = tx * (kV2Cols / 2) + wx;
-    __half* dst = p.y + ((static_cast<long long>(img) * oh + py) * ow + px) * kC0Out;
+    wgmma_wait<0>();
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint32_t v[4][8];
+    for (int j = 0; j < 4; ++j) { fence_regs(acc[j][0]); fence_regs(acc[j][1]); }
+    // ---- 3. epilogue: as the first form, window m = accumulator row ----
 #pragma unroll
-      for (int j = 0; j < 4; ++j) tmem_ld_32x32b_x8(lane_addr + j * kC0Out + g * 8, v[j]);
-      tmem_ld_wait();
-      if constexpr (kRaw) {
-        // pixel (row, col) of the tile lives at slot col' = col / 2 + (col & 1) * 8 of its row (the eight lanes of a quarter-warp then fill
-        // eight consecutive 64-byte slots), 16-byte chunk g at g ^ ((col / 4) & 3)
+    for (int h = 0; h < 2; ++h) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int row = 2 * wy + (j >> 1), slot = wx + (j & 1) * 8;
-          *reinterpret_cast<uint4*>(stage + (row * kV2Cols + slot) * (kC0Out * 2) + ((g ^ ((wx >> 1) & 3)) << 4)) =
-              make_uint4(pack_h2(__uint_as_float(v[j][0]), __uint_as_float(v[j][1])), pack_h2(__uint_as_float(v[j][2]), __uint_as_float(v[j][3])),
-                         pack_h2(__uint_as_float(v[j][4]), __uint_as_float(v[j][5])), pack_h2(__uint_as_float(v[j][6]), __uint_as_float(v[j][7])));
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = 64 * h + 16 * warp + (lane >> 2) + 8 * hh;
+        const int wy = m >> 3, wx = m & 7;
+        const int py = ty * (kV2Rows / 2) + wy, px = tx * (kV2Cols / 2) + wx;
+        __half* dst = p.y + ((static_cast<long long>(img) * oh + py) * ow + px) * kC0Out;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int c = 8 * jj + 2 * (lane & 3);
+          if constexpr (kRaw) {
+            // pixel (row, col) of the tile lives at slot col' = col / 2 + (col & 1) * 8 of its row (the eight windows of a window row
+            // then fill eight consecutive 64-byte slots), 16-byte chunk jj at jj ^ ((col / 4) & 3)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const int row = 2 * wy + (j >> 1), slot = wx + (j & 1) * 8;
+              *reinterpret_cast<uint32_t*>(stage + (row * kV2Cols + slot) * (kC0Out * 2) + ((jj ^ ((wx >> 1) & 3)) << 4) + (lane & 3) * 4) =
+                  pack_h2(acc[j][h][4 * jj + 2 * hh], acc[j][h][4 * jj + 2 * hh + 1]);
+            }
+            continue;
+          }
+          float mm[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float s = sc[c + e], b = sh[c + e];
+            float best = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              float t = acc[j][h][4 * jj + 2 * hh + e] * s + b;
+              t = t > 0.f ? t : t * p.slope;
+              best = fmaxf(best, t);
+            }
+            mm[e] = best;
+          }
+          *reinterpret_cast<uint32_t*>(dst + c) = pack_h2(mm[0], mm[1]);
         }
-        continue;
       }
-      float m[8];
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const float s = sc[g * 8 + e], b = sh[g * 8 + e];
-        float best = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float t = __uint_as_float(v[j][e]) * s + b;
-          t = t > 0.f ? t : t * p.slope;
-          best = fmaxf(best, t);
-        }
-        m[e] = best;
-      }
-      *reinterpret_cast<uint4*>(dst + g * 8) = make_uint4(pack_h2(m[0], m[1]), pack_h2(m[2], m[3]), pack_h2(m[4], m[5]), pack_h2(m[6], m[7]));
     }
-    tc_fence_before();
     if constexpr (kRaw) {
       __syncthreads();                              // the whole tile is staged
       // 2048 chunks of 16 B: chunk c = i * 128 + tid -> row c / 64, (col, g) = c % 64 = tid % 64 on every trip
@@ -476,12 +446,6 @@ __global__ void __launch_bounds__(128, 4) conv0_k16_kernel(const Conv0Params p) 
     __syncthreads();
     if (tid < 2 * kC0Out) atomicAdd(p.stats + tid, static_cast<double>(s_stats[tid]));
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
-  }
 }
 
 int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -506,7 +470,7 @@ int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* sc
   YB_REQUIRE(stats == nullptr || (raw && v2 && !x_is_u8), "conv0: fused statistics need the raw fp32-input form on a 32 x 16-tileable image");
   if (raw) { p.scale = w; p.shift = w; }   // unused in raw mode, must be readable
   p.dbg = debug_word_device();
-  const int max_ctas = sm_count() * 4;
+  const int max_ctas = sm_count() * kC0CtasPerSm;
   const int grid = p.num_tiles < max_ctas ? p.num_tiles : max_ctas;
   if (v2) {
     if (x_is_u8) {

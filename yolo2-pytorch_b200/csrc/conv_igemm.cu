@@ -1,7 +1,7 @@
-// K1: convolution as an implicit GEMM on the 5th-gen tensor cores (tcgen05), sm_100a only.
+// K1: convolution as an implicit GEMM on the Hopper tensor cores (wgmma), sm_90a.
 //
 // Replaces the reference's  nn.Conv2d -> nn.BatchNorm2d(eval) -> nn.LeakyReLU(0.1)  unit
-// (/root/reference model/yolo2.py:49-65) for k in {1,3}, stride 1, pad (k-1)/2.
+// (reference model/yolo2.py:49-65) for k in {1,3}, stride 1, pad (k-1)/2.
 //
 //   D[M = B*H*W pixels, N = Cout] = A[M, K = k*k*Cin] * W[N, K]^T
 //
@@ -9,14 +9,15 @@
 //     M-tile is fetched by ONE im2col-mode TMA (cp.async.bulk.tensor.4d...im2col) straight from
 //     the NHWC fp16 activation into 128B- (or 64B-) swizzled shared memory; halo pixels are
 //     zero-filled by the TMA unit.  W (KRSC fp16, K-major) comes in by a tiled 2D TMA.
-//   * one elected thread issues tcgen05.mma (M=128, N=BN, K=16) with the fp32 accumulator in TMEM
-//     (two accumulator stages so the epilogue of tile i overlaps the mainloop of tile i+1);
-//   * the epilogue warps read TMEM with tcgen05.ld, apply the folded BatchNorm (fp32 scale/shift per
-//     channel) + leaky-ReLU and store fp16 NHWC (optionally into a channel slice of a wider buffer,
-//     which is how torch.cat at yolo2.py:129 disappears) or fp32 NCHW (the head, the tensor the
-//     reference hands to the decoder).
-//   * persistent: grid = min(#tiles, #SMs); warp 0 = TMA producer, warp 1 = MMA issuer + TMEM
-//     owner, warps 2..5 = epilogue (TMEM lane quadrant = warp_id % 4).
+//   * one warpgroup issues wgmma (M=64 x2, N=BN, K=16) with the fp32 accumulator in registers, then
+//     parks the finished tile in a shared-memory accumulator (yb_ptx.cuh) and starts the next tile,
+//     so the epilogue of tile i overlaps the mainloop of tile i+1;
+//   * the epilogue warps read that tile one pixel row per thread, apply the folded BatchNorm (fp32
+//     scale/shift per channel) + leaky-ReLU and store fp16 NHWC (optionally into a channel slice of a
+//     wider buffer, which is how torch.cat at yolo2.py:129 disappears) or fp32 NCHW (the head, the
+//     tensor the reference hands to the decoder).
+//   * persistent: grid = min(#tiles, #SMs); warps 0..3 = MMA warpgroup, warp 4 = TMA producer,
+//     warps 5..8 = epilogue (rows 32 * (warp - 5) .. + 31 of the tile).
 #include "yb_common.h"
 #include "yb_ptx.cuh"
 #include <stdlib.h>
@@ -43,28 +44,28 @@ struct ConvParams {
   int skip;         // profiling ablation (results are garbage): 1 = no A loads, 2 = no B loads, 4 = no MMA, 8 = no stores
   int* dbg;
   // stream-K (streamk != 0): the tiles x K-blocks iteration space is cut into gridDim.x equal contiguous ranges, so a
-  // layer whose tile count does not fill the SMs (13x13: 88 tiles on 148 SMs) still keeps every SM busy.  A CTA
+  // layer whose tile count does not fill the SMs (13x13 at batch 32: 169 tiles of 128 x 128 on 132 SMs) still keeps every SM busy.  A CTA
   // whose range ends inside a tile dumps that partial fp32 accumulator to ws[blockIdx] and raises flags[blockIdx];
   // the CTA that holds the tile's last K-block adds the partials of the (lower-numbered) CTAs and runs the epilogue.
   int streamk;
   int sk_base, sk_rem;         // units per CTA = sk_base (+1 for the first sk_rem CTAs)
   float* ws;                   // [gridDim.x][MT][BN/32][128][32] fp32
   unsigned* flags;             // [gridDim.x], 0 = empty, 1 = partial ready (reset by the consumer)
-  unsigned long long* trace;   // optional (tools/conv_trace.py): block 0 records clock64() per pipeline event, 3 roles x 256 slots
+  unsigned long long* trace;   // optional (yb_conv_set_trace): block 0 records clock64() per pipeline event, 3 roles x 256 slots
   // optional (training): per-channel sum and sum of squares of the STORED (fp16-rounded) outputs, added into
   // stats[0..Cout) / stats[Cout..2Cout) -- the batch statistics of train-mode BatchNorm without a second pass over z
   double* stats;
   // split-precision ("strict") mode.  The reduction dimension of the GEMM is a concatenation of fp16 terms,
   //   A = [a_hi | a_lo | a_hi] (channels of one pixel),  W = [w_hi | w_hi | w_lo] (per tap),
-  // so a_hi*w_hi + a_lo*w_hi + a_hi*w_lo accumulate into ONE fp32 TMEM accumulator: the fp16 rounding of either operand
+  // so a_hi*w_hi + a_lo*w_hi + a_hi*w_lo accumulate into ONE fp32 accumulator: the fp16 rounding of either operand
   // (2^-11 relative, the source of the 1.6e-3 end-to-end drift) drops to ~2^-22.  `cin` is then the concatenated width,
   // `a_wrap` the number of channels the activation tensor really holds (C or 2C): channel offsets past it wrap around.
   // `lo_off` != 0: the epilogue also stores lo = fp16(v - fp32(fp16(v))) at y + lo_off (fp16 NHWC only).
   int a_wrap;
   long long lo_off;
-  // fp16 NHWC output through shared memory + TMA store (tmap_y): the epilogue stages 128 rows x 64 channels (128B-swizzled) and one
-  // thread ships them with a single bulk store.  The per-thread 16 B stores it replaces write 32 half-used sectors per instruction
-  // (lanes = pixels, 2*y_ld bytes apart) and cost 15-30 % of the 104x104 / 1x1 layers (tools/conv_ablate.py: full vs no-store).
+  // fp16 NHWC output through shared memory + TMA store (tmap_y): each epilogue warp stages 32 rows x 64 channels (128B-swizzled) and
+  // one lane ships them with a single bulk store, instead of per-thread 16 B stores that write 32 half-used sectors per instruction
+  // (lanes = pixels, 2*y_ld bytes apart).
   int tma_store;
 };
 
@@ -75,8 +76,12 @@ struct ConvParams {
 constexpr int BM = 128;
 
 constexpr int UMMA_K = 16;
-constexpr int kNumThreads = 192;
+constexpr int kMmaThreads = 128;                // warps 0..3: the MMA warpgroup
+constexpr int kProducerWarp = 4;
+constexpr int kEpiWarp0 = 5;                    // warps 5..8: epilogue
 constexpr int kEpiThreads = 128;
+constexpr int kThreads = kMmaThreads + 32 + kEpiThreads;
+constexpr int kSmemLimit = 232448;              // 227 KB: the per-block opt-in maximum of sm_90
 
 // Work iteration shared by the three warp roles.  Plain mode: whole tiles, strided over the CTAs.  Stream-K mode: the
 // CTA's unit range [s, e) (unit = one K-block of one tile) is walked from its END backwards, one tile segment at a
@@ -122,95 +127,76 @@ __device__ __forceinline__ void st_release_gpu(unsigned* p, unsigned v) {
 
 // MT = number of 128-pixel M-subtiles per CTA tile (1 or 2).  MT = 2 makes the CTA tile 256 x BN: both
 // subtiles reuse the same weight (B) tile from shared memory, halving the L2->SM weight traffic per MAC.
-// kPair = true runs two CTAs of a (2,1,1) cluster as one cta_group::2 unit: every MMA is M = 256 (128 rows
-// from each CTA), each CTA stages only HALF of the weight tile (N/2 rows) and the tensor cores read the other
-// half from the peer SM, so the per-SM operand feed drops again by 25-33%.
-template <int BN, int BK, int MT, bool kPair, int EW = 4>
+// The MMA warpgroup holds MT * BN fp32 accumulators per thread, so MT * BN <= 128.
+template <int BN, int BK, int MT>
 struct ConvCfg {
   static constexpr int kSwizzle = BK * 2;                       // bytes per smem row
   static constexpr int kASubBytes = BM * BK * 2;
   static constexpr int kABytes = MT * kASubBytes;
-  static constexpr int kBRows = kPair ? BN / 2 : BN;            // weight rows staged by this CTA
-  static constexpr int kBBytes = kBRows * BK * 2;
+  static constexpr int kBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kEpiWarps = EW;                          // 4, or 8 = two warps per TMEM lane quarter taking alternate 64-column chunks
-  static constexpr int kThreads = 64 + 32 * EW;
-  static constexpr int kOperandBudget = 196608 - (EW == 8 ? BM * 128 : 0);
-  static constexpr int kStages = (kOperandBudget / kStageBytes) > 8 ? 8 : (kOperandBudget / kStageBytes);
-  static constexpr int kAccCols = MT * BN;                      // TMEM columns of one accumulator stage
-  static constexpr int kAccStages = (2 * kAccCols <= 512) ? 2 : 1;
-  static constexpr int kTmemCols = kAccStages * kAccCols;       // power of two in [64, 512]
-  static constexpr int kRowsPerCta = BM * MT;
-  static constexpr bool kMergedA = (MT == 2 && !kPair);        // A tile fetched by one 256-pixel TMA box
-  static constexpr int kRowsPerTile = kRowsPerCta * (kPair ? 2 : 1);
-  static constexpr int kOutBytes = (EW / 4) * BM * 128;         // TMA-store staging: one 32-row x 64-channel fp16 slice (4 KB) per epilogue warp
-  static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + 1024 /*align slack*/ + 2 * 2 * BN * 4 /*scale/shift x2*/ + 2 * BN * 4 /*stats*/ + 256 /*barriers*/;
-  static_assert(kSmemBytes <= 232448, "shared memory budget");
-  static_assert(kAccCols <= 512, "accumulator does not fit TMEM");
+  static constexpr int kAccCols = MT * BN;                      // columns of the shared-memory accumulator tile
+  static constexpr int kAccBytes = kAccCols * kAccPitch * 4;
+  static constexpr bool kMergedA = (MT == 2);                   // A tile fetched by one 256-pixel TMA box
+  static constexpr int kRowsPerTile = BM * MT;
+  static constexpr int kOutBytes = BM * 128;                    // TMA-store staging: one 32-row x 64-channel fp16 slice (4 KB) per epilogue warp
+  static constexpr int kFixedBytes = kAccBytes + kOutBytes + 1024 /*align slack*/ + 2 * 2 * BN * 4 /*scale/shift x2*/ + 2 * BN * 4 /*stats*/ + 256 /*barriers*/;
+  static constexpr int kStages = ((kSmemLimit - kFixedBytes) / kStageBytes) > 8 ? 8 : ((kSmemLimit - kFixedBytes) / kStageBytes);
+  static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
+  static_assert(kAccCols <= 128, "accumulator does not fit the MMA warpgroup's registers");
+  static_assert(kStages >= 2, "shared memory budget");
 };
 
-template <int BN, int BK, int MT, bool kPair, int EW>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
+template <int BN, int BK, int MT>
+__global__ void __launch_bounds__(kThreads, 1)
 conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
-  using Cfg = ConvCfg<BN, BK, MT, kPair, EW>;
-  constexpr int kEpiThreads = 32 * EW;          // shadows the file-scope constant of the 4-warp form
-  constexpr int kAccStages = Cfg::kAccStages;
+  using Cfg = ConvCfg<BN, BK, MT>;
   constexpr int kStages = Cfg::kStages;
   constexpr bool kMergedA = Cfg::kMergedA;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment for the swizzle atoms (identical offsets in both CTAs of a pair)
+  // 1024-byte alignment for the swizzle atoms
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t smem_a = smem_base;
   const uint32_t smem_b = smem_base + kStages * Cfg::kABytes;
   const uint32_t smem_o = smem_base + kStages * Cfg::kStageBytes;                       // 1024-aligned: stage sizes are multiples of 1 KB
-  float* ep_scale = reinterpret_cast<float*>(smem_gen + kStages * Cfg::kStageBytes + Cfg::kOutBytes);  // [2][BN]
+  float* sacc = reinterpret_cast<float*>(smem_gen + kStages * Cfg::kStageBytes + Cfg::kOutBytes);
+  float* ep_scale = sacc + Cfg::kAccCols * kAccPitch;                                   // [2][BN]
   float* ep_shift = ep_scale + 2 * BN;                                                  // [2][BN]
   float* ep_stats = ep_shift + 2 * BN;                                                  // [2][BN] sum, sum of squares of this tile
   uint64_t* bars = reinterpret_cast<uint64_t*>(ep_stats + 2 * BN);
-  const uint32_t bar_full = smem_u32(bars);                 // [kStages]  (pair: only the leader's are used)
+  const uint32_t bar_full = smem_u32(bars);                 // [kStages]
   const uint32_t bar_empty = bar_full + 8 * kStages;        // [kStages]
-  const uint32_t bar_tfull = bar_empty + 8 * kStages;       // [2]
-  const uint32_t bar_tempty = bar_tfull + 16;               // [2]        (pair: only the leader's are used)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
+  const uint32_t bar_tfull = bar_empty + 8 * kStages;       // accumulator tile written
+  const uint32_t bar_tempty = bar_tfull + 8;                // accumulator tile read
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.m_tiles * p.n_tiles;
-  const uint32_t rank = kPair ? cluster_ctarank() : 0u;     // 0 = leader
-  const int unit_id = kPair ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int num_units = kPair ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
+  const int unit_id = static_cast<int>(blockIdx.x);
+  const int num_units = static_cast<int>(gridDim.x);
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
-      mbar_init(bar_full + 8 * i, kPair ? 2 : 1);
-      mbar_init(bar_empty + 8 * i, 1);
+      mbar_init(bar_full + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, 4);                      // one arrival per MMA warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar_tfull + 8 * i, 1);
-      mbar_init(bar_tempty + 8 * i, (kPair ? 2 : 1) * EW);
-    }
+    mbar_init(bar_tfull, 4);
+    mbar_init(bar_tempty, 4);
     fence_mbar_init();
     fence_proxy_async_smem();
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     if (p.tma_store) tma_prefetch_desc(&tmap_y);
   }
-  if (warp == 1) {
-    if (kPair) { tmem_alloc_pair(smem_u32(tmem_slot), Cfg::kTmemCols); tmem_relinquish_pair(); }
-    else { tmem_alloc(smem_u32(tmem_slot), Cfg::kTmemCols); tmem_relinquish(); }
-  }
-  tc_fence_before();
-  if (kPair) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // PDL: everything above (barrier init, TMEM allocation, descriptor prefetch) overlapped the tail of the previous kernel of the
+  __syncthreads();
+  // PDL: everything above (barrier init, descriptor prefetch) overlapped the tail of the previous kernel of the
   // stream; nothing below may run before that kernel's outputs (our activations / the stream-K workspace) are complete
   pdl_trigger();
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
@@ -220,7 +206,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         const int tile = it.tile;
         const int n_tile = tile % p.n_tiles;
         const int m_tile = tile / p.n_tiles;
-        const int m_cta = m_tile * Cfg::kRowsPerTile + static_cast<int>(rank) * Cfg::kRowsPerCta;
+        const int m_cta = m_tile * Cfg::kRowsPerTile;
         int img[MT], h0[MT], w0[MT];
         int nsub = 0;                      // subtiles that start inside the tensor (the rest are skipped)
 #pragma unroll
@@ -234,17 +220,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
         if (p.skip & 1) nsub = 0;
         if (kMergedA && nsub) nsub = MT;      // the merged box always transfers (and zero-fills) both subtiles
-        uint32_t tx_bytes = nsub * Cfg::kASubBytes + ((p.skip & 2) ? 0 : Cfg::kBBytes);
-        if (kPair) {
-          // the leader's barrier also counts the peer's bytes: recompute the peer's live subtiles
-          const int m_peer = m_tile * Cfg::kRowsPerTile + Cfg::kRowsPerCta;
-          int nsub_peer = 0;
-#pragma unroll
-          for (int t = 0; t < MT; ++t)
-            if (m_peer + t * BM < p.m_total) nsub_peer = t + 1;
-          if (p.skip & 1) nsub_peer = 0;
-          tx_bytes += nsub_peer * Cfg::kASubBytes + ((p.skip & 2) ? 0 : Cfg::kBBytes);     // (only used by rank 0, whose own nsub is MT here or the tile is the last one)
-        }
+        const uint32_t tx_bytes = nsub * Cfg::kASubBytes + ((p.skip & 2) ? 0 : Cfg::kBBytes);
         for (int kb = it.kb0; kb < it.kb1; ++kb) {
           const int tap = kb / p.kb_per_tap;
           const int c0 = (kb - tap * p.kb_per_tap) * BK;    // offset inside the (possibly concatenated) weight row of this tap
@@ -253,12 +229,11 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           const int s = tap - r * p.ksize;
           mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x100 | stage);
           YB_TRACE(0, tr_p); ++tr_p;
-          const uint32_t full = kPair ? leader_addr(bar_full + 8 * stage) : (bar_full + 8 * stage);
-          if (!kPair || rank == 0) mbar_arrive_expect_tx(bar_full + 8 * stage, tx_bytes);
-          else mbar_arrive_remote(bar_full + 8 * stage, 0);
+          const uint32_t full = bar_full + 8 * stage;
+          mbar_arrive_expect_tx(full, tx_bytes);
           if (kMergedA) {
             // one TMA box covers both 128-pixel subtiles (the tensor map's box is BM * MT pixels): the im2col-mode TMA has
-            // a large per-instruction cost (profiles/r01_wgrad_variants.txt), rows past the tensor end are zero-filled
+            // a large per-instruction cost, rows past the tensor end are zero-filled
             if (!(p.skip & 1)) {
               const uint32_t dst = smem_a + stage * Cfg::kABytes;
               if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[0] - p.pad, h0[0] - p.pad, img[0], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
@@ -269,70 +244,71 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           for (int t = 0; t < MT; ++t) {
             if (t < nsub) {
               const uint32_t dst = smem_a + stage * Cfg::kABytes + t * Cfg::kASubBytes;
-              if (p.a_im2col) {
-                if (kPair) tma_load_im2col_4d_pair(dst, &tmap_a, full, ca, w0[t] - p.pad, h0[t] - p.pad, img[t], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
-                else tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[t] - p.pad, h0[t] - p.pad, img[t], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
-              } else {
-                if (kPair) tma_load_2d_pair(dst, &tmap_a, full, ca, m_cta + t * BM);
-                else tma_load_2d(dst, &tmap_a, full, ca, m_cta + t * BM);
-              }
+              if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[t] - p.pad, h0[t] - p.pad, img[t], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+              else tma_load_2d(dst, &tmap_a, full, ca, m_cta + t * BM);
             }
           }
           }
-          const int brow = n_tile * BN + static_cast<int>(rank) * Cfg::kBRows;
-          if (p.skip & 2) { /* ablation: weights not fetched */ }
-          else if (kPair) tma_load_2d_pair(smem_b + stage * Cfg::kBBytes, &tmap_b, full, tap * p.cin + c0, brow);
-          else tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, full, tap * p.cin + c0, brow);
+          if (!(p.skip & 2)) tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, full, tap * p.cin + c0, n_tile * BN);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (pair: leader CTA only) =====================
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(kPair ? 2 * BM : BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int tr_m = 0;
-      for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
-        mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1, p.dbg, 0x200 | acc);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::kAccCols;
-        const int kb_first = it.kb0, kb_last = it.kb1 - 1;
-        for (int kb = kb_first; kb <= kb_last; ++kb) {
-          mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x300 | stage);
-          tc_fence_after();
-          YB_TRACE(1, tr_m); ++tr_m;
+  } else if (warp < kProducerWarp) {
+    // ===================== MMA warpgroup =====================
+    float acc[MT][2][BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t acc_phase = 0;
+    int tr_m = 0;
+    for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
+      const int kb_first = it.kb0, kb_last = it.kb1 - 1;
+      int prev = -1;
+      for (int kb = kb_first; kb <= kb_last; ++kb) {
+        mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x300 | stage);
+        if (threadIdx.x == 0) { YB_TRACE(1, tr_m); ++tr_m; }
+        if (!(p.skip & 4)) {
           const uint64_t bdesc = make_kmajor_desc<Cfg::kSwizzle>(smem_b + stage * Cfg::kBBytes);
+          wgmma_fence();
 #pragma unroll
           for (int t = 0; t < MT; ++t) {
-            if (p.skip & 4) break;
-            const uint64_t adesc = make_kmajor_desc<Cfg::kSwizzle>(smem_a + stage * Cfg::kABytes + t * Cfg::kASubBytes);
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              // advance 16 fp16 = 32 bytes inside the swizzled row: +2 in the 16-byte address field
-              if (kPair) umma_f16_pair(d_tmem + t * BN, adesc + 2 * k, bdesc + 2 * k, idesc, ((kb - kb_first) | k) != 0);
-              else umma_f16(d_tmem + t * BN, adesc + 2 * k, bdesc + 2 * k, idesc, ((kb - kb_first) | k) != 0);
+            for (int h = 0; h < 2; ++h) {
+              const uint64_t adesc = make_kmajor_desc<Cfg::kSwizzle>(smem_a + stage * Cfg::kABytes + t * Cfg::kASubBytes + h * 64 * Cfg::kSwizzle);
+#pragma unroll
+              for (int k = 0; k < BK / UMMA_K; ++k)      // advance 16 fp16 = 32 bytes inside the swizzled row: +2 in the 16-byte address field
+                wgmma_f16<BN>(acc[t][h], adesc + 2 * k, bdesc + 2 * k, ((kb - kb_first) | k) != 0);
             }
           }
-          // free the smem slot (in both CTAs of a pair) once these MMAs retire
-          if (kPair) umma_commit_pair(bar_empty + 8 * stage); else umma_commit(bar_empty + 8 * stage);
-          if (kb == kb_last) {
-            if (kPair) umma_commit_pair(bar_tfull + 8 * acc); else umma_commit(bar_tfull + 8 * acc);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          wgmma_commit();
+          // one group in flight: the previous K-block's MMAs have retired, so its smem slot can be refilled
+          wgmma_wait<1>();
         }
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int t = 0; t < MT; ++t)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) fence_regs(acc[t][h]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      // park the tile for the epilogue once it has drained the previous one
+      mbar_wait(bar_tempty, acc_phase ^ 1, p.dbg, 0x200);
+#pragma unroll
+      for (int t = 0; t < MT; ++t)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) sacc_store<BN>(sacc, h * 64, t * BN, acc[t][h]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_tfull);
+      acc_phase ^= 1;
     }
   } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                    // TMEM lane quadrant this warp may read
-    const int eh = (warp - 2) >> 2;            // EW = 8: which of the quadrant's two warps (they take alternate 64- / 32-column chunks)
-    const int et = threadIdx.x - 64;           // 0 .. 32 * EW - 1
-    int acc = 0;
+    // ===================== epilogue (warps 5..8) =====================
+    const int q = warp - kEpiWarp0;            // tile rows 32 q .. 32 q + 31
+    const int et = threadIdx.x - kEpiWarp0 * 32;   // 0 .. kEpiThreads - 1
     uint32_t acc_phase = 0;
     int buf = 0;
     for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
@@ -345,7 +321,7 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       const bool sk_dump = it.kb1 < p.num_kb;
       const bool sk_collect = !sk_dump && it.kb0 > 0;
       int sk_lo = 0;                           // partials come from CTAs [sk_lo, blockIdx.x)
-      const int m_cta = m_tile * Cfg::kRowsPerTile + static_cast<int>(rank) * Cfg::kRowsPerCta;
+      const int m_cta = m_tile * Cfg::kRowsPerTile;
       // stage this tile's per-channel scale/shift (double-buffered: a warp can be one tile ahead)
       float* sc = ep_scale + buf * BN;
       float* sh = ep_shift + buf * BN;
@@ -378,34 +354,29 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           }
         }
       }
-      asm volatile("bar.sync 1, %0;" :: "n"(32 * EW) : "memory");
-      mbar_wait(bar_tfull + 8 * acc, acc_phase, p.dbg, 0x400 | acc);
-      tc_fence_after();
+      asm volatile("bar.sync 1, %0;" :: "n"(kEpiThreads) : "memory");
+      mbar_wait(bar_tfull, acc_phase, p.dbg, 0x400);
       if (sk_dump) {
         float* wsp = p.ws + static_cast<size_t>(blockIdx.x) * (MT * BN * 128);
 #pragma unroll 1
         for (int t = 0; t < MT; ++t) {
           if (m_cta + t * BM >= p.m_total) break;
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * Cfg::kAccCols + t * BN;
 #pragma unroll 1
           for (int cc = 0; cc < BN / 32; ++cc) {
             if (n0 + cc * 32 >= p.cout) break;
-            if (EW == 8 && (((t * (BN / 32) + cc) & 1) != eh)) continue;
             uint32_t v[32];
-            tmem_ld_32x32b_x32(taddr + cc * 32, v);
-            tmem_ld_wait();
+            sacc_ld_x32(sacc, q * 32 + lane, t * BN + cc * 32, v);
             float4* dst = reinterpret_cast<float4*>(wsp + (static_cast<size_t>(t * (BN / 32) + cc) * 128 + q * 32 + lane) * 32);
 #pragma unroll
             for (int g = 0; g < 8; ++g)
               dst[g] = make_float4(__uint_as_float(v[4 * g]), __uint_as_float(v[4 * g + 1]), __uint_as_float(v[4 * g + 2]), __uint_as_float(v[4 * g + 3]));
           }
         }
-        tc_fence_before();
         __threadfence();
-        asm volatile("bar.sync 1, %0;" :: "n"(32 * EW) : "memory");
+        asm volatile("bar.sync 1, %0;" :: "n"(kEpiThreads) : "memory");
         if (et == 0) st_release_gpu(p.flags + blockIdx.x, 1u);
-        if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+        if (lane == 0) mbar_arrive(bar_tempty);
+        acc_phase ^= 1;
         continue;
       }
 #pragma unroll 1
@@ -413,21 +384,17 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         if (m_cta + t * BM >= p.m_total) break;   // warp-uniform: subtile entirely past the end
         const int row = m_cta + t * BM + q * 32 + lane;
         const bool row_ok = row < p.m_total;
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * Cfg::kAccCols + t * BN;
         int img = 0, pix = 0;
         if (p.out_mode == 1) { img = row / p.hw; pix = row - img * p.hw; }
         if (p.tma_store) {
-          // ---- fp16 NHWC through the staging buffer: 64 channels (two TMEM loads) per bulk store ----
+          // ---- fp16 NHWC through the staging buffer: 64 channels per bulk store ----
 #pragma unroll 1
           for (int c2 = 0; c2 < BN / 64; ++c2) {
             if (n0 + c2 * 64 >= p.cout) break;
-            if (EW == 8 && (((t * (BN / 64) + c2) & 1) != eh)) continue;      // the quadrant's other warp takes this chunk
             uint4 pk[8];
-            // both 32-column halves in flight before the single wait (a TMEM load is a few hundred cycles of latency)
             uint32_t vv[2][32];
-            tmem_ld_32x32b_x32(taddr + (c2 * 2) * 32, vv[0]);
-            tmem_ld_32x32b_x32(taddr + (c2 * 2 + 1) * 32, vv[1]);
-            tmem_ld_wait();
+            sacc_ld_x32(sacc, q * 32 + lane, t * BN + (c2 * 2) * 32, vv[0]);
+            sacc_ld_x32(sacc, q * 32 + lane, t * BN + (c2 * 2 + 1) * 32, vv[1]);
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
               const int cc = c2 * 2 + hh;
@@ -487,19 +454,18 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               }
             }
             // Each epilogue warp ships its own 32 rows (4 KB of the staging tile) with its own bulk store: no block-level barrier in the
-            // epilogue, so while one warp waits for TMEM the others convert / store.  The warp's previous store must have drained its
-            // slice (that wait overlapped the TMEM loads and the math above).
+            // epilogue, so while one warp waits the others convert / store.  The warp's previous store must have drained its slice.
             if (lane == 0) tma_store_wait_read<0>();
             __syncwarp();
             {
-              const uint32_t slice = smem_o + (eh * 4 + q) * 4096 + lane * 128;
+              const uint32_t slice = smem_o + q * 4096 + lane * 128;
 #pragma unroll
               for (int c = 0; c < 8; ++c) st_shared_v4(slice + ((c ^ (lane & 7)) << 4), pk[c]);
             }
             fence_proxy_async_smem();
             __syncwarp();
             if (lane == 0 && !(p.skip & 8)) {
-              tma_store_2d(&tmap_y, smem_o + (eh * 4 + q) * 4096, n0 + c2 * 64, m_cta + t * BM + q * 32);      // rows >= M and channels >= Cout are clipped by the tensor map
+              tma_store_2d(&tmap_y, smem_o + q * 4096, n0 + c2 * 64, m_cta + t * BM + q * 32);      // rows >= M and channels >= Cout are clipped by the tensor map
               tma_store_commit();
             }
           }
@@ -507,10 +473,8 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
 #pragma unroll 1
         for (int cc = 0; cc < BN / 32; ++cc) {
-          if (EW == 8 && (((t * (BN / 32) + cc) & 1) != eh)) continue;
           uint32_t v[32];
-          tmem_ld_32x32b_x32(taddr + cc * 32, v);
-          tmem_ld_wait();
+          sacc_ld_x32(sacc, q * 32 + lane, t * BN + cc * 32, v);
           const int cbase = n0 + cc * 32;
           if (cbase >= p.cout) continue;           // warp-uniform
           if (sk_collect) {
@@ -601,252 +565,40 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           }
         }
       }  // M-subtiles
-      // release this accumulator stage back to the MMA warp (of the leader CTA)
-      tc_fence_before();
+      // hand the accumulator tile back to the MMA warpgroup
       __syncwarp();
-      if (lane == 0) {
-        if (!kPair || rank == 0) mbar_arrive(bar_tempty + 8 * acc);
-        else mbar_arrive_remote(bar_tempty + 8 * acc, 0);
-      }
+      if (lane == 0) mbar_arrive(bar_tempty);
       if (p.stats != nullptr) {
         // this tile's column sums -> the global double accumulators (the bar.sync at the top of the next tile orders the
         // re-zeroing of ep_stats after these reads)
-        asm volatile("bar.sync 1, %0;" :: "n"(32 * EW) : "memory");
+        asm volatile("bar.sync 1, %0;" :: "n"(kEpiThreads) : "memory");
         for (int i = et; i < BN; i += kEpiThreads) {
           if (n0 + i < p.cout) {
             atomicAdd(p.stats + n0 + i, static_cast<double>(ep_stats[i]));
             atomicAdd(p.stats + p.cout + n0 + i, static_cast<double>(ep_stats[BN + i]));
           }
         }
-        asm volatile("bar.sync 1, %0;" :: "n"(32 * EW) : "memory");
+        asm volatile("bar.sync 1, %0;" :: "n"(kEpiThreads) : "memory");
       }
       if (sk_collect) {
         // every reader is done with the partials: hand the slots back (the next writer is a later launch)
-        asm volatile("bar.sync 1, %0;" :: "n"(32 * EW) : "memory");
+        asm volatile("bar.sync 1, %0;" :: "n"(kEpiThreads) : "memory");
         for (int j = sk_lo + et; j < static_cast<int>(blockIdx.x); j += kEpiThreads) p.flags[j] = 0u;
       }
-      if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+      acc_phase ^= 1;
     }
     if (p.tma_store && lane == 0) tma_store_wait<0>();     // every bulk store of this warp has landed before the CTA's shared memory goes away
   }
-
-  tc_fence_before();
-  if (kPair) cluster_sync_all(); else __syncthreads();   // pair: nobody leaves while the peer may still touch its smem / barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if (kPair) tmem_dealloc_pair(tmem_base, Cfg::kTmemCols); else tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
-// Small-K variant for 3x3 convs with Cin = 32 (layers1.2: K = 288).  With the generic kernel every K-block is a
-// 32-channel sliver (2 MMAs), so the producer->MMA->commit hand-shake (~250 ns per K-block) dominates.  Here the
-// whole weight matrix (9 taps x [BN x 32]) stays resident in shared memory for the life of the CTA and one pipeline
-// stage carries ALL 9 taps of a 128-pixel tile: one barrier round trip and 18 MMAs per tile instead of 9 and 2.
-// ---------------------------------------------------------------------------------------------
-template <int BN>
-struct SmallKCfg {
-  static constexpr int kTaps = 9, BK = 32;
-  static constexpr int kATap = BM * BK * 2;            // 8 KB
-  static constexpr int kAStage = kTaps * kATap;        // 72 KB
-  static constexpr int kBTap = BN * BK * 2;            // 4 KB (BN = 64)
-  static constexpr int kBBytes = kTaps * kBTap;        // 36 KB, resident
-  static constexpr int kStages = 2;
-  static constexpr int kThreads = 64 + 256;            // TMA warp, MMA warp, 8 epilogue warps (two per TMEM lane quarter)
-  static constexpr int kOutBytes = BM * BN * 2;       // 16 KB staging tile for the TMA-store epilogue (x2)
-  static constexpr int kSmemBytes = kStages * kAStage + kBBytes + 2 * kOutBytes + 1024 + 2 * 2 * BN * 4 + 256;
-};
-
-template <int BN>
-__global__ void __launch_bounds__(SmallKCfg<BN>::kThreads, 1)
-conv_smallk_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const __grid_constant__ CUtensorMap tmap_y, const ConvParams p, const int tma_store) {
-  using Cfg = SmallKCfg<BN>;
-  constexpr int kStages = Cfg::kStages;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t smem_a = smem_base;
-  const uint32_t smem_b = smem_base + kStages * Cfg::kAStage;
-  const uint32_t smem_o = smem_b + Cfg::kBBytes;       // 1024-aligned (72K, 36K are multiples of 1024)
-  float* ep_scale = reinterpret_cast<float*>(smem_gen + kStages * Cfg::kAStage + Cfg::kBBytes + 2 * Cfg::kOutBytes);
-  float* ep_shift = ep_scale + 2 * BN;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ep_shift + 2 * BN);
-  const uint32_t bar_full = smem_u32(bars);
-  const uint32_t bar_empty = bar_full + 8 * kStages;
-  const uint32_t bar_tfull = bar_empty + 8 * kStages;
-  const uint32_t bar_tempty = bar_tfull + 16;
-  const uint32_t bar_w = bar_tempty + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 5);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = p.m_tiles * p.n_tiles;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kStages; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(bar_tfull + 8 * i, 1); mbar_init(bar_tempty + 8 * i, 8); }
-    mbar_init(bar_w, 1);
-    fence_mbar_init();
-    fence_proxy_async_smem();
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_y);
-  }
-  if (warp == 1) { tmem_alloc(smem_u32(tmem_slot), 2 * BN); tmem_relinquish(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // resident weights: this CTA works on one column tile only when n_tiles == 1 (checked on the host)
-      mbar_arrive_expect_tx(bar_w, Cfg::kBBytes);
-      for (int t = 0; t < Cfg::kTaps; ++t) tma_load_2d(smem_b + t * Cfg::kBTap, &tmap_b, bar_w, t * p.cin, 0);
-      int stage = 0; uint32_t phase = 0; int tr = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = tile * BM;
-        const int img = m0 / p.hw;
-        const int rem = m0 - img * p.hw;
-        const int h0 = rem / p.width, w0 = rem - h0 * p.width;
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x900 | stage);
-        YB_TRACE(0, tr); ++tr;
-        if (p.skip & 1) { mbar_arrive(bar_full + 8 * stage); if (++stage == kStages) { stage = 0; phase ^= 1; } continue; }
-        mbar_arrive_expect_tx(bar_full + 8 * stage, Cfg::kAStage);
-        for (int t = 0; t < Cfg::kTaps; ++t)
-          tma_load_im2col_4d(smem_a + stage * Cfg::kAStage + t * Cfg::kATap, &tmap_a, bar_full + 8 * stage, 0, w0 - 1, h0 - 1, img,
-                             static_cast<uint16_t>(t % 3), static_cast<uint16_t>(t / 3));
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN);
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0; int tr = 0;
-      mbar_wait(bar_w, 0, p.dbg, 0xA00);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1, p.dbg, 0xA10 | acc);
-        YB_TRACE(1, tr); ++tr;
-        mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0xA20 | stage);
-        tc_fence_after();
-        YB_TRACE(1, tr); ++tr;
-#pragma unroll
-        for (int t = 0; t < Cfg::kTaps; ++t) {
-          if (p.skip & 4) break;
-          const uint64_t adesc = make_kmajor_desc<64>(smem_a + stage * Cfg::kAStage + t * Cfg::kATap);
-          const uint64_t bdesc = make_kmajor_desc<64>(smem_b + t * Cfg::kBTap);
-          umma_f16(tmem_base + acc * BN, adesc, bdesc, idesc, t != 0);
-          umma_f16(tmem_base + acc * BN, adesc + 2, bdesc + 2, idesc, 1);
-        }
-        umma_commit(bar_empty + 8 * stage);
-        umma_commit(bar_tfull + 8 * acc);
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else {
-    const int q = warp & 3;                 // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;       // which 32-column half of the 64-wide tile this warp converts
-    const int et = threadIdx.x - 64;
-    int acc = 0; uint32_t acc_phase = 0; int tr = 0;
-    for (int i = et; i < BN; i += 256) {
-      ep_scale[i] = (i < p.cout) ? __ldg(p.scale + i) : 0.f;
-      ep_shift[i] = (i < p.cout) ? __ldg(p.shift + i) : 0.f;
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(bar_tfull + 8 * acc, acc_phase, p.dbg, 0xA30 | acc);
-      tc_fence_after();
-      if (et == 0) { YB_TRACE(2, tr); ++tr; }
-      const int row = tile * BM + q * 32 + lane;
-      const bool row_ok = row < p.m_total;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      if (tma_store) {
-        // stage the 128 x 64 fp16 tile in shared memory (128 B rows, 128B-swizzled so the 16 B chunk writes of a
-        // quarter-warp hit distinct banks) and let one thread ship it with a single TMA store; the tensor map clips
-        // rows >= M and channels >= Cout.
-        const uint32_t obuf = smem_o + acc * Cfg::kOutBytes;
-        if (et == 0) tma_store_wait_read<1>();          // the store issued two tiles ago has finished reading this buffer
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (et == 0) { YB_TRACE(2, tr); ++tr; }
-        const int r = q * 32 + lane;
-        {
-          const int cc = half;
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(taddr + cc * 32, v);
-          tmem_ld_wait();
-          const int cbase = cc * 32;
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float f[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float x = __uint_as_float(v[g * 8 + j]) * ep_scale[cbase + g * 8 + j] + ep_shift[cbase + g * 8 + j];
-              f[j] = x > 0.f ? x : x * p.slope;
-            }
-            uint4 pk;
-            __half2 h0 = __floats2half2_rn(f[0], f[1]), h1 = __floats2half2_rn(f[2], f[3]), h2 = __floats2half2_rn(f[4], f[5]), h3 = __floats2half2_rn(f[6], f[7]);
-            pk.x = *reinterpret_cast<uint32_t*>(&h0); pk.y = *reinterpret_cast<uint32_t*>(&h1);
-            pk.z = *reinterpret_cast<uint32_t*>(&h2); pk.w = *reinterpret_cast<uint32_t*>(&h3);
-            const int chunk = cc * 4 + g;
-            st_shared_v4(obuf + r * 128 + ((chunk ^ (r & 7)) << 4), pk);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-        if (et == 0) { YB_TRACE(2, tr); ++tr; }
-        fence_proxy_async_smem();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (et == 0 && !(p.skip & 8)) { tma_store_2d(&tmap_y, obuf, 0, tile * BM); tma_store_commit(); }
-        if (et == 0) { YB_TRACE(2, tr); ++tr; }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        continue;
-      }
-      for (int cc = half; cc <= half; ++cc) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr + cc * 32, v);
-        tmem_ld_wait();
-        const int cbase = cc * 32;
-        if (cbase >= p.cout || !row_ok || (p.skip & 8)) continue;
-        __half* dst = reinterpret_cast<__half*>(p.y) + static_cast<long long>(row) * p.y_ld + p.y_ch_off + cbase;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          if (cbase + g * 8 < p.cout) {
-            float f[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float x = __uint_as_float(v[g * 8 + j]) * ep_scale[cbase + g * 8 + j] + ep_shift[cbase + g * 8 + j];
-              f[j] = x > 0.f ? x : x * p.slope;
-            }
-            uint4 pk;
-            __half2 h0 = __floats2half2_rn(f[0], f[1]), h1 = __floats2half2_rn(f[2], f[3]), h2 = __floats2half2_rn(f[4], f[5]), h3 = __floats2half2_rn(f[6], f[7]);
-            pk.x = *reinterpret_cast<uint32_t*>(&h0); pk.y = *reinterpret_cast<uint32_t*>(&h1);
-            pk.z = *reinterpret_cast<uint32_t*>(&h2); pk.w = *reinterpret_cast<uint32_t*>(&h3);
-            *reinterpret_cast<uint4*>(dst + g * 8) = pk;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
-    if (tma_store && et == 0) tma_store_wait<0>();      // all bulk stores complete before the CTA's smem goes away
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 2 * BN); }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Halo-tile kernel for 3x3, Cin = 32 (layers1.2).  The im2col formulations above pull every input pixel through the
-// L2 -> SM path nine times (once per tap) -- 779 MB for 88 MB of input at batch 32, and the clock64 trace
-// (profiles/r01_conv_trace.txt) shows the MMA warp waiting on exactly that.  Here an output tile is a 16 x 8 pixel
+// Halo-tile kernel for 3x3, Cin = 32 (layers1.2).  The im2col formulation above pulls every input pixel through the
+// L2 -> SM path nine times (once per tap): 779 MB for 88 MB of input at batch 32.  Here an output tile is a 16 x 8 pixel
 // rectangle and its 18 x 10 x 32ch input halo is fetched ONCE (11.5 KB instead of 72 KB) as four 8-channel planes
 // [pixel][16 B].  In that layout a 3x3 tap is just a shifted window: 8 consecutive pixels of a halo row form one 8 x 16 B
 // core matrix of the un-swizzled K-major operand format, the next output row is +10 pixels (SBO = 160 B) and the second
-// K chunk is the next plane (LBO), so tcgen05.mma reads all nine taps straight out of the halo tile by moving the
-// descriptor's start address by (r * 10 + s) * 16 B.  Weights stay resident (as in the small-K kernel); the epilogue can
+// K chunk is the next plane (LBO), so wgmma reads all nine taps straight out of the halo tile by moving the
+// descriptor's start address by (r * 10 + s) * 16 B.  Weights stay resident in shared memory; the epilogue can
 // apply the 2x2 max-pool that follows this layer (lane ^ 1 and lane ^ 8 hold the horizontal / vertical neighbours) and
 // ships the tile with one TMA store, so the un-pooled activation never reaches HBM in inference.
 // ---------------------------------------------------------------------------------------------
@@ -869,16 +621,17 @@ struct C32Cfg {
   static constexpr int kPlaneData = HH * HW * 16;                 // 2880 B written by one TMA box
   static constexpr int kPlane = (kPlaneData + 127) / 128 * 128;   // 2944: TMA destinations are 128 B aligned
   static constexpr int kHalo = 4 * kPlane;                        // 11776
-  static constexpr int kStages = 6;
+  static constexpr int kStages = 4;
   static constexpr int BN = 64;
   static constexpr int kBTap = BN * 32 * 2;                       // 4 KB
   static constexpr int kBBytes = 9 * kBTap;                       // 36 KB resident
   static constexpr int kOutBytes = 128 * 128;                     // staging tile for the TMA store (2 per epilogue group)
-  static constexpr int kAccStages = 4;
-  static constexpr int kGroups = 3;                               // epilogue groups of four warps (tools/conv_ablate.py: the per-tile epilogue chain, not the MMA, bounds this kernel)
+  static constexpr int kGroups = 2;                               // epilogue groups of four warps, one accumulator tile each
+  static constexpr int kAccBytes = BN * kAccPitch * 4;
   static constexpr int kEpiThreads = kGroups * 128;
-  static constexpr int kThreads = 64 + kEpiThreads;
-  static constexpr int kSmemBytes = 1024 + kBBytes + 2 * kGroups * kOutBytes + kStages * kHalo + 2 * BN * 4 + 256 + 2 * BN * 4 /*stats*/;
+  static constexpr int kThreads = 128 + 32 + kEpiThreads;         // MMA warpgroup, TMA warp, epilogue groups
+  static constexpr int kSmemBytes = 1024 + kBBytes + 2 * kGroups * kOutBytes + kStages * kHalo + kGroups * kAccBytes + 2 * BN * 4 + 256 + 2 * BN * 4 /*stats*/;
+  static_assert(kSmemBytes <= kSmemLimit, "c32: shared memory budget");
 };
 
 __global__ void __launch_bounds__(C32Cfg::kThreads, 1)
@@ -886,27 +639,28 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
                 const __grid_constant__ CUtensorMap tmap_y, const C32Params p) {
   using Cfg = C32Cfg;
   constexpr int BN = Cfg::BN;
+  constexpr int kGroups = Cfg::kGroups;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t smem_b = smem_base;
   const uint32_t smem_o = smem_b + Cfg::kBBytes;
-  const uint32_t smem_h = smem_o + 2 * Cfg::kGroups * Cfg::kOutBytes;
-  float* ep_scale = reinterpret_cast<float*>(smem_gen + Cfg::kBBytes + 2 * Cfg::kGroups * Cfg::kOutBytes + Cfg::kStages * Cfg::kHalo);
+  const uint32_t smem_h = smem_o + 2 * kGroups * Cfg::kOutBytes;
+  float* sacc = reinterpret_cast<float*>(smem_gen + Cfg::kBBytes + 2 * kGroups * Cfg::kOutBytes + Cfg::kStages * Cfg::kHalo);  // [kGroups] tiles
+  float* ep_scale = sacc + kGroups * BN * kAccPitch;
   float* ep_shift = ep_scale + BN;
   uint64_t* bars = reinterpret_cast<uint64_t*>(ep_shift + BN);
   const uint32_t bar_full = smem_u32(bars);
   const uint32_t bar_empty = bar_full + 8 * Cfg::kStages;
   const uint32_t bar_tfull = bar_empty + 8 * Cfg::kStages;
-  const uint32_t bar_tempty = bar_tfull + 8 * Cfg::kAccStages;
-  const uint32_t bar_w = bar_tempty + 8 * Cfg::kAccStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::kStages + 2 * Cfg::kAccStages + 1);
+  const uint32_t bar_tempty = bar_tfull + 8 * kGroups;
+  const uint32_t bar_w = bar_tempty + 8 * kGroups;
   float* ep_stats = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);      // [2][BN], accumulated over all of this CTA's tiles
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    for (int i = 0; i < Cfg::kAccStages; ++i) { mbar_init(bar_tfull + 8 * i, 1); mbar_init(bar_tempty + 8 * i, 4); }
+    for (int i = 0; i < Cfg::kStages; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 4); }
+    for (int i = 0; i < kGroups; ++i) { mbar_init(bar_tfull + 8 * i, 4); mbar_init(bar_tempty + 8 * i, 4); }
     mbar_init(bar_w, 1);
     fence_mbar_init();
     fence_proxy_async_smem();
@@ -914,14 +668,10 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_y);
   }
-  if (warp == 1) { tmem_alloc(smem_u32(tmem_slot), Cfg::kAccStages * BN); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_trigger();        // an ordinary launch itself; lets a PDL successor set up while this grid drains
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       mbar_arrive_expect_tx(bar_w, Cfg::kBBytes);
       for (int t = 0; t < 9; ++t) tma_load_2d(smem_b + t * Cfg::kBTap, &tmap_w, bar_w, t * 32, 0);
@@ -943,43 +693,59 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN);
-      const uint32_t lbo = p.swap_lbo ? Cfg::HW * 16 : Cfg::kPlane;
-      const uint32_t sbo = p.swap_lbo ? Cfg::kPlane : Cfg::HW * 16;
-      int stage = 0; uint32_t phase = 0; int acc = 0; uint32_t acc_phase = 0; int tr = 0;
-      mbar_wait(bar_w, 0, p.dbg, 0xB10);
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        mbar_wait(bar_tempty + 8 * acc, acc_phase ^ 1, p.dbg, 0xB20 | acc);
-        YB_TRACE(1, tr); ++tr;
-        mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0xB30 | stage);
-        tc_fence_after();
-        YB_TRACE(1, tr); ++tr;
-        const uint32_t halo = smem_h + stage * Cfg::kHalo;
-        if (!(p.skip & 4)) {
+  } else if (warp < kProducerWarp) {
+    // MMA warpgroup: rows 0..63 of the 16 x 8 tile are output rows 0..7 (one 8-pixel core matrix each), rows 64..127 start
+    // 8 halo rows further down
+    const uint32_t lbo = p.swap_lbo ? Cfg::HW * 16 : Cfg::kPlane;
+    const uint32_t sbo = p.swap_lbo ? Cfg::kPlane : Cfg::HW * 16;
+    float acc[2][BN / 2];
+    int stage = 0; uint32_t phase = 0; int tr = 0;
+    mbar_wait(bar_w, 0, p.dbg, 0xB10);
+    int local = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++local) {
+      mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0xB30 | stage);
+      if (threadIdx.x == 0) { YB_TRACE(1, tr); ++tr; }
+      const uint32_t halo = smem_h + stage * Cfg::kHalo;
+      if (!(p.skip & 4)) {
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
           for (int t = 0; t < 9; ++t) {
-            const uint32_t win = halo + ((t / 3) * Cfg::HW + (t % 3)) * 16;      // tap (r, s): window shifted by r rows, s pixels
+            const uint32_t win = halo + ((h * 8 + t / 3) * Cfg::HW + (t % 3)) * 16;      // tap (r, s): window shifted by r rows, s pixels
             const uint64_t bdesc = make_kmajor_desc<64>(smem_b + t * Cfg::kBTap);
-            umma_f16(tmem_base + acc * BN, make_kmajor_desc_noswz(win, lbo, sbo), bdesc, idesc, t != 0);
-            umma_f16(tmem_base + acc * BN, make_kmajor_desc_noswz(win + 2 * Cfg::kPlane, lbo, sbo), bdesc + 2, idesc, 1);
+            wgmma_f16<BN>(acc[h], make_kmajor_desc_noswz(win, lbo, sbo), bdesc, t != 0);
+            wgmma_f16<BN>(acc[h], make_kmajor_desc_noswz(win + 2 * Cfg::kPlane, lbo, sbo), bdesc + 2, 1);
           }
         }
-        umma_commit(bar_empty + 8 * stage);
-        umma_commit(bar_tfull + 8 * acc);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        if (++acc == Cfg::kAccStages) { acc = 0; acc_phase ^= 1; }
+        wgmma_commit();
+        wgmma_wait<0>();
       }
+      fence_regs(acc[0]);
+      fence_regs(acc[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      // tile `local` goes to epilogue group local % kGroups, through that group's accumulator tile
+      const int grp = local % kGroups;
+      const uint32_t use = static_cast<uint32_t>(local / kGroups);
+      mbar_wait(bar_tempty + 8 * grp, (use & 1) ^ 1, p.dbg, 0xB20 | grp);
+      float* tile_acc = sacc + grp * BN * kAccPitch;
+      sacc_store<BN>(tile_acc, 0, 0, acc[0]);
+      sacc_store<BN>(tile_acc, 64, 0, acc[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_tfull + 8 * grp);
     }
   } else {
     // Independent epilogue groups of four warps take the tiles round-robin: one tile's epilogue is a chain of latencies
-    // (tcgen05.ld, two named barriers, the async-proxy fence, the TMA store issue -- ~1300 cycles even with nothing else
-    // running, see profiles/r01_conv_trace.txt), so kGroups of them in flight multiply the tile rate.
-    const int q = warp & 3;                 // TMEM lane quarter: tile rows 4q .. 4q+3
-    const int grp = (warp - 2) >> 2;
-    const int gt = (threadIdx.x - 64) & 127;
-    const int et = threadIdx.x - 64;
+    // (accumulator reads, two named barriers, the async-proxy fence, the TMA store issue), so kGroups of them in flight
+    // multiply the tile rate.
+    const int ew = warp - kEpiWarp0;
+    const int q = ew & 3;                   // tile pixels 32 q .. 32 q + 31: rows 4q .. 4q+3
+    const int grp = ew >> 2;
+    const int gt = (threadIdx.x - kEpiWarp0 * 32) & 127;
+    const int et = threadIdx.x - kEpiWarp0 * 32;
+    const float* tile_acc = sacc + grp * BN * kAccPitch;
     int tr = 0;
     for (int i = et; i < BN; i += Cfg::kEpiThreads) {
       ep_scale[i] = (i < p.cout) ? __ldg(p.scale + i) : 0.f;
@@ -996,26 +762,22 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
     }
     int local = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++local) {
-      if (local % Cfg::kGroups != grp) continue;
-      const int acc = local & 3;
-      const uint32_t acc_phase = (local >> 2) & 1;
+      if (local % kGroups != grp) continue;
+      const uint32_t use = static_cast<uint32_t>(local / kGroups);
       const int tw = tile % p.tiles_w;
       const int rest = tile / p.tiles_w;
       const int th = rest % p.tiles_h;
       const int n = rest / p.tiles_h;
-      mbar_wait(bar_tfull + 8 * acc, acc_phase, p.dbg, 0xB40 | acc);
-      tc_fence_after();
+      mbar_wait(bar_tfull + 8 * grp, use & 1, p.dbg, 0xB40 | grp);
       if (et == 0) { YB_TRACE(2, tr); ++tr; }
       uint4 pk[8];
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
         uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN + half * 32, v);
-        tmem_ld_wait();
-        if (half == 1) {                      // both halves are in registers: hand the accumulator back
-          tc_fence_before();
+        sacc_ld_x32(tile_acc, m, half * 32, v);
+        if (half == 1) {                      // both halves are in registers: hand the accumulator tile back
           __syncwarp();
-          if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);
+          if (lane == 0) mbar_arrive(bar_tempty + 8 * grp);
         }
         float f[32];
 #pragma unroll
@@ -1064,7 +826,7 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
           pk[half * 4 + g].z = *reinterpret_cast<uint32_t*>(&h2); pk[half * 4 + g].w = *reinterpret_cast<uint32_t*>(&h3);
         }
       }
-      const uint32_t obuf = smem_o + (grp * 2 + ((local / Cfg::kGroups) & 1)) * Cfg::kOutBytes;
+      const uint32_t obuf = smem_o + (grp * 2 + (use & 1)) * Cfg::kOutBytes;
       if (gt == 0) tma_store_wait_read<1>();      // this group's store from two of its tiles ago has drained the buffer
       asm volatile("bar.sync %0, 128;" :: "r"(1 + grp) : "memory");
       if (et == 0) { YB_TRACE(2, tr); ++tr; }
@@ -1090,16 +852,13 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, Cfg::kAccStages * BN); }
 }
 
 // ---------------------------------------------------------------------------------------------
 // Host side: tensor-map encoding through the driver entry points (no link-time libcuda dependency)
 // ---------------------------------------------------------------------------------------------
 constexpr long long kSkFlagBytes = 4096;          // room for 1024 CTA flags
-constexpr long long kSkSlotBytes = 512 * 128 * 4;  // one CTA's largest partial accumulator (MT*BN = 512 columns x 128 rows x fp32)
+constexpr long long kSkSlotBytes = 128 * 128 * 4;  // one CTA's largest partial accumulator (MT*BN = 128 columns x 128 rows x fp32)
 long long conv_workspace_bytes() { return kSkFlagBytes + kSkSlotBytes * sm_count(); }
 
 static unsigned long long* g_conv_trace = nullptr;
@@ -1133,77 +892,44 @@ static int get_encoders(EncodeTiledFn* tiled, EncodeIm2colFn* im2col) {
 
 int get_tensor_map_encoders(EncodeTiledFn* tiled, EncodeIm2colFn* im2col) { return get_encoders(tiled, im2col); }
 
-template <int BN, int BK, int MT, bool kPair, int EW = 4>
+template <int BN, int BK, int MT>
 static int launch_conv(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, cudaStream_t stream) {
-  using Cfg = ConvCfg<BN, BK, MT, kPair, EW>;
+  using Cfg = ConvCfg<BN, BK, MT>;
   static bool attr_set = false;
   if (!attr_set) {
-    YB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BN, BK, MT, kPair, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    YB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BN, BK, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
   const int tiles = p.m_tiles * p.n_tiles;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int nattr = 0;
-  // Programmatic dependent launch: this kernel's prologue may overlap the previous kernel's tail.  OFF by default -- measured on B200
-  // (profiles/r02_pdl_ab.md): one batch in flight 24.30 k vs 24.43 k img/s (no gain: the prologue is ~2 us of a 20-130 us kernel), two
-  // batches in flight 29.3 k vs 31.2 k img/s (early-resident CTAs spinning in griddepcontrol.wait take the SMs the other lane's kernels
-  // would have used).  YB_PDL=1 switches it on for A/B runs.
+  // Programmatic dependent launch: this kernel's prologue may overlap the previous kernel's tail.  Off by default (the prologue is
+  // a small share of a conv, and early-resident CTAs spinning in griddepcontrol.wait hold SMs another stream's kernels could use);
+  // YB_PDL=1 switches it on for A/B runs.
   static const int use_pdl = getenv("YB_PDL") ? atoi(getenv("YB_PDL")) : 0;
   if (use_pdl) {
     attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[nattr].val.programmaticStreamSerializationAllowed = 1;
     ++nattr;
   }
-  if (kPair) {
-    const int pairs = sm_count() / 2;
-    cfg.gridDim = dim3(2 * (tiles < pairs ? tiles : pairs));
-    attr[nattr].id = cudaLaunchAttributeClusterDimension;
-    attr[nattr].val.clusterDim.x = 2; attr[nattr].val.clusterDim.y = 1; attr[nattr].val.clusterDim.z = 1;
-    ++nattr;
-  } else if (p.streamk) {
-    cfg.gridDim = dim3(sm_count());          // sk_base / sk_rem were computed for exactly this many CTAs
-  } else {
-    cfg.gridDim = dim3(tiles < sm_count() ? tiles : sm_count());
-  }
-  cfg.blockDim = dim3(Cfg::kThreads);
+  if (p.streamk) cfg.gridDim = dim3(sm_count());          // sk_base / sk_rem were computed for exactly this many CTAs
+  else cfg.gridDim = dim3(tiles < sm_count() ? tiles : sm_count());
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
   cfg.attrs = attr; cfg.numAttrs = nattr;
-  YB_CUDA(cudaLaunchKernelEx(&cfg, conv_igemm_kernel<BN, BK, MT, kPair, EW>, ta, tb, ty, p));
+  YB_CUDA(cudaLaunchKernelEx(&cfg, conv_igemm_kernel<BN, BK, MT>, ta, tb, ty, p));
   return check_launch("conv_igemm_kernel");
 }
 
-// Eight epilogue warps (two per TMEM lane quarter, alternate 64-column chunks, own staging slices) for BLOCK_N <= 128, non-pair, non-stream-K
-// launches: built to test whether the per-tile epilogue chain bounds the 104^2 / 52^2 / 1x1 layers.  Measured on B200
-// (profiles/r02_epi_warps_ab.md): one batch in flight 25.77 k -> 25.97 k img/s, two lanes 33.67 k -> 33.52 k -- no gain, so the four-warp
-// form stays the default and YB_CONV_EPI_WARPS=8 selects this one.
-static int epi_warps_default() {
-  static const int v = getenv("YB_CONV_EPI_WARPS") ? atoi(getenv("YB_CONV_EPI_WARPS")) : 4;
-  return v == 8 ? 8 : 4;
-}
-
-template <int BK, bool kPair>
+// CTA tile shapes (BLOCK_N, M-subtiles): the MMA warpgroup keeps MT * BLOCK_N <= 128 accumulators per thread
+template <int BK>
 static int dispatch_conv(int bn, int mt, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, cudaStream_t stream) {
-  if constexpr (!kPair) {
-    if (bn <= 128 && !p.streamk && epi_warps_default() == 8) {
-      if (mt == 1) {
-        if (bn == 64) return launch_conv<64, BK, 1, false, 8>(ta, tb, ty, p, stream);
-        return launch_conv<128, BK, 1, false, 8>(ta, tb, ty, p, stream);
-      }
-      if (bn == 64) return launch_conv<64, BK, 2, false, 8>(ta, tb, ty, p, stream);
-      return launch_conv<128, BK, 2, false, 8>(ta, tb, ty, p, stream);
-    }
-  }
-  if (mt == 1) {
-    if (bn == 64) return launch_conv<64, BK, 1, kPair>(ta, tb, ty, p, stream);
-    if (bn == 128) return launch_conv<128, BK, 1, kPair>(ta, tb, ty, p, stream);
-    return launch_conv<256, BK, 1, kPair>(ta, tb, ty, p, stream);
-  }
-  if (bn == 64) return launch_conv<64, BK, 2, kPair>(ta, tb, ty, p, stream);
-  if (bn == 128) return launch_conv<128, BK, 2, kPair>(ta, tb, ty, p, stream);
-  return launch_conv<256, BK, 2, kPair>(ta, tb, ty, p, stream);
+  if (mt == 2) return launch_conv<64, BK, 2>(ta, tb, ty, p, stream);
+  if (bn == 64) return launch_conv<64, BK, 1>(ta, tb, ty, p, stream);
+  return launch_conv<128, BK, 1>(ta, tb, ty, p, stream);
 }
 
 static int conv_c32_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -1301,75 +1027,65 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
     return conv_c32_forward(x, w, scale, shift, slope, y, batch, height, width, cout, x_ld, y_ld, y_ch_off, pool, flags, stats, stream);
   if (pool) return fail(YB_ERR_UNSUPPORTED, "conv: YB_CONV_POOL2X2 is only implemented for the Cin = 32 3x3 layer");
   const int bk = (cin % 64 == 0 && a_channels % 64 == 0) ? 64 : 32;     // K-blocks never straddle the wrap point
-  // tile shape: flags may force BLOCK_N (bits 8..17) and the number of M-subtiles (bits 20..21);
-  // otherwise pick the (BLOCK_N, M-subtiles) pair with the lowest modelled time.  The model was
-  // fitted to tools/conv_sweep.py on B200 (profiles/r01_conv_sweep.md): the kernel is bound by the
-  // L2->SM operand feed (~95 B/ns per SM, ~11 TB/s chip-wide), a tile costs its operand bytes at
-  // that rate (or its MMA time if larger), tiles run in ceil(tiles/SMs) rounds, and a CTA tile whose
-  // accumulator fills all of TMEM (256x256) cannot overlap its epilogue with the next mainloop.
-  int bn = 0, mt = 0, pair = 0, streamk = 0;
+  // tile shape: flags may force BLOCK_N (bits 8..17) and the number of M-subtiles (bits 20..21); otherwise pick the
+  // (BLOCK_N, M-subtiles) pair with the lowest modelled time.  The model treats the kernel as bound by the L2->SM operand
+  // feed (a tile costs its operand bytes at a per-SM rate, or its MMA time if larger, and tiles run in ceil(tiles/SMs)
+  // rounds, capped by a chip-wide L2 rate); its rates are estimates for H100, not fitted measurements.
+  int bn = 0, mt = 0, streamk = 0;
   // stream-K needs the caller's workspace (one per stream: partial sums + flags); flags bit 3 forbids, bit 30 forces it
   const bool sk_possible = stats == nullptr && workspace != nullptr && workspace_bytes >= conv_workspace_bytes() && (flags & 8) == 0 &&
                            (reinterpret_cast<uintptr_t>(workspace) & 255) == 0;
   const bool sk_force = sk_possible && ((flags >> 30) & 1);
   const int force_bn = (flags >> 8) & 0x3FF;
   const int force_mt = (flags >> 20) & 0x3;
-  const int force_pair = (flags >> 22) & 0x3;      // 0 = auto, 1 = single-CTA, 2 = CTA pair (cta_group::2)
+  const int force_pair = (flags >> 22) & 0x3;      // 0 = auto, 1 = single-CTA tiles (the only form), 2 = CTA pair (not on sm_90)
+  YB_REQUIRE(force_pair != 2, "conv: CTA-pair tiles need two-CTA tensor-core instructions, which sm_90 does not have");
+  YB_REQUIRE(!force_bn || ((force_bn == 64 || force_bn == 128) && (force_mt != 2 || force_bn == 64)),
+             "conv: BLOCK_N=%d x %d M-subtiles is not a tile shape of this kernel (64 x 1, 128 x 1, 64 x 2)", force_bn, force_mt ? force_mt : 1);
   {
     double best = 1e300;
     const int sms = sm_count();
     const int num_kb = ksize * ksize * (cin / bk);
-    for (int cpair = 0; cpair <= 1; ++cpair) {
-      if (force_pair && cpair != force_pair - 1) continue;
-      if (!force_pair && cpair == 1 && (flags & 4) == 0) continue;   // pairs are opt-in (YB_CONV_ALLOW_PAIR) until tuned
-      for (int cbn = 64; cbn <= 256; cbn *= 2) {
-        if (force_bn && cbn != force_bn) continue;
-        if (!force_bn && cbn > 64 && cbn / 2 >= cout) continue;       // do not pad Cout by more than 2x
-        for (int cmt = 1; cmt <= 2; ++cmt) {
-          if (force_mt && cmt != force_mt) continue;
-          const int rows_tile = BM * cmt * (cpair ? 2 : 1);
-          const double tiles = static_cast<double>((m_total_ll + rows_tile - 1) / rows_tile) * ((cout + cbn - 1) / cbn);
-          const int units = cpair ? sms / 2 : sms;
-          const double rounds = static_cast<double>((static_cast<long long>(tiles) + units - 1) / units);
-          const double bytes_kb = (cmt * BM + (cpair ? cbn / 2 : cbn)) * bk * 2.0;        // per CTA
-          const double mma_ns_kb = cmt * (bk / 16) * (cbn >= 128 ? cbn / 2.0 : 64.0) / 1.9;   // cycles(N) = max(N,128)/2 @ ~1.9 GHz
-          const double kb_ns = bytes_kb / 95.0 > mma_ns_kb ? bytes_kb / 95.0 : mma_ns_kb;
-          const bool single_acc = 2 * cmt * cbn > 512;
-          const double tile_ns = num_kb * kb_ns + (single_acc ? 8000.0 : 500.0);
-          const double agg_ns = tiles * (cpair ? 2 : 1) * num_kb * bytes_kb / 11000.0;
-          double t = rounds * tile_ns;
-          if (agg_ns > t) t = agg_ns;
-          int csk = 0;
-          if (sk_possible && !cpair) {
-            // stream-K: every SM gets units/SMs K-blocks; on top, roughly one partial dump + one collecting epilogue
-            // per CTA (proportional to the accumulator size, not overlapped when it fills TMEM)
-            const double units = tiles * num_kb;
-            const double per_cta = static_cast<double>((static_cast<long long>(units) + sms - 1) / sms);
-            const double epi_ns = 8000.0 * (cmt * cbn / 512.0);
-            double tsk = per_cta * kb_ns + (single_acc ? 2.0 : 1.0) * epi_ns + 1500.0;
-            if (agg_ns > tsk) tsk = agg_ns;
-            // Measured (tools/conv_sweep_sk.py, profiles/r01_conv_sweep_sk.md): at batch 32 the 13x13 / 26x26 layers are
-            // already limited chip-wide (L2 -> SM operand bandwidth, board power), so spreading them over all SMs gains
-            // nothing; stream-K pays when the layer leaves most of the GPU idle (single images, small batches).
-            const bool ok = per_cta >= 4.0 && num_kb >= 2;
-            const bool idle = tiles <= sms / 2;
-            if (ok && (sk_force || (idle && tsk < 0.93 * t))) { t = tsk; csk = 1; }
-          }
-          if (sk_force && !csk) continue;
-          // ties (e.g. 256x128 vs 128x256, same operand bytes) go to the wider-N shape, which measured ~8% faster
-          if (t < best * 0.9999 || (t <= best * 1.0001 && cbn > bn)) { best = t; bn = cbn; mt = cmt; pair = cpair; streamk = csk; }
+    for (int cbn = 64; cbn <= 128; cbn *= 2) {
+      if (force_bn && cbn != force_bn) continue;
+      if (!force_bn && cbn > 64 && cbn / 2 >= cout) continue;       // do not pad Cout by more than 2x
+      for (int cmt = 1; cmt <= 2; ++cmt) {
+        if (force_mt && cmt != force_mt) continue;
+        if (cmt * cbn > 128) continue;
+        const int rows_tile = BM * cmt;
+        const double tiles = static_cast<double>((m_total_ll + rows_tile - 1) / rows_tile) * ((cout + cbn - 1) / cbn);
+        const double rounds = static_cast<double>((static_cast<long long>(tiles) + sms - 1) / sms);
+        const double bytes_kb = (cmt * BM + cbn) * bk * 2.0;        // per CTA
+        const double mma_ns_kb = cmt * BM * cbn * bk * 2.0 / 7000.0;  // ~7 TFLOP/s per SM of dense fp16
+        const double kb_ns = bytes_kb / 60.0 > mma_ns_kb ? bytes_kb / 60.0 : mma_ns_kb;
+        const double tile_ns = num_kb * kb_ns + 500.0;
+        const double agg_ns = tiles * num_kb * bytes_kb / 7000.0;
+        double t = rounds * tile_ns;
+        if (agg_ns > t) t = agg_ns;
+        int csk = 0;
+        if (sk_possible) {
+          // stream-K: every SM gets units/SMs K-blocks; on top, roughly one partial dump + one collecting epilogue per CTA
+          const double units = tiles * num_kb;
+          const double per_cta = static_cast<double>((static_cast<long long>(units) + sms - 1) / sms);
+          const double epi_ns = 8000.0 * (cmt * cbn / 512.0);
+          double tsk = per_cta * kb_ns + epi_ns + 1500.0;
+          if (agg_ns > tsk) tsk = agg_ns;
+          // stream-K pays when the layer leaves most of the GPU idle (single images, small batches); layers that already fill
+          // the chip gain nothing from the spread
+          const bool ok = per_cta >= 4.0 && num_kb >= 2;
+          const bool idle = tiles <= sms / 2;
+          if (ok && (sk_force || (idle && tsk < 0.93 * t))) { t = tsk; csk = 1; }
         }
+        if (sk_force && !csk) continue;
+        // ties go to the wider-N shape (more reuse of each A tile)
+        if (t < best * 0.9999 || (t <= best * 1.0001 && cbn > bn)) { best = t; bn = cbn; mt = cmt; streamk = csk; }
       }
     }
-    if (bn == 0) { bn = force_bn ? force_bn : 128; mt = force_mt ? force_mt : 1; pair = force_pair == 2; streamk = 0; }
+    if (bn == 0) { bn = force_bn ? force_bn : 128; mt = force_mt ? force_mt : 1; streamk = 0; }
   }
-  // small-K specialisation (Cin = 32, 3x3, Cout <= 64, fp16 NHWC out): all 9 taps per stage, resident weights
-  const bool smallk = (!split && cin == 32 && ksize == 3 && cout <= 64 && out_mode == 0 && !force_bn && !force_mt && !force_pair && ((flags >> 28) & 1) == 0);
-  if (smallk) { bn = 64; mt = 1; pair = 0; streamk = 0; }
-  YB_REQUIRE(bn == 64 || bn == 128 || bn == 256, "conv: BN=%d", bn);
-  YB_REQUIRE(mt == 1 || mt == 2, "conv: MT=%d", mt);
-  // 1x1 layers read A as a plain [pixels, Cin] matrix (2-D tiled TMA: cheaper per instruction than im2col mode and measured
-  // 2 us faster on the 13x13 layers); YB_CONV_1X1_IM2COL=1 switches back for A/B runs
+  YB_REQUIRE((bn == 64 || bn == 128) && (mt == 1 || mt == 2) && mt * bn <= 128, "conv: tile %d x %d", bn, mt);
+  // 1x1 layers read A as a plain [pixels, Cin] matrix (2-D tiled TMA: cheaper per instruction than im2col mode);
+  // YB_CONV_1X1_IM2COL=1 switches back for A/B runs
   static const int k1x1_im2col = getenv("YB_CONV_1X1_IM2COL") ? atoi(getenv("YB_CONV_1X1_IM2COL")) : 0;
   const int a_im2col = (ksize == 3) ? 1 : ((k1x1_im2col && !(flags & 1)) ? 1 : 0);
 
@@ -1383,7 +1099,7 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
   p.height = height; p.width = width; p.cin = cin; p.cout = cout; p.ksize = ksize; p.pad = (ksize - 1) / 2;
   p.kb_per_tap = cin / bk;
   p.num_kb = ksize * ksize * p.kb_per_tap;
-  const int rows_tile = BM * mt * (pair ? 2 : 1);
+  const int rows_tile = BM * mt;
   p.m_tiles = (p.m_total + rows_tile - 1) / rows_tile;
   p.n_tiles = (cout + bn - 1) / bn;
   p.a_im2col = a_im2col;
@@ -1411,7 +1127,7 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
   const CUtensorMapSwizzle swz = (bk == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   alignas(64) CUtensorMap ta, tb;
   CUresult cr;
-  const int a_rows = (mt == 2 && !pair && !smallk) ? 2 * BM : BM;   // pixels per A box (ConvCfg::kMergedA)
+  const int a_rows = BM * mt;     // pixels per A box (ConvCfg::kMergedA)
   if (a_im2col) {
     const cuuint64_t dims[4] = {static_cast<cuuint64_t>(a_channels), static_cast<cuuint64_t>(width), static_cast<cuuint64_t>(height),
                                 static_cast<cuuint64_t>(batch)};
@@ -1443,36 +1159,13 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
     const cuuint64_t k_total = static_cast<cuuint64_t>(ksize) * ksize * cin;
     const cuuint64_t dims[2] = {k_total, static_cast<cuuint64_t>(cout)};
     const cuuint64_t strides[1] = {k_total * 2};
-    const cuuint32_t box[2] = {static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(pair ? bn / 2 : bn)};   // a pair CTA stages half the tile
+    const cuuint32_t box[2] = {static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(bn)};
     const cuuint32_t estr[2] = {1, 1};
     cr = enc_tiled(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(w), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(W) failed (%d)", static_cast<int>(cr));
   }
 
-  if (smallk) {
-    using Cfg = SmallKCfg<64>;
-    static bool attr_set = false;
-    if (!attr_set) {
-      YB_CUDA(cudaFuncSetAttribute(conv_smallk_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-      attr_set = true;
-    }
-    const int tiles = p.m_tiles;
-    const int grid = tiles < sm_count() ? tiles : sm_count();
-    alignas(64) CUtensorMap ty;
-    {
-      const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cout), static_cast<cuuint64_t>(p.m_total)};
-      const cuuint64_t strides[1] = {static_cast<cuuint64_t>(y_ld) * 2};
-      const cuuint32_t box[2] = {64, BM};
-      const cuuint32_t estr[2] = {1, 1};
-      cr = enc_tiled(&ty, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, static_cast<__half*>(y) + y_ch_off, dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
-    }
-    const int tma_store = ((flags >> 29) & 1) ? 0 : 1;     // bit 29: plain per-thread stores (A/B switch)
-    conv_smallk_kernel<64><<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(ta, tb, ty, p, tma_store);
-    return check_launch("conv_smallk_kernel");
-  }
   // output tensor map of the TMA-store epilogue (fp16 NHWC, no residual output); flags bit 29 (YB_CONV_PLAIN_STORE) keeps the
   // per-thread stores for A/B runs
   alignas(64) CUtensorMap ty;
@@ -1487,12 +1180,8 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
   }
-  if (pair) {
-    if (bk == 64) return dispatch_conv<64, true>(bn, mt, ta, tb, ty, p, stream);
-    return dispatch_conv<32, true>(bn, mt, ta, tb, ty, p, stream);
-  }
-  if (bk == 64) return dispatch_conv<64, false>(bn, mt, ta, tb, ty, p, stream);
-  return dispatch_conv<32, false>(bn, mt, ta, tb, ty, p, stream);
+  if (bk == 64) return dispatch_conv<64>(bn, mt, ta, tb, ty, p, stream);
+  return dispatch_conv<32>(bn, mt, ta, tb, ty, p, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

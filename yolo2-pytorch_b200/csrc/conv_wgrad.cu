@@ -1,32 +1,34 @@
-// K11: convolution weight gradient on the tensor cores (tcgen05), sm_100a only.
-// Replaces what torch autograd runs for nn.Conv2d.weight.grad (/root/reference model/yolo2.py:57,
+// K11: convolution weight gradient on the Hopper tensor cores (wgmma), sm_90a.
+// Replaces what torch autograd runs for nn.Conv2d.weight.grad (reference model/yolo2.py:57,
 // train.py:351 loss_total.backward()).
 //
 //   dW[co][r][s][ci] = sum over output pixels p of  dz[p, co] * x[p + (r-1, s-1), ci]        (zero outside the image)
 //
 // As a GEMM the reduction runs over PIXELS:  D[M = 128 co, N = ci-chunk] += A[M, K = pixels] * B[N, K]^T with
 // A(m, k) = dz[p0 + k][co0 + m] and B(n, k) = x[shift(p0 + k)][ci0 + n].  Both tensors are NHWC (channel
-// contiguous), so both operands are "MN-major": a TMA box of [64 channels x 32 pixels] lands in shared memory as
-// 32 rows of 128 bytes and is described to tcgen05.mma with a_major = b_major = MN (leading-dim offset = next
-// 64-channel box, stride offset = next group of 8 pixel rows).  The shifted activation tile comes from the same
-// im2col-mode TMA the forward kernel uses (halo zero-filled by the unit).
+// contiguous), so both operands are "MN-major": a TMA box of [64 channels x KP pixels] lands in shared memory as
+// KP rows of 128 bytes and is described to wgmma as transposed (leading-dim offset = next 64-channel box, stride
+// offset = next group of 8 pixel rows).  The shifted activation tile comes from the same im2col-mode TMA the forward
+// kernel uses (halo zero-filled by the unit).
 //
-// One CTA owns a 128-row slice of Cout and up to 512 accumulator columns = G (tap, ci-chunk) groups, so the dz tile
-// is fetched once per K-block and reused by all G groups; the pixel range is split across CTAs (split-K) and the
-// fp32 partial sums are added into a zero-initialised [Cout][k][k][Cin] buffer with 16-byte vector atomics.
+// One CTA owns a 128-row slice of Cout (two warpgroups of 64) and up to 256 accumulator columns = G (tap, ci-chunk)
+// groups, so the dz tile is fetched once per K-block and reused by all G groups; the pixel range is split across CTAs
+// (split-K) and the fp32 partial sums are added into a zero-initialised [Cout][k][k][Cin] buffer with 8-byte vector
+// atomics.
 #include "yb_common.h"
 #include "yb_ptx.cuh"
 #include <stdlib.h>
 
 namespace yb {
 
-constexpr int WG_THREADS = 192;
+constexpr int WG_MMA_THREADS = 256;                 // two warpgroups: output channels 0..63 / 64..127 of the CTA's slice
+constexpr int WG_THREADS = WG_MMA_THREADS + 32;     // + the TMA producer warp
 constexpr int WG_MAX_GROUPS = 9;
 
 struct WgradParams {
   int m_total, hw, width;
   int cin, cout, ksize, pad;
-  int n_per_group;      // N of one MMA group (32, 64, 128 or 256)
+  int n_per_group;      // N of one (tap, ci-chunk) group (32, 64, 128, 192 or 256)
   int groups_per_cta;   // G
   int col_tiles;        // taps * ceil(cin / n_per_group)
   int chunks_per_tap;   // ceil(cin / n_per_group)
@@ -43,15 +45,15 @@ struct WgradParams {
 // per row, 8-row groups `8 * kRowBytes` apart (SBO), 64- (or 32-) channel boxes `lbo_bytes` apart (LBO).
 template <int kRowBytes>
 __device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-  constexpr uint64_t layout = (kRowBytes == 128) ? 2ull : 4ull;
+  constexpr uint64_t layout = (kRowBytes == 128) ? 1ull : 2ull;
   constexpr uint64_t sbo = (8ull * kRowBytes) >> 4;
-  return static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4) | (static_cast<uint64_t>(lbo_bytes >> 4) << 16) | (sbo << 32) | (1ull << 46) | (layout << 61);
+  return static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4) | (static_cast<uint64_t>(lbo_bytes >> 4) << 16) | (sbo << 32) | (layout << 62);
 }
 
 // kBRow = bytes per pixel row of the activation (B) boxes: 128 (64 channels) or 64 (32 channels, Cin = 32)
 // WG_KP = pixels (K) per pipeline stage = pixels per TMA box; WG_STAGES = pipeline depth; NMAX = accumulator columns
 // (activation channels x taps) one CTA owns.  The im2col-mode TMA has a large per-instruction cost, so few big boxes
-// (KP = 64..128) feed the tensor cores far better than many 32-pixel ones (tools/wgrad_ablate.py).
+// (KP = 64..128) feed the tensor cores far better than many 32-pixel ones.
 template <int kBRow, int WG_KP, int WG_STAGES, int NMAX>
 struct WgradCfg {
   static constexpr int kABox = WG_KP * 128;
@@ -63,13 +65,16 @@ struct WgradCfg {
   static constexpr int kStageBytes = kABytes + kBBytes;
   static constexpr int kSmemBytes = WG_STAGES * kStageBytes + 1024 + 256;
   static_assert(kSmemBytes <= 232448, "wgrad: shared memory");
-  static_assert(NMAX <= 512, "wgrad: TMEM columns");
+  static_assert(NMAX <= 256, "wgrad: accumulator columns (one wgmma, registers)");
 };
 
-template <int kBRow, int WG_KP, int WG_STAGES, int NMAX>
+// N = accumulator columns of every CTA of the launch (groups_per_cta x n_per_group); a CTA with fewer groups computes the
+// surplus columns from stale shared memory and never stores them
+template <int kBRow, int WG_KP, int WG_STAGES, int NMAX, int N>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_constant__ CUtensorMap tmap_x, const WgradParams p) {
   using Cfg = WgradCfg<kBRow, WG_KP, WG_STAGES, NMAX>;
+  static_assert(N <= NMAX, "wgrad: N");
   constexpr int kABox = Cfg::kABox;                  // bytes of one [64 co x KP px] box
   constexpr int kBBox = Cfg::kBBox;                  // bytes of one activation box
   constexpr int kBCh = Cfg::kBCh;                    // channels per activation box
@@ -81,8 +86,6 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_gen + WG_STAGES * kStageBytes);
   const uint32_t bar_full = smem_u32(bars);
   const uint32_t bar_empty = bar_full + 8 * WG_STAGES;
-  const uint32_t bar_done = bar_empty + 8 * WG_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * WG_STAGES + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work item
@@ -99,111 +102,96 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   const int boxes_per_group = p.n_per_group / kBCh;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < WG_STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 1); }
-    mbar_init(bar_done, 1);
+    for (int i = 0; i < WG_STAGES; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, WG_MMA_THREADS / 32); }
     fence_mbar_init();
     fence_proxy_async_smem();
     tma_prefetch_desc(&tmap_dz);
     tma_prefetch_desc(&tmap_x);
   }
-  if (warp == 1) { tmem_alloc(smem_u32(tmem_slot), 512); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  if (kb1 <= kb0) return;
 
-  if (kb1 > kb0) {
-    if (warp == 0) {
-      if (lane == 0) {
-        int stage = 0; uint32_t phase = 0;
-        const uint32_t tx_bytes = ((p.skip & 2) ? 0 : kABytes) + ((p.skip & 1) ? 0 : ngroups * boxes_per_group * kBBox);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          const int p0 = kb * WG_KP;
-          const int img = p0 / p.hw;
-          const int rem = p0 - img * p.hw;
-          const int h0 = rem / p.width, w0 = rem - h0 * p.width;
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x600 | stage);
-          mbar_arrive_expect_tx(bar_full + 8 * stage, tx_bytes);
-          const uint32_t sa = smem_base + stage * kStageBytes;
-          if (!(p.skip & 2)) {
-            tma_load_2d(sa, &tmap_dz, bar_full + 8 * stage, co_tile * 128, p0);
-            tma_load_2d(sa + kABox, &tmap_dz, bar_full + 8 * stage, co_tile * 128 + 64, p0);
-          }
-          uint32_t sb = sa + kABytes;
-          for (int g = 0; g < ((p.skip & 1) ? 0 : ngroups); ++g) {
-            const int t = first_tile + g;
-            const int tap = t / p.chunks_per_tap;
-            const int ci0 = (t - tap * p.chunks_per_tap) * p.n_per_group;
-            const int r = tap / p.ksize, s = tap - r * p.ksize;
-            for (int j = 0; j < boxes_per_group; ++j) {
-              tma_load_im2col_4d(sb, &tmap_x, bar_full + 8 * stage, ci0 + j * kBCh, w0 - p.pad, h0 - p.pad, img, static_cast<uint16_t>(s),
-                                 static_cast<uint16_t>(r));
-              sb += kBBox;
-            }
-          }
-          if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+  if (warp == WG_MMA_THREADS / 32) {
+    if (lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      const uint32_t tx_bytes = ((p.skip & 2) ? 0 : kABytes) + ((p.skip & 1) ? 0 : ngroups * boxes_per_group * kBBox);
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const int p0 = kb * WG_KP;
+        const int img = p0 / p.hw;
+        const int rem = p0 - img * p.hw;
+        const int h0 = rem / p.width, w0 = rem - h0 * p.width;
+        mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x600 | stage);
+        mbar_arrive_expect_tx(bar_full + 8 * stage, tx_bytes);
+        const uint32_t sa = smem_base + stage * kStageBytes;
+        if (!(p.skip & 2)) {
+          tma_load_2d(sa, &tmap_dz, bar_full + 8 * stage, co_tile * 128, p0);
+          tma_load_2d(sa + kABox, &tmap_dz, bar_full + 8 * stage, co_tile * 128 + 64, p0);
         }
-      }
-    } else if (warp == 1) {
-      if (lane == 0) {
-        // M = 128, A and B MN-major (bits 15, 16).  The (tap, ci-chunk) groups of this CTA are consecutive TMA boxes in
-        // shared memory and consecutive accumulator columns, so one MMA covers all of them (N = groups x n_per_group,
-        // up to 256 columns per instruction): far fewer, larger MMAs than one per group.
-        const int n_total = ngroups * p.n_per_group;
-        int stage = 0; uint32_t phase = 0;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x700 | stage);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * kStageBytes;
-          const uint64_t adesc = make_mnmajor_desc<128>(sa, kABox);
-          for (int c0 = (p.skip & 4) ? n_total : 0; c0 < n_total; c0 += 256) {
-            const int n = n_total - c0 < 256 ? n_total - c0 : 256;
-            const uint32_t idesc = make_idesc_f16(128, n) | (1u << 15) | (1u << 16);
-            const uint64_t bdesc = make_mnmajor_desc<kBRow>(sa + kABytes + (c0 / kBCh) * kBBox, kBBox);
-#pragma unroll
-            for (int ks = 0; ks < WG_KP / 16; ++ks) {
-              // advance 16 pixel rows: 16 * rowbytes, in 16-byte units
-              umma_f16(tmem_base + c0, adesc + ks * (16 * 128 / 16), bdesc + ks * (16 * kBRow / 16), idesc, (kb > kb0 || ks > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(bar_empty + 8 * stage);
-          if (kb == kb1 - 1) umma_commit(bar_done);
-          if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    } else {
-      // epilogue: thread = one output channel (TMEM lane), 32 accumulator columns per tcgen05.ld
-      const int q = warp & 3;
-      mbar_wait(bar_done, 0, p.dbg, 0x800);
-      tc_fence_after();
-      const int co = co_tile * 128 + q * 32 + lane;
-      const long long ktot = static_cast<long long>(p.ksize) * p.ksize * p.cin;
-      for (int g = 0; g < ngroups; ++g) {
-        const int t = first_tile + g;
-        const int tap = t / p.chunks_per_tap;
-        const int ci0 = (t - tap * p.chunks_per_tap) * p.n_per_group;
-        for (int cc = 0; cc < p.n_per_group; cc += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + g * p.n_per_group + cc, v);
-          tmem_ld_wait();
-          if (co < p.cout) {
-            float* dst = p.dw + static_cast<long long>(co) * ktot + static_cast<long long>(tap) * p.cin + ci0 + cc;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (ci0 + cc + j < p.cin && !(p.skip & 8)) {
-                const float4 val = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                if (p.use_atomics) atomicAdd(reinterpret_cast<float4*>(dst + j), val);
-                else *reinterpret_cast<float4*>(dst + j) = val;
-              }
-            }
+        uint32_t sb = sa + kABytes;
+        for (int g = 0; g < ((p.skip & 1) ? 0 : ngroups); ++g) {
+          const int t = first_tile + g;
+          const int tap = t / p.chunks_per_tap;
+          const int ci0 = (t - tap * p.chunks_per_tap) * p.n_per_group;
+          const int r = tap / p.ksize, s = tap - r * p.ksize;
+          for (int j = 0; j < boxes_per_group; ++j) {
+            tma_load_im2col_4d(sb, &tmap_x, bar_full + 8 * stage, ci0 + j * kBCh, w0 - p.pad, h0 - p.pad, img, static_cast<uint16_t>(s),
+                               static_cast<uint16_t>(r));
+            sb += kBBox;
           }
         }
+        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
       }
     }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
+  // MMA warpgroups: M = 64 output channels each (their dz box), A and B MN-major.  The (tap, ci-chunk) groups of this CTA are
+  // consecutive TMA boxes in shared memory and consecutive accumulator columns, so one wgmma covers all of them.
+  const int wg = threadIdx.x >> 7;
+  float acc[N / 2];
+  int stage = 0; uint32_t phase = 0;
+  int prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x700 | stage);
+    if (!(p.skip & 4)) {
+      const uint32_t sa = smem_base + stage * kStageBytes;
+      const uint64_t adesc = make_mnmajor_desc<128>(sa + wg * kABox, kABox);
+      const uint64_t bdesc = make_mnmajor_desc<kBRow>(sa + kABytes, kBBox);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < WG_KP / 16; ++ks)      // advance 16 pixel rows: 16 * rowbytes, in 16-byte units
+        wgmma_f16<N, 1, 1>(acc, adesc + ks * (16 * 128 / 16), bdesc + ks * (16 * kBRow / 16), (kb > kb0 || ks > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+    }
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+    prev = stage;
+    if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  fence_regs(acc);
+  // epilogue straight from the fragment: rows = output channels, column pairs = two consecutive input channels of one group
+  const long long ktot = static_cast<long long>(p.ksize) * p.ksize * p.cin;
+  const int w4 = warp & 3;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int co = co_tile * 128 + wg * 64 + 16 * w4 + (lane >> 2) + 8 * hh;
+    if (co >= p.cout || (p.skip & 8)) continue;
+    float* dst_row = p.dw + static_cast<long long>(co) * ktot;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+      const int g = col / p.n_per_group;
+      if (g >= ngroups) continue;
+      const int t = first_tile + g;
+      const int tap = t / p.chunks_per_tap;
+      const int ci = (t - tap * p.chunks_per_tap) * p.n_per_group + (col - g * p.n_per_group);
+      if (ci >= p.cin) continue;
+      float* dst = dst_row + static_cast<long long>(tap) * p.cin + ci;
+      const float2 val = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+      if (p.use_atomics) atomicAdd(reinterpret_cast<float2*>(dst), val);
+      else *reinterpret_cast<float2*>(dst) = val;
+    }
+  }
 }
 
 // tensor-map encoders live in conv_igemm.cu
@@ -215,21 +203,22 @@ typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 int get_tensor_map_encoders(EncodeTiledFn* tiled, EncodeIm2colFn* im2col);
 
-template <int kBRow, int KP, int STAGES, int NMAX>
+template <int kBRow, int KP, int STAGES, int NMAX, int N>
 static int launch_wgrad(const CUtensorMap& tdz, const CUtensorMap& tx, const WgradParams& p, int grid, cudaStream_t stream) {
   using Cfg = WgradCfg<kBRow, KP, STAGES, NMAX>;
   static bool set = false;
   if (!set) {
-    YB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<kBRow, KP, STAGES, NMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    YB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<kBRow, KP, STAGES, NMAX, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     set = true;
   }
-  conv_wgrad_kernel<kBRow, KP, STAGES, NMAX><<<grid, WG_THREADS, Cfg::kSmemBytes, stream>>>(tdz, tx, p);
+  conv_wgrad_kernel<kBRow, KP, STAGES, NMAX, N><<<grid, WG_THREADS, Cfg::kSmemBytes, stream>>>(tdz, tx, p);
   return check_launch("conv_wgrad_kernel");
 }
 
-// (pixels per stage, stages, accumulator columns) variants of the wide kernel; YB_WGRAD_CFG selects one for tools/wgrad_ablate.py
-struct WgradVariant { int kp, stages, nmax; };
-static const WgradVariant kWgradVariants[] = {{32, 4, 512}, {64, 2, 512}, {64, 4, 256}, {128, 2, 256}, {64, 3, 384}, {128, 3, 128}};
+// pixels per stage (one TMA box) and pipeline depth: 128-pixel boxes, two stages
+constexpr int kWgKP = 128, kWgStages = 2;
+constexpr int kWgNmaxWide = 256;    // Cin >= 64: 64-channel boxes
+constexpr int kWgNmaxNarrow = 96;   // Cin = 32: three taps of 32 channels per CTA
 
 int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch, int height, int width, int cin, int cout, int ksize, int x_ld,
                        int dz_ld, cudaStream_t stream) {
@@ -245,22 +234,18 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
   if (rc) return rc;
 
   const bool narrow = (cin == 32);
-  int variant = 3;                                               // 128-pixel boxes, 2 stages, 256 columns: fastest on every wide layer
-  if (const char* e = getenv("YB_WGRAD_CFG")) variant = atoi(e);
-  if (variant < 0 || variant >= static_cast<int>(sizeof(kWgradVariants) / sizeof(kWgradVariants[0]))) variant = 3;
-  static const WgradVariant kNarrow[] = {{32, 4, 288}, {64, 3, 288}, {64, 4, 288}, {128, 2, 288}};
-  const WgradVariant var = narrow ? kNarrow[variant & 3] : kWgradVariants[variant];
-  const int KP = var.kp;
+  const int KP = kWgKP;
+  const int nmax = narrow ? kWgNmaxNarrow : kWgNmaxWide;
 
   WgradParams p;
   p.m_total = static_cast<int>(m_total); p.hw = height * width; p.width = width;
   p.cin = cin; p.cout = cout; p.ksize = ksize; p.pad = (ksize - 1) / 2;
   const int taps = ksize * ksize;
   p.n_per_group = cin >= 256 ? 256 : cin;                       // 32, 64, 128 or 256
-  if (p.n_per_group > var.nmax) p.n_per_group = var.nmax;
+  if (p.n_per_group > nmax) p.n_per_group = nmax;
   p.chunks_per_tap = (cin + p.n_per_group - 1) / p.n_per_group;
   p.col_tiles = taps * p.chunks_per_tap;
-  int g = var.nmax / p.n_per_group;                              // accumulator columns available
+  int g = nmax / p.n_per_group;                                  // accumulator columns available
   if (taps == 9 && g > 3 && g < 9) g = 3;                        // 3 taps per CTA: 9 taps split evenly
   if (g > p.col_tiles) g = p.col_tiles;
   if (g > WG_MAX_GROUPS) g = WG_MAX_GROUPS;
@@ -269,14 +254,14 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
   p.co_tiles = (cout + 127) / 128;
   p.kb_total = (p.m_total + KP - 1) / KP;
   const int base_items = p.co_tiles * p.col_groups;
-  // Split the pixel range so that the CTAs fill whole waves of SMs.  Cost model fitted to tools/wgrad_ablate.py:
-  // time ~ waves * (K-blocks per CTA + the atomic epilogue, worth ~11 K-blocks of 128 pixels).
+  // Split the pixel range so that the CTAs fill whole waves of SMs.  Cost model: time ~ waves * (K-blocks per CTA + the atomic
+  // epilogue, worth ~11 K-blocks of 128 pixels).
   const int sms = sm_count();
   const int max_splits = (p.kb_total + 7) / 8;                   // at least 8 K-blocks per split
   int splits = 1;
   {
     double best = 1e30;
-    const double epi = KP >= 128 ? 11.0 : 18.0;   // atomic dump of the accumulator tile, in K-block times (measured)
+    const double epi = 11.0;   // atomic dump of the accumulator tile, in K-block times
     for (int s_ = 1; s_ <= max_splits && s_ <= 512; ++s_) {
       const int ctas = base_items * s_;
       const int waves = (ctas + sms - 1) / sms;
@@ -326,22 +311,18 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
     if (drv <= 13010 && span_bytes < 131072ull) reinterpret_cast<uint64_t*>(&tx)[1] &= ~(1ull << 21);
   }
   const int grid = p.co_tiles * p.col_groups * p.splits;
+  const int n = p.groups_per_cta * p.n_per_group;
   if (narrow) {
-    switch (variant & 3) {
-      case 1: return launch_wgrad<64, 64, 3, 288>(tdz, tx, p, grid, stream);
-      case 2: return launch_wgrad<64, 64, 4, 288>(tdz, tx, p, grid, stream);
-      case 3: return launch_wgrad<64, 128, 2, 288>(tdz, tx, p, grid, stream);
-      default: return launch_wgrad<64, 32, 4, 288>(tdz, tx, p, grid, stream);
-    }
+    if (n == 32) return launch_wgrad<64, kWgKP, kWgStages, kWgNmaxNarrow, 32>(tdz, tx, p, grid, stream);
+    if (n == 64) return launch_wgrad<64, kWgKP, kWgStages, kWgNmaxNarrow, 64>(tdz, tx, p, grid, stream);
+    if (n == 96) return launch_wgrad<64, kWgKP, kWgStages, kWgNmaxNarrow, 96>(tdz, tx, p, grid, stream);
+  } else {
+    if (n == 64) return launch_wgrad<128, kWgKP, kWgStages, kWgNmaxWide, 64>(tdz, tx, p, grid, stream);
+    if (n == 128) return launch_wgrad<128, kWgKP, kWgStages, kWgNmaxWide, 128>(tdz, tx, p, grid, stream);
+    if (n == 192) return launch_wgrad<128, kWgKP, kWgStages, kWgNmaxWide, 192>(tdz, tx, p, grid, stream);
+    if (n == 256) return launch_wgrad<128, kWgKP, kWgStages, kWgNmaxWide, 256>(tdz, tx, p, grid, stream);
   }
-  switch (variant) {
-    case 1: return launch_wgrad<128, 64, 2, 512>(tdz, tx, p, grid, stream);
-    case 2: return launch_wgrad<128, 64, 4, 256>(tdz, tx, p, grid, stream);
-    case 3: return launch_wgrad<128, 128, 2, 256>(tdz, tx, p, grid, stream);
-    case 4: return launch_wgrad<128, 64, 3, 384>(tdz, tx, p, grid, stream);
-    case 5: return launch_wgrad<128, 128, 3, 128>(tdz, tx, p, grid, stream);
-    default: return launch_wgrad<128, 32, 4, 512>(tdz, tx, p, grid, stream);
-  }
+  return fail(YB_ERR_UNSUPPORTED, "wgrad: %d accumulator columns per CTA (Cin=%d, k=%d) has no kernel", n, cin, ksize);
 }
 
 }  // namespace yb

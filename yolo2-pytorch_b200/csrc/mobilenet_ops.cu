@@ -3,7 +3,7 @@
 //              fp16 NHWC out -- the layout boundary of this backbone.
 //   dwconv3x3  conv_dw: depthwise nn.Conv2d(C,C,3,stride,1,groups=C) + BatchNorm2d + ReLU (:33-38) on fp16 NHWC.
 //              HBM-bound: one thread = 8 channels (16 B) of one output pixel, 9 vector loads, fp32 FMA, 16 B store.
-// The pointwise convs (conv_pw, :41-46) and the 1x1 head reuse the tcgen05 implicit-GEMM kernel (slope = 0 -> ReLU).
+// The pointwise convs (conv_pw, :41-46) and the 1x1 head reuse the wgmma implicit-GEMM kernel (slope = 0 -> ReLU).
 #include "yb_common.h"
 #include <cuda_fp16.h>
 #include <stdint.h>

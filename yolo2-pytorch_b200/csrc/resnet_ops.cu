@@ -2,7 +2,7 @@
 //   stem7x7     nn.Conv2d(3, 64, 7, stride 2, pad 3) + BatchNorm2d + ReLU (:107-109): fp32 NCHW image in, fp16 NHWC out -- the layout boundary.
 //   maxpool3x3  nn.MaxPool2d(3, stride 2, pad 1) (:110) on fp16 NHWC.
 //   subsample2  x[:, ::2, ::2, :]: a stride-2 conv with "same" padding equals its stride-1 form at the even pixels, so the three stride-2 3x3
-//               convs and the 1x1 stride-2 downsample convs (:33,:39,:65,:73) run on the stride-1 tcgen05 kernel + this selection.
+//               convs and the 1x1 stride-2 downsample convs (:33,:39,:65,:73) run on the stride-1 wgmma kernel + this selection.
 //   add_relu    out += residual; relu (:58-59, :100-101).
 // The 3x3 / 1x1 convs themselves (with folded BN and ReLU or identity) are yb_conv_bn_act_fwd.
 #include "yb_common.h"

@@ -533,7 +533,7 @@ int head_grad_prepare(const float* dfeature, void* dz, float* dbias, int batch, 
 // ------------------------------------------------------------------------------------------------
 // conv0 weight gradient: dW[co][ci][r][s] = sum_{b,y,x} dz[b,y,x,co] * x[b,ci,y+r-1,x+s-1]   (Cout = 32, Cin = 3)
 // A [27 taps (padded to 32) x pixels] x [pixels x 32 co] product with the pixels as the reduction dimension.  K = 27 is
-// far too thin for a tcgen05 tile, and the op is HBM-bound (709 MB of dz at batch 64), so this uses warp-level
+// far too thin for a wgmma tile, and the op is HBM-bound (709 MB of dz at batch 64), so this uses warp-level
 // mma.sync.m16n8k16 (fp16 in, fp32 accumulate): persistent blocks over 8x32-pixel tiles, the haloed fp32 input patch
 // and the fp16 dz tile staged in shared memory; warp w owns image row w of the tile (2 K-steps of 16 pixels), builds
 // the tap-major A fragments from the patch (two adjacent pixels -> one half2 register) and reads the dz fragments

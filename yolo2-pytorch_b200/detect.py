@@ -1,7 +1,7 @@
 """detect -- detection post-filter on the GPU (reference detect.py:43-80).
 
 `get_logits`, `filter_visible`, `postprocess` keep the reference's single-image signatures and
-return values; `postprocess_batch` is the B200-native entry point that processes every image of a
+return values; `postprocess_batch` is the H100-native entry point that processes every image of a
 batch in ONE kernel launch (yb_filter_nms: threshold filter -> stable sort -> greedy NMS ->
 per-class expansion, one CTA per image, no host round trips until the results are read).
 The cv2 capture/draw loop of the reference's `Detect` class is host glue outside the hot path.
@@ -23,7 +23,7 @@ def get_prob(pred):
     """Class probabilities: the decode kernel's fused softmax when present (pred['prob'])."""
     if 'prob' in pred:
         return pred['prob']
-    raise RuntimeError('pred has no fused `prob`; build it with model._inference on the B200 Inference module')
+    raise RuntimeError('pred has no fused `prob`; build it with model._inference on the GPU Inference module')
 
 
 def _config_filter(config):

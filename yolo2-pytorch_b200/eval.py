@@ -1,4 +1,4 @@
-"""eval -- detection-quality bookkeeping immediately downstream of NMS (SURVEY 8f rank 3), B200-native where it is per-image
+"""eval -- detection-quality bookkeeping immediately downstream of NMS (SURVEY 8f rank 3), H100-native where it is per-image
 work: the greedy true-positive matching of reference eval.py:57-75 (`_matching` / `matching`, called per image and per class
 from `Eval.filter_cls`, eval.py:210-216) runs as one CUDA launch for a whole batch (`matching_batch`, yb_eval_match); the
 per-dataset reductions `voc_ap` / `average_precision` (eval.py:78-121) are the same few numpy lines as in the reference --
@@ -18,7 +18,7 @@ def matching_batch(det_yx_min, det_yx_max, det_cls, det_off, gt_yx_min, gt_yx_ma
     classes and offsets integer tensors, everything on the GPU.  Returns a uint8 device tensor tp[num_detections]."""
     for name, t in (('det_yx_min', det_yx_min), ('det_yx_max', det_yx_max), ('gt_yx_min', gt_yx_min), ('gt_yx_max', gt_yx_max)):
         if not (isinstance(t, torch.Tensor) and t.is_cuda):
-            raise RuntimeError('eval.matching_batch (B200): %s must be a CUDA tensor; there is no CPU fallback' % name)
+            raise RuntimeError('eval.matching_batch: %s must be a CUDA tensor; there is no CPU fallback' % name)
     dev = det_yx_min.device
     i32 = lambda t: t.to(device=dev, dtype=torch.int32).contiguous()
     f32 = lambda t: t.to(dtype=torch.float32).contiguous()

@@ -1,4 +1,4 @@
-"""model -- detection head helpers of the plugin surface, B200-native.
+"""model -- detection head helpers of the plugin surface, H100-native.
 
 Mirrors the public names of ruiminshen/yolo2-pytorch `model/__init__.py` (reference file:line per
 item) so `detect.py`/`train.py`-style callers keep working: `ConfigChannels` (:29-43),
@@ -72,7 +72,7 @@ class Inference(nn.Module):
     def forward(self, x):
         feature = self.dnn(x)
         if not feature.is_cuda:
-            raise RuntimeError('model.Inference (B200): the backbone must return a CUDA tensor; there is no CPU fallback')
+            raise RuntimeError('model.Inference: the backbone must return a CUDA tensor; there is no CPU fallback')
         anchors = self._anchors_on(feature.device)
         a = anchors.size(0)
         per = feature.size(1) // a
@@ -127,7 +127,7 @@ def loss(anchors, data, pred, threshold, cross_entropy=True):
     train/cross_entropy (config.ini:77; the reference infers it from the rank of data['cls'])."""
     feature = pred['feature']
     if not feature.is_cuda:
-        raise RuntimeError('model.loss (B200): tensors must be on the GPU; there is no CPU fallback')
+        raise RuntimeError('model.loss: tensors must be on the GPU; there is no CPU fallback')
     dev = feature.device
     anchors = anchors.detach().to(device=dev, dtype=torch.float32).contiguous()
     yx_min = data['yx_min'].to(device=dev, dtype=torch.float32).contiguous()

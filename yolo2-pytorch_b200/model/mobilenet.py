@@ -1,17 +1,17 @@
-"""model.mobilenet -- MobileNet backbone plugin on the B200 kernels (inference and training).
+"""model.mobilenet -- MobileNet backbone plugin on the CUDA kernels (inference and training).
 
 Drop-in for the reference's `model/mobilenet.py` (file:line cited per item): same constructor contract
 `MobileNet(config_channels, anchors, num_cls)` (:56-77), same state_dict keys (`layers.0.conv.weight`,
 `layers.N.dw.conv.weight`, `layers.N.pw.bn.running_var`, `layers.14.weight`, `layers.14.bias`), same forward
 contract x[B,3,H,W] fp32 -> [B, A*(5+C), H/32, W/32] fp32 (:84-85).  Modules only hold parameters; the forward pass is:
   conv_bn(3,32,s2)   -> yb_mb_conv0_bn_relu_fwd  (fp32 NCHW image in, fp16 NHWC out)
-  13 x conv_unit      -> yb_dwconv3x3_bn_relu_fwd (depthwise, HBM-bound) + tcgen05 1x1 conv with fused BN + ReLU
-  nn.Conv2d(1024, A*(5+C), 1) with bias -> tcgen05 1x1 conv writing fp32 NCHW.
+  13 x conv_unit      -> yb_dwconv3x3_bn_relu_fwd (depthwise, HBM-bound) + wgmma 1x1 conv with fused BN + ReLU
+  nn.Conv2d(1024, A*(5+C), 1) with bias -> wgmma 1x1 conv writing fp32 NCHW.
 BatchNorm uses the PyTorch-default momentum 0.1 (unlike model.yolo2's 0.01) and the activation is ReLU (:28-29).
 
 Two inference precisions, as for Darknet (`set_precision`, `[b200] precision` in the INI, YB_PRECISION): `fast` (fp16 operands, 1.4e-3 from
 the fp32 reference after 27 layers) and `strict`: activations travel as [hi | lo] fp16 pairs, the pointwise convs and the head run the
-split-precision tcgen05 kernel (operands [a_hi | a_lo | a_hi] x [w_hi | w_hi | w_lo] in one fp32 accumulator), the first conv and the depthwise
+split-precision wgmma kernel (operands [a_hi | a_lo | a_hi] x [w_hi | w_hi | w_lo] in one fp32 accumulator), the first conv and the depthwise
 convs compute in fp32 on hi + lo -- within 1e-3 of the reference.
 """
 import os
@@ -164,14 +164,14 @@ class MobileNet(nn.Module):
             from model.yolo2 import _DarknetTrainFunction
             return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
         if not x.is_cuda:
-            raise RuntimeError('MobileNet (B200): input must be a CUDA tensor; there is no CPU fallback')
+            raise RuntimeError('MobileNet: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape
         if c != 3 or h % 32 or w % 32:
             raise ValueError('MobileNet expects [B,3,H,W] with H, W multiples of 32')
         x = x.contiguous().float()
         first = self.layers[0]
         if first.conv.weight.shape[0] != 32:
-            raise ValueError('MobileNet (B200): the first layer must have 32 output channels')
+            raise ValueError('MobileNet: the first layer must have 32 output channels')
         if self.precision == 'strict':
             return self._forward_strict(x)
         scale, shift = self._fold('bn0', first.bn)

@@ -1,4 +1,4 @@
-"""model.resnet -- ResNet backbone plugin on the B200 kernels (inference).
+"""model.resnet -- ResNet backbone plugin on the CUDA kernels (inference).
 
 Drop-in for the reference's `model/resnet.py` (file:line cited per item): same constructors `resnet18 / resnet34 / resnet50
 (config_channels, anchors, num_cls)` (:161-197), same state_dict keys as torchvision's ResNet (`conv1.weight`, `bn1.*`,
@@ -7,12 +7,12 @@ Drop-in for the reference's `model/resnet.py` (file:line cited per item): same c
 parameters; the forward pass is:
   conv1 7x7 s2 + bn1 + relu      -> yb_stem7x7_bn_relu_fwd   (fp32 NCHW image in, fp16 NHWC out)
   maxpool 3x3 s2 p1              -> yb_maxpool3x3_s2_f16
-  3x3 / 1x1 conv + bn (+ relu)   -> tcgen05 implicit-GEMM conv with the folded BatchNorm in its epilogue (slope 0 = ReLU, 1 = none)
+  3x3 / 1x1 conv + bn (+ relu)   -> wgmma implicit-GEMM conv with the folded BatchNorm in its epilogue (slope 0 = ReLU, 1 = none)
   stride-2 3x3 conv              -> the same kernel at stride 1, then yb_subsample2_f16 (a padded stride-2 conv IS its stride-1
                                     form at the even pixels); stride-2 1x1 downsample -> yb_subsample2_f16, then the 1x1 conv
   out += residual; relu          -> yb_add_relu_f16
-  nn.Conv2d(C, A*(5+C), 1) + bias-> tcgen05 1x1 conv writing fp32 NCHW.
-Training this plugin is not on the B200 path (train() forward raises); Darknet, Tiny and MobileNet are.
+  nn.Conv2d(C, A*(5+C), 1) + bias-> wgmma 1x1 conv writing fp32 NCHW.
+Training this plugin is not on the GPU path (train() forward raises); Darknet, Tiny and MobileNet are.
 """
 import re
 
@@ -158,14 +158,14 @@ class ResNet(nn.Module):
 
     def forward(self, x):
         if self.training:
-            raise NotImplementedError('ResNet (B200): the training step of this plugin is not built; use eval() -- Darknet, Tiny and MobileNet train')
+            raise NotImplementedError('ResNet: the training step of this plugin is not built; use eval() -- Darknet, Tiny and MobileNet train')
         if not x.is_cuda:
-            raise RuntimeError('ResNet (B200): input must be a CUDA tensor; there is no CPU fallback')
+            raise RuntimeError('ResNet: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape
         if c != 3 or h % 32 or w % 32:
             raise ValueError('ResNet expects [B,3,H,W] with H, W multiples of 32')
         if self.conv1.weight.shape[0] != 64:
-            raise ValueError('ResNet (B200): the stem must have 64 output channels')
+            raise ValueError('ResNet: the stem must have 64 output channels')
         x = x.contiguous().float()
         scale, shift = self._fold('bn1', self.bn1)
         stem = torch.empty(b, h // 2, w // 2, 64, dtype=torch.float16, device=x.device)

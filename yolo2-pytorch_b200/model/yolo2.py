@@ -1,4 +1,4 @@
-"""model.yolo2 -- Darknet-19 backbone plugin, B200-native.
+"""model.yolo2 -- Darknet-19 backbone plugin, H100-native.
 
 Drop-in for the plugin surface of ruiminshen/yolo2-pytorch `model/yolo2.py` (reference file:line
 cited per item): same constructor contract `Darknet(config_channels, anchors, num_cls, stride=2,
@@ -9,7 +9,7 @@ the module-level `reorg()` (:33-46).
 
 The modules here only HOLD parameters (so `.cuda()`, `.state_dict()`, `load_state_dict()`,
 `.parameters()` and torch.optim work unchanged).  No torch.nn forward is ever executed: the forward
-pass is the kernel chain in b200.engine (tcgen05 implicit-GEMM convs with fused BN + leaky-ReLU,
+pass is the kernel chain in b200.engine (wgmma implicit-GEMM convs with fused BN + leaky-ReLU,
 fp16 NHWC activations, in-place concat).  There is no CPU fallback.
 """
 import torch
@@ -57,7 +57,7 @@ class Conv2d(nn.Module):
         if isinstance(padding, bool):
             padding = (kernel_size - 1) // 2 if padding else 0
         if stride != 1 or padding != (kernel_size - 1) // 2 or kernel_size not in (1, 3):
-            raise ValueError('B200 Conv2d supports k in {1,3}, stride 1, "same" padding (got k=%d stride=%d pad=%d)'
+            raise ValueError('Conv2d supports k in {1,3}, stride 1, "same" padding (got k=%d stride=%d pad=%d)'
                              % (kernel_size, stride, padding))
         self.conv = nn.Conv2d(in_channels, out_channels, kernel_size, stride, padding=padding, bias=not bn)
         self.has_bn, self.has_act = bool(bn), bool(act)
@@ -67,7 +67,7 @@ class Conv2d(nn.Module):
 
     def forward(self, x):
         """Stand-alone use of one unit on an fp32 NCHW tensor (tests, pruning tools).  Layout/dtype
-        conversion at this boundary is plain data movement; the conv runs on the tcgen05 kernel."""
+        conversion at this boundary is plain data movement; the conv runs on the wgmma kernel."""
         if self.training and self.has_bn:
             raise NotImplementedError('a stand-alone Conv2d unit runs in eval mode only; training goes through Darknet.forward (b200.train_engine)')
         if self._unit is None:
@@ -110,7 +110,7 @@ class Darknet(nn.Module):
     def __init__(self, config_channels, anchors, num_cls, stride=2, ratio=1):
         nn.Module.__init__(self)
         if stride != 2:
-            raise ValueError('Darknet (B200): passthrough stride must be 2')
+            raise ValueError('Darknet: passthrough stride must be 2')
         self.stride = stride
         bn = config_channels.config.getboolean('batch_norm', 'enable')
         cc = config_channels
@@ -233,13 +233,13 @@ class MaxPool2dStride1(nn.Module):
 
 class Tiny(nn.Module):
     """Tiny YOLOv2 backbone plugin (reference model/yolo2.py:140-173; the repo's default `model/dnn`, config.ini:25),
-    inference and training on the B200 kernels.  Same constructor contract `Tiny(config_channels, anchors, num_cls, channels=16)`, same
+    inference and training on the CUDA kernels.  Same constructor contract `Tiny(config_channels, anchors, num_cls, channels=16)`, same
     state_dict keys (`layers.{0,2,4,6,8,10,13,14,15}.conv.*`, `.bn.*`), `init()` (xavier-normal, :159-165), `scope()`
     (:170-171) and forward contract x[B,3,H,W] fp32 -> [B, A*(5+C), H/32, W/32] fp32.
 
     Kernel chain: the 3->16 first layer runs on the fused first-layer kernel with its 16 filters zero-padded to 32 (the
     extra channels come out as exact zeros and the next layer's weights are zero-padded on the input side to match), the
-    two Cin = 32 layers on the halo-tile tcgen05 kernel with the 2x2 max-pool fused, the rest on the implicit-GEMM
+    two Cin = 32 layers on the halo-tile wgmma kernel with the 2x2 max-pool fused, the rest on the implicit-GEMM
     kernel; `ConstantPad2d + MaxPool2d(2, stride=1)` is one HBM kernel."""
 
     def __init__(self, config_channels, anchors, num_cls, channels=16):
@@ -334,7 +334,7 @@ class Tiny(nn.Module):
             # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.TinyTrainer)
             return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
         if not x.is_cuda:
-            raise RuntimeError('Tiny (B200): input must be a CUDA tensor; there is no CPU fallback')
+            raise RuntimeError('Tiny: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape
         if c != 3 or h % 32 or w % 32:
             raise ValueError('Tiny expects fp32 [B,3,H,W] with H, W multiples of 32, got %s' % (tuple(x.shape),))
@@ -344,7 +344,7 @@ class Tiny(nn.Module):
             u.refresh(first_layer=(i == 0))
         u0, after0 = plan[0]
         if after0 != 'pool' or u0.cout > 32:
-            raise RuntimeError('Tiny (B200): the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
+            raise RuntimeError('Tiny: the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
         w0, sc0, sh0 = self._padded('u0', u0, 32, 3, True)
         cur = _ops.conv0_bn_leaky_pool(x, w0, sc0, sh0, u0.slope)          # [B,H/2,W/2,32], channels >= cout are exact zeros
         chan = 32

@@ -1,4 +1,4 @@
-"""train -- the training step of the reference (train.py:57-71,338-362) on the B200 path.
+"""train -- the training step of the reference (train.py:57-71,338-362) on the GPU path.
 
 `norm_data`, `ensure_model` and `iterate` keep the reference's meaning:
   iterate: forward (train-mode Darknet: batch-statistics BatchNorm) -> region loss -> hparam-weighted sum ->
@@ -35,7 +35,7 @@ def ensure_model(module):
     (torch.distributed): nothing is wrapped, every rank's parameters and buffers are made equal to rank 0's once, and the
     gradient exchange (b200.ddp) is attached by `iterate`."""
     if not torch.cuda.is_available():
-        raise RuntimeError('train (B200): a CUDA device is required; there is no CPU fallback')
+        raise RuntimeError('train: a CUDA device is required; there is no CPU fallback')
     module = module.cuda()
     reducer = _ddp.default_reducer()
     if reducer is not None:
@@ -109,7 +109,7 @@ def iterate(inference, optimizer, anchors, config, data, reducer=None):
 class GraphedStep(object):
     """`iterate` captured once per input shape into a CUDA graph and replayed: the ~300 kernel launches, the autograd
     bookkeeping and the optimizer step of one training iteration cost one graph launch, which removes the host
-    launch overhead that dominates the eager step (tcgen05 kernels of 20-100 us each).
+    launch overhead that dominates the eager step (wgmma kernels of 20-100 us each).
 
         step = train.GraphedStep(inference, optimizer, anchors, config)
         out = step(dict(tensor=..., yx_min=..., yx_max=..., cls=...))      # same dict as iterate()

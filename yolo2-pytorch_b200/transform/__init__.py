@@ -59,7 +59,7 @@ def to_tensor(frames_u8):
     """uint8 CUDA tensor [B, H, W, 3] -> float32 [B, 3, H, W] in [0, 1] (torchvision ToTensor, one kernel).  The training
     forward needs this form; inference takes the uint8 batch directly."""
     if not (isinstance(frames_u8, torch.Tensor) and frames_u8.is_cuda and frames_u8.dtype == torch.uint8 and frames_u8.dim() == 4 and frames_u8.shape[3] == 3):
-        raise RuntimeError('transform.to_tensor (B200): expected a uint8 CUDA tensor [B, H, W, 3]')
+        raise RuntimeError('transform.to_tensor: expected a uint8 CUDA tensor [B, H, W, 3]')
     frames_u8 = frames_u8.contiguous()
     b, h, w, _ = frames_u8.shape
     out = torch.empty(b, 3, h, w, dtype=torch.float32, device=frames_u8.device)

@@ -25,7 +25,7 @@ def fixed(image, height, width):
     h, w = int(image.shape[0]), int(image.shape[1])
     scale = height / h if h / w > height / width else width / w
     if scale >= 1:
-        raise NotImplementedError('transform.resize.image.fixed (B200): the INTER_CUBIC branch (scale >= 1) is not built')
+        raise NotImplementedError('transform.resize.image.fixed: the INTER_CUBIC branch (scale >= 1) is not built')
     return _aug.warp_affine(image, [[scale, 0.0, 0.0], [0.0, scale, 0.0]], (width, height), 0)
 
 

@@ -15,7 +15,7 @@ def nms(score, yx_min, yx_max, overlap=0.5, limit=200):
     if score.numel() == 0:
         return []
     if not score.is_cuda:
-        raise RuntimeError('utils.postprocess.nms (B200): inputs must be CUDA tensors; there is no CPU fallback')
+        raise RuntimeError('utils.postprocess.nms: inputs must be CUDA tensors; there is no CPU fallback')
     n = score.numel()
     res = _ops.filter_nms(score.reshape(1, n).contiguous().float(), yx_min.reshape(1, n, 2).contiguous().float(),
                           yx_max.reshape(1, n, 2).contiguous().float(), None, _ops.FILTER_NONE, 0.0, 0.0, overlap, limit)

@@ -1,4 +1,4 @@
-"""utils.train -- checkpoint files on either side of the B200 path (host code, no kernel).
+"""utils.train -- checkpoint files on either side of the GPU path (host code, no kernel).
 
 Same names and on-disk format as the reference's `utils/train.py` (file:line cited per item), so a model directory written by the
 reference is read here and vice versa:
