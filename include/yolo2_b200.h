@@ -301,6 +301,23 @@ int yb_maxpool3x3_s2_f16(const void* x, void* y, int batch, int height, int widt
 int yb_subsample2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
 int yb_add_relu_f16(const void* a, const void* b, void* out, long long count, yb_stream_t stream);
 
+/* Training of the ResNet plugin: what torch autograd does for the stem, the max-pool, the stride-2 selection and the residual join.  BatchNorm and
+ * the activations are the generic train-mode kernels above (slope 0 = ReLU, slope 1 = identity); the 3x3 / 1x1 convs and their gradients are the
+ * wgmma kernels, a stride-2 conv's backward being the stride-1 gradients of the zero-inserted dz (yb_upsample2_zero_f16).
+ *   stem7x7_raw   the stem conv output z, fp16 NHWC [B,H/2,W/2,64], no BatchNorm, no ReLU;
+ *   stem7x7_wgrad dw fp32 OIHW [64,3,7,7] (overwritten) from the fp32 NCHW image and dz fp16 NHWC [B,H/2,W/2,64];
+ *   maxpool bwd   dx [B,H,W,C] from the pool's input x [B,H,W,C] and dy [B,(H+1)/2,(W+1)/2,C]: each output's gradient goes to the first maximum of
+ *                 its window in scan order (torch's CPU rule); deterministic;
+ *   upsample2_zero y [B,H,W,C] = x [B,(H+1)/2,(W+1)/2,C] at the even pixels, 0 elsewhere (the transpose of yb_subsample2_f16);
+ *   residual_bwd  out [B,H,W,C] = (y > 0) ? g_a + S^T g_b : 0 with one rounding: y = the block input (NULL = no mask), g_a [B,H,W,C], g_b (NULL =
+ *                 none) [B,H,W,C] for stride_b = 1 or [B,(H+1)/2,(W+1)/2,C] zero-inserted for stride_b = 2.  C % 8 == 0 for all four fp16 kernels. */
+int yb_stem7x7_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, yb_stream_t stream);
+int yb_stem7x7_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream);
+int yb_maxpool3x3_s2_bwd_f16(const void* x, const void* dy, void* dx, int batch, int height, int width, int channels, yb_stream_t stream);
+int yb_upsample2_zero_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
+int yb_residual_bwd_f16(const void* y, const void* g_a, const void* g_b, int stride_b, void* out, int batch, int height, int width, int channels,
+                        yb_stream_t stream);
+
 /* Training of the MobileNet plugin: what torch autograd does for conv_bn / conv_dw (model/mobilenet.py:25-38).  The raw forms return the conv
  * output before BatchNorm / ReLU (train-mode statistics come from yb_bn_stats / yb_bn_finalize, the activation from yb_bn_act_apply with slope 0);
  * height / width are always those of the conv INPUT.  dgrad: da fp16 [B,H,W,C] from dz fp16 [B,H/stride,W/stride,C]; wgrad: dw fp32 [C][9]

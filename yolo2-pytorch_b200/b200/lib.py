@@ -72,6 +72,11 @@ SIGNATURES = {
     'yb_maxpool3x3_s2_f16': [P, P, c_int, c_int, c_int, c_int, P],
     'yb_subsample2_f16': [P, P, c_int, c_int, c_int, c_int, P],
     'yb_add_relu_f16': [P, P, P, c_longlong, P],
+    'yb_stem7x7_raw_fwd': [P, P, P, c_int, c_int, c_int, P],
+    'yb_stem7x7_wgrad': [P, P, P, c_int, c_int, c_int, P],
+    'yb_maxpool3x3_s2_bwd_f16': [P, P, P, c_int, c_int, c_int, c_int, P],
+    'yb_upsample2_zero_f16': [P, P, c_int, c_int, c_int, c_int, P],
+    'yb_residual_bwd_f16': [P, P, P, c_int, P, c_int, c_int, c_int, c_int, P],
     'yb_comm_version': [ctypes.POINTER(c_int)],
     'yb_comm_unique_id': [P],
     'yb_comm_init': [ctypes.POINTER(P), c_int, P, c_int],

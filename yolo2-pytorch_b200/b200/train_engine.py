@@ -103,6 +103,16 @@ class DarknetTrainer(object):
             self._tracked = []
 
     # ---- helpers -------------------------------------------------------------------------------------
+    def _slope(self, u):
+        """Activation slope of a unit's train-mode BatchNorm + activation: its own `train_slope` (ResNet units: 0 = ReLU, 1 = identity),
+        else the trainer's."""
+        return getattr(u, 'train_slope', self.slope)
+
+    @staticmethod
+    def _pnames(key, u):
+        """State-dict names of a unit's (conv weight, BN weight, BN bias): `key.conv.weight`, `key.bn.*` unless the unit carries `pnames`."""
+        return getattr(u, 'pnames', None) or (key + '.conv.weight', key + '.bn.weight', key + '.bn.bias')
+
     def _emit(self, name, grads):
         if self.reducer is not None:
             dev = grads[name].device
@@ -211,7 +221,7 @@ class DarknetTrainer(object):
         c = u.cout
         if out is None:
             out = torch.empty(b, h // 2 if pool else h, w // 2 if pool else w, c, dtype=torch.float16, device=z.device)
-        ops.call('yb_bn_act_apply', z, z.shape[-1], mean, invstd, u.bn.weight.detach(), u.bn.bias.detach(), self.slope, out, out.shape[-1], a_off,
+        ops.call('yb_bn_act_apply', z, z.shape[-1], mean, invstd, u.bn.weight.detach(), u.bn.bias.detach(), self._slope(u), out, out.shape[-1], a_off,
                  b, h, w, c, int(pool))
         return out
 
@@ -220,15 +230,16 @@ class DarknetTrainer(object):
         c = u.cout
         dev = s.z.device
         sums = self._sums(('b', key), c, dev)
-        args = (s.z, s.z.shape[-1], s.mean, s.invstd, u.bn.weight.detach(), u.bn.bias.detach(), self.slope, da, 0 if da is None else da.shape[-1], 0, dap,
+        args = (s.z, s.z.shape[-1], s.mean, s.invstd, u.bn.weight.detach(), u.bn.bias.detach(), self._slope(u), da, 0 if da is None else da.shape[-1], 0, dap,
                 0 if dap is None else dap.shape[-1], 0, b, s.h, s.w, c, 1 if dap is not None else 0, sums)
         ops.call('yb_bn_act_bwd', 0, *args, None, 0, 1)
         ops.call('yb_bn_act_bwd', 1, *args, dz, ld_dz, 1)
-        dgamma, dbeta = self.arena.views[key + '.bn.weight'], self.arena.views[key + '.bn.bias']
+        _, gname, bname = self._pnames(key, u)
+        dgamma, dbeta = self.arena.views[gname], self.arena.views[bname]
         ops.call('yb_bn_param_grad', sums, c, dgamma, dbeta, 1, self._unscale)
-        grads[key + '.bn.weight'], grads[key + '.bn.bias'] = dgamma, dbeta
-        self._emit(key + '.bn.weight', grads)
-        self._emit(key + '.bn.bias', grads)
+        grads[gname], grads[bname] = dgamma, dbeta
+        self._emit(gname, grads)
+        self._emit(bname, grads)
 
     # ---- forward -------------------------------------------------------------------------------------
     def forward(self, x):
@@ -350,10 +361,11 @@ class DarknetTrainer(object):
         with torch.cuda.stream(side) if side is not None else _NullCtx():
             dw_krsc = torch.empty(cout, k, k, cin, dtype=torch.float32, device=dev)
             ops.call('yb_conv_wgrad', ain, dz, dw_krsc, b, hh, ww, cin, cout, k, ain.shape[-1], dz.shape[-1])
-            dw = self.arena.views[name + '.conv.weight']                                  # [cout, cin, k, k] slot of the gradient arena
+            wname = self._pnames(name, u)[0]
+            dw = self.arena.views[wname]                                                     # [cout, cin, k, k] slot of the gradient arena
             ops.call('yb_unpack_wgrad', dw_krsc, dw, cout, cin, k, self._unscale)            # layout change + inverse loss scale (/ world)
-            grads[name + '.conv.weight'] = dw
-            self._emit(name + '.conv.weight', grads)
+            grads[wname] = dw
+            self._emit(wname, grads)
 
     def _side(self, dev):
         # only while the step is being captured into a CUDA graph: in eager mode the step is host-bound and the extra
@@ -380,18 +392,19 @@ class DarknetTrainer(object):
         window = 1 if (dap is not None) else 0
         sums = self._sums(('b', key), c, dev)
         bnw, bnb = u.bn.weight.detach(), u.bn.bias.detach()
-        args = (s.z, s.z.shape[-1], s.mean, s.invstd, bnw, bnb, self.slope, da, 0 if da is None else da.shape[-1], da_off, dap,
+        args = (s.z, s.z.shape[-1], s.mean, s.invstd, bnw, bnb, self._slope(u), da, 0 if da is None else da.shape[-1], da_off, dap,
                 0 if dap is None else dap.shape[-1], dap_off, b, s.h, s.w, c, window, sums)
         ops.call('yb_bn_act_bwd', 0, *args, None, 0, 1)
-        dgamma = self.arena.views[key + '.bn.weight']
-        dbeta = self.arena.views[key + '.bn.bias']
+        _, gname, bname = self._pnames(key, u)
+        dgamma = self.arena.views[gname]
+        dbeta = self.arena.views[bname]
         dz = torch.empty(b, s.h, s.w, c, dtype=torch.float16, device=dev)
         ops.call('yb_bn_act_bwd', 1, *args, dz, c, 1)
         ops.call('yb_bn_param_grad', sums, c, dgamma, dbeta, 1, self._unscale)     # un-scales (/ world), then clears the accumulators
-        grads[key + '.bn.weight'] = dgamma
-        grads[key + '.bn.bias'] = dbeta
-        self._emit(key + '.bn.weight', grads)
-        self._emit(key + '.bn.bias', grads)
+        grads[gname] = dgamma
+        grads[bname] = dbeta
+        self._emit(gname, grads)
+        self._emit(bname, grads)
         if s.ain is None:
             return dz
         self._wgrad(u, s.ain, dz, b, s.h, s.w, grads, key)
@@ -792,6 +805,223 @@ class MobileNetTrainer(DarknetTrainer):
         ops.call('yb_mb_conv0_wgrad', saved.x, dz0, dw0, b, saved.h, saved.w)
         grads['layers.0.conv.weight'] = dw0.mul_(self._unscale)
         self._emit('layers.0.conv.weight', grads)
+        self._join(dev)
+        if self.reducer is not None:
+            self.reducer.finish()
+        if self.found_inf is None or self.found_inf.device != dev:
+            self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
+        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+        return grads
+
+
+class _ResUnit(object):
+    """One conv + BatchNorm unit of a ResNet (stem, block conv, downsample) as the trainer helpers read it: its own activation slope
+    (0 = ReLU, 1 = identity before the residual join) and its torchvision-style state-dict names."""
+
+    def __init__(self, key, conv, bn, slope, pnames):
+        self.key, self.conv, self.bn, self.train_slope, self.pnames = key, conv, bn, slope, pnames
+        self.stride, self.ksize = conv.stride[0], conv.kernel_size[0]
+        self.cout, self.cin = conv.weight.shape[0], conv.weight.shape[1]
+        self.w16 = None
+        self._bver = None
+
+
+class ResNetTrainer(DarknetTrainer):
+    """Training-mode forward / backward of `model.resnet.ResNet` (reference model/resnet.py:28-142): stem conv 7x7 stride 2 + BN + ReLU,
+    MaxPool2d(3, 2, 1), BasicBlock / Bottleneck stacks, a 1x1 head with bias.
+
+    Forward per unit: raw wgmma conv -> batch statistics -> running-stat update (momentum read from the module, 0.1) -> normalise + ReLU
+    (slope 0), or identity (slope 1) on the last unit of a block and on the downsample; the join is yb_add_relu_f16.  A stride-2 3x3 conv runs
+    at stride 1 and keeps the even pixels (yb_subsample2_f16), its statistics taken after the selection; the 1x1 stride-2 downsample reads the
+    subsampled input.  Backward of a stride-2 3x3 conv is the transpose: dz zero-inserted to full resolution (yb_upsample2_zero_f16), then the
+    stride-1 weight and data gradients.  At each block boundary yb_residual_bwd_f16 sums the main path's data gradient and the skip path's and
+    applies the previous block's ReLU mask in one pass.  The stem's gradient runs through the max-pool backward (first maximum of each window),
+    the BN + ReLU backward and a CUDA-core weight-gradient kernel on the fp32 image."""
+
+    def __init__(self, dnn, grad_scale=16384.0):
+        DarknetTrainer.__init__(self, _TinyEngineView(dnn), grad_scale)
+        self.dnn = dnn
+        self.slope = 0.0
+        self._blocks = None
+
+    def _plan(self):
+        if self._blocks is None:
+            net = self.dnn
+            blocks = []
+            for lname in ('layer1', 'layer2', 'layer3', 'layer4'):
+                for bname, blk in getattr(net, lname).named_children():
+                    p = '%s.%s' % (lname, bname)
+                    units = []
+                    for name, conv, bn, relu in blk.units():
+                        bnn = '%s.bn%s' % (p, name[len('conv'):])
+                        units.append(_ResUnit('%s.%s' % (p, name), conv, bn, 0.0 if relu else 1.0, ('%s.%s.weight' % (p, name), bnn + '.weight', bnn + '.bias')))
+                    ds = None
+                    if blk.downsample is not None:
+                        ds = _ResUnit(p + '.downsample', blk.downsample[0], blk.downsample[1], 1.0,
+                                      (p + '.downsample.0.weight', p + '.downsample.1.weight', p + '.downsample.1.bias'))
+                    blocks.append((p, units, ds))
+            self._stem = _ResUnit('conv1', net.conv1, net.bn1, 0.0, ('conv1.weight', 'bn1.weight', 'bn1.bias'))
+            self._head = _ResUnit('conv', net.conv, None, 1.0, ('conv.weight', None, None))
+            self._blocks = blocks
+        return self._blocks
+
+    def _conv_units(self):
+        return [u for _, units, ds in self._plan() for u in units + ([ds] if ds is not None else [])]
+
+    def grad_order(self):
+        names = ['conv.bias', 'conv.weight']
+        for _, units, ds in reversed(self._plan()):
+            for u in list(reversed(units)) + ([ds] if ds is not None else []):
+                names += [u.pnames[1], u.pnames[2], u.pnames[0]]
+        return names + ['bn1.weight', 'bn1.bias', 'conv1.weight']
+
+    def _repack(self, device):
+        """Forward and data-gradient fp16 operands of every 1x1 / 3x3 conv and the head in ONE batched launch (the stem reads its fp32
+        weights in place)."""
+        units = self._conv_units() + [self._head]
+        ptrs = tuple(u.conv.weight.data_ptr() for u in units)
+        plan = self._pack_plan
+        if plan is None or plan.key != ptrs or plan.table.device != device:
+            cpad = (self._head.cout + 31) // 32 * 32          # the head's filters are padded to the dz buffer's width
+            plan = self._pack_plan = PackPlan([(u.key, u.conv.weight.detach(), True, True, cpad if u is self._head else 0) for u in units], device)
+        plan.run()
+        for u in units:
+            u.w16 = plan.fwd[u.key]
+            self.wd_cache[u.key] = plan.dgrad[u.key]
+
+    def _subsample(self, x):
+        b, h, w, c = x.shape
+        out = torch.empty(b, (h + 1) // 2, (w + 1) // 2, c, dtype=torch.float16, device=x.device)
+        ops.call('yb_subsample2_f16', x, out, b, h, w, c)
+        return out
+
+    def _unit_forward(self, u, src, b, hh, ww):
+        s = _Saved()
+        if u.stride == 2 and u.ksize == 1:
+            src = self._subsample(src)                     # kept: the weight gradient reads it
+            hh, ww = src.shape[1], src.shape[2]
+        s.u, s.ain, s.in_h, s.in_w = u, src, hh, ww
+        if u.stride == 2 and u.ksize == 3:
+            # statistics over the selected (stride-2) pixels only: not from the full-resolution conv epilogue
+            z = self._subsample(self._raw_conv(u, src))
+            oh, ow = z.shape[1], z.shape[2]
+        else:
+            z = self._raw_conv(u, src, key=u.key)
+            oh, ow = hh, ww
+        mean, invstd = self._bn_forward(u.key, u, z, b * oh * ow)
+        a = self._apply(u, z, mean, invstd, b, oh, ow, False)
+        s.z, s.mean, s.invstd, s.h, s.w = z, mean, invstd, oh, ow
+        return a, s
+
+    def forward(self, x):
+        self._tracked = []
+        if not x.is_cuda:
+            raise RuntimeError('ResNet training: input must be a CUDA tensor')
+        b, c, h, w = x.shape
+        if c != 3 or h % 32 or w % 32:
+            raise ValueError('ResNet expects [B,3,H,W] with H, W multiples of 32')
+        net = self.dnn
+        if tuple(net.conv1.weight.shape) != (64, 3, 7, 7):
+            raise ValueError('ResNet: the stem must be a 7x7 conv with 64 output channels')
+        x = x.contiguous().float()
+        dev = x.device
+        blocks = self._plan()
+        self._repack(dev)
+        saved = _Saved()
+        saved.x, saved.b, saved.h, saved.w = x, b, h, w
+        # stem: raw conv -> BN (batch statistics) -> ReLU -> max-pool
+        st = self._stem
+        hh, ww = h // 2, w // 2
+        z = torch.empty(b, hh, ww, 64, dtype=torch.float16, device=dev)
+        ops.call('yb_stem7x7_raw_fwd', x, st.conv.weight.detach(), z, b, h, w)
+        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww)
+        a = self._apply(st, z, mean, invstd, b, hh, ww, False)
+        s = _Saved()
+        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w = st, None, z, mean, invstd, hh, ww
+        saved.stem, saved.stem_a = s, a
+        cur = torch.empty(b, hh // 2, ww // 2, 64, dtype=torch.float16, device=dev)
+        ops.call('yb_maxpool3x3_s2_f16', a, cur, b, hh, ww, 64)
+        hh, ww = hh // 2, ww // 2
+        saved.pool = cur
+        saved.blocks = []
+        for _, units, ds in blocks:
+            xin, in_h, in_w = cur, hh, ww
+            recs = []
+            for u in units:
+                cur, s = self._unit_forward(u, cur, b, hh, ww)
+                hh, ww = s.h, s.w
+                recs.append(s)
+            if ds is not None:
+                res, sds = self._unit_forward(ds, xin, b, in_h, in_w)
+            else:
+                res, sds = xin, None
+            if res.shape != cur.shape:
+                raise RuntimeError('ResNet training: residual %s does not match the block output %s' % (tuple(res.shape), tuple(cur.shape)))
+            ops.call('yb_add_relu_f16', cur, res, cur, cur.numel())      # in place: the units keep z, not their output
+            saved.blocks.append((xin, in_h, in_w, recs, sds))
+        head = self._head
+        one, _ = self._ones(head.cout, dev)
+        feature = ops.conv_bn_act(cur, head.w16, one, head.conv.bias.detach(), 1.0, out_mode=ops.OUT_F32_NCHW)
+        saved.a_last, saved.hh, saved.ww = cur, hh, ww
+        self._bump_tracked()
+        return feature, saved
+
+    def _res_unit_backward(self, s, b, grads, da):
+        """Backward of one block unit from the gradient of its output; returns the gradient of its input (s.ain's resolution)."""
+        u = s.u
+        if not (u.stride == 2 and u.ksize == 3):
+            return self._unit_backward(u.key, s, b, grads, da=da)
+        dev = s.z.device
+        dz = torch.empty(b, s.h, s.w, u.cout, dtype=torch.float16, device=dev)
+        self._bn_backward(u.key, s, b, grads, da, None, dz, u.cout)
+        dzf = torch.empty(b, s.in_h, s.in_w, u.cout, dtype=torch.float16, device=dev)
+        ops.call('yb_upsample2_zero_f16', dz, dzf, b, s.in_h, s.in_w, u.cout)
+        self._wgrad(u, s.ain, dzf, b, s.in_h, s.in_w, grads, u.key)
+        one, zero = self._ones(u.cin, dev)
+        return ops.conv_bn_act(dzf, self._wd(u.key, u), one, zero, 1.0)
+
+    def backward(self, saved, dfeature, dnn=None):
+        b = saved.b
+        grads = {}
+        dev = dfeature.device
+        self._ensure_arena(self.dnn, dev)
+        self._main = torch.cuda.current_stream(dev)
+        head = self._head
+        hh, ww = saved.hh, saved.ww
+        chead, cin = head.cout, head.cin
+        cpad = (chead + 31) // 32 * 32
+        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
+        dbias = self.arena.views['conv.bias']
+        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
+        grads['conv.bias'] = dbias.mul_(self._unscale)
+        self._emit('conv.bias', grads)
+        self._wgrad(head, saved.a_last, dzh, b, hh, ww, grads, head.key, cout=chead)
+        one, zero = self._ones(cin, dev)
+        gh = ops.conv_bn_act(dzh, self._wd(head.key, head, cpad), one, zero, 1.0)
+        g = torch.empty_like(gh)
+        ops.call('yb_residual_bwd_f16', saved.a_last, gh, None, 1, g, b, hh, ww, cin)        # through the last block's ReLU
+        # g: gradient of the pre-ReLU sum of the current block (main path + skip)
+        for (xin, in_h, in_w, recs, sds), (_, units, ds) in reversed(list(zip(saved.blocks, self._plan()))):
+            gm = g
+            for s in reversed(recs):
+                gm = self._res_unit_backward(s, b, grads, gm)
+            if sds is not None:
+                gb, stride_b = self._res_unit_backward(sds, b, grads, g), sds.u.stride
+            else:
+                gb, stride_b = g, 1
+            mask = None if xin is saved.pool else xin           # layer1.0's input is the max-pool output: no ReLU in between
+            g = torch.empty_like(xin)
+            ops.call('yb_residual_bwd_f16', mask, gm, gb, stride_b, g, b, in_h, in_w, xin.shape[-1])
+        # stem: max-pool backward -> BN + ReLU backward -> weight gradient from the fp32 image
+        st = saved.stem
+        da = torch.empty_like(saved.stem_a)
+        ops.call('yb_maxpool3x3_s2_bwd_f16', saved.stem_a, g, da, b, st.h, st.w, 64)
+        dz = torch.empty(b, st.h, st.w, 64, dtype=torch.float16, device=dev)
+        self._bn_backward(st.u.key, st, b, grads, da, None, dz, 64)
+        dw = self.arena.views['conv1.weight']
+        ops.call('yb_stem7x7_wgrad', saved.x, dz, dw, b, saved.h, saved.w)
+        grads['conv1.weight'] = dw.mul_(self._unscale)
+        self._emit('conv1.weight', grads)
         self._join(dev)
         if self.reducer is not None:
             self.reducer.finish()

@@ -107,10 +107,14 @@ int eval_match(const float*, const float*, const int*, const int*, const float*,
 int unpack_wgrad(const float*, float*, int, int, int, float, cudaStream_t);
 int grad_guard(float*, long long, float*, int, cudaStream_t);
 int conv_wgrad_forward(const void*, const void*, float*, int, int, int, int, int, int, int, int, cudaStream_t);
-int stem7x7(const float*, const float*, const float*, const float*, void*, int, int, int, cudaStream_t);
+int stem7x7(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
+int stem7x7_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
 int maxpool3x3_s2(const void*, void*, int, int, int, int, cudaStream_t);
+int maxpool3x3_s2_bwd(const void*, const void*, void*, int, int, int, int, cudaStream_t);
 int subsample2(const void*, void*, int, int, int, int, cudaStream_t);
+int upsample2_zero(const void*, void*, int, int, int, int, cudaStream_t);
 int add_relu(const void*, const void*, void*, long long, cudaStream_t);
+int residual_bwd(const void*, const void*, const void*, int, void*, int, int, int, int, cudaStream_t);
 int comm_version(int*);
 int comm_unique_id(void*);
 int comm_init(void**, int, const void*, int);
@@ -410,7 +414,7 @@ int yb_dwconv3x3_bn_relu_fwd(const void* x, const float* w_c9, const float* scal
 
 int yb_stem7x7_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height, int width,
                            yb_stream_t stream) {
-  return yb::stem7x7(x_nchw, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, S(stream));
+  return yb::stem7x7(x_nchw, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, S(stream));
 }
 
 int yb_maxpool3x3_s2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
@@ -422,6 +426,27 @@ int yb_subsample2_f16(const void* x, void* y, int batch, int height, int width, 
 }
 
 int yb_add_relu_f16(const void* a, const void* b, void* out, long long count, yb_stream_t stream) { return yb::add_relu(a, b, out, count, S(stream)); }
+
+int yb_stem7x7_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, yb_stream_t stream) {
+  return yb::stem7x7(x_nchw, w_oihw, nullptr, nullptr, z_nhwc_f16, batch, height, width, 1, S(stream));
+}
+
+int yb_stem7x7_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream) {
+  return yb::stem7x7_wgrad(x_nchw, dz_nhwc_f16, dw_oihw, batch, height, width, S(stream));
+}
+
+int yb_maxpool3x3_s2_bwd_f16(const void* x, const void* dy, void* dx, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::maxpool3x3_s2_bwd(x, dy, dx, batch, height, width, channels, S(stream));
+}
+
+int yb_upsample2_zero_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::upsample2_zero(x, y, batch, height, width, channels, S(stream));
+}
+
+int yb_residual_bwd_f16(const void* y, const void* g_a, const void* g_b, int stride_b, void* out, int batch, int height, int width, int channels,
+                        yb_stream_t stream) {
+  return yb::residual_bwd(y, g_a, g_b, stride_b, out, batch, height, width, channels, S(stream));
+}
 
 int yb_comm_version(int* nccl_version) { return yb::comm_version(nccl_version); }
 

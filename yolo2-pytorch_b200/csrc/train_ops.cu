@@ -400,7 +400,7 @@ static int grid_for(long long work_items, int items_per_thread = 1) {
 static int grid_for_groups(long long work_items, int c8) {
   static const int items = getenv("YB_BN_ITEMS") ? atoi(getenv("YB_BN_ITEMS")) : 16;   // tuning knob (tools): work items per thread
   int g = grid_for(work_items, items > 0 ? items : 16);    // every block pays ~50 parameter loads per thread and 2C global double atomics
-  (void)c8;  // blockDim (256) is a multiple of every supported c8 (4..128), so any grid size works
+  (void)c8;  // blockDim (256) is a multiple of every supported c8 (4..256), so any grid size works
   return g;
 }
 
@@ -443,7 +443,7 @@ int bn_act_apply(const void* z, long long ld_z, const float* mean, const float* 
 int bn_act_bwd(int mode, const void* z, long long ld_z, const float* mean, const float* invstd, const float* gamma, const float* beta,
                float slope, const void* da, long long ld_da, int da_off, const void* dap, long long ld_dap, int dap_off, int batch, int height,
                int width, int channels, int window, double* sums, void* dz, long long ld_dz, int has_bn, cudaStream_t stream) {
-  YB_REQUIRE(z && sums && (da || dap) && channels % 8 == 0 && channels <= 1024 && kTrainThreads % (channels / 8) == 0, "bn_act_bwd: bad argument (C=%d)", channels);
+  YB_REQUIRE(z && sums && (da || dap) && channels % 8 == 0 && channels <= 2048 && kTrainThreads % (channels / 8) == 0, "bn_act_bwd: bad argument (C=%d)", channels);
   YB_REQUIRE(!has_bn || (mean && invstd && gamma && beta), "bn_act_bwd: BN parameters missing");
   YB_REQUIRE(mode == 0 || dz != nullptr, "bn_act_bwd: dz missing");
   YB_REQUIRE(!window || (height % 2 == 0 && width % 2 == 0), "bn_act_bwd: window mode needs even H, W");

@@ -1,4 +1,4 @@
-"""model.resnet -- ResNet backbone plugin on the CUDA kernels (inference).
+"""model.resnet -- ResNet backbone plugin on the CUDA kernels (inference and training).
 
 Drop-in for the reference's `model/resnet.py` (file:line cited per item): same constructors `resnet18 / resnet34 / resnet50
 (config_channels, anchors, num_cls)` (:161-197), same state_dict keys as torchvision's ResNet (`conv1.weight`, `bn1.*`,
@@ -12,7 +12,10 @@ parameters; the forward pass is:
                                     form at the even pixels); stride-2 1x1 downsample -> yb_subsample2_f16, then the 1x1 conv
   out += residual; relu          -> yb_add_relu_f16
   nn.Conv2d(C, A*(5+C), 1) + bias-> wgmma 1x1 conv writing fp32 NCHW.
-Training this plugin is not on the GPU path (train() forward raises); Darknet, Tiny and MobileNet are.
+In train() mode the forward is one autograd node (model.yolo2._DarknetTrainFunction) over b200.train_engine.ResNetTrainer: batch-statistics
+BatchNorm (momentum 0.1, read from the modules) on the raw conv outputs, the explicit backward chain (stride-2 convs as the stride-1 gradients of the
+zero-inserted dz, max-pool backward to the first maximum of each window, the stem's weight gradient on the fp32 image).  There is no CPU path.
+Switching back to eval() drops the cached folded BatchNorm and packed weights, so inference uses the trained state.
 """
 import re
 
@@ -21,6 +24,7 @@ import torch.nn as nn
 
 import model
 from b200 import ops as _ops
+from b200 import train_engine as _train
 
 
 def conv3x3(in_planes, out_planes, stride=1):
@@ -87,6 +91,7 @@ class ResNet(nn.Module):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
         self._cache = {}
+        self._trainer = None
 
     def _make_layer(self, config_channels, prefix, block, channels, blocks, stride=1):
         seq = [block(config_channels, '%s.0' % prefix, channels, stride)]
@@ -107,7 +112,15 @@ class ResNet(nn.Module):
             assert comp[-1] == 'conv', name
         return '.'.join(comp)
 
+    @property
+    def trainer(self):
+        if self._trainer is None:
+            self._trainer = _train.ResNetTrainer(self)
+        return self._trainer
+
     def train(self, mode=True):
+        """nn.Module.train + drop cached kernel operands (training updates running statistics and, with fused optimizers, parameters behind
+        torch's version counters)."""
         if bool(mode) != self.training:
             self._cache = {}
         return nn.Module.train(self, mode)
@@ -158,7 +171,11 @@ class ResNet(nn.Module):
 
     def forward(self, x):
         if self.training:
-            raise NotImplementedError('ResNet: the training step of this plugin is not built; use eval() -- Darknet, Tiny and MobileNet train')
+            if not x.is_cuda:
+                raise NotImplementedError('ResNet training: no CPU path, input must be a CUDA tensor')
+            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.ResNetTrainer)
+            from model.yolo2 import _DarknetTrainFunction
+            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
         if not x.is_cuda:
             raise RuntimeError('ResNet: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape

@@ -196,7 +196,12 @@ class GraphedStep(object):
 
     def finish(self):
         """Drop operand caches that the graph kept current on its own buffers (see the class docstring)."""
-        self.inference.dnn.engine.invalidate()
+        dnn = self.inference.dnn
+        engine = getattr(dnn, 'engine', None)
+        if engine is not None:
+            engine.invalidate()
+        elif hasattr(dnn, '_cache'):
+            dnn._cache = {}          # plugins that cache their operands on the module (MobileNet, ResNet)
 
     def close(self):
         """Destroy the captured graphs (required before the NCCL communicator whose collectives they captured is destroyed)."""
