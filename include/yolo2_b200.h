@@ -96,6 +96,10 @@ int yb_conv_bn_act_stats_fwd(const void* x, const void* w, const float* scale, c
                              int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int flags,
                              double* sums, yb_stream_t stream);
 long long yb_conv_workspace_bytes(void);
+/* The kernel and tile shape yb_conv_bn_act_fwd (with_workspace = 0) or yb_conv_bn_act_fwd_ws (1) picks for this shape and these
+ * flags -- the same selection function the launch runs.  out = {kernel: 0 one-warpgroup implicit GEMM, 1 two-consumer 256 x 128
+ * implicit GEMM, 2 Cin = 32 halo tiles; BK; BLOCK_N; pixels per CTA tile; stream-K 0/1; grid}. */
+int yb_conv_choice(int batch, int height, int width, int cin, int cout, int ksize, int out_mode, int flags, int with_workspace, int out[6]);
 int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                           int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);

@@ -141,6 +141,17 @@ def conv_workspace(device='cuda'):
     return torch.zeros(int(_l.load().yb_conv_workspace_bytes()), dtype=torch.uint8, device=device)
 
 
+CONV_KERNELS = ('conv_igemm_kernel', 'conv_wide_kernel', 'conv_c32_kernel')
+
+
+def conv_choice(batch, height, width, cin, cout, k, out_mode=OUT_F16_NHWC, flags=0, workspace=True):
+    """The kernel and tile shape conv_bn_act picks for this shape (the library's own selection, yb_conv_choice)."""
+    out = (ctypes.c_int * 6)()
+    _l.check(_l.load().yb_conv_choice(batch, height, width, cin, cout, k, out_mode, flags, int(bool(workspace)), ctypes.byref(out)),
+             'yb_conv_choice')
+    return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5])
+
+
 def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, ref=False, workspace=None):
     """x: fp16 [B,H,W,x_ld] (uses the first `cin` channels, default all); w: fp16 [Cout,k,k,Cin].
     out (fp16): [B,H,W,y_ld] written at channels [y_ch_off, y_ch_off+Cout); out (fp32): [B,Cout,H,W]."""

@@ -61,6 +61,7 @@ int* debug_word_device() {
 
 // implemented in the kernel translation units
 long long conv_workspace_bytes();
+int conv_choice(int, int, int, int, int, int, int, int, int, int*);
 int conv_igemm_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, long long,
                        int, int, int, void*, long long, double*, int, int, cudaStream_t);
 int pack_weight_split(const float*, void*, int, int, int, int, int, cudaStream_t);
@@ -181,6 +182,10 @@ int yb_conv_bn_act_stats_fwd(const void* x, const void* w, const float* scale, c
 }
 
 long long yb_conv_workspace_bytes(void) { return yb::conv_workspace_bytes(); }
+
+int yb_conv_choice(int batch, int height, int width, int cin, int cout, int ksize, int out_mode, int flags, int with_workspace, int out[6]) {
+  return yb::conv_choice(batch, height, width, cin, cout, ksize, out_mode, flags, with_workspace, out);
+}
 
 int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                           int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,

@@ -592,6 +592,231 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 }
 
 // ---------------------------------------------------------------------------------------------
+// Wide family: a 256 x 128 CTA tile on two consumer warpgroups.  Warpgroup 0 is the producer (one thread issues the TMAs,
+// the group gives its registers back), warpgroups 1 and 2 each accumulate 128 pixels x 128 channels in registers
+// (128 fp32 per thread) from the same stage: A is one 256-pixel box, B is read by both.  Per FLOP that moves 2/3 of the
+// operand bytes of the 128 x 128 tile.  The epilogue runs from the registers (scale / shift, leaky, fp16, a 128B-swizzled
+// staging slice, TMA store), so there is no accumulator park; stream-K partials go to and come from `ws` out of the
+// registers.  Each accumulator sees the same K-blocks and k16 steps in the same order as in the 128 x 128 kernel, so a
+// launch without stream-K is bit-identical to it.  fp16 NHWC output only: the head, the residual (lo) output and the
+// training statistics stay on conv_igemm_kernel.
+// ---------------------------------------------------------------------------------------------
+constexpr int kWideThreads = 384;
+constexpr int kWideRows = 256;
+constexpr int kWideBN = 128;
+
+template <int BK>
+struct WideCfg {
+  static constexpr int kSwizzle = BK * 2;
+  static constexpr int kABytes = kWideRows * BK * 2;
+  static constexpr int kBBytes = kWideBN * BK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kOutBytes = 128 * 128;                   // per consumer: 128 rows x 64 channels fp16, 128B-swizzled
+  static constexpr int kFixedBytes = 2 * kOutBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kStages = ((kSmemLimit - kFixedBytes) / kStageBytes) > 8 ? 8 : ((kSmemLimit - kFixedBytes) / kStageBytes);
+  static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
+  static constexpr int kWsFloats = kWideRows * kWideBN;         // one CTA's stream-K partial tile
+  static_assert(kStages >= 3, "shared memory budget");
+};
+
+template <int BK>
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
+  using Cfg = WideCfg<BK>;
+  constexpr int kStages = Cfg::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_a = smem_base;
+  const uint32_t smem_b = smem_base + kStages * Cfg::kABytes;
+  const uint32_t smem_o = smem_base + kStages * Cfg::kStageBytes;         // [2 consumers][kOutBytes]
+  const uint32_t bar_full = smem_o + 2 * Cfg::kOutBytes;                 // [kStages]
+  const uint32_t bar_empty = bar_full + 8 * kStages;                     // [kStages]
+  const int num_tiles = p.m_tiles * p.n_tiles;
+  const int unit_id = static_cast<int>(blockIdx.x);
+  const int num_units = static_cast<int>(gridDim.x);
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(bar_full + 8 * i, 1);
+      mbar_init(bar_empty + 8 * i, 8);                     // one arrival per consumer warp
+    }
+    fence_mbar_init();
+    fence_proxy_async_smem();
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_y);
+  }
+  __syncthreads();
+  pdl_trigger();
+  pdl_wait();
+
+  if (threadIdx.x < 128) {
+    // ===================== producer warpgroup =====================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
+        const int n_tile = it.tile % p.n_tiles;
+        const int m_cta = (it.tile / p.n_tiles) * kWideRows;
+        const int img = m_cta / p.hw;
+        const int rem = m_cta - img * p.hw;
+        const int h0 = rem / p.width;
+        const int w0 = rem - h0 * p.width;
+        for (int kb = it.kb0; kb < it.kb1; ++kb) {
+          const int tap = kb / p.kb_per_tap;
+          const int c0 = (kb - tap * p.kb_per_tap) * BK;
+          const int ca = c0 >= p.a_wrap ? c0 - p.a_wrap : c0;
+          const int r = tap / p.ksize;
+          const int s = tap - r * p.ksize;
+          mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x600 | stage);
+          const uint32_t full = bar_full + 8 * stage;
+          mbar_arrive_expect_tx(full, Cfg::kStageBytes);      // the A box always transfers (and zero-fills) all 256 rows
+          const uint32_t dst = smem_a + stage * Cfg::kABytes;
+          if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0 - p.pad, h0 - p.pad, img, static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+          else tma_load_2d(dst, &tmap_a, full, ca, m_cta);
+          tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, full, tap * p.cin + c0, n_tile * kWideBN);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+  // ===================== consumer warpgroups =====================
+  setmaxnreg_inc<232>();
+  const int cw = (threadIdx.x >> 7) - 1;       // consumer 0: tile rows 0..127, consumer 1: rows 128..255
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5;
+  const int lane = t & 31;
+  const bool leader = threadIdx.x == 128;
+  const uint32_t stage_o = smem_o + cw * Cfg::kOutBytes;
+  float acc[2][64];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
+    const int kb_first = it.kb0, kb_last = it.kb1 - 1;
+    int prev = -1;
+    for (int kb = kb_first; kb <= kb_last; ++kb) {
+      mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x700 | stage);
+      const uint64_t bdesc = make_kmajor_desc<Cfg::kSwizzle>(smem_b + stage * Cfg::kBBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint64_t adesc = make_kmajor_desc<Cfg::kSwizzle>(smem_a + stage * Cfg::kABytes + (cw * 128 + h * 64) * Cfg::kSwizzle);
+#pragma unroll
+        for (int k = 0; k < BK / UMMA_K; ++k)
+          wgmma_f16<kWideBN>(acc[h], adesc + 2 * k, bdesc + 2 * k, ((kb - kb_first) | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc[0]);
+    fence_regs(acc[1]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+
+    const int tile = it.tile;
+    const int n0 = (tile % p.n_tiles) * kWideBN;
+    const int m_base = (tile / p.n_tiles) * kWideRows + cw * 128;
+    const bool sk_dump = it.kb1 < p.num_kb;
+    const bool sk_collect = !sk_dump && it.kb0 > 0;
+    // per-thread partial layout: float4 g of thread t of consumer cw at ((cw * 32 + g) * 128 + t) * 4 -- coalesced both ways
+    if (sk_dump) {
+      float4* dst = reinterpret_cast<float4*>(p.ws + static_cast<size_t>(blockIdx.x) * Cfg::kWsFloats) + cw * 32 * 128 + t;
+#pragma unroll
+      for (int g = 0; g < 32; ++g)
+        dst[g * 128] = make_float4(acc[g >> 4][4 * (g & 15)], acc[g >> 4][4 * (g & 15) + 1], acc[g >> 4][4 * (g & 15) + 2], acc[g >> 4][4 * (g & 15) + 3]);
+      __threadfence();
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (leader) st_release_gpu(p.flags + blockIdx.x, 1u);
+      continue;
+    }
+    int sk_lo = 0;
+    if (sk_collect) {
+      const int u = tile * p.num_kb;
+      const int wide = p.sk_rem * (p.sk_base + 1);
+      sk_lo = u < wide ? u / (p.sk_base + 1) : p.sk_rem + (u - wide) / p.sk_base;
+      if (leader) {
+        for (int j = sk_lo; j < static_cast<int>(blockIdx.x); ++j) {
+          uint32_t spins = 0;
+          uint64_t t0 = 0;
+          while (ld_acquire_gpu(p.flags + j) == 0u) {
+            if ((++spins & 0x3FFu) == 0) {
+              const uint64_t now = globaltimer_ns();
+              if (t0 == 0) t0 = now;
+              if (now - t0 > 4000000000ull) {
+                if (p.dbg != nullptr) { p.dbg[0] = 0x0BAD0800; p.dbg[1] = static_cast<int>(blockIdx.x); p.dbg[2] = j; p.dbg[3] = tile; __threadfence_system(); }
+                __trap();
+              }
+            }
+          }
+        }
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      for (int j = sk_lo; j < static_cast<int>(blockIdx.x); ++j) {
+        const float4* src = reinterpret_cast<const float4*>(p.ws + static_cast<size_t>(j) * Cfg::kWsFloats) + cw * 32 * 128 + t;
+#pragma unroll
+        for (int g = 0; g < 32; ++g) {
+          const float4 a = __ldcg(src + g * 128);
+          float* d = &acc[g >> 4][4 * (g & 15)];
+          d[0] += a.x; d[1] += a.y; d[2] += a.z; d[3] += a.w;
+        }
+      }
+    }
+    // fragment of thread t: acc[h][4 j + 2 hh + e] is tile row 64 h + 16 warp + lane / 4 + 8 hh, column 8 j + 2 (lane % 4) + e
+#pragma unroll
+    for (int c2 = 0; c2 < 2; ++c2) {
+      if (n0 + c2 * 64 < p.cout) {                 // uniform over the CTA
+        // the previous bulk store of this consumer has read the staging slice
+        if (t == 0) tma_store_wait_read<0>();
+        asm volatile("bar.sync %0, 128;" :: "r"(2 + cw) : "memory");
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int col = n0 + c2 * 64 + 8 * jj + 2 * (lane & 3);
+          const bool ok = col < p.cout;            // Cout % 8 == 0: both columns of the pair agree
+          const float sc0 = ok ? __ldg(p.scale + col) : 0.f, sc1 = ok ? __ldg(p.scale + col + 1) : 0.f;
+          const float sh0 = ok ? __ldg(p.shift + col) : 0.f, sh1 = ok ? __ldg(p.shift + col + 1) : 0.f;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              const int j = c2 * 8 + jj;
+              float x0 = acc[h][4 * j + 2 * hh] * sc0 + sh0;
+              float x1 = acc[h][4 * j + 2 * hh + 1] * sc1 + sh1;
+              x0 = x0 > 0.f ? x0 : x0 * p.slope;
+              x1 = x1 > 0.f ? x1 : x1 * p.slope;
+              __half2 v = __floats2half2_rn(x0, x1);
+              const int r = h * 64 + warp * 16 + (lane >> 2) + hh * 8;
+              const uint32_t addr = stage_o + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
+              asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(*reinterpret_cast<uint32_t*>(&v)) : "memory");
+            }
+          }
+        }
+        fence_proxy_async_smem();
+        asm volatile("bar.sync %0, 128;" :: "r"(2 + cw) : "memory");
+        if (t == 0) {
+#pragma unroll
+          for (int g = 0; g < 4; ++g)     // rows >= M and channels >= Cout are clipped by the tensor map
+            if (m_base + 32 * g < p.m_total) tma_store_2d(&tmap_y, stage_o + g * 4096, n0 + c2 * 64, m_base + 32 * g);
+          tma_store_commit();
+        }
+      }
+    }
+    if (sk_collect) {
+      // every reader is done with the partials: hand the slots back (the next writer is a later launch)
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      for (int j = sk_lo + t + 128 * cw; j < static_cast<int>(blockIdx.x); j += 256) p.flags[j] = 0u;
+    }
+  }
+  if (t == 0) tma_store_wait<0>();
+}
+
+// ---------------------------------------------------------------------------------------------
 // Halo-tile kernel for 3x3, Cin = 32 (layers1.2).  The im2col formulation above pulls every input pixel through the
 // L2 -> SM path nine times (once per tap): 779 MB for 88 MB of input at batch 32.  Here an output tile is a 16 x 8 pixel
 // rectangle and its 18 x 10 x 32ch input halo is fetched ONCE (11.5 KB instead of 72 KB) as four 8-channel planes
@@ -858,8 +1083,15 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
 // Host side: tensor-map encoding through the driver entry points (no link-time libcuda dependency)
 // ---------------------------------------------------------------------------------------------
 constexpr long long kSkFlagBytes = 4096;          // room for 1024 CTA flags
-constexpr long long kSkSlotBytes = 128 * 128 * 4;  // one CTA's largest partial accumulator (MT*BN = 128 columns x 128 rows x fp32)
+constexpr long long kSkSlotBytes = kWideRows * kWideBN * 4;  // one CTA's largest partial accumulator (the 256 x 128 fp32 tile)
 long long conv_workspace_bytes() { return kSkFlagBytes + kSkSlotBytes * sm_count(); }
+
+constexpr int kKernelIgemm = 0;      // conv_igemm_kernel (one MMA warpgroup, shared-memory accumulator)
+constexpr int kKernelWide = 1;       // conv_wide_kernel (256 x 128, two consumer warpgroups)
+constexpr int kKernelC32 = 2;        // conv_c32_kernel (3x3, Cin = 32 halo tiles)
+struct ConvChoice {
+  int kernel, bk, bn, mt, streamk, grid;
+};
 
 static unsigned long long* g_conv_trace = nullptr;
 void conv_set_trace(void* dev_ptr) { g_conv_trace = static_cast<unsigned long long*>(dev_ptr); }
@@ -924,9 +1156,39 @@ static int launch_conv(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   return check_launch("conv_igemm_kernel");
 }
 
-// CTA tile shapes (BLOCK_N, M-subtiles): the MMA warpgroup keeps MT * BLOCK_N <= 128 accumulators per thread
 template <int BK>
-static int dispatch_conv(int bn, int mt, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, cudaStream_t stream) {
+static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, int grid, cudaStream_t stream) {
+  using Cfg = WideCfg<BK>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    YB_CUDA(cudaFuncSetAttribute(conv_wide_kernel<BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    attr_set = true;
+  }
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cudaLaunchAttribute attr[1];
+  int nattr = 0;
+  static const int use_pdl = getenv("YB_PDL") ? atoi(getenv("YB_PDL")) : 0;     // as launch_conv: A/B runs only
+  if (use_pdl) {
+    attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[nattr].val.programmaticStreamSerializationAllowed = 1;
+    ++nattr;
+  }
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(kWideThreads);
+  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.stream = stream;
+  cfg.attrs = attr; cfg.numAttrs = nattr;
+  YB_CUDA(cudaLaunchKernelEx(&cfg, conv_wide_kernel<BK>, ta, tb, ty, p));
+  return check_launch("conv_wide_kernel");
+}
+
+// CTA tile shapes (BLOCK_N, M-subtiles): the one-warpgroup kernel keeps MT * BLOCK_N <= 128 accumulators per thread; 128 x 2 is
+// the two-consumer kernel
+template <int BK>
+static int dispatch_conv(int bn, int mt, int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p,
+                         cudaStream_t stream) {
+  if (mt == 2 && bn == 128) return launch_wide<BK>(ta, tb, ty, p, grid, stream);
   if (mt == 2) return launch_conv<64, BK, 2>(ta, tb, ty, p, stream);
   if (bn == 64) return launch_conv<64, BK, 1>(ta, tb, ty, p, stream);
   return launch_conv<128, BK, 1>(ta, tb, ty, p, stream);
@@ -998,13 +1260,111 @@ static int conv_c32_forward(const void* x, const void* w, const float* scale, co
   return check_launch("conv_c32_kernel");
 }
 
+// Kernel and tile shape of one conv launch.  flags may force BLOCK_N (bits 8..17) and the number of 128-row M-subtiles
+// (bits 20..21), forbid (bit 3) or force (bit 30) stream-K; otherwise the (BLOCK_N, M-subtiles, stream-K) triple with the lowest
+// modelled time wins.  Model (constants fitted to profiles/conv_layers_h100.json: every shape of the 21 implicit-GEMM launches of
+// C2 timed alone on an H100 SXM at a 700 W power limit): tiles run in ceil(tiles / SMs) rounds; a K-block costs a fixed issue latency (im2col boxes cost
+// more than plain tiled ones) plus its operand bytes at a per-SM L2->SM rate; the one-warpgroup kernel's epilogue overlaps the
+// next main loop (a tile costs the larger of the two), the two-consumer kernel's register epilogue does not (they add).  With
+// these constants the model picks, on each of those 21 launches, a shape within 3 % of the fastest one measured.
+constexpr double kKbNsIm2col = 240.0;     // ns per K-block, 3x3 layers (im2col-mode A box)
+constexpr double kKbNsTiled = 100.0;      // ns per K-block, 1x1 layers (plain 2-D tiled A box)
+constexpr double kFeedBytesPerNs = 130.0; // L2 -> SM operand bytes per ns per SM
+constexpr double kEpiNsPerOut = 0.15;     // one-warpgroup epilogue, ns per output element (overlapped with the main loop)
+constexpr double kWideEpiNsPerOut = 0.08; // two-consumer register epilogue, ns per output element (not overlapped)
+constexpr double kSkNs = 16000.0;         // stream-K partial dump + collect, one-warpgroup kernel
+constexpr double kSkNsWide = 9000.0;      // the same from registers, two-consumer kernel
+int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, int a_channels, int out_mode, int flags, bool workspace_ok,
+                bool stats, bool lo, ConvChoice* out) {
+  ConvChoice c;
+  memset(&c, 0, sizeof(c));
+  const int sms = sm_count();
+  const bool split = a_channels != cin || lo;
+  // 3x3, Cin = 32, Cout <= 64 (layers1.2): halo-tile kernel unless a test asks for one of the im2col kernels
+  if (!split && cin == 32 && ksize == 3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 8) & 0xFFFF) == 0) {
+    const long long tiles = static_cast<long long>(batch) * ((width + C32Cfg::TW - 1) / C32Cfg::TW) * ((height + C32Cfg::TH - 1) / C32Cfg::TH);
+    c.kernel = kKernelC32; c.bk = 32; c.bn = C32Cfg::BN; c.mt = 1;
+    c.grid = static_cast<int>(tiles < sms ? tiles : sms);
+    *out = c;
+    return 0;
+  }
+  if ((flags >> 4) & 1) return fail(YB_ERR_UNSUPPORTED, "conv: YB_CONV_POOL2X2 is only implemented for the Cin = 32 3x3 layer");
+  const int bk = (cin % 64 == 0 && a_channels % 64 == 0) ? 64 : 32;     // K-blocks never straddle the wrap point
+  const bool sk_possible = !stats && workspace_ok && (flags & 8) == 0;
+  const bool sk_force = sk_possible && ((flags >> 30) & 1);
+  // the two-consumer kernel: fp16 NHWC through the TMA store, no residual output, statistics or profiling ablation
+  const bool wide_ok = out_mode == 0 && !lo && !stats && ((flags >> 24) & 0xF) == 0 && ((flags >> 29) & 1) == 0;
+  const int force_bn = (flags >> 8) & 0x3FF;
+  const int force_mt = (flags >> 20) & 0x3;
+  const int force_pair = (flags >> 22) & 0x3;      // 0 = auto, 1 = single-CTA tiles (the only form), 2 = CTA pair (not on sm_90)
+  YB_REQUIRE(force_pair != 2, "conv: CTA-pair tiles need two-CTA tensor-core instructions, which sm_90 does not have");
+  YB_REQUIRE(!force_bn || ((force_bn == 64 || force_bn == 128) && (force_mt != 2 || force_bn == 64 || wide_ok)),
+             "conv: BLOCK_N=%d x %d M-subtiles is not a tile shape of this launch (64 x 1, 128 x 1, 64 x 2; 128 x 2 for fp16 NHWC "
+             "outputs without residual or statistics)", force_bn, force_mt ? force_mt : 1);
+  const long long m_total = static_cast<long long>(batch) * height * width;
+  const int num_kb = ksize * ksize * (cin / bk);
+  double best = 1e300;
+  for (int cbn = 64; cbn <= 128; cbn *= 2) {
+    if (force_bn && cbn != force_bn) continue;
+    if (!force_bn && cbn > 64 && cbn / 2 >= cout) continue;       // do not pad Cout by more than 2x
+    for (int cmt = 1; cmt <= 2; ++cmt) {
+      if (force_mt && cmt != force_mt) continue;
+      const bool cwide = cmt * cbn > 128;
+      if (cwide && !wide_ok) continue;
+      const int rows_tile = BM * cmt;
+      const double tiles = static_cast<double>((m_total + rows_tile - 1) / rows_tile) * ((cout + cbn - 1) / cbn);
+      const double rounds = static_cast<double>((static_cast<long long>(tiles) + sms - 1) / sms);
+      const double kb_ns = (ksize == 3 ? kKbNsIm2col : kKbNsTiled) + (cmt * BM + cbn) * bk * 2.0 / kFeedBytesPerNs;
+      const double main_ns = num_kb * kb_ns;
+      const double outs = static_cast<double>(rows_tile) * cbn;
+      const double tile_ns = cwide ? main_ns + outs * kWideEpiNsPerOut : (main_ns > outs * kEpiNsPerOut ? main_ns : outs * kEpiNsPerOut);
+      double t = rounds * tile_ns;
+      int csk = 0;
+      if (sk_possible) {
+        // stream-K: every SM gets units/SMs K-blocks, plus one partial dump / collect
+        const double units = tiles * num_kb;
+        const double per_cta = static_cast<double>((static_cast<long long>(units) + sms - 1) / sms);
+        const double tsk = per_cta * kb_ns + (cwide ? kSkNsWide : kSkNs);
+        // stream-K only spreads layers that leave most of the GPU idle (single images, small batches).  On layers that fill
+        // the chip it changes the fp32 summation order of most outputs, which the fp16 activations of the next layers turn
+        // into a head-feature difference of ~1.2e-3 (max|d| / max|y|) at C2.
+        const bool ok = per_cta >= 4.0 && num_kb >= 2;
+        const bool idle = tiles <= sms / 2;
+        if (ok && (sk_force || (idle && tsk < 0.93 * t))) { t = tsk; csk = 1; }
+      }
+      if (sk_force && !csk) continue;
+      // ties go to the wider-N shape (more reuse of each A tile)
+      if (t < best * 0.9999 || (t <= best * 1.0001 && cbn > c.bn)) { best = t; c.bn = cbn; c.mt = cmt; c.streamk = csk; }
+    }
+  }
+  if (c.bn == 0) { c.bn = force_bn ? force_bn : 128; c.mt = force_mt ? force_mt : 1; c.streamk = 0; }
+  YB_REQUIRE((c.bn == 64 || c.bn == 128) && (c.mt == 1 || c.mt == 2) && (c.mt * c.bn <= 128 || wide_ok), "conv: tile %d x %d", c.bn, c.mt);
+  c.kernel = c.mt * c.bn > 128 ? kKernelWide : kKernelIgemm;
+  c.bk = bk;
+  const long long tiles = ((m_total + BM * c.mt - 1) / (BM * c.mt)) * ((cout + c.bn - 1) / c.bn);
+  c.grid = c.streamk ? sms : static_cast<int>(tiles < sms ? tiles : sms);      // sk_base / sk_rem are computed for exactly sms CTAs
+  *out = c;
+  return 0;
+}
+
+// out = {kernel (kKernel*), BK, BLOCK_N, rows per CTA tile, stream-K, grid} of a yb_conv_bn_act_fwd(_ws) launch
+int conv_choice(int batch, int height, int width, int cin, int cout, int ksize, int out_mode, int flags, int with_workspace, int* out) {
+  YB_REQUIRE(out != nullptr && batch > 0 && height > 0 && width > 0 && cin % 32 == 0 && cout > 0 && (ksize == 1 || ksize == 3),
+             "conv_choice: bad shape");
+  ConvChoice c;
+  const int rc = conv_choose(batch, height, width, cin, cout, ksize, cin, out_mode, flags, with_workspace != 0, false, false, &c);
+  if (rc) return rc;
+  out[0] = c.kernel; out[1] = c.bk; out[2] = c.bn; out[3] = c.kernel == kKernelC32 ? C32Cfg::TH * C32Cfg::TW : BM * c.mt;
+  out[4] = c.streamk; out[5] = c.grid;
+  return 0;
+}
+
 int conv_igemm_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                        int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                        int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off, cudaStream_t stream) {
   YB_REQUIRE(x && w && scale && shift && y, "conv: null pointer");
   // split-precision operands (see ConvParams::a_wrap): cin is the concatenated reduction width, a_channels what x really holds
   if (a_channels <= 0) a_channels = cin;
-  const bool split = a_channels != cin || lo_ch_off >= 0;
   YB_REQUIRE(a_channels <= cin && a_channels % 32 == 0 && cin - a_channels <= a_channels, "conv: a_channels=%d does not fit cin=%d", a_channels, cin);
   YB_REQUIRE(lo_ch_off < 0 || (out_mode == 0 && stats == nullptr && lo_ch_off % 8 == 0 && lo_ch_off >= y_ch_off + cout && lo_ch_off + cout <= y_ld),
              "conv: lo_ch_off=%d (needs fp16 NHWC output with room for a second Cout-wide slice)", lo_ch_off);
@@ -1020,70 +1380,15 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
                "conv: fp16 NHWC output needs Cout, y_ld, y_ch_off multiples of 8 and a 16B aligned pointer");
   }
   const long long m_total_ll = static_cast<long long>(batch) * height * width;
-  YB_REQUIRE(m_total_ll < (1ll << 31) - BM, "conv: too many pixels");
-  const int pool = (flags >> 4) & 1;        // YB_CONV_POOL2X2
-  // 3x3, Cin = 32, Cout <= 64 (layers1.2): halo-tile kernel unless a test asks for one of the im2col kernels
-  if (!split && cin == 32 && ksize == 3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 8) & 0xFFFF) == 0)
-    return conv_c32_forward(x, w, scale, shift, slope, y, batch, height, width, cout, x_ld, y_ld, y_ch_off, pool, flags, stats, stream);
-  if (pool) return fail(YB_ERR_UNSUPPORTED, "conv: YB_CONV_POOL2X2 is only implemented for the Cin = 32 3x3 layer");
-  const int bk = (cin % 64 == 0 && a_channels % 64 == 0) ? 64 : 32;     // K-blocks never straddle the wrap point
-  // tile shape: flags may force BLOCK_N (bits 8..17) and the number of M-subtiles (bits 20..21); otherwise pick the
-  // (BLOCK_N, M-subtiles) pair with the lowest modelled time.  The model treats the kernel as bound by the L2->SM operand
-  // feed (a tile costs its operand bytes at a per-SM rate, or its MMA time if larger, and tiles run in ceil(tiles/SMs)
-  // rounds, capped by a chip-wide L2 rate); its rates are estimates for H100, not fitted measurements.
-  int bn = 0, mt = 0, streamk = 0;
-  // stream-K needs the caller's workspace (one per stream: partial sums + flags); flags bit 3 forbids, bit 30 forces it
-  const bool sk_possible = stats == nullptr && workspace != nullptr && workspace_bytes >= conv_workspace_bytes() && (flags & 8) == 0 &&
-                           (reinterpret_cast<uintptr_t>(workspace) & 255) == 0;
-  const bool sk_force = sk_possible && ((flags >> 30) & 1);
-  const int force_bn = (flags >> 8) & 0x3FF;
-  const int force_mt = (flags >> 20) & 0x3;
-  const int force_pair = (flags >> 22) & 0x3;      // 0 = auto, 1 = single-CTA tiles (the only form), 2 = CTA pair (not on sm_90)
-  YB_REQUIRE(force_pair != 2, "conv: CTA-pair tiles need two-CTA tensor-core instructions, which sm_90 does not have");
-  YB_REQUIRE(!force_bn || ((force_bn == 64 || force_bn == 128) && (force_mt != 2 || force_bn == 64)),
-             "conv: BLOCK_N=%d x %d M-subtiles is not a tile shape of this kernel (64 x 1, 128 x 1, 64 x 2)", force_bn, force_mt ? force_mt : 1);
-  {
-    double best = 1e300;
-    const int sms = sm_count();
-    const int num_kb = ksize * ksize * (cin / bk);
-    for (int cbn = 64; cbn <= 128; cbn *= 2) {
-      if (force_bn && cbn != force_bn) continue;
-      if (!force_bn && cbn > 64 && cbn / 2 >= cout) continue;       // do not pad Cout by more than 2x
-      for (int cmt = 1; cmt <= 2; ++cmt) {
-        if (force_mt && cmt != force_mt) continue;
-        if (cmt * cbn > 128) continue;
-        const int rows_tile = BM * cmt;
-        const double tiles = static_cast<double>((m_total_ll + rows_tile - 1) / rows_tile) * ((cout + cbn - 1) / cbn);
-        const double rounds = static_cast<double>((static_cast<long long>(tiles) + sms - 1) / sms);
-        const double bytes_kb = (cmt * BM + cbn) * bk * 2.0;        // per CTA
-        const double mma_ns_kb = cmt * BM * cbn * bk * 2.0 / 7000.0;  // ~7 TFLOP/s per SM of dense fp16
-        const double kb_ns = bytes_kb / 60.0 > mma_ns_kb ? bytes_kb / 60.0 : mma_ns_kb;
-        const double tile_ns = num_kb * kb_ns + 500.0;
-        const double agg_ns = tiles * num_kb * bytes_kb / 7000.0;
-        double t = rounds * tile_ns;
-        if (agg_ns > t) t = agg_ns;
-        int csk = 0;
-        if (sk_possible) {
-          // stream-K: every SM gets units/SMs K-blocks; on top, roughly one partial dump + one collecting epilogue per CTA
-          const double units = tiles * num_kb;
-          const double per_cta = static_cast<double>((static_cast<long long>(units) + sms - 1) / sms);
-          const double epi_ns = 8000.0 * (cmt * cbn / 512.0);
-          double tsk = per_cta * kb_ns + epi_ns + 1500.0;
-          if (agg_ns > tsk) tsk = agg_ns;
-          // stream-K pays when the layer leaves most of the GPU idle (single images, small batches); layers that already fill
-          // the chip gain nothing from the spread
-          const bool ok = per_cta >= 4.0 && num_kb >= 2;
-          const bool idle = tiles <= sms / 2;
-          if (ok && (sk_force || (idle && tsk < 0.93 * t))) { t = tsk; csk = 1; }
-        }
-        if (sk_force && !csk) continue;
-        // ties go to the wider-N shape (more reuse of each A tile)
-        if (t < best * 0.9999 || (t <= best * 1.0001 && cbn > bn)) { best = t; bn = cbn; mt = cmt; streamk = csk; }
-      }
-    }
-    if (bn == 0) { bn = force_bn ? force_bn : 128; mt = force_mt ? force_mt : 1; streamk = 0; }
-  }
-  YB_REQUIRE((bn == 64 || bn == 128) && (mt == 1 || mt == 2) && mt * bn <= 128, "conv: tile %d x %d", bn, mt);
+  YB_REQUIRE(m_total_ll < (1ll << 31) - kWideRows, "conv: too many pixels");
+  // stream-K needs the caller's workspace (one per stream: partial sums + flags)
+  const bool ws_ok = workspace != nullptr && workspace_bytes >= conv_workspace_bytes() && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0;
+  ConvChoice ch;
+  int rc = conv_choose(batch, height, width, cin, cout, ksize, a_channels, out_mode, flags, ws_ok, stats != nullptr, lo_ch_off >= 0, &ch);
+  if (rc) return rc;
+  if (ch.kernel == kKernelC32)
+    return conv_c32_forward(x, w, scale, shift, slope, y, batch, height, width, cout, x_ld, y_ld, y_ch_off, (flags >> 4) & 1, flags, stats, stream);
+  const int bk = ch.bk, bn = ch.bn, mt = ch.mt, streamk = ch.streamk;
   // 1x1 layers read A as a plain [pixels, Cin] matrix (2-D tiled TMA: cheaper per instruction than im2col mode);
   // YB_CONV_1X1_IM2COL=1 switches back for A/B runs
   static const int k1x1_im2col = getenv("YB_CONV_1X1_IM2COL") ? atoi(getenv("YB_CONV_1X1_IM2COL")) : 0;
@@ -1091,7 +1396,7 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
 
   EncodeTiledFn enc_tiled;
   EncodeIm2colFn enc_im2col;
-  int rc = get_encoders(&enc_tiled, &enc_im2col);
+  rc = get_encoders(&enc_tiled, &enc_im2col);
   if (rc) return rc;
 
   ConvParams p;
@@ -1180,8 +1485,8 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
   }
-  if (bk == 64) return dispatch_conv<64>(bn, mt, ta, tb, ty, p, stream);
-  return dispatch_conv<32>(bn, mt, ta, tb, ty, p, stream);
+  if (bk == 64) return dispatch_conv<64>(bn, mt, ch.grid, ta, tb, ty, p, stream);
+  return dispatch_conv<32>(bn, mt, ch.grid, ta, tb, ty, p, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

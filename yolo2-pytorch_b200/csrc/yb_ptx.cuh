@@ -135,6 +135,13 @@ __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// Per-warpgroup register budget (executed by all 128 threads of a warpgroup): a producer warpgroup hands registers back so
+// the MMA warpgroups can hold larger accumulator tiles than the block-wide launch bound allows.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(N)); }
+
 
 // ---------------------------------------------------------------------------------------------
 // wgmma: one warpgroup (4 consecutive warps, the first one a multiple of 4) issues D(64 x N, fp32 registers) (+)= A * B
