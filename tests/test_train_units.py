@@ -1,0 +1,666 @@
+"""Train-mode parity of the ResNet and MobileNet trainers one unit at a time, against an fp64 restatement fed its own activations and gradients.
+
+End to end, train-mode BatchNorm amplifies every fp16 rounding through the chain (see test_resnet_train.py and the MobileNet step test), so
+those checks can only bound gradient cosines.  Here the chain is removed: an fp64 "teacher" runs one train-mode step of the restatement with
+autograd and records, for every conv + BatchNorm unit, the input the GPU unit reads and the loss gradient at its output.  Each unit of the
+trainer (`ResNetTrainer._unit_forward / _res_unit_backward / _stem_* / _head_backward / _join_*`, `MobileNetTrainer._first_* / _dw_* /
+_pw_forward / _unit_backward / _head_backward`) is then run on exactly those operands, stored the way the GPU path stores them (fp16
+activations, fp16 gradients times `grad_scale`), and compared with an fp64 recomputation of that single unit from the same operands.  The
+bounds are per unit, near the fp16 rounding level, and every failure names the unit and the quantity.
+
+CPU: the teacher's records chain into the float32 restatement's feature and parameter gradients (which the executed-reference tests pin).
+GPU: every unit of resnet18, resnet50 and MobileNet at 8 x 160^2, resnet50 and MobileNet at 2 x 416^2 (the 13^2 head grid and every
+2048-channel BatchNorm of resnet50); eval() after 15 SGD steps block by block on the eval oracle's own inputs; resnet50's eval path at 416^2.
+"""
+import configparser
+import json
+import os
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+import resnet_train_oracle as RT
+from oracle import yolo2_oracle as O
+
+DEV = 'cuda'
+SCALE = 16384.0          # the trainers' static loss scale (DarknetTrainer.grad_scale)
+EPS = 1e-5
+FP16_MAX = 65504.0
+
+
+def rel_err(got, ref):
+    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
+    return ((got - ref).abs().max() / ref.abs().max().clamp_min(1e-30)).item()
+
+
+def rel_l2(got, ref):
+    got, ref = got.detach().double().cpu(), ref.detach().double().cpu()
+    return ((got - ref).norm() / ref.norm().clamp_min(1e-30)).item()
+
+
+def record(name, value):
+    """Measured per-unit figures of this run -> $YB_PARITY_OUT/parity_train_units.json when that directory is given."""
+    out = os.environ.get('YB_PARITY_OUT')
+    if not out:
+        return
+    os.makedirs(out, exist_ok=True)
+    path = os.path.join(out, 'parity_train_units.json')
+    data = json.load(open(path)) if os.path.exists(path) else {}
+    data[name] = value
+    with open(path, 'w') as f:
+        json.dump(data, f, indent=1, sort_keys=True)
+
+
+def make_config():
+    config = configparser.ConfigParser()
+    config.read_dict({'batch_norm': {'enable': '1'}, 'model': {'threshold': '0.6', 'pretrained': '0'},
+                      'detect': {'threshold': '0.3', 'threshold_cls': '0.005', 'fix': '1', 'overlap': '0.45'},
+                      'hparam': {k: str(v) for k, v in O.HPARAM_DEFAULT.items()}, 'train': {'cross_entropy': '1'}})
+    return config
+
+
+def make_resnet(name, sd):
+    import model
+    import model.resnet
+    net = getattr(model.resnet, name)(model.ConfigChannels(make_config()), O.anchors_yolo_voc(), 20)
+    res = net.load_state_dict(sd, strict=False)
+    assert not res.unexpected_keys and all(k.endswith('num_batches_tracked') for k in res.missing_keys), res
+    return net
+
+
+def make_mobilenet(sd):
+    import model
+    import model.mobilenet
+    net = model.mobilenet.MobileNet(model.ConfigChannels(make_config()), O.anchors_yolo_voc(), 20)
+    net.load_state_dict(sd, strict=False)
+    return net
+
+
+# ------------------------------------------------------------------------------------------------
+# fp64 teacher: one train-mode step of the restatement with autograd, every unit's operands recorded
+# ------------------------------------------------------------------------------------------------
+class Teacher(object):
+    """units[key] = dict(src, z, mean, var, count, out, stride, k, relu, conv, bn) in execution order; `src` is the tensor the unit's conv
+    reads (a 1x1 stride-2 downsample: the subsampled block input), `inp` what the trainer's unit method is handed.  After backward()
+    `.grad` of src / out / the joins' tensors hold the loss gradients."""
+
+    def __init__(self):
+        self.units, self.joins = {}, {}
+        self.sd, self.feature, self.losses = None, None, None
+
+    def unit(self, key, inp, conv, bn, stride, k, relu, sub=False, groups=1):
+        src = (inp[:, :, ::2, ::2] if sub else inp).clone()
+        if src.requires_grad:             # not the image
+            src.retain_grad()
+        w = self.sd[conv]
+        z = F.conv2d(src, w, None, 1 if sub else stride, (k - 1) // 2, groups=groups)
+        y = F.batch_norm(z, None, None, self.sd[bn + '.weight'], self.sd[bn + '.bias'], True, 0.0, EPS)
+        out = F.relu(y) if relu else y
+        out.retain_grad()
+        self.units[key] = dict(inp=inp, src=src, z=z, mean=z.mean(dim=(0, 2, 3)), var=z.var(dim=(0, 2, 3), unbiased=False),
+                               count=z.numel() // z.shape[1], out=out, stride=1 if sub else stride, k=k, relu=relu, conv=conv, bn=bn,
+                               groups=groups, sub=sub)
+        return out
+
+    def finish(self, feature, data):
+        feature.retain_grad()
+        anchors = O.anchors_yolo_voc()
+        fc = feature.cpu()                  # the region loss runs on the CPU; autograd carries its gradient back to the backbone's device
+        pred = O.decode(fc, anchors)
+        pred['feature'] = fc
+        self.losses, _ = O.loss(anchors, data, pred, 0.6)
+        O.loss_total(self.losses).backward()
+        self.feature = feature
+        return self
+
+
+def _leaf_sd(sd0, dtype, device):
+    return {k: (v.to(device, dtype).requires_grad_(True) if v.is_floating_point() and 'running' not in k else v.to(device))
+            for k, v in sd0.items()}
+
+
+def resnet_teacher(sd0, x, data, name, dtype=torch.float64, device='cpu'):
+    """The arithmetic of RT.resnet_train_forward with every unit, join, the stem and the head recorded."""
+    t = Teacher()
+    t.sd = _leaf_sd(sd0, dtype, device)
+    x = x.to(device, dtype)
+    stem = t.unit('conv1', x, 'conv1.weight', 'bn1', 2, 7, True)
+    pool = F.max_pool2d(stem, 3, 2, 1)
+    pool.retain_grad()
+    t.stem = dict(x=x, out=stem, pool=pool)
+    cur = pool
+    for blk in O.resnet_blocks(name):
+        p, s = blk['prefix'], blk['stride']
+        xm = cur.clone()
+        xm.retain_grad()
+        names = [('conv1', 3, s, True), ('conv2', 3, 1, False)] if blk['kind'] == 'basic' else \
+            [('conv1', 1, 1, True), ('conv2', 3, s, True), ('conv3', 1, 1, False)]
+        out, keys = xm, []
+        for i, (cname, k, st, relu) in enumerate(names):
+            key = '%s.%s' % (p, cname)
+            out = t.unit(key, out, key + '.weight', '%s.bn%s' % (p, cname[-1]), st, k, relu)
+            keys.append(key)
+        if blk['downsample']:
+            res = t.unit(p + '.downsample', cur, p + '.downsample.0.weight', p + '.downsample.1', s, 1, False, sub=s == 2)
+            skip = t.units[p + '.downsample']['src']
+        else:
+            res = cur.clone()
+            res.retain_grad()
+            skip = res
+        pre = out + res
+        pre.retain_grad()
+        new = F.relu(pre)
+        new.retain_grad()
+        t.joins[p] = dict(xin=cur, xm=xm, skip=skip, main=out, res=res, pre=pre, out=new, stride=s if blk['downsample'] else 1,
+                          units=keys, ds=p + '.downsample' if blk['downsample'] else None)
+        cur = new
+    cur.retain_grad()
+    t.head = dict(a=cur, w='conv.weight', b='conv.bias')
+    return t.finish(F.conv2d(cur, t.sd['conv.weight'], t.sd['conv.bias']), data)
+
+
+def mobilenet_teacher(sd0, x, data, dtype=torch.float64, device='cpu'):
+    """The arithmetic of O.mobilenet_forward(train=True) with the first conv, every depthwise and pointwise unit and the head recorded."""
+    t = Teacher()
+    t.sd = _leaf_sd(sd0, dtype, device)
+    x = x.to(device, dtype)
+    cur = t.unit('layers.0', x, 'layers.0.conv.weight', 'layers.0.bn', 2, 3, True)
+    for i, (_, stride) in enumerate(O.MOBILENET_UNITS, 1):
+        cur = t.unit('layers.%d.dw' % i, cur, 'layers.%d.dw.conv.weight' % i, 'layers.%d.dw.bn' % i, stride, 3, True, groups=cur.shape[1])
+        cur = t.unit('layers.%d.pw' % i, cur, 'layers.%d.pw.conv.weight' % i, 'layers.%d.pw.bn' % i, 1, 1, True)
+    t.head = dict(a=cur, w='layers.14.weight', b='layers.14.bias')
+    return t.finish(F.conv2d(cur, t.sd['layers.14.weight'], t.sd['layers.14.bias']), data)
+
+
+def unit_ref(src, w, gamma, beta, stride, k, relu, gout, groups=1, round_z=False, mask=None):
+    """One conv + train-mode BatchNorm (+ ReLU) unit in fp64 from the given operands, and its backward from `gout`.  round_z passes z through
+    fp16 rounding (straight-through in backward), as the GPU stores it; `mask` (the GPU's own activation > 0) makes the ReLU take the GPU's
+    decisions, so an element within rounding of 0 does not move its whole gradient between the two sides."""
+    src, w, gamma, beta = (t.detach().double().clone().requires_grad_(True) for t in (src, w, gamma, beta))
+    z = F.conv2d(src, w, None, stride, (k - 1) // 2, groups=groups)
+    if round_z:
+        z = z + (z.detach().half().double() - z.detach())
+    y = F.batch_norm(z, None, None, gamma, beta, True, 0.0, EPS)
+    out = (y * mask if mask is not None else F.relu(y)) if relu else y
+    out.backward(gout.double())
+    return dict(z=z.detach(), mean=z.detach().mean(dim=(0, 2, 3)), var=z.detach().var(dim=(0, 2, 3), unbiased=False),
+                count=z.numel() // z.shape[1], out=out.detach(), dx=src.grad, dw=w.grad, dgamma=gamma.grad, dbeta=beta.grad)
+
+
+CPU_CASES = {'resnet18': (4, 128, 40, 41), 'resnet50': (2, 64, 42, 43), 'mobilenet': (2, 96, 44, 45)}
+# fp64 vs fp32 parameter gradients (worst rel L2): resnet18 5.9e-6, MobileNet 9.2e-5; resnet50 at 2 x 64^2 measures 3.0e-2, because its
+# last stages see 32 and 8 values per channel, and train-mode BatchNorm on so few values amplifies even fp32 rounding
+GRAD_FP32 = {'resnet18': 1e-4, 'resnet50': 6e-2, 'mobilenet': 1e-3}
+
+
+def _case_inputs(b, size, seed_x, seed_t, slots=6):
+    s = size // 32
+    x = O.synth_images(b, size, size, seed=seed_x)
+    tgt = O.synth_targets(b, size, size, slots=slots, seed=seed_t)
+    return x, tgt, O.norm_data(tgt, size, size, s, s)
+
+
+@pytest.mark.parametrize('net', ['resnet18', 'resnet50', 'mobilenet'])
+def test_teacher_records_chain_to_the_fp32_restatement(net):
+    """The fp64 teacher is what every GPU unit is judged against, so it must be the restatement: its feature, loss terms and every parameter
+    gradient agree with the float32 restatement (pinned to the executed reference by test_resnet_train_oracle_matches_executed_reference and
+    test_mobilenet_oracle_matches_reference) to fp32 rounding; every unit recomputed alone by `unit_ref` from its recorded input and output
+    gradient reproduces its recorded z, statistics, output and the parameter and input gradients; and the records chain (each unit's input
+    is its producer's output, each join's gradients add up to the block input's)."""
+    b, size, seed_x, seed_t = CPU_CASES[net]
+    x, _, data = _case_inputs(b, size, seed_x, seed_t)
+    if net == 'mobilenet':
+        sd0 = O.make_mobilenet_state_dict(0)
+        t = mobilenet_teacher(sd0, x, data)
+        sd = {k: (v.clone().requires_grad_(True) if v.is_floating_point() and 'running' not in k else v.clone()) for k, v in sd0.items()}
+        f32 = O.mobilenet_forward(sd, x, train=True)
+    else:
+        sd0 = O.make_resnet_state_dict(net, 0)
+        t = resnet_teacher(sd0, x, data, net)
+        sd = {k: (v.clone().requires_grad_(True) if v.is_floating_point() and 'running' not in k else v.clone()) for k, v in sd0.items()}
+        f32 = RT.resnet_train_forward(sd, x, net)
+    pred = O.decode(f32, O.anchors_yolo_voc())
+    pred['feature'] = f32
+    l32, _ = O.loss(O.anchors_yolo_voc(), data, pred, 0.6)
+    O.loss_total(l32).backward()
+    # fp64 against fp32: the only difference is fp32 rounding, amplified through the train-mode BatchNorm chain (resnet50's 53 layers
+    # take the feature to 1.4e-4)
+    assert rel_err(t.feature, f32) <= 1e-3, ('feature', rel_err(t.feature, f32))
+    for k, v in t.losses.items():
+        assert abs(v.item() - l32[k].item()) <= 1e-4 * abs(l32[k].item()) + 1e-9, ('loss', k)
+    params = [k for k, v in sd.items() if v.requires_grad]
+    worst = max((rel_l2(t.sd[k].grad, sd[k].grad), k) for k in params)
+    print('%s: fp64 teacher vs fp32 restatement: feature %.2e, worst gradient rel L2 %.2e (%s)' % (net, rel_err(t.feature, f32), *worst))
+    assert worst[0] <= GRAD_FP32[net], worst
+    # each unit alone, from its own records
+    owned = set()
+    for key, u in t.units.items():
+        r = unit_ref(u['src'], t.sd[u['conv']], t.sd[u['bn'] + '.weight'], t.sd[u['bn'] + '.bias'], u['stride'], u['k'], u['relu'],
+                     u['out'].grad, groups=u['groups'])
+        assert rel_err(r['out'], u['out']) <= 1e-10 and rel_err(r['z'], u['z']) <= 1e-10, key
+        assert rel_err(r['mean'], u['mean']) <= 1e-8 and rel_err(r['var'], u['var']) <= 1e-10 and r['count'] == u['count'], key
+        assert u['src'].grad is None or rel_err(r['dx'], u['src'].grad) <= 1e-9, ('dx', key)
+        for name, got in ((u['conv'], r['dw']), (u['bn'] + '.weight', r['dgamma']), (u['bn'] + '.bias', r['dbeta'])):
+            assert rel_err(got, t.sd[name].grad) <= 1e-9, (name, key)
+            owned.add(name)
+    head = t.head
+    hr_w, hr_b, hr_a = (v.detach().clone().requires_grad_(True) for v in (t.sd[head['w']], t.sd[head['b']], head['a']))
+    F.conv2d(hr_a, hr_w, hr_b).backward(t.feature.grad)
+    assert rel_err(hr_w.grad, t.sd[head['w']].grad) <= 1e-9 and rel_err(hr_b.grad, t.sd[head['b']].grad) <= 1e-9
+    assert rel_err(hr_a.grad, head['a'].grad) <= 1e-9
+    owned |= {head['w'], head['b']}
+    assert owned == set(params), sorted(set(params) ^ owned)
+    # chaining
+    keys = list(t.units)
+    if net == 'mobilenet':
+        for prev, key in zip(keys, keys[1:]):
+            assert t.units[key]['inp'] is t.units[prev]['out'], key
+        return
+    st = t.stem
+    xs = st['out'].detach().clone().requires_grad_(True)
+    F.max_pool2d(xs, 3, 2, 1).backward(st['pool'].grad)
+    assert rel_err(xs.grad, st['out'].grad) <= 1e-12, 'stem max-pool backward'
+    for p, j in t.joins.items():
+        up = torch.zeros_like(j['xin'])
+        if j['stride'] == 2:
+            up[:, :, ::2, ::2] = j['skip'].grad
+        else:
+            up = j['skip'].grad
+        gin = j['xm'].grad + up
+        assert torch.equal(j['pre'].grad, j['main'].grad) and torch.equal(j['pre'].grad, j['res'].grad), p
+        assert rel_err(j['xin'].grad, gin) <= 1e-12, ('join', p)
+        assert rel_err(torch.where(j['out'] > 0, j['out'].grad, torch.zeros(())), j['pre'].grad) <= 1e-12, ('join relu', p)
+        assert t.units[j['units'][0]]['inp'] is j['xm']
+
+
+# ------------------------------------------------------------------------------------------------
+# GPU: teacher-forced units
+# ------------------------------------------------------------------------------------------------
+# about 2x the worst unit measured on an H100 (DESIGN.md section 2), never above the fp16-level ceilings of the Darknet per-unit test;
+# join_* compares a join's exact output with the fp64 teacher, where a block input within fp16 rounding of 0 flips the ReLU mask
+TOL = dict(z=2e-3, act=3e-3, mean=1e-4, var=3e-4, running=2e-3, dgamma=3e-3, dbeta=5e-3, dbias=1e-6, dw_l2=1.5e-3, dw_max=3e-3, dx_l2=1e-3,
+           dx_max=2e-3, pool=3e-3, pool_dx_l2=1e-3, pool_dx_max=1e-3, join_l2=1e-3, join_max=5e-2)
+
+
+def nhwc16(t):
+    return t.detach().permute(0, 2, 3, 1).contiguous().to(DEV).half()
+
+
+def nchw(t):
+    return t.detach().permute(0, 3, 1, 2).double().cpu()
+
+
+class Figures(object):
+    """Per-unit figures and the worst of each quantity; `check` asserts with the unit and the quantity named."""
+
+    def __init__(self, tag):
+        self.tag, self.units, self.worst = tag, {}, {}
+
+    def add(self, unit, **fig):
+        self.units.setdefault(unit, {}).update(fig)
+        for q, v in fig.items():
+            if v > self.worst.get(q, (0.0, None))[0]:
+                self.worst[q] = (v, unit)
+
+    def check(self):
+        record(self.tag, dict(units=self.units, worst=self.worst))
+        bad = ['%s %s = %.3e > %.1e' % (u, q, v, TOL[q]) for u, fig in self.units.items() for q, v in fig.items() if q in TOL and v > TOL[q]]
+        assert not bad, '%s: %s' % (self.tag, '; '.join(bad[:12]))
+
+
+def _bn_figures(fig, unit, s, ref, bn, rm0, rv0, a, a_ref):
+    """z, batch statistics, running statistics after the step and the activation of one unit against its fp64 recomputation."""
+    mean, invstd = s.mean.double().cpu(), s.invstd.double().cpu()
+    n = ref['count']
+    mom = bn.momentum
+    rm_ref = (1 - mom) * rm0.double() + mom * ref['mean']
+    rv_ref = (1 - mom) * rv0.double() + mom * ref['var'] * n / (n - 1)
+    fig.add(unit, z=rel_err(nchw(s.z), ref['z']),
+            mean=((mean - ref['mean']).abs().max() / ref['var'].sqrt().max()).item(),
+            var=rel_err(1.0 / invstd ** 2 - EPS, ref['var']),
+            running=max(((bn.running_mean.double().cpu() - rm_ref).abs() / rm_ref.abs().clamp_min(1e-3)).max().item(),
+                        ((bn.running_var.double().cpu() - rv_ref).abs() / rv_ref.abs()).max().item()),
+            act=rel_err(nchw(a), a_ref))
+
+
+def _grad_figures(fig, unit, arena, names, ref, dx=None, dx_ref=None):
+    wname, gname, bname = names
+    f = dict(dw_l2=rel_l2(arena.views[wname], ref['dw']), dw_max=rel_err(arena.views[wname], ref['dw']))
+    if gname is not None:
+        f.update(dgamma=rel_err(arena.views[gname], ref['dgamma']), dbeta=rel_err(arena.views[bname], ref['dbeta']))
+    if dx is not None:
+        f.update(dx_l2=rel_l2(nchw(dx) / SCALE, dx_ref), dx_max=rel_err(nchw(dx) / SCALE, dx_ref))
+    fig.add(unit, **f)
+
+
+def _snap(bn):
+    return bn.running_mean.detach().double().cpu().clone(), bn.running_var.detach().double().cpu().clone()
+
+
+def _gout16(t):
+    """A loss gradient as the GPU path carries it: times the loss scale, in fp16; and the fp64 value of exactly that operand."""
+    g16 = nhwc16(t * SCALE)
+    return g16, nchw(g16) / SCALE
+
+
+def _head_check(fig, tr, t, a16, w16_ref, hh, ww):
+    """Head: bias gradient, weight gradient from the 128-wide padded dz, data gradient through the padded dgrad pack."""
+    head = t.head
+    df = t.feature.grad.float().cpu()
+    grads = {}
+    gh = tr._head_backward(a16, hh, ww, df.to(DEV), grads)
+    dz = (df * SCALE).half().double() / SCALE          # yb_head_grad_prepare rounds the scaled gradient to fp16
+    a = nchw(a16).requires_grad_(True)
+    wr = w16_ref.clone().requires_grad_(True)
+    br = t.sd[head['b']].detach().double().cpu().requires_grad_(True)
+    F.conv2d(a, wr, br).backward(dz)
+    bref = df.double().sum(dim=(0, 2, 3))
+    fig.add('head', dbias=rel_err(tr.arena.views[head['b']], bref), dw_l2=rel_l2(tr.arena.views[head['w']], wr.grad),
+            dw_max=rel_err(tr.arena.views[head['w']], wr.grad), dx_l2=rel_l2(nchw(gh) / SCALE, a.grad), dx_max=rel_err(nchw(gh) / SCALE, a.grad))
+    assert fig.units['head']['dbias'] <= TOL['dbeta'], ('head dbias', fig.units['head'])
+    return gh
+
+
+def _resnet_units(name, b, size, seed):
+    from b200 import ops
+    sd0 = O.make_resnet_state_dict(name, 0)
+    x, _, data = _case_inputs(b, size, seed, seed + 1, slots=5)
+    t = resnet_teacher(sd0, x, data, name, device=DEV)
+    net = make_resnet(name, sd0).to(DEV).train()
+    tr = net.trainer
+    tr._plan()
+    tr._repack(torch.device(DEV))
+    tr._ensure_arena(net, torch.device(DEV))
+    tr._main = torch.cuda.current_stream()
+    fig = Figures('%s_%dx%d' % (name, b, size))
+    units = {u.key: u for u in tr._conv_units()}
+    # stem: 7x7 raw conv on the fp32 image with the fp32 weights, BN, ReLU, 3x3 / s2 max-pool, and back
+    st = tr._stem
+    rm0, rv0 = _snap(st.bn)
+    xg = x.to(DEV).float().contiguous()
+    s, a, pooled = tr._stem_forward(xg)
+    g16, g64 = _gout16(t.stem['pool'].grad)
+    sw, sg, sb = (sd0[k].double().clone().requires_grad_(True) for k in ('conv1.weight', 'bn1.weight', 'bn1.bias'))
+    z = F.conv2d(x.double(), sw, None, 2, 3)
+    z = z + (z.detach().half().double() - z.detach())
+    act = F.batch_norm(z, None, None, sg, sb, True, 0.0, EPS) * (nchw(a) > 0).double()      # the GPU's ReLU decisions
+    act.retain_grad()
+    act16 = act + (act.detach().half().double() - act.detach())        # the pool reads the fp16 activation: same argmax on ties
+    pool_ref = F.max_pool2d(act16, 3, 2, 1)
+    pool_ref.backward(g64)
+    ref = dict(z=z.detach(), mean=z.detach().mean(dim=(0, 2, 3)), var=z.detach().var(dim=(0, 2, 3), unbiased=False),
+               count=z.numel() // 64, dw=sw.grad, dgamma=sg.grad, dbeta=sb.grad)
+    _bn_figures(fig, 'conv1', s, ref, st.bn, rm0, rv0, a, act.detach())
+    fig.add('conv1', pool=rel_err(nchw(pooled), pool_ref.detach()))
+    grads = {}
+    da = tr._stem_backward(xg, s, a, g16, grads)
+    fig.add('conv1', pool_dx_l2=rel_l2(nchw(da) / SCALE, act.grad), pool_dx_max=rel_err(nchw(da) / SCALE, act.grad))
+    _grad_figures(fig, 'conv1', tr.arena, st.pnames, ref)
+    # every block unit and downsample on the teacher's own input and output gradient
+    for key, tu in t.units.items():
+        if key == 'conv1':
+            continue
+        u = units[key]
+        rm0, rv0 = _snap(u.bn)
+        inp16 = nhwc16(tu['inp'])
+        bb, hh, ww = inp16.shape[0], inp16.shape[1], inp16.shape[2]
+        a, s = tr._unit_forward(u, inp16, bb, hh, ww)
+        g16, g64 = _gout16(tu['out'].grad)
+        src = nchw(inp16)
+        if tu['sub']:
+            src = src[:, :, ::2, ::2]
+        w16 = t.sd[tu['conv']].detach().half().double().cpu()
+        ref = unit_ref(src, w16, sd0[tu['bn'] + '.weight'], sd0[tu['bn'] + '.bias'], tu['stride'], tu['k'], tu['relu'], g64, round_z=True,
+                       mask=(nchw(a) > 0).double())
+        _bn_figures(fig, key, s, ref, u.bn, rm0, rv0, a, ref['out'])
+        grads = {}
+        dx = tr._res_unit_backward(s, bb, grads, g16)
+        _grad_figures(fig, key, tr.arena, u.pnames, ref, dx, ref['dx'])
+    # block joins: forward relu(main + residual) and the boundary gradient, both one fp32 sum rounded once
+    first = list(t.joins)[0]
+    for p, j in t.joins.items():
+        m16, r16 = nhwc16(j['main']), nhwc16(j['res'])
+        exp = torch.relu(m16.float() + r16.float()).half()
+        tr._join_forward(m16, r16)
+        assert torch.equal(m16, exp), '%s join forward (yb_add_relu_f16) is not the fp32 sum rounded once' % p
+        bb, hh, ww = j['xin'].shape[0], j['xin'].shape[2], j['xin'].shape[3]
+        mask = None if p == first else nhwc16(j['xin'])
+        gm16, gb16 = nhwc16(j['xm'].grad * SCALE), nhwc16(j['skip'].grad * SCALE)
+        g = tr._join_backward(mask, gm16, gb16, j['stride'], bb, hh, ww)
+        up = torch.zeros_like(gm16, dtype=torch.float32)
+        up[:, ::j['stride'], ::j['stride']] = gb16.float()
+        exp = gm16.float() + up
+        if mask is not None:
+            exp = torch.where(mask.float() > 0, exp, torch.zeros((), device=DEV))
+        assert torch.equal(g, exp.half()), '%s join backward (yb_residual_bwd_f16) is not the fp32 sum rounded once' % p
+        # against the teacher: the gradient of the previous block's pre-ReLU sum (of the max-pool output for the first block)
+        prev = list(t.joins)[list(t.joins).index(p) - 1] if p != first else None
+        gref = t.stem['pool'].grad if prev is None else t.joins[prev]['pre'].grad
+        fig.add('join ' + p, join_l2=rel_l2(nchw(g) / SCALE, gref), join_max=rel_err(nchw(g) / SCALE, gref))
+    # last block's ReLU, then the head
+    a_last16 = nhwc16(t.head['a'])
+    hh, ww = a_last16.shape[1], a_last16.shape[2]
+    gh = _head_check(fig, tr, t, a_last16, t.sd['conv.weight'].detach().half().double().cpu(), hh, ww)
+    g = tr._join_backward(a_last16, gh, None, 1, a_last16.shape[0], hh, ww)
+    exp = torch.where(a_last16.float() > 0, gh.float(), torch.zeros((), device=DEV)).half()
+    assert torch.equal(g, exp), 'last join backward (yb_residual_bwd_f16 without a skip) is not exact'
+    last = list(t.joins)[-1]
+    fig.add('join head', join_l2=rel_l2(nchw(g) / SCALE, t.joins[last]['pre'].grad), join_max=rel_err(nchw(g) / SCALE, t.joins[last]['pre'].grad))
+    assert sum(1 for k in fig.units if not k.startswith('join') and k != 'head') == len(t.units)
+    return fig
+
+
+RESNET_UNIT_CASES = [('resnet18', 8, 160), ('resnet50', 8, 160), ('resnet50', 2, 416)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('case', RESNET_UNIT_CASES, ids=['%s_%dx%d' % c for c in RESNET_UNIT_CASES])
+def test_resnet_units_on_teacher_operands(case):
+    """Every unit of the ResNet trainer on the fp64 teacher's own input and output gradient: the stem (7x7 raw forward, BN, ReLU, max-pool
+    forward and backward, its weight gradient), every block conv (the stride-2 3x3 as zero-insert plus stride-1 gradients, its statistics
+    after the selection), every downsample (the 1x1 stride-2 on the subsampled input), every block join forward and backward, and the head
+    (padded dz through weight and data gradient).  z, batch and running statistics, activation, dgamma, dbeta, dW and dx per unit."""
+    name, b, size = case
+    fig = _resnet_units(name, b, size, 90 if size == 160 else 92)
+    if name == 'resnet50':
+        assert any(k.startswith('layer4') and k.endswith('conv3') for k in fig.units)
+    fig.check()
+
+
+def _mobilenet_units(b, size, seed):
+    sd0 = O.make_mobilenet_state_dict(0)
+    x, _, data = _case_inputs(b, size, seed, seed + 1, slots=5)
+    t = mobilenet_teacher(sd0, x, data, device=DEV)
+    net = make_mobilenet(sd0).to(DEV).train()
+    tr = net.trainer
+    plan = tr._plan()
+    tr._ensure_arena(net, torch.device(DEV))
+    tr._main = torch.cuda.current_stream()
+    fig = Figures('mobilenet_%dx%d' % (b, size))
+    # first conv (stride 2, fp32 weights on the fp32 image)
+    u0 = plan['first']
+    rm0, rv0 = _snap(u0.bn)
+    xg = x.to(DEV).float().contiguous()
+    s0, a0 = tr._first_forward(xg)
+    tu = t.units['layers.0']
+    g16, g64 = _gout16(tu['out'].grad)
+    ref = unit_ref(x, sd0['layers.0.conv.weight'], sd0['layers.0.bn.weight'], sd0['layers.0.bn.bias'], 2, 3, True, g64, round_z=True,
+                   mask=(nchw(a0) > 0).double())
+    _bn_figures(fig, 'layers.0', s0, ref, u0.bn, rm0, rv0, a0, ref['out'])
+    grads = {}
+    tr._first_backward(xg, s0, g16, grads)
+    _grad_figures(fig, 'layers.0', tr.arena, ('layers.0.conv.weight', 'layers.0.bn.weight', 'layers.0.bn.bias'), ref)
+    for i, rec in enumerate(plan['units'], 1):
+        key = rec['key']
+        # depthwise: fp32 weights, fp16 activations
+        tu = t.units[key + '.dw']
+        rm0, rv0 = _snap(rec['dw'].bn)
+        inp16 = nhwc16(tu['inp'])
+        bb, hh, ww = inp16.shape[:3]
+        ad, sd = tr._dw_forward(rec, inp16, bb, hh, ww)
+        g16, g64 = _gout16(tu['out'].grad)
+        ch = inp16.shape[-1]
+        ref = unit_ref(nchw(inp16), sd0[key + '.dw.conv.weight'], sd0[key + '.dw.bn.weight'], sd0[key + '.dw.bn.bias'], tu['stride'], 3, True,
+                       g64, groups=ch, round_z=True, mask=(nchw(ad) > 0).double())
+        _bn_figures(fig, key + '.dw', sd, ref, rec['dw'].bn, rm0, rv0, ad, ref['out'])
+        grads = {}
+        gin = tr._dw_backward(key, sd, bb, grads, g16)
+        _grad_figures(fig, key + '.dw', tr.arena, (key + '.dw.conv.weight', key + '.dw.bn.weight', key + '.dw.bn.bias'), ref, gin, ref['dx'])
+        # pointwise: fp16-packed weights on the wgmma conv
+        tu = t.units[key + '.pw']
+        up = rec['pw']
+        rm0, rv0 = _snap(up.bn)
+        inp16 = nhwc16(tu['inp'])
+        ap, sp = tr._pw_forward(rec, inp16, bb, inp16.shape[1], inp16.shape[2])
+        g16, g64 = _gout16(tu['out'].grad)
+        w16 = sd0[key + '.pw.conv.weight'].half().double()
+        ref = unit_ref(nchw(inp16), w16, sd0[key + '.pw.bn.weight'], sd0[key + '.pw.bn.bias'], 1, 1, True, g64, round_z=True,
+                       mask=(nchw(ap) > 0).double())
+        _bn_figures(fig, key + '.pw', sp, ref, up.bn, rm0, rv0, ap, ref['out'])
+        grads = {}
+        gin = tr._unit_backward(key + '.pw', sp, bb, grads, da=g16)
+        _grad_figures(fig, key + '.pw', tr.arena, (key + '.pw.conv.weight', key + '.pw.bn.weight', key + '.pw.bn.bias'), ref, gin, ref['dx'])
+    a16 = nhwc16(t.head['a'])
+    _head_check(fig, tr, t, a16, sd0['layers.14.weight'].half().double(), a16.shape[1], a16.shape[2])
+    assert len(fig.units) == len(t.units) + 1 == 28
+    return fig
+
+
+MOBILENET_UNIT_CASES = [(8, 160), (2, 416)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('case', MOBILENET_UNIT_CASES, ids=['%dx%d' % c for c in MOBILENET_UNIT_CASES])
+def test_mobilenet_units_on_teacher_operands(case):
+    """Every unit of the MobileNet trainer on the fp64 teacher's own input and output gradient: the stride-2 first conv, all 13 depthwise
+    units (stride 1 and 2, the depthwise BatchNorm backward chain and weight / data gradients), all 13 pointwise units and the head."""
+    b, size = case
+    _mobilenet_units(b, size, 80 if size == 160 else 82).check()
+
+
+# ------------------------------------------------------------------------------------------------
+# GPU: eval() after training, and resnet50's eval path at 416^2, block by block on the oracle's own inputs
+# ------------------------------------------------------------------------------------------------
+def _resnet_eval_blocks(net, sd, x, name):
+    """Each block of the eval path (`ResNet._block`) on the eval oracle's own block input; and the end-to-end feature."""
+    collect = {}
+    with torch.no_grad():
+        f_o = O.resnet_forward(sd, x, name, collect=collect)
+    prev, blocks = collect['maxpool'], {}
+    for blk in O.resnet_blocks(name):
+        p = blk['prefix']
+        lname, bname = p.split('.')
+        out = net._block(p, getattr(net, lname)[int(bname)], nhwc16(prev))
+        blocks[p] = dict(rel=rel_err(nchw(out), collect[p]), absmax=collect[p].abs().max().item() / FP16_MAX)
+        prev = collect[p]
+    with torch.no_grad():
+        f = net(x.to(DEV))
+    return rel_err(f, f_o), blocks
+
+
+def _train_resnet_15_steps(name):
+    """The setup of test_resnet_training_step_vs_oracle_and_descent: one step through the plugin surface, then 15 SGD steps on one batch."""
+    import model
+    import train as yb_train
+    cfg = make_config()
+    anchors = O.anchors_yolo_voc()
+    sd0 = O.make_resnet_state_dict(name, 0)
+    b, size = 8, 160
+    s = size // 32
+    x = O.synth_images(b, size, size, seed=90)
+    tgt = O.synth_targets(b, size, size, slots=5, seed=91)
+    data = O.norm_data(tgt, size, size, s, s)
+    net = make_resnet(name, sd0).to(DEV).train()
+    inference = model.Inference(cfg, net, anchors).train()
+    pred = model._inference(inference, x.to(DEV))
+    losses, _ = model.loss(anchors, {k: v.to(DEV) for k, v in data.items()}, pred, 0.6)
+    sum(losses[k] * O.HPARAM_DEFAULT[k] for k in losses).backward()
+    opt = torch.optim.SGD(net.parameters(), 1e-3, momentum=0.9)
+    batch = dict(tensor=x, yx_min=tgt['yx_min'], yx_max=tgt['yx_max'], cls=tgt['cls'])
+    for _ in range(15):
+        yb_train.iterate(inference, opt, anchors, cfg, batch)
+    return net.eval(), x
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('name', ['resnet18', 'resnet50'])
+def test_resnet_eval_after_training_block_by_block(name):
+    """After the 15 SGD steps of the training test, each block of the eval path on the eval oracle's own input under the trained
+    state_dict stays at the per-block level the golden test allows (3e-3), and no activation approaches the fp16 range: the end-to-end
+    eval() difference is the compounding of these per-block errors, not one wrong block."""
+    net, x = _train_resnet_15_steps(name)
+    sd_t = {k: v.detach().float().cpu() for k, v in net.state_dict().items() if not k.endswith('num_batches_tracked')}
+    e2e, blocks = _resnet_eval_blocks(net, sd_t, x[:2], name)
+    record('%s_eval_after_training_blocks' % name, dict(feature=e2e, blocks=blocks))
+    for p, v in blocks.items():
+        assert v['rel'] <= 3e-3, '%s block %s after training: rel err %.3e' % (name, p, v['rel'])
+        assert v['absmax'] <= 0.1, '%s block %s: |activation| %.3g of the fp16 range' % (name, p, v['absmax'])
+    assert e2e <= {'resnet18': 1e-2, 'resnet50': 5e-2}[name], e2e
+
+
+@pytest.mark.gpu
+def test_resnet50_eval_at_416_block_by_block():
+    """resnet50's eval path at the production size (2 x 416^2: 26 -> 13 stride-2 selections, a 13^2 head) on the initial state: each block
+    on the oracle's own input and the head feature end to end."""
+    sd0 = O.make_resnet_state_dict('resnet50', 0)
+    net = make_resnet('resnet50', sd0).to(DEV).eval()
+    x = O.synth_images(2, 416, 416, seed=93)
+    e2e, blocks = _resnet_eval_blocks(net, sd0, x, 'resnet50')
+    record('resnet50_eval_416_blocks', dict(feature=e2e, blocks=blocks))
+    for p, v in blocks.items():
+        assert v['rel'] <= 3e-3, 'resnet50 block %s at 416: rel err %.3e' % (p, v['rel'])
+    assert e2e <= 1e-2, e2e
+
+
+@pytest.mark.gpu
+def test_mobilenet_eval_after_training_vs_oracle():
+    """MobileNet eval() after the 15 SGD steps of the training test against the eval oracle on the trained state_dict, end to end and each
+    [depthwise, pointwise] unit pair on the oracle's own input."""
+    import model
+    import train as yb_train
+    cfg = make_config()
+    cfg.read_dict({'hparam': {'foreground': '5', 'background': '1', 'center': '1', 'size': '1', 'cls': '1'}})
+    anchors = O.anchors_yolo_voc()
+    sd0 = O.make_mobilenet_state_dict(0)
+    b, size = 8, 160
+    s = size // 32
+    x = O.synth_images(b, size, size, seed=80)
+    tgt = O.synth_targets(b, size, size, slots=5, seed=81)
+    data = O.norm_data(tgt, size, size, s, s)
+    net = make_mobilenet(sd0).to(DEV).train()
+    inference = model.Inference(cfg, net, anchors).train()
+    pred = model._inference(inference, x.to(DEV))
+    losses, _ = model.loss(anchors, {k: v.to(DEV) for k, v in data.items()}, pred, 0.6)
+    sum(losses[k] * O.HPARAM_DEFAULT[k] for k in losses).backward()
+    opt = torch.optim.SGD(net.parameters(), 1e-3, momentum=0.9)
+    batch = dict(tensor=x, yx_min=tgt['yx_min'], yx_max=tgt['yx_max'], cls=tgt['cls'])
+    hist = [float(yb_train.iterate(inference, opt, anchors, cfg, batch)['loss_total'].item()) for _ in range(15)]
+    assert hist[-1] < 0.9 * hist[0], hist
+    net.eval()
+    sd_t = {k: v.detach().float().cpu() for k, v in net.state_dict().items() if not k.endswith('num_batches_tracked')}
+    xe = x[:2]
+    collect = {}
+    with torch.no_grad():
+        f = net(xe.to(DEV))
+        f_o = O.mobilenet_forward(sd_t, xe, collect=collect)
+        f_stale = O.mobilenet_forward(sd0, xe)
+    e_eval, e_stale = rel_err(f, f_o), rel_err(f_stale, f_o)
+    # each unit pair with the eval path's kernels and operands (MobileNet._fold / _packed) on the oracle's own input
+    from b200 import ops
+    units = {}
+    for i, unit in enumerate(list(net.layers)[1:-1], 1):
+        cur = nhwc16(collect['layers.%d' % (i - 1)])
+        bb, hh, ww, ch = cur.shape
+        stride = unit.dw.conv.stride[0]
+        scale, shift = net._fold('dw%d' % i, unit.dw.bn)
+        out = torch.empty(bb, hh // stride, ww // stride, ch, dtype=torch.float16, device=DEV)
+        ops.call('yb_dwconv3x3_bn_relu_fwd', cur, unit.dw.conv.weight.detach().contiguous().view(ch, 9), scale, shift, out, bb, hh, ww, ch, stride)
+        scale, shift = net._fold('pw%d' % i, unit.pw.bn)
+        y = ops.conv_bn_act(out, net._packed('pww%d' % i, unit.pw.conv.weight), scale, shift, 0.0)
+        units['layers.%d' % i] = rel_err(nchw(y), collect['layers.%d' % i])
+    record('mobilenet_eval_after_training', dict(vs_trained_state=e_eval, stale_state_would_be=e_stale, units=units))
+    for k, v in units.items():
+        assert v <= 3e-3, 'MobileNet eval unit %s after training: rel err %.3e' % (k, v)
+    assert e_eval <= 5e-2, e_eval          # measured 1.8e-2 and 2.2e-2 (the training steps are not bit-deterministic)
+    assert e_eval <= 0.2 * e_stale, (e_eval, e_stale)

@@ -719,37 +719,13 @@ class MobileNetTrainer(DarknetTrainer):
         first = self.dnn.layers[0]
         if first.conv.weight.shape[0] != 32:
             raise ValueError('MobileNet: the first layer must have 32 output channels')
+        saved.first, cur = self._first_forward(x)
         hh, ww = h // 2, w // 2
-        z = torch.empty(b, hh, ww, 32, dtype=torch.float16, device=dev)
-        ops.call('yb_mb_conv0_raw_fwd', x, first.conv.weight.detach().contiguous(), z, b, h, w)
-        u0 = plan['first']
-        mean, invstd = self._bn_forward('layers.0', u0, z, b * hh * ww)
-        cur = self._apply(u0, z, mean, invstd, b, hh, ww, False)
-        s0 = _Saved()
-        s0.u, s0.z, s0.mean, s0.invstd, s0.h, s0.w = u0, z, mean, invstd, hh, ww
-        saved.first = s0
         for rec in plan['units']:
-            key, stride = rec['key'], rec['stride']
-            ch = rec['dw'].cout
-            oh, ow = hh // stride, ww // stride
-            # depthwise
-            zd = torch.empty(b, oh, ow, ch, dtype=torch.float16, device=dev)
-            wd = rec['dw_conv'].weight.detach().contiguous().view(ch, 9)
-            ops.call('yb_dwconv3x3_raw_fwd', cur, wd, zd, b, hh, ww, ch, stride)
-            mean, invstd = self._bn_forward(key + '.dw', rec['dw'], zd, b * oh * ow)
-            ad = self._apply(rec['dw'], zd, mean, invstd, b, oh, ow, False)
-            sd = _Saved()
-            sd.u, sd.ain, sd.z, sd.mean, sd.invstd, sd.h, sd.w, sd.in_h, sd.in_w, sd.stride, sd.wd = rec['dw'], cur, zd, mean, invstd, oh, ow, hh, ww, stride, wd
-            # pointwise
-            up = rec['pw']
-            up.refresh(force=True)
-            zp = self._raw_conv(up, ad, key=key + '.pw')
-            mean, invstd = self._bn_forward(key + '.pw', up, zp, b * oh * ow)
-            ap = self._apply(up, zp, mean, invstd, b, oh, ow, False)
-            sp = _Saved()
-            sp.u, sp.ain, sp.z, sp.mean, sp.invstd, sp.h, sp.w, sp.pooled = up, ad, zp, mean, invstd, oh, ow, False
-            saved.units.append((key, sd, sp))
-            cur, hh, ww = ap, oh, ow
+            ad, sd = self._dw_forward(rec, cur, b, hh, ww)
+            cur, sp = self._pw_forward(rec, ad, b, sd.h, sd.w)
+            saved.units.append((rec['key'], sd, sp))
+            hh, ww = sd.h, sd.w
         head = plan['head']
         cout = head.weight.shape[0]
         w16 = ops.pack_weight_f16(head.weight.detach().contiguous(), 0)
@@ -759,14 +735,75 @@ class MobileNetTrainer(DarknetTrainer):
         self._bump_tracked()
         return feature, saved
 
-    def backward(self, saved, dfeature, dnn=None):
-        b = saved.b
-        grads = {}
-        dev = dfeature.device
-        self._ensure_arena(self.dnn, dev)
-        self._main = torch.cuda.current_stream(dev)
+    def _first_forward(self, x):
+        """conv_bn(3, 32, stride 2) on the fp32 image: raw conv -> BN (batch statistics) -> ReLU.  Returns (saved unit, activation)."""
+        b, _, h, w = x.shape
+        hh, ww = h // 2, w // 2
+        z = torch.empty(b, hh, ww, 32, dtype=torch.float16, device=x.device)
+        ops.call('yb_mb_conv0_raw_fwd', x, self.dnn.layers[0].conv.weight.detach().contiguous(), z, b, h, w)
+        u0 = self._plan()['first']
+        mean, invstd = self._bn_forward('layers.0', u0, z, b * hh * ww)
+        a = self._apply(u0, z, mean, invstd, b, hh, ww, False)
+        s0 = _Saved()
+        s0.u, s0.z, s0.mean, s0.invstd, s0.h, s0.w = u0, z, mean, invstd, hh, ww
+        return s0, a
+
+    def _dw_forward(self, rec, cur, b, hh, ww):
+        """Depthwise 3x3 unit (stride 1 or 2) on its input cur [B,hh,ww,C]: raw conv -> BN -> ReLU.  Returns (activation, saved unit)."""
+        key, stride = rec['key'], rec['stride']
+        ch = rec['dw'].cout
+        oh, ow = hh // stride, ww // stride
+        zd = torch.empty(b, oh, ow, ch, dtype=torch.float16, device=cur.device)
+        wd = rec['dw_conv'].weight.detach().contiguous().view(ch, 9)
+        ops.call('yb_dwconv3x3_raw_fwd', cur, wd, zd, b, hh, ww, ch, stride)
+        mean, invstd = self._bn_forward(key + '.dw', rec['dw'], zd, b * oh * ow)
+        ad = self._apply(rec['dw'], zd, mean, invstd, b, oh, ow, False)
+        sd = _Saved()
+        sd.u, sd.ain, sd.z, sd.mean, sd.invstd, sd.h, sd.w, sd.in_h, sd.in_w, sd.stride, sd.wd = rec['dw'], cur, zd, mean, invstd, oh, ow, hh, ww, stride, wd
+        return ad, sd
+
+    def _pw_forward(self, rec, ad, b, oh, ow):
+        """Pointwise 1x1 unit on the wgmma conv: raw conv (statistics in its epilogue) -> BN -> ReLU.  Returns (activation, saved unit)."""
+        key = rec['key']
+        up = rec['pw']
+        up.refresh(force=True)
+        zp = self._raw_conv(up, ad, key=key + '.pw')
+        mean, invstd = self._bn_forward(key + '.pw', up, zp, b * oh * ow)
+        ap = self._apply(up, zp, mean, invstd, b, oh, ow, False)
+        sp = _Saved()
+        sp.u, sp.ain, sp.z, sp.mean, sp.invstd, sp.h, sp.w, sp.pooled = up, ad, zp, mean, invstd, oh, ow, False
+        return ap, sp
+
+    def _dw_backward(self, key, sd, b, grads, g):
+        """Depthwise unit backward from the gradient g of its activation: BN + ReLU backward, depthwise weight and data gradients.  Returns the
+        gradient of the unit's input."""
+        ch = sd.u.cout
+        dev = g.device
+        dz = torch.empty(b, sd.h, sd.w, ch, dtype=torch.float16, device=dev)
+        self._bn_backward(key + '.dw', sd, b, grads, g, None, dz, ch)
+        dwd = self.arena.views[key + '.dw.conv.weight']
+        ops.call('yb_dwconv3x3_wgrad', sd.ain, dz, dwd, b, sd.in_h, sd.in_w, ch, sd.stride)
+        grads[key + '.dw.conv.weight'] = dwd.mul_(self._unscale)
+        self._emit(key + '.dw.conv.weight', grads)
+        gin = torch.empty(b, sd.in_h, sd.in_w, ch, dtype=torch.float16, device=dev)
+        ops.call('yb_dwconv3x3_dgrad', dz, sd.wd, gin, b, sd.in_h, sd.in_w, ch, sd.stride)
+        return gin
+
+    def _first_backward(self, x, s0, g, grads):
+        """First layer backward from the gradient g of its activation: BN + ReLU backward, then the weight gradient from the fp32 image."""
+        b, _, h, w = x.shape
+        dz0 = torch.empty(b, s0.h, s0.w, 32, dtype=torch.float16, device=g.device)
+        self._bn_backward('layers.0', s0, b, grads, g, None, dz0, 32)
+        dw0 = self.arena.views['layers.0.conv.weight']
+        ops.call('yb_mb_conv0_wgrad', x, dz0, dw0, b, h, w)
+        grads['layers.0.conv.weight'] = dw0.mul_(self._unscale)
+        self._emit('layers.0.conv.weight', grads)
+
+    def _head_backward(self, a_last, hh, ww, dfeature, grads):
+        """Head (1x1 conv with bias): bias gradient, dz scaled into fp16 and padded to 128 channels, weight gradient, and the data gradient at
+        the head's input."""
+        b, dev = a_last.shape[0], a_last.device
         head = self._plan()['head']
-        hh, ww = saved.hh, saved.ww
         chead, cin = head.weight.shape[0], head.weight.shape[1]
         cpad = (chead + 31) // 32 * 32
         dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
@@ -776,7 +813,7 @@ class MobileNetTrainer(DarknetTrainer):
         self._emit('layers.14.bias', grads)
         # head weight gradient / data gradient (1x1)
         dw_krsc = torch.empty(chead, 1, 1, cin, dtype=torch.float32, device=dev)
-        ops.call('yb_conv_wgrad', saved.a_last, dzh, dw_krsc, b, hh, ww, cin, chead, 1, saved.a_last.shape[-1], dzh.shape[-1])
+        ops.call('yb_conv_wgrad', a_last, dzh, dw_krsc, b, hh, ww, cin, chead, 1, a_last.shape[-1], dzh.shape[-1])
         dwh = self.arena.views['layers.14.weight']
         ops.call('yb_unpack_wgrad', dw_krsc, dwh, chead, cin, 1, self._unscale)
         grads['layers.14.weight'] = dwh
@@ -784,27 +821,20 @@ class MobileNetTrainer(DarknetTrainer):
         wdh = torch.empty(cin, 1, 1, cpad, dtype=torch.float16, device=dev)
         ops.call('yb_pack_weight_dgrad_f16', head.weight.detach().contiguous(), wdh, chead, cin, 1, cpad)
         one, zero = self._ones(cin, dev)
-        g = ops.conv_bn_act(dzh, wdh, one, zero, 1.0)
+        return ops.conv_bn_act(dzh, wdh, one, zero, 1.0)
+
+    def backward(self, saved, dfeature, dnn=None):
+        b = saved.b
+        grads = {}
+        dev = dfeature.device
+        self._ensure_arena(self.dnn, dev)
+        self._main = torch.cuda.current_stream(dev)
+        g = self._head_backward(saved.a_last, saved.hh, saved.ww, dfeature, grads)
         for key, sd, sp in reversed(saved.units):
             # pointwise unit: generic BN backward + wgmma weight / data gradient (state-dict names layers.N.pw.*)
             g = self._unit_backward(key + '.pw', sp, b, grads, da=g)
-            # depthwise unit
-            ch = sd.u.cout
-            dz = torch.empty(b, sd.h, sd.w, ch, dtype=torch.float16, device=dev)
-            self._bn_backward(key + '.dw', sd, b, grads, g, None, dz, ch)
-            dwd = self.arena.views[key + '.dw.conv.weight']
-            ops.call('yb_dwconv3x3_wgrad', sd.ain, dz, dwd, b, sd.in_h, sd.in_w, ch, sd.stride)
-            grads[key + '.dw.conv.weight'] = dwd.mul_(self._unscale)
-            self._emit(key + '.dw.conv.weight', grads)
-            g = torch.empty(b, sd.in_h, sd.in_w, ch, dtype=torch.float16, device=dev)
-            ops.call('yb_dwconv3x3_dgrad', dz, sd.wd, g, b, sd.in_h, sd.in_w, ch, sd.stride)
-        s0 = saved.first
-        dz0 = torch.empty(b, s0.h, s0.w, 32, dtype=torch.float16, device=dev)
-        self._bn_backward('layers.0', s0, b, grads, g, None, dz0, 32)
-        dw0 = self.arena.views['layers.0.conv.weight']
-        ops.call('yb_mb_conv0_wgrad', saved.x, dz0, dw0, b, saved.h, saved.w)
-        grads['layers.0.conv.weight'] = dw0.mul_(self._unscale)
-        self._emit('layers.0.conv.weight', grads)
+            g = self._dw_backward(key, sd, b, grads, g)
+        self._first_backward(saved.x, saved.first, g, grads)
         self._join(dev)
         if self.reducer is not None:
             self.reducer.finish()
@@ -929,19 +959,8 @@ class ResNetTrainer(DarknetTrainer):
         self._repack(dev)
         saved = _Saved()
         saved.x, saved.b, saved.h, saved.w = x, b, h, w
-        # stem: raw conv -> BN (batch statistics) -> ReLU -> max-pool
-        st = self._stem
-        hh, ww = h // 2, w // 2
-        z = torch.empty(b, hh, ww, 64, dtype=torch.float16, device=dev)
-        ops.call('yb_stem7x7_raw_fwd', x, st.conv.weight.detach(), z, b, h, w)
-        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww)
-        a = self._apply(st, z, mean, invstd, b, hh, ww, False)
-        s = _Saved()
-        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w = st, None, z, mean, invstd, hh, ww
-        saved.stem, saved.stem_a = s, a
-        cur = torch.empty(b, hh // 2, ww // 2, 64, dtype=torch.float16, device=dev)
-        ops.call('yb_maxpool3x3_s2_f16', a, cur, b, hh, ww, 64)
-        hh, ww = hh // 2, ww // 2
+        saved.stem, saved.stem_a, cur = self._stem_forward(x)
+        hh, ww = h // 4, w // 4
         saved.pool = cur
         saved.blocks = []
         for _, units, ds in blocks:
@@ -955,9 +974,7 @@ class ResNetTrainer(DarknetTrainer):
                 res, sds = self._unit_forward(ds, xin, b, in_h, in_w)
             else:
                 res, sds = xin, None
-            if res.shape != cur.shape:
-                raise RuntimeError('ResNet training: residual %s does not match the block output %s' % (tuple(res.shape), tuple(cur.shape)))
-            ops.call('yb_add_relu_f16', cur, res, cur, cur.numel())      # in place: the units keep z, not their output
+            self._join_forward(cur, res)
             saved.blocks.append((xin, in_h, in_w, recs, sds))
         head = self._head
         one, _ = self._ones(head.cout, dev)
@@ -965,6 +982,69 @@ class ResNetTrainer(DarknetTrainer):
         saved.a_last, saved.hh, saved.ww = cur, hh, ww
         self._bump_tracked()
         return feature, saved
+
+    def _stem_forward(self, x):
+        """Stem on the fp32 image x [B,3,H,W]: raw 7x7 stride-2 conv -> BN (batch statistics) -> ReLU -> 3x3 stride-2 max-pool.
+        Returns (saved unit, activation before the pool, pooled output)."""
+        b, _, h, w = x.shape
+        dev = x.device
+        st = self._stem
+        hh, ww = h // 2, w // 2
+        z = torch.empty(b, hh, ww, 64, dtype=torch.float16, device=dev)
+        ops.call('yb_stem7x7_raw_fwd', x, st.conv.weight.detach(), z, b, h, w)
+        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww)
+        a = self._apply(st, z, mean, invstd, b, hh, ww, False)
+        s = _Saved()
+        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w = st, None, z, mean, invstd, hh, ww
+        pooled = torch.empty(b, hh // 2, ww // 2, 64, dtype=torch.float16, device=dev)
+        ops.call('yb_maxpool3x3_s2_f16', a, pooled, b, hh, ww, 64)
+        return s, a, pooled
+
+    @staticmethod
+    def _join_forward(cur, res):
+        """Block join: cur = relu(cur + res), in place (the units keep z, not their output)."""
+        if res.shape != cur.shape:
+            raise RuntimeError('ResNet training: residual %s does not match the block output %s' % (tuple(res.shape), tuple(cur.shape)))
+        ops.call('yb_add_relu_f16', cur, res, cur, cur.numel())
+
+    @staticmethod
+    def _join_backward(mask, gm, gb, stride_b, b, h, w):
+        """Gradient at a block boundary: (mask > 0) ? gm + S^T gb : 0 in one pass, where gm is the main path's input gradient, gb the skip
+        path's (at 1 / stride_b resolution, or None) and mask the previous block's ReLU output (None: no ReLU in between)."""
+        g = torch.empty_like(gm)
+        ops.call('yb_residual_bwd_f16', mask, gm, gb, stride_b, g, b, h, w, gm.shape[-1])
+        return g
+
+    def _head_backward(self, a_last, hh, ww, dfeature, grads):
+        """Head (1x1 conv with bias): bias gradient from the fp32 gradient, dz scaled into fp16 and padded to 128 channels, weight gradient,
+        and the data gradient at the head's input (before the last block's ReLU mask)."""
+        b, dev = a_last.shape[0], a_last.device
+        head = self._head
+        chead, cin = head.cout, head.cin
+        cpad = (chead + 31) // 32 * 32
+        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
+        dbias = self.arena.views['conv.bias']
+        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
+        grads['conv.bias'] = dbias.mul_(self._unscale)
+        self._emit('conv.bias', grads)
+        self._wgrad(head, a_last, dzh, b, hh, ww, grads, head.key, cout=chead)
+        one, zero = self._ones(cin, dev)
+        return ops.conv_bn_act(dzh, self._wd(head.key, head, cpad), one, zero, 1.0)
+
+    def _stem_backward(self, x, st, stem_a, g, grads):
+        """Stem backward from the gradient g at the max-pool output: max-pool backward -> BN + ReLU backward -> weight gradient from the fp32
+        image.  Returns the gradient at the stem's activation (the max-pool's input)."""
+        b, _, h, w = x.shape
+        dev = g.device
+        da = torch.empty_like(stem_a)
+        ops.call('yb_maxpool3x3_s2_bwd_f16', stem_a, g, da, b, st.h, st.w, 64)
+        dz = torch.empty(b, st.h, st.w, 64, dtype=torch.float16, device=dev)
+        self._bn_backward(st.u.key, st, b, grads, da, None, dz, 64)
+        dw = self.arena.views['conv1.weight']
+        ops.call('yb_stem7x7_wgrad', x, dz, dw, b, h, w)
+        grads['conv1.weight'] = dw.mul_(self._unscale)
+        self._emit('conv1.weight', grads)
+        return da
 
     def _res_unit_backward(self, s, b, grads, da):
         """Backward of one block unit from the gradient of its output; returns the gradient of its input (s.ain's resolution)."""
@@ -986,20 +1066,9 @@ class ResNetTrainer(DarknetTrainer):
         dev = dfeature.device
         self._ensure_arena(self.dnn, dev)
         self._main = torch.cuda.current_stream(dev)
-        head = self._head
         hh, ww = saved.hh, saved.ww
-        chead, cin = head.cout, head.cin
-        cpad = (chead + 31) // 32 * 32
-        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views['conv.bias']
-        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
-        grads['conv.bias'] = dbias.mul_(self._unscale)
-        self._emit('conv.bias', grads)
-        self._wgrad(head, saved.a_last, dzh, b, hh, ww, grads, head.key, cout=chead)
-        one, zero = self._ones(cin, dev)
-        gh = ops.conv_bn_act(dzh, self._wd(head.key, head, cpad), one, zero, 1.0)
-        g = torch.empty_like(gh)
-        ops.call('yb_residual_bwd_f16', saved.a_last, gh, None, 1, g, b, hh, ww, cin)        # through the last block's ReLU
+        gh = self._head_backward(saved.a_last, hh, ww, dfeature, grads)
+        g = self._join_backward(saved.a_last, gh, None, 1, b, hh, ww)        # through the last block's ReLU
         # g: gradient of the pre-ReLU sum of the current block (main path + skip)
         for (xin, in_h, in_w, recs, sds), (_, units, ds) in reversed(list(zip(saved.blocks, self._plan()))):
             gm = g
@@ -1010,18 +1079,8 @@ class ResNetTrainer(DarknetTrainer):
             else:
                 gb, stride_b = g, 1
             mask = None if xin is saved.pool else xin           # layer1.0's input is the max-pool output: no ReLU in between
-            g = torch.empty_like(xin)
-            ops.call('yb_residual_bwd_f16', mask, gm, gb, stride_b, g, b, in_h, in_w, xin.shape[-1])
-        # stem: max-pool backward -> BN + ReLU backward -> weight gradient from the fp32 image
-        st = saved.stem
-        da = torch.empty_like(saved.stem_a)
-        ops.call('yb_maxpool3x3_s2_bwd_f16', saved.stem_a, g, da, b, st.h, st.w, 64)
-        dz = torch.empty(b, st.h, st.w, 64, dtype=torch.float16, device=dev)
-        self._bn_backward(st.u.key, st, b, grads, da, None, dz, 64)
-        dw = self.arena.views['conv1.weight']
-        ops.call('yb_stem7x7_wgrad', saved.x, dz, dw, b, saved.h, saved.w)
-        grads['conv1.weight'] = dw.mul_(self._unscale)
-        self._emit('conv1.weight', grads)
+            g = self._join_backward(mask, gm, gb, stride_b, b, in_h, in_w)
+        self._stem_backward(saved.x, saved.stem, saved.stem_a, g, grads)
         self._join(dev)
         if self.reducer is not None:
             self.reducer.finish()
