@@ -225,6 +225,50 @@ class DarknetTrainer(object):
                  b, h, w, c, int(pool))
         return out
 
+    @staticmethod
+    def _saved_unit(u, ain, z, mean, invstd, hh, ww, pooled):
+        s = _Saved()
+        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w, s.pooled = u, ain, z, mean, invstd, hh, ww, pooled
+        return s
+
+    def _first_forward(self, x):
+        """layers1.0 on the fp32 image: raw conv (batch statistics in its copy-out loop when the shape allows) -> BN -> leaky + 2x2 max-pool.
+        Returns (saved unit, pooled activation)."""
+        u0 = self.engine.units1[0]
+        b, _, h, w = x.shape
+        dev = x.device
+        z = torch.empty(b, h, w, u0.cout, dtype=torch.float16, device=dev)
+        if self.fuse_stats and h % 32 == 0 and w % 16 == 0:
+            # batch statistics accumulated by the conv kernel's copy-out loop: z is not read again for them
+            ops.call('yb_conv0_raw_stats_fwd', x, u0.w16, z, self._sums(('f', 'layers1.0'), u0.cout, dev), b, h, w, u0.cout)
+            self._fused_stats = True
+        else:
+            ops.call('yb_conv0_raw_fwd', x, u0.w16, z, b, h, w, u0.cout)
+        mean, invstd = self._bn_forward('layers1.0', u0, z, b * h * w)
+        a = self._apply(u0, z, mean, invstd, b, h, w, True)
+        return self._saved_unit(u0, None, z, mean, invstd, h, w, True), a
+
+    def _bn_unit_forward(self, key, u, src, b, hh, ww, pool, pooled=None, out=None, a_off=0):
+        """One BN unit on its input src [B,hh,ww,*]: raw conv -> batch statistics -> normalise + leaky (+ 2x2 max-pool), the activation
+        written into `out` at channel `a_off` when given.  `pooled` (default: `pool`) is what the backward chain is told about the unit's
+        output.  Returns (activation, saved unit)."""
+        z = self._raw_conv(u, src, key=key)
+        mean, invstd = self._bn_forward(key, u, z, b * hh * ww)
+        a = self._apply(u, z, mean, invstd, b, hh, ww, pool, out=out, a_off=a_off)
+        return a, self._saved_unit(u, src, z, mean, invstd, hh, ww, pool if pooled is None else pooled)
+
+    @staticmethod
+    def _reorg_forward(a_pt, cat):
+        """Passthrough activation [B,h,w,C] -> space-to-depth(2) into channels [0, 4C) of the concat buffer [B,h/2,w/2,*]."""
+        ops.reorg_f16(a_pt, cat, 0)
+
+    @staticmethod
+    def _reorg_backward(dcat, b, h, w, c):
+        """Gradient of the passthrough activation [B,h,w,C] from channels [0, 4C) of the concat gradient (the transpose of reorg)."""
+        d_apt = torch.empty(b, h, w, c, dtype=torch.float16, device=dcat.device)
+        ops.call('yb_reorg_bwd_f16', dcat, dcat.shape[-1], 0, d_apt, b, h, w, c)
+        return d_apt
+
     def _bn_backward(self, key, s, b, grads, da, dap, dz, ld_dz):
         u = s.u
         c = u.cout
@@ -260,32 +304,12 @@ class DarknetTrainer(object):
         saved = _Saved()
         saved.x, saved.b, saved.h, saved.w = x, b, h, w
         saved.units = {}
-
-        def record(key, u, ain, z, mean, invstd, hh, ww, pooled):
-            s = _Saved()
-            s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w, s.pooled = u, ain, z, mean, invstd, hh, ww, pooled
-            saved.units[key] = s
-
         # layers1.0 (direct from the fp32 image)
-        u0 = eng.units1[0]
-        z = torch.empty(b, h, w, u0.cout, dtype=torch.float16, device=dev)
-        if self.fuse_stats and h % 32 == 0 and w % 16 == 0:
-            # batch statistics accumulated by the conv kernel's copy-out loop: z is not read again for them
-            ops.call('yb_conv0_raw_stats_fwd', x, u0.w16, z, self._sums(('f', 'layers1.0'), u0.cout, dev), b, h, w, u0.cout)
-            self._fused_stats = True
-        else:
-            ops.call('yb_conv0_raw_fwd', x, u0.w16, z, b, h, w, u0.cout)
-        mean, invstd = self._bn_forward('layers1.0', u0, z, b * h * w)
-        cur = self._apply(u0, z, mean, invstd, b, h, w, True)
-        record('layers1.0', u0, None, z, mean, invstd, h, w, True)
+        saved.units['layers1.0'], cur = self._first_forward(x)
         hh, ww = h // 2, w // 2
         for u, key, pooled in zip(eng.units1[1:], eng._k1[1:], eng.pools1[1:]):
-            z = self._raw_conv(u, cur, key=key)
-            mean, invstd = self._bn_forward(key, u, z, b * hh * ww)
             last = key == eng._k1[-1]
-            a = self._apply(u, z, mean, invstd, b, hh, ww, pooled and not last)
-            record(key, u, cur, z, mean, invstd, hh, ww, pooled)
-            cur = a
+            cur, saved.units[key] = self._bn_unit_forward(key, u, cur, b, hh, ww, pooled and not last, pooled)
             if pooled and not last:
                 hh, ww = hh // 2, ww // 2
         x1 = cur                                    # layers1.16 output, unpooled (hh x ww)
@@ -293,30 +317,19 @@ class DarknetTrainer(object):
         upt = eng.unit_pt
         cat_ch = upt.cout * 4 + eng.units2[-1].cout
         cat = torch.empty(b, hh // 2, ww // 2, cat_ch, dtype=torch.float16, device=dev)
-        z = self._raw_conv(upt, x1, key='passthrough')
-        mean, invstd = self._bn_forward('passthrough', upt, z, b * hh * ww)
-        a_pt = self._apply(upt, z, mean, invstd, b, hh, ww, False)
-        record('passthrough', upt, x1, z, mean, invstd, hh, ww, False)
-        ops.reorg_f16(a_pt, cat, 0)
+        a_pt, saved.units['passthrough'] = self._bn_unit_forward('passthrough', upt, x1, b, hh, ww, False)
+        self._reorg_forward(a_pt, cat)
         # trunk
         cur = ops.maxpool2x2(x1)
         h32, w32 = hh // 2, ww // 2
         for i, (u, key) in enumerate(zip(eng.units2, eng._k2)):
-            z = self._raw_conv(u, cur, key=key)
-            mean, invstd = self._bn_forward(key, u, z, b * h32 * w32)
             if i == len(eng.units2) - 1:
-                self._apply(u, z, mean, invstd, b, h32, w32, False, out=cat, a_off=upt.cout * 4)
-                a = cat
+                cur, saved.units[key] = self._bn_unit_forward(key, u, cur, b, h32, w32, False, out=cat, a_off=upt.cout * 4)
             else:
-                a = self._apply(u, z, mean, invstd, b, h32, w32, False)
-            record(key, u, cur, z, mean, invstd, h32, w32, False)
-            cur = a
+                cur, saved.units[key] = self._bn_unit_forward(key, u, cur, b, h32, w32, False)
         saved.keys2 = list(eng._k2[:len(eng.units2)])
         u30, u31 = eng.units3
-        z = self._raw_conv(u30, cat, key='layers3.0')
-        mean, invstd = self._bn_forward('layers3.0', u30, z, b * h32 * w32)
-        a30 = self._apply(u30, z, mean, invstd, b, h32, w32, False)
-        record('layers3.0', u30, cat, z, mean, invstd, h32, w32, False)
+        a30, saved.units['layers3.0'] = self._bn_unit_forward('layers3.0', u30, cat, b, h32, w32, False)
         feature = ops.conv_bn_act(a30, u31.w16, u31.scale, u31.shift, 1.0, out_mode=ops.OUT_F32_NCHW)
         saved.a30, saved.cat, saved.x1, saved.h16, saved.w16, saved.h32, saved.w32 = a30, cat, x1, hh, ww, h32, w32
         self._bump_tracked()
@@ -413,6 +426,49 @@ class DarknetTrainer(object):
         one, zero = self._ones(u.cin, dev)
         return ops.conv_bn_act(dz, self._wd(key, u), one, zero, 1.0)
 
+    def _head_backward(self, a_last, hh, ww, dfeature, grads):
+        """Head (layers3.1, 1x1 conv with bias): bias gradient from the unscaled fp32 gradient, dz scaled into fp16 and padded to a multiple of
+        32 channels, weight gradient, and the data gradient at the head's input."""
+        u31 = self.engine.units3[1]
+        b, dev = a_last.shape[0], a_last.device
+        chead = u31.cout
+        cpad = (chead + 31) // 32 * 32
+        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
+        dbias = self.arena.views['layers3.1.conv.bias']
+        scaled = (dfeature.contiguous().float() * self.grad_scale)
+        ops.call('yb_head_grad_prepare', scaled, dzh, dbias, b, chead, cpad, hh * ww)
+        grads['layers3.1.conv.bias'] = dbias.mul_(self._unscale)
+        self._emit('layers3.1.conv.bias', grads)
+        self._wgrad(u31, a_last, dzh, b, hh, ww, grads, 'layers3.1', cout=chead)
+        one, zero = self._ones(u31.cin, dev)
+        return ops.conv_bn_act(dzh, self._wd('layers3.1', u31, cpad), one, zero, 1.0)
+
+    def _first_backward(self, x, s0, g_da, g_dap, grads):
+        """layers1.0 backward from the gradient of its activation (g_da unpooled, g_dap through its max-pool): BN + leaky (+ pool) backward
+        and the weight gradient from the fp32 image x."""
+        b, _, h, w = x.shape
+        dev = s0.z.device
+        dw0 = self.arena.views['layers1.0.conv.weight']
+        if g_da is None and g_dap is not None and h % 8 == 0 and w % 32 == 0 and os.environ.get('YB_CONV0_WGRAD_FUSED', '1') != '0':
+            # reduce pass of the BatchNorm backward, then the weight-gradient kernel forms dz itself (in shared memory, from z and the pooled
+            # gradient): the 2 x 708 MB (B = 64 @ 416) write + read of dz and one launch disappear
+            u0 = s0.u
+            sums = self._sums(('b', 'layers1.0'), u0.cout, dev)
+            bnw, bnb = u0.bn.weight.detach(), u0.bn.bias.detach()
+            ops.call('yb_bn_act_bwd', 0, s0.z, s0.z.shape[-1], s0.mean, s0.invstd, bnw, bnb, self.slope, None, 0, 0, g_dap, g_dap.shape[-1], 0,
+                     b, s0.h, s0.w, u0.cout, 1, sums, None, 0, 1)
+            ops.call('yb_conv0_wgrad_bn', x, s0.z, g_dap, g_dap.shape[-1], 0, s0.mean, s0.invstd, bnw, bnb, self.slope, sums, dw0, b, h, w)
+            dgamma, dbeta = self.arena.views['layers1.0.bn.weight'], self.arena.views['layers1.0.bn.bias']
+            ops.call('yb_bn_param_grad', sums, u0.cout, dgamma, dbeta, 1, self._unscale)          # also clears the accumulators (after their last reader)
+            grads['layers1.0.bn.weight'], grads['layers1.0.bn.bias'] = dgamma, dbeta
+            self._emit('layers1.0.bn.weight', grads)
+            self._emit('layers1.0.bn.bias', grads)
+        else:
+            dz0 = self._unit_backward('layers1.0', s0, b, grads, da=g_da, dap=g_dap)
+            ops.call('yb_conv0_wgrad', x, dz0, dw0, b, h, w)
+        grads['layers1.0.conv.weight'] = dw0.mul_(self._unscale)
+        self._emit('layers1.0.conv.weight', grads)
+
     def backward(self, saved, dfeature, dnn=None):
         """dfeature: fp32 NCHW gradient of the loss w.r.t. the head output.  Returns {state_dict key: fp32 grad}: views of the
         persistent gradient arena, already averaged over the data-parallel ranks when a reducer is attached."""
@@ -422,20 +478,7 @@ class DarknetTrainer(object):
         dev = dfeature.device
         self._ensure_arena(dnn if dnn is not None else self._dnn, dev)
         self._main = torch.cuda.current_stream(dev)
-        u30, u31 = eng.units3
-        h32, w32 = saved.h32, saved.w32
-        chead = u31.cout
-        cpad = (chead + 31) // 32 * 32
-        # head: bias gradient from the unscaled fp32 gradient, dz scaled into fp16
-        dzh = torch.empty(b, h32, w32, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views['layers3.1.conv.bias']
-        scaled = (dfeature.contiguous().float() * self.grad_scale)
-        ops.call('yb_head_grad_prepare', scaled, dzh, dbias, b, chead, cpad, h32 * w32)
-        grads['layers3.1.conv.bias'] = dbias.mul_(self._unscale)
-        self._emit('layers3.1.conv.bias', grads)
-        self._wgrad(u31, saved.a30, dzh, b, h32, w32, grads, 'layers3.1', cout=chead)
-        one, zero = self._ones(u31.cin, dev)
-        da = ops.conv_bn_act(dzh, self._wd('layers3.1', u31, cpad), one, zero, 1.0)
+        da = self._head_backward(saved.a30, saved.h32, saved.w32, dfeature, grads)
         # layers3.0 -> gradient of the concat buffer
         dcat = self._unit_backward('layers3.0', saved.units['layers3.0'], b, grads, da=da)
         cpt4 = eng.unit_pt.cout * 4
@@ -446,8 +489,7 @@ class DarknetTrainer(object):
             g_off = 0
         d_x1_pool = g                                              # [B,h32,w32,C16]
         # passthrough branch
-        d_apt = torch.empty(b, saved.h16, saved.w16, eng.unit_pt.cout, dtype=torch.float16, device=dev)
-        ops.call('yb_reorg_bwd_f16', dcat, dcat.shape[-1], 0, d_apt, b, saved.h16, saved.w16, eng.unit_pt.cout)
+        d_apt = self._reorg_backward(dcat, b, saved.h16, saved.w16, eng.unit_pt.cout)
         d_x1 = self._unit_backward('passthrough', saved.units['passthrough'], b, grads, da=d_apt)
         # layers1.* in reverse; the branch point layers1.16 gets both gradients
         keys1 = eng._k1
@@ -459,27 +501,7 @@ class DarknetTrainer(object):
             prev_pooled = saved.units[prev_key].pooled
             g_da, g_dap = (None, g) if prev_pooled else (g, None)
         # layers1.0: weight gradient straight from the fp32 image
-        s0 = saved.units['layers1.0']
-        dw0 = self.arena.views['layers1.0.conv.weight']
-        if g_da is None and g_dap is not None and saved.h % 8 == 0 and saved.w % 32 == 0 and os.environ.get('YB_CONV0_WGRAD_FUSED', '1') != '0':
-            # reduce pass of the BatchNorm backward, then the weight-gradient kernel forms dz itself (in shared memory, from z and the pooled
-            # gradient): the 2 x 708 MB (B = 64 @ 416) write + read of dz and one launch disappear
-            u0 = s0.u
-            sums = self._sums(('b', 'layers1.0'), u0.cout, dev)
-            bnw, bnb = u0.bn.weight.detach(), u0.bn.bias.detach()
-            ops.call('yb_bn_act_bwd', 0, s0.z, s0.z.shape[-1], s0.mean, s0.invstd, bnw, bnb, self.slope, None, 0, 0, g_dap, g_dap.shape[-1], 0,
-                     b, s0.h, s0.w, u0.cout, 1, sums, None, 0, 1)
-            ops.call('yb_conv0_wgrad_bn', saved.x, s0.z, g_dap, g_dap.shape[-1], 0, s0.mean, s0.invstd, bnw, bnb, self.slope, sums, dw0, b, saved.h, saved.w)
-            dgamma, dbeta = self.arena.views['layers1.0.bn.weight'], self.arena.views['layers1.0.bn.bias']
-            ops.call('yb_bn_param_grad', sums, u0.cout, dgamma, dbeta, 1, self._unscale)          # also clears the accumulators (after their last reader)
-            grads['layers1.0.bn.weight'], grads['layers1.0.bn.bias'] = dgamma, dbeta
-            self._emit('layers1.0.bn.weight', grads)
-            self._emit('layers1.0.bn.bias', grads)
-        else:
-            dz0 = self._unit_backward('layers1.0', s0, b, grads, da=g_da, dap=g_dap)
-            ops.call('yb_conv0_wgrad', saved.x, dz0, dw0, b, saved.h, saved.w)
-        grads['layers1.0.conv.weight'] = dw0.mul_(self._unscale)
-        self._emit('layers1.0.conv.weight', grads)
+        self._first_backward(saved.x, saved.units['layers1.0'], g_da, g_dap, grads)
         self._join(dev)
         if self.reducer is not None:
             self.reducer.finish()          # main stream waits for every bucket's all-reduce (no host wait)
@@ -535,7 +557,27 @@ class TinyTrainer(DarknetTrainer):
         saved = _Saved()
         saved.x, saved.b, saved.h, saved.w, saved.units, saved.order = x, b, h, w, {}, []
         # unit 0: 3 -> C0 (<= 32) on the first-layer kernel, filters zero-padded to 32
-        key0, u0, after0 = plan[0]
+        key0, _, after0 = plan[0]
+        saved.units[key0], cur = self._first_forward(x)
+        saved.order.append((key0, after0))
+        hh, ww = h // 2, w // 2
+        for key, u, after in plan[1:-1]:
+            cur, saved.units[key] = self._chain_unit_forward(key, u, after, cur, b, hh, ww)
+            saved.order.append((key, after))
+            if after == 'pool':
+                hh, ww = hh // 2, ww // 2
+        key_h, u_h, _ = plan[-1]
+        feature = ops.conv_bn_act(cur, u_h.w16, u_h.scale, u_h.shift, 1.0, out_mode=ops.OUT_F32_NCHW)
+        saved.a_last, saved.hh, saved.ww, saved.head = cur, hh, ww, (key_h, u_h)
+        self._bump_tracked()
+        return feature, saved
+
+    def _first_forward(self, x):
+        """Unit 0 (3 -> C0 <= 32) on the first-layer kernel with its filters zero-padded to 32: raw conv -> BN over the C0 real channels ->
+        leaky + 2x2 max-pool into a persistent 32-wide buffer whose padding channels stay zero.  Returns (saved unit, pooled activation)."""
+        b, _, h, w = x.shape
+        dev = x.device
+        key0, u0, after0 = self.dnn.unit_keys()[0]
         c0 = u0.cout
         if c0 > 32 or after0 != 'pool':
             raise RuntimeError('Tiny: the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
@@ -546,43 +588,52 @@ class TinyTrainer(DarknetTrainer):
         mean, invstd = self._bn_forward(key0, u0, z, b * h * w)
         cur = self._zeros(('a0', b, h, w), (b, h // 2, w // 2, 32), dev)
         self._apply(u0, z, mean, invstd, b, h, w, True, out=cur)
-        s = _Saved()
-        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w, s.pooled = u0, None, z, mean, invstd, h, w, True
-        saved.units[key0] = s
-        saved.order.append((key0, after0))
-        hh, ww, chan = h // 2, w // 2, 32
-        for key, u, after in plan[1:-1]:
-            if u.cin != chan:
-                # input side zero-padded to the producer's buffer width (unit 1: 16 -> 32)
-                wp = torch.zeros(u.cout, chan, u.ksize, u.ksize, dtype=torch.float32, device=dev)
-                wp[:, :u.cin].copy_(u.conv.weight.detach())
-                w16 = ops.pack_weight_f16(wp, 0)
-            else:
-                w16 = u.w16
-            one, zero = self._ones(u.cout, dev)
-            if self.fuse_stats and not (chan == 32 and u.ksize == 3 and u.cout <= 64):
-                z = ops.conv_bn_act_stats(cur, w16, one, zero, 1.0, self._sums(('f', key), u.cout, dev))
-                self._fused_stats = True
-            else:
-                z = ops.conv_bn_act(cur, w16, one, zero, 1.0)
-                self._fused_stats = False
-            mean, invstd = self._bn_forward(key, u, z, b * hh * ww)
-            a = self._apply(u, z, mean, invstd, b, hh, ww, after == 'pool')
-            s = _Saved()
-            s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w, s.pooled, s.cin_pad = u, cur, z, mean, invstd, hh, ww, after == 'pool', chan
-            if after == 'pool':
-                hh, ww = hh // 2, ww // 2
-            elif after == 'pool_s1':
-                s.a_unpooled = a
-                a = ops.maxpool2x2_s1(a)
-            saved.units[key] = s
-            saved.order.append((key, after))
-            cur, chan = a, u.cout
-        key_h, u_h, _ = plan[-1]
-        feature = ops.conv_bn_act(cur, u_h.w16, u_h.scale, u_h.shift, 1.0, out_mode=ops.OUT_F32_NCHW)
-        saved.a_last, saved.hh, saved.ww, saved.head = cur, hh, ww, (key_h, u_h)
-        self._bump_tracked()
-        return feature, saved
+        return self._saved_unit(u0, None, z, mean, invstd, h, w, True), cur
+
+    def _chain_unit_forward(self, key, u, after, cur, b, hh, ww):
+        """One chain unit on its input cur [B,hh,ww,chan]: raw conv (weights zero-padded on the input side when chan > Cin) -> BN -> leaky,
+        then the 2x2 max-pool (after = 'pool', fused) or ConstantPad2d + MaxPool2d(2, stride 1) (after = 'pool_s1').  Returns (output,
+        saved unit)."""
+        dev = cur.device
+        chan = cur.shape[-1]
+        if u.cin != chan:
+            # input side zero-padded to the producer's buffer width (unit 1: 16 -> 32)
+            wp = torch.zeros(u.cout, chan, u.ksize, u.ksize, dtype=torch.float32, device=dev)
+            wp[:, :u.cin].copy_(u.conv.weight.detach())
+            w16 = ops.pack_weight_f16(wp, 0)
+        else:
+            w16 = u.w16
+        one, zero = self._ones(u.cout, dev)
+        if self.fuse_stats and not (chan == 32 and u.ksize == 3 and u.cout <= 64):
+            z = ops.conv_bn_act_stats(cur, w16, one, zero, 1.0, self._sums(('f', key), u.cout, dev))
+            self._fused_stats = True
+        else:
+            z = ops.conv_bn_act(cur, w16, one, zero, 1.0)
+            self._fused_stats = False
+        mean, invstd = self._bn_forward(key, u, z, b * hh * ww)
+        a = self._apply(u, z, mean, invstd, b, hh, ww, after == 'pool')
+        s = self._saved_unit(u, cur, z, mean, invstd, hh, ww, after == 'pool')
+        s.cin_pad = chan
+        if after == 'pool_s1':
+            s.a_unpooled = a
+            a = ops.maxpool2x2_s1(a)
+        return a, s
+
+    def _head_backward(self, a_last, hh, ww, dfeature, grads):
+        """Head (1x1 conv with bias): bias gradient, dz scaled into fp16 and padded to a multiple of 32 channels, weight gradient, and the data
+        gradient at the head's input."""
+        key_h, u_h, _ = self.dnn.unit_keys()[-1]
+        b, dev = a_last.shape[0], a_last.device
+        chead = u_h.cout
+        cpad = (chead + 31) // 32 * 32
+        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
+        dbias = self.arena.views[key_h + '.conv.bias']
+        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
+        grads[key_h + '.conv.bias'] = dbias.mul_(self._unscale)
+        self._emit(key_h + '.conv.bias', grads)
+        self._wgrad(u_h, a_last, dzh, b, hh, ww, grads, key_h, cout=chead)
+        one, zero = self._ones(u_h.cin, dev)
+        return ops.conv_bn_act(dzh, self._wd(key_h, u_h, cpad), one, zero, 1.0)
 
     def backward(self, saved, dfeature, dnn=None):
         b = saved.b
@@ -591,18 +642,7 @@ class TinyTrainer(DarknetTrainer):
         self._ensure_arena(self.dnn, dev)
         self._main = torch.cuda.current_stream(dev)
         self._x = saved.x
-        key_h, u_h = saved.head
-        hh, ww = saved.hh, saved.ww
-        chead = u_h.cout
-        cpad = (chead + 31) // 32 * 32
-        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views[key_h + '.conv.bias']
-        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
-        grads[key_h + '.conv.bias'] = dbias.mul_(self._unscale)
-        self._emit(key_h + '.conv.bias', grads)
-        self._wgrad(u_h, saved.a_last, dzh, b, hh, ww, grads, key_h, cout=chead)
-        one, zero = self._ones(u_h.cin, dev)
-        g = ops.conv_bn_act(dzh, self._wd(key_h, u_h, cpad), one, zero, 1.0)
+        g = self._head_backward(saved.a_last, saved.hh, saved.ww, dfeature, grads)
         for key, after in reversed(saved.order):
             s = saved.units[key]
             u = s.u
