@@ -278,6 +278,21 @@ int yb_warp_affine_u8(const void* src, int src_h, int src_w, void* dst, int dst_
  * value / 255.  Only the training path needs the fp32 image (inference reads the uint8 frames in the first conv kernel). */
 int yb_totensor_u8(const void* src_nhwc_u8, float* dst_nchw_f32, int batch, int height, int width, yb_stream_t stream);
 
+/* One segment of the photometric chain of transform/image.py (RandomBlur, BGR2HSV, RandomHue, RandomSaturation, RandomBrightness, HSV2RGB,
+ * RandomGamma; config.ini `transform/image_train`) over a resized uint8 batch [B,H,W,3], out of place (dst != src), bit-exact with cv2 4.13.
+ * `stages`: 4-bit codes, first stage in the low bits, 0 ends the list: YB_PH_BLUR (cv2.blur, REFLECT_101, kernels up to 5 x 5; only as
+ * the first stage), YB_PH_SWAP (BGR<->RGB), YB_PH_BGR2HSV, YB_PH_HSV2RGB, YB_PH_LUT (a per-image, per-channel 256-entry table); at most 7
+ * stages and 4 tables.  params: DEVICE buffer, per image `param_stride` = 16 + 768 * (number of LUT stages) bytes: int32 kw, kh (blur
+ * kernel width and height, read when the first stage is a blur; values outside 1..5 are clamped into it), 8 bytes of padding, then each table as uint8 [3][256].  Nothing else
+ * varies with the draws, so a launch captured in a CUDA graph replays new draws after one copy into params. */
+#define YB_PH_BLUR 1
+#define YB_PH_SWAP 2
+#define YB_PH_BGR2HSV 3
+#define YB_PH_HSV2RGB 4
+#define YB_PH_LUT 5
+int yb_photometric_batch_u8(const void* src, void* dst, int batch, int height, int width, const void* params, int param_stride, int stages,
+                            yb_stream_t stream);
+
 /* ---- evaluation matching (SURVEY 8f rank 3; eval.py:57-75 `_matching`/`matching`, called per image and class at eval.py:210-216) ----
  * Segmented batch: image i owns detections [det_off[i], det_off[i+1]) (descending score within the image, as postprocess returns
  * them) and ground-truth boxes [gt_off[i], gt_off[i+1]); boxes are (y, x) float pairs, classes int32.  tp[d] = 1 iff detection d's

@@ -100,6 +100,7 @@ int conv0_wgrad_bn(const float*, const void*, const void*, long long, int, const
                    cudaStream_t);
 int resize_batch_u8(const void*, const long long*, const int*, void*, int, int, int, int, float*, float*, int, cudaStream_t);
 int totensor_u8(const void*, float*, int, int, int, cudaStream_t);
+int photometric_batch_u8(const void*, void*, int, int, int, const void*, int, int, cudaStream_t);
 int warp_affine_u8(const void*, int, int, void*, int, int, const double*, const int*, cudaStream_t);
 int resize_aug_batch_u8(const void*, const long long*, const int*, const int*, const float*, const unsigned char*, void*, int, int, int, int, float*, float*,
                         int, cudaStream_t);
@@ -368,6 +369,11 @@ int yb_warp_affine_u8(const void* src, int src_h, int src_w, void* dst, int dst_
 
 int yb_totensor_u8(const void* src_nhwc_u8, float* dst_nchw_f32, int batch, int height, int width, yb_stream_t stream) {
   return yb::totensor_u8(src_nhwc_u8, dst_nchw_f32, batch, height, width, S(stream));
+}
+
+int yb_photometric_batch_u8(const void* src, void* dst, int batch, int height, int width, const void* params, int param_stride, int stages,
+                            yb_stream_t stream) {
+  return yb::photometric_batch_u8(src, dst, batch, height, width, params, param_stride, stages, S(stream));
 }
 
 int yb_eval_match(const float* det_yx_min, const float* det_yx_max, const int* det_cls, const int* det_off, const float* gt_yx_min,

@@ -238,6 +238,175 @@ int warp_affine_u8(const void* src, int sh, int sw, void* dst, int dh, int dw, c
   return check_launch("warp_affine_u8_kernel");
 }
 
+// ------------------------------------------------------------------------------------------------
+// The photometric chain of the reference's `transform/image.py` (RandomBlur, BGR2HSV, RandomHue, RandomSaturation, RandomBrightness,
+// HSV2RGB, RandomGamma; config.ini `transform/image_train`) over a resized uint8 batch [B, H, W, 3], out of place, bit-exact with cv2 4.13
+// (tests/photometric_oracle.py states the rules and tests/golden/photometric.npz pins them).  One launch runs one segment of the chain:
+// an optional box blur, then per-pixel stages in registers.  `stages` holds 4-bit codes, first stage in the low bits.  Per image the
+// parameter buffer holds {int kw, kh, 0, 0} and then one 3 x 256 lookup table per LUT stage (hue / saturation / brightness / gamma draws,
+// composed on the host); it is the only thing a new draw changes, so a captured launch replays with new draws after one copy into it.
+constexpr int PH_TW = 32, PH_TH = 32, PH_HALO = 2;  // output tile; halo of the largest pinned kernel, 5 x 5
+constexpr int PH_MAX_STAGES = 7, PH_MAX_LUTS = 4;
+enum { PH_END = 0, PH_BLUR = 1, PH_SWAP = 2, PH_BGR2HSV = 3, PH_HSV2RGB = 4, PH_LUT = 5 };
+
+struct PhTables {
+  int sdiv[256], hdiv[256];
+  uint8_t lut[PH_MAX_LUTS][3][256];
+};
+
+__device__ __forceinline__ int reflect101(int i, int n) {  // BORDER_REFLECT_101 for i in [-2, n + 1]
+  if (n == 1) return 0;
+  i = i < 0 ? -i : i;
+  i = i >= n ? 2 * n - 2 - i : i;
+  return i < 0 ? -i : i;
+}
+
+// cv2 COLOR_BGR2HSV, 8-bit: OpenCV's integer rule with hsv_shift = 12
+__device__ __forceinline__ void bgr2hsv_px(const PhTables& t, int& c0, int& c1, int& c2) {
+  const int b = c0, g = c1, r = c2;
+  const int v = max(max(b, g), r), diff = v - min(min(b, g), r);
+  const int s = (diff * t.sdiv[v] + (1 << 11)) >> 12;
+  const int hp = v == r ? g - b : (v == g ? b - r + 2 * diff : r - g + 4 * diff);
+  int h = (hp * t.hdiv[diff] + (1 << 11)) >> 12;
+  c0 = h < 0 ? h + 180 : h; c1 = s; c2 = v;
+}
+
+// cv2 COLOR_HSV2RGB, 8-bit: float32 sectors with fused multiply-adds (any h, taken mod 180 through the sector); the result is truncated
+// in the vector body of a row and rounded half to even in its scalar tail (`tail`: the last w mod 32 pixels)
+__device__ __forceinline__ void hsv2rgb_px(bool tail, int& c0, int& c1, int& c2) {
+  const float h = __fmul_rn(static_cast<float>(c0), 6.f / 180.f);
+  const float s = __fmul_rn(static_cast<float>(c1), 1.f / 255.f), v = __fmul_rn(static_cast<float>(c2), 1.f / 255.f);
+  const float pre = floorf(h), f = __fsub_rn(h, pre);
+  const float t0 = v, t1 = __fmul_rn(v, __fsub_rn(1.f, s)), t2 = __fmul_rn(v, __fmaf_rn(-s, f, 1.f)),
+              t3 = __fmul_rn(v, __fmaf_rn(-s, __fsub_rn(1.f, f), 1.f));
+  float b, g, r;
+  switch (static_cast<int>(pre) % 6) {
+    case 0: b = t1; g = t3; r = t0; break;
+    case 1: b = t1; g = t0; r = t2; break;
+    case 2: b = t3; g = t0; r = t1; break;
+    case 3: b = t0; g = t2; r = t1; break;
+    case 4: b = t0; g = t1; r = t3; break;
+    default: b = t2; g = t1; r = t0; break;
+  }
+  r = __fmul_rn(r, 255.f); g = __fmul_rn(g, 255.f); b = __fmul_rn(b, 255.f);
+  c0 = min(255, tail ? __float2int_rn(r) : static_cast<int>(r));
+  c1 = min(255, tail ? __float2int_rn(g) : static_cast<int>(g));
+  c2 = min(255, tail ? __float2int_rn(b) : static_cast<int>(b));
+}
+
+__device__ __forceinline__ void ph_pixel(const PhTables& t, int stages, bool hsv_tail, int& c0, int& c1, int& c2) {
+  int lut = 0;
+#pragma unroll 1
+  for (; stages != PH_END; stages >>= 4) {
+    const int op = stages & 15;
+    if (op == PH_SWAP) { const int x = c0; c0 = c2; c2 = x; }
+    else if (op == PH_BGR2HSV) bgr2hsv_px(t, c0, c1, c2);
+    else if (op == PH_HSV2RGB) hsv2rgb_px(hsv_tail, c0, c1, c2);
+    else { c0 = t.lut[lut][0][c0]; c1 = t.lut[lut][1][c1]; c2 = t.lut[lut][2][c2]; ++lut; }
+  }
+}
+
+// cv2.blur's window sum -> pixel (d = kw kh): copy for d = 1; the 16-bit fixed-point rule up to d = 24, whose only overflow (d = 2,
+// s = 510) saturates in the 16-byte vector body of a row and wraps to 0 in its scalar tail; the exact quotient rounded half up at d = 25
+__device__ __forceinline__ int blur_divide(int s, int d, int m, int delta, bool tail) {
+  if (d == 1) return s;
+  if (d == 25) return (2 * s + 25) / 50;
+  const int v = ((s + delta) * m) >> 16;
+  return v > 255 ? (tail ? v & 255 : 255) : v;
+}
+
+// one CTA = a 32 x 32 output tile of one image (blockIdx.z); 256 threads, 4 rows each.  BLUR: tile + halo into shared memory with
+// REFLECT_101 indexing, integer row sums, then column sums in the epilogue.
+template <bool BLUR>
+__global__ void __launch_bounds__(256) photometric_u8_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int height, int width,
+                                                             const uint8_t* __restrict__ params, int stride, int stages, int nlut) {
+  __shared__ PhTables t;
+  constexpr int IW = PH_TW + 2 * PH_HALO, IH = PH_TH + 2 * PH_HALO;
+  __shared__ uint8_t tin[BLUR ? IH * IW * 3 : 1];
+  __shared__ uint16_t trow[BLUR ? IH * PH_TW * 3 : 1];
+  const int tid = threadIdx.x, img = blockIdx.z;
+  const int x0 = blockIdx.x * PH_TW, y0 = blockIdx.y * PH_TH;
+  const uint8_t* p = params + static_cast<long long>(img) * stride;
+  const uint8_t* s_img = src + static_cast<long long>(img) * height * width * 3;
+  uint8_t* d_img = dst + static_cast<long long>(img) * height * width * 3;
+  t.sdiv[tid] = tid ? (2 * (255 << 12) + tid) / (2 * tid) : 0;      // round((255 << 12) / i)
+  t.hdiv[tid] = tid ? (2 * (180 << 12) + 6 * tid) / (12 * tid) : 0;  // round((180 << 12) / (6 i))
+  for (int i = tid; i < nlut * 768; i += 256) (&t.lut[0][0][0])[i] = p[16 + i];
+  int kw = 1, kh = 1, d = 1, m = 0, delta = 0;
+  if (BLUR) {
+    // clamped to the pinned 1..5 (the host rejects larger draws): a bad parameter block must not index outside tin / trow
+    kw = min(max(reinterpret_cast<const int*>(p)[0], 1), 2 * PH_HALO + 1);
+    kh = min(max(reinterpret_cast<const int*>(p)[1], 1), 2 * PH_HALO + 1);
+    d = kw * kh;
+    m = 65536 / d;
+    if (2 * (65536 % d) < d) delta = d / 2 + 1; else { ++m; delta = d / 2; }
+    for (int i = tid; i < IH * IW * 3; i += 256) {
+      const int r = i / (IW * 3), rem = i - r * IW * 3, cx = rem / 3, c = rem - cx * 3;
+      const int gy = reflect101(min(max(y0 - PH_HALO + r, -PH_HALO), height + 1), height);
+      const int gx = reflect101(min(max(x0 - PH_HALO + cx, -PH_HALO), width + 1), width);
+      tin[i] = s_img[(static_cast<long long>(gy) * width + gx) * 3 + c];
+    }
+    __syncthreads();
+    const int xo = PH_HALO - kw / 2;
+    for (int i = tid; i < IH * PH_TW * 3; i += 256) {
+      const int r = i / (PH_TW * 3), rem = i - r * PH_TW * 3, x = rem / 3, c = rem - x * 3;
+      const uint8_t* q = tin + (r * IW + x + xo) * 3 + c;
+      int sum = 0;
+      for (int j = 0; j < kw; ++j) sum += q[3 * j];
+      trow[i] = static_cast<uint16_t>(sum);
+    }
+  }
+  __syncthreads();
+  const int tail_start = 3 * width - (3 * width) % 16;
+  const int tx = tid & 31;
+#pragma unroll 1
+  for (int ty = tid >> 5; ty < PH_TH; ty += 8) {
+    const int x = x0 + tx, y = y0 + ty;
+    if (x >= width || y >= height) continue;
+    const long long off = (static_cast<long long>(y) * width + x) * 3;
+    int c[3];
+    if (BLUR) {
+      const uint16_t* q = trow + ((ty + PH_HALO - kh / 2) * PH_TW + tx) * 3;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        int sum = 0;
+        for (int i = 0; i < kh; ++i) sum += q[i * PH_TW * 3 + k];
+        c[k] = blur_divide(sum, d, m, delta, 3 * x + k >= tail_start);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) c[k] = s_img[off + k];
+    }
+    ph_pixel(t, stages, x >= width - width % 32, c[0], c[1], c[2]);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) d_img[off + k] = static_cast<uint8_t>(c[k]);
+  }
+}
+
+int photometric_batch_u8(const void* src, void* dst, int batch, int height, int width, const void* params, int param_stride, int stages,
+                         cudaStream_t stream) {
+  YB_REQUIRE(src && dst && params && batch > 0 && batch <= 65535 && height > 0 && width > 0 && src != dst, "photometric_batch_u8: bad argument");
+  YB_REQUIRE(static_cast<long long>(height) * width * 3 < (1ll << 31) && stages >= 0, "photometric_batch_u8: bad argument");
+  const bool blur = (stages & 15) == PH_BLUR;
+  const int pixel_stages = blur ? stages >> 4 : stages;
+  int n = 0, nlut = 0, rest = pixel_stages;
+  for (; rest != 0; rest >>= 4, ++n) {
+    const int op = rest & 15;
+    YB_REQUIRE(op >= PH_SWAP && op <= PH_LUT, "photometric_batch_u8: unknown stage code, or a blur that is not the first stage");
+    nlut += op == PH_LUT;
+  }
+  YB_REQUIRE(n + blur <= PH_MAX_STAGES && nlut <= PH_MAX_LUTS, "photometric_batch_u8: too many stages for one launch");
+  YB_REQUIRE(param_stride == 16 + 768 * nlut, "photometric_batch_u8: param_stride must be 16 + 768 * (number of LUT stages)");
+  const dim3 grid((width + PH_TW - 1) / PH_TW, (height + PH_TH - 1) / PH_TH, batch);
+  if (blur)
+    photometric_u8_kernel<true><<<grid, 256, 0, stream>>>(static_cast<const uint8_t*>(src), static_cast<uint8_t*>(dst), height, width,
+                                                          static_cast<const uint8_t*>(params), param_stride, pixel_stages, nlut);
+  else
+    photometric_u8_kernel<false><<<grid, 256, 0, stream>>>(static_cast<const uint8_t*>(src), static_cast<uint8_t*>(dst), height, width,
+                                                           static_cast<const uint8_t*>(params), param_stride, pixel_stages, nlut);
+  return check_launch("photometric_u8_kernel");
+}
+
 int totensor_u8(const void* src, float* dst, int batch, int height, int width, cudaStream_t stream) {
   YB_REQUIRE(src && dst && batch > 0 && height > 0 && width > 0, "totensor_u8: bad argument");
   const long long total = static_cast<long long>(batch) * height * width;

@@ -4,10 +4,32 @@
 frames in one launch -- optionally through the horizontal flip and the random-crop window of the reference's training pipeline
 (`transform.augmentation.flip_horizontally`, `transform.resize.label.random_crop`), which are index transforms on the source of the same
 resize; `transform.augmentation.random_rotate` / `Rotator` and `transform.resize.image.fixed` (shrinking) run cv2.warpAffine's bilinear path in
-one kernel.  The photometric augmentations of `transform/image.py` (blur / hue / saturation / brightness / gamma) are not part of this build."""
+one kernel.  The photometric augmentations of `transform/image.py` (RandomBlur, BGR2HSV, RandomHue, RandomSaturation, RandomBrightness,
+HSV2RGB, RandomGamma) run bit-exactly with cv2 in one launch per chain segment over the resized batch (`transform.image.Compose`);
+`parse_transform` / `get_transform` build a configured sequence such as `transform/image_train` the way the reference does."""
+import inspect
+
 import torch
 
 from b200 import ops as _ops
+
+
+def parse_transform(config, method):
+    """A dotted name such as 'transform.image.RandomBlur' -> an instance, given `config` when its constructor takes one (reference
+    transform/__init__.py); anything else is returned as is."""
+    if isinstance(method, str):
+        import utils
+        attr = utils.parse_attr(method)
+        return attr(config) if len(inspect.signature(attr).parameters) == 1 else attr()
+    return method
+
+
+def get_transform(config, sequence, compose=None):
+    """`sequence` (dotted names or instances) -> `compose(list)`, by default `transform.image.Compose`, which compiles the image ops
+    into device launches."""
+    if compose is None:
+        from transform.image import Compose as compose
+    return compose([parse_transform(config, method) for method in sequence])
 
 
 def resize_batch(frames, height, width, bgr2rgb=True, yx_min=None, yx_max=None, flip=None, crop=None, margin=None):

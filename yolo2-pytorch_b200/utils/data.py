@@ -56,11 +56,17 @@ class Collate(object):
                  into the first conv kernel)
         yx_min / yx_max float32 [B, G, 2] in pixels of the resized image, zero-padded (train.norm_data scales to grid units)
         cls int64 [B, G], difficult uint8 [B, G], size int64 [B, 2] (original sizes), height, width
-    The reference's `resize` config choice maps to `rescale` (the default, transform/resize/label.py:25-31)."""
+    The reference's `resize` config choice maps to `rescale` (the default, transform/resize/label.py:25-31).
+    `transform_image` (a `transform.image.Compose`, e.g. `transform.get_transform(config, config.get('transform', 'image_train').split())`)
+    runs on the whole resized batch, with its draws made image by image as the reference's Collate makes them (utils/data.py:114-133);
+    a sequence of `BGR2RGB` alone keeps the swap fused in the resize kernel, as does the default None."""
 
-    def __init__(self, sizes, maintain=1, seed=None, bgr2rgb=True):
+    def __init__(self, sizes, maintain=1, seed=None, bgr2rgb=True, transform_image=None):
         self.schedule = SizeSchedule(sizes, maintain, seed)
         self.bgr2rgb = bgr2rgb
+        self.transform_image = transform_image
+        if transform_image is not None and transform_image.swap_only:
+            self.bgr2rgb, self.transform_image = True, None
 
     def __call__(self, batch):
         import transform
@@ -79,7 +85,10 @@ class Collate(object):
             rows.append(padding_labels(d, dim))
         yx_min = torch.from_numpy(np.stack([r['yx_min'] for r in rows]).astype(np.float32))
         yx_max = torch.from_numpy(np.stack([r['yx_max'] for r in rows]).astype(np.float32))
-        tensor, yx_min, yx_max = transform.resize_batch(frames, height, width, bgr2rgb=self.bgr2rgb, yx_min=yx_min, yx_max=yx_max)
+        chain = self.transform_image
+        tensor, yx_min, yx_max = transform.resize_batch(frames, height, width, bgr2rgb=self.bgr2rgb and chain is None, yx_min=yx_min, yx_max=yx_max)
+        if chain is not None:
+            tensor = chain.batch(tensor)
         dev = tensor.device
         return dict(tensor=tensor, yx_min=yx_min, yx_max=yx_max,
                     cls=torch.from_numpy(np.stack([np.asarray(r['cls']) for r in rows]).astype(np.int64)).to(dev),
