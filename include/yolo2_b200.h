@@ -320,6 +320,25 @@ int yb_maxpool3x3_s2_f16(const void* x, void* y, int batch, int height, int widt
 int yb_subsample2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
 int yb_add_relu_f16(const void* a, const void* b, void* out, long long count, yb_stream_t stream);
 
+/* ---- DenseNet plugin (model/densenet.py:29-65, torchvision's _DenseLayer / _Transition), inference ------------------------------
+ * DenseNet's norm -> relu -> 1x1 conv, with the BatchNorm + ReLU applied to the conv's INPUT (each dense layer has its own norm1 over the
+ * concatenation of all earlier feature maps of its block, so it cannot be folded into the producer or into the weights):
+ *   a[p][c] = fp16_rn( act( fmaf(pre_scale[c], x[p][c], pre_shift[c]) ) ),  act = ReLU (pre_relu = 1) or identity (0)
+ *   y = epilogue(a . W^T) exactly as yb_conv_bn_act_fwd_ws (scale / shift / slope; fp16 NHWC at y_ld / y_ch_off, or fp32 NCHW).
+ * x fp16 NHWC with pixel pitch x_ld >= cin (reads channels [0, cin) only), cin % 32 == 0 and cin <= 1920, w from yb_pack_weight_f16 (k = 1).
+ * The transform runs on the A tile in shared memory, between the TMA load and the tensor-core MMA; a bit-identical result is K1 on the
+ * materialised a with the same tile shape.  Tile selection is yb_conv_choice's for a 1x1 layer, restricted to the one-warpgroup kernel. */
+int yb_conv1x1_preact_fwd(const void* x, const void* w, const float* pre_scale, const float* pre_shift, int pre_relu, const float* scale,
+                          const float* shift, float slope, void* y, int batch, int height, int width, int cin, int cout, int x_ld, long long y_ld,
+                          int y_ch_off, int out_mode, int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);
+/* A transition's norm -> relu -> AvgPool2d(2) (torchvision _Transition): x fp16 NHWC [B,H,W,x_ld] (channels [0, C)) -> y [B,H/2,W/2,C],
+ * y = fp16(((r00 + r01) + (r10 + r11)) * 0.25) with r = max(fmaf(scale, x, shift), 0) in fp32.  The transition's 1x1 conv then runs on the
+ * pooled tensor (pooling and a 1x1 conv commute in exact arithmetic).  H, W even, C and x_ld multiples of 8. */
+int yb_bn_relu_avgpool2x2_f16(const void* x, int x_ld, const float* scale, const float* shift, void* y, int batch, int height, int width,
+                              int channels, yb_stream_t stream);
+/* yb_maxpool3x3_s2_f16 writing channels [y_ch_off, y_ch_off + C) of y [B,(H+1)/2,(W+1)/2,y_ld] (the stem pool into the first block's buffer). */
+int yb_maxpool3x3_s2_ld_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
+
 /* Training of the ResNet plugin: what torch autograd does for the stem, the max-pool, the stride-2 selection and the residual join.  BatchNorm and
  * the activations are the generic train-mode kernels above (slope 0 = ReLU, slope 1 = identity); the 3x3 / 1x1 convs and their gradients are the
  * wgmma kernels, a stride-2 conv's backward being the stride-1 gradients of the zero-inserted dz (yb_upsample2_zero_f16).

@@ -87,6 +87,10 @@ SIGNATURES = {
     'yb_broadcast_buffer': [P, P, c_longlong, c_int, c_int, P],
     'yb_mb_conv0_bn_relu_fwd': [P, P, P, P, P, c_int, c_int, c_int, P],
     'yb_dwconv3x3_bn_relu_fwd': [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_conv1x1_preact_fwd': [P, P, P, P, c_int, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int, P,
+                              c_longlong, P],
+    'yb_bn_relu_avgpool2x2_f16': [P, c_int, P, P, P, c_int, c_int, c_int, c_int, P],
+    'yb_maxpool3x3_s2_ld_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
 }
 
 _lib = None

@@ -176,6 +176,36 @@ def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch
     return out
 
 
+def conv1x1_preact(x, w, pre_scale, pre_shift, pre_relu, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0,
+                   workspace=None):
+    """DenseNet's norm -> relu -> 1x1 conv (yb_conv1x1_preact_fwd): the conv reads a = fp16(act(fmaf(pre_scale, x, pre_shift))) with act = ReLU
+    (pre_relu) or identity, then applies the conv_bn_act epilogue (scale, shift, slope).  x: fp16 [B,H,W,x_ld] (the first `cin` channels,
+    default the weight's Cin); w: fp16 [Cout,1,1,Cin]; out as conv_bn_act."""
+    _req(x, torch.float16, 'x'); _req(w, torch.float16, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    _req(pre_scale, torch.float32, 'pre_scale'); _req(pre_shift, torch.float32, 'pre_shift')
+    b, h, wd, x_ld = x.shape
+    cout, k, _, wcin = w.shape
+    cin = wcin if cin is None else cin
+    if cin != wcin or k != 1:
+        raise ValueError('conv1x1_preact: weight [%d,%d,%d,%d] does not match a 1x1 conv over %d channels' % (cout, k, k, wcin, cin))
+    if pre_scale.numel() < cin or pre_shift.numel() < cin:
+        raise ValueError('conv1x1_preact: pre_scale / pre_shift need %d channels' % cin)
+    if out is None:
+        out = (torch.empty(b, h, wd, cout, dtype=torch.float16, device=x.device) if out_mode == OUT_F16_NHWC
+               else torch.empty(b, cout, h, wd, dtype=torch.float32, device=x.device))
+    if out_mode == OUT_F16_NHWC:
+        _req(out, torch.float16, 'out')
+        y_ld = out.shape[-1]
+    else:
+        _req(out, torch.float32, 'out')
+        y_ld = 0
+    ws_ptr, ws_bytes = (None, 0) if workspace is None else (_p(_req(workspace, torch.uint8, 'workspace')), workspace.numel())
+    _ck(_l.load().yb_conv1x1_preact_fwd(_p(x), _p(w), _p(pre_scale), _p(pre_shift), int(bool(pre_relu)), _p(scale), _p(shift), float(slope),
+                                        _p(out), b, h, wd, cin, cout, x_ld, y_ld, y_ch_off, out_mode, flags, ws_ptr, ws_bytes, _s()),
+        'yb_conv1x1_preact_fwd')
+    return out
+
+
 def conv_bn_act_split(x, w, scale, shift, slope, out, a_channels, y_ch_off=0, lo_ch_off=-1, out_mode=OUT_F16_NHWC, flags=0, workspace=None):
     """Split-precision conv unit (yb_conv_bn_act_split_fwd).  x: fp16 [B,H,W,x_ld] holding `a_channels` usable channels
     (C, or 2C = [hi | lo]); w: fp16 [Cout,k,k,K'] from pack_weight_split_f16; out fp16 [B,H,W,y_ld]: hi at y_ch_off, and the fp16

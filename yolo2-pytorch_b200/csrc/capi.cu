@@ -63,7 +63,9 @@ int* debug_word_device() {
 long long conv_workspace_bytes();
 int conv_choice(int, int, int, int, int, int, int, int, int, int*);
 int conv_igemm_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, long long,
-                       int, int, int, void*, long long, double*, int, int, cudaStream_t);
+                       int, int, int, void*, long long, double*, int, int, const float*, const float*, int, cudaStream_t);
+int bn_relu_avgpool2x2(const void*, int, const float*, const float*, void*, int, int, int, int, cudaStream_t);
+int maxpool3x3_s2_ld(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 int pack_weight_split(const float*, void*, int, int, int, int, int, cudaStream_t);
 int maxpool2x2_split(const void*, void*, int, int, int, int, int, int, int, int, cudaStream_t);
 int conv_ref_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, long long,
@@ -172,14 +174,14 @@ int yb_conv_bn_act_fwd(const void* x, const void* w, const float* scale, const f
                        int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                        int flags, yb_stream_t stream) {
   return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, x_ld, y_ld, y_ch_off, out_mode,
-                                flags, nullptr, 0, nullptr, 0, -1, S(stream));
+                                flags, nullptr, 0, nullptr, 0, -1, nullptr, nullptr, 0, S(stream));
 }
 
 int yb_conv_bn_act_stats_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                              int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int flags,
                              double* sums, yb_stream_t stream) {
   return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, x_ld, y_ld, y_ch_off, 0, flags, nullptr, 0,
-                                sums, 0, -1, S(stream));
+                                sums, 0, -1, nullptr, nullptr, 0, S(stream));
 }
 
 long long yb_conv_workspace_bytes(void) { return yb::conv_workspace_bytes(); }
@@ -192,7 +194,7 @@ int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, cons
                           int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
   return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, x_ld, y_ld, y_ch_off, out_mode,
-                                flags, workspace, workspace_bytes, nullptr, 0, -1, S(stream));
+                                flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, S(stream));
 }
 
 int yb_conv_bn_act_split_fwd(const void* x, const void* w_split, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -200,7 +202,25 @@ int yb_conv_bn_act_split_fwd(const void* x, const void* w_split, const float* sc
                              int y_ch_off, int lo_ch_off, int out_mode, int flags, void* workspace, long long workspace_bytes,
                              yb_stream_t stream) {
   return yb::conv_igemm_forward(x, w_split, scale, shift, slope, y, batch, height, width, k_channels, cout, ksize, x_ld, y_ld, y_ch_off,
-                                out_mode, flags, workspace, workspace_bytes, nullptr, a_channels, lo_ch_off, S(stream));
+                                out_mode, flags, workspace, workspace_bytes, nullptr, a_channels, lo_ch_off, nullptr, nullptr, 0,
+                                S(stream));
+}
+
+int yb_conv1x1_preact_fwd(const void* x, const void* w, const float* pre_scale, const float* pre_shift, int pre_relu, const float* scale,
+                          const float* shift, float slope, void* y, int batch, int height, int width, int cin, int cout, int x_ld, long long y_ld,
+                          int y_ch_off, int out_mode, int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
+  if (pre_scale == nullptr) return yb::fail(YB_ERR_BAD_ARG, "conv_preact: null pre_scale");
+  return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, 1, x_ld, y_ld, y_ch_off, out_mode, flags,
+                                workspace, workspace_bytes, nullptr, 0, -1, pre_scale, pre_shift, pre_relu, S(stream));
+}
+
+int yb_bn_relu_avgpool2x2_f16(const void* x, int x_ld, const float* scale, const float* shift, void* y, int batch, int height, int width,
+                              int channels, yb_stream_t stream) {
+  return yb::bn_relu_avgpool2x2(x, x_ld, scale, shift, y, batch, height, width, channels, S(stream));
+}
+
+int yb_maxpool3x3_s2_ld_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::maxpool3x3_s2_ld(x, y, y_ld, y_ch_off, batch, height, width, channels, S(stream));
 }
 
 int yb_pack_weight_split_f16(const float* w_oihw, void* w_f16, int cout, int cin, int ksize, int segments, int lo_mask, yb_stream_t stream) {

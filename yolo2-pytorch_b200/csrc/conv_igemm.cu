@@ -128,7 +128,8 @@ __device__ __forceinline__ void st_release_gpu(unsigned* p, unsigned v) {
 // MT = number of 128-pixel M-subtiles per CTA tile (1 or 2).  MT = 2 makes the CTA tile 256 x BN: both
 // subtiles reuse the same weight (B) tile from shared memory, halving the L2->SM weight traffic per MAC.
 // The MMA warpgroup holds MT * BN fp32 accumulators per thread, so MT * BN <= 128.
-template <int BN, int BK, int MT>
+// kPreCh > 0 (the pre-activation form, conv_preact_kernel): room for a per-input-channel scale / shift table of up to kPreCh channels.
+template <int BN, int BK, int MT, int kPreCh = 0>
 struct ConvCfg {
   static constexpr int kSwizzle = BK * 2;                       // bytes per smem row
   static constexpr int kASubBytes = BM * BK * 2;
@@ -140,18 +141,67 @@ struct ConvCfg {
   static constexpr bool kMergedA = (MT == 2);                   // A tile fetched by one 256-pixel TMA box
   static constexpr int kRowsPerTile = BM * MT;
   static constexpr int kOutBytes = BM * 128;                    // TMA-store staging: one 32-row x 64-channel fp16 slice (4 KB) per epilogue warp
-  static constexpr int kFixedBytes = kAccBytes + kOutBytes + 1024 /*align slack*/ + 2 * 2 * BN * 4 /*scale/shift x2*/ + 2 * BN * 4 /*stats*/ + 256 /*barriers*/;
+  static constexpr int kFixedBytes = kAccBytes + kOutBytes + 1024 /*align slack*/ + 2 * 2 * BN * 4 /*scale/shift x2*/ + 2 * BN * 4 /*stats*/ + 256 /*barriers*/ +
+                                     2 * kPreCh * 4 /*pre-activation scale / shift*/;
   static constexpr int kStages = ((kSmemLimit - kFixedBytes) / kStageBytes) > 8 ? 8 : ((kSmemLimit - kFixedBytes) / kStageBytes);
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static_assert(kAccCols <= 128, "accumulator does not fit the MMA warpgroup's registers");
   static_assert(kStages >= 2, "shared memory budget");
 };
 
-template <int BN, int BK, int MT>
-__global__ void __launch_bounds__(kThreads, 1)
-conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
-  using Cfg = ConvCfg<BN, BK, MT>;
+// Pre-activation of the A operand (DenseNet's norm -> relu -> 1x1 conv, conv_preact_kernel):
+//   a[p][c] = fp16_rn(act(fmaf(scale[c], x[p][c], shift[c]))), act = ReLU (relu = 1) or identity (0).
+struct PreAct {
+  const float* scale;
+  const float* shift;
+  int relu;
+};
+constexpr int kPreMaxCh = 1920;                 // DenseNet-201's widest block input; the table is staged whole, once per CTA
+
+// Applies the pre-activation in place to one swizzled A stage (MT * 128 pixel rows x BK channels starting at channel c0).  The TMA
+// swizzle permutes 16-byte chunks inside a row: logical chunk c of row r sits at chunk c ^ (r % 8) (BK = 64, 128-byte rows) or
+// c ^ ((r / 2) % 4) (BK = 32, 64-byte rows).  A thread keeps one chunk column, so its scale / shift values stay in registers, and a
+// warp covers 512 contiguous bytes per pass.  A thread handles its chunk in two 8-byte halves; threads whose rows fall on alternate
+// 128-byte lines take the halves in opposite order, so each instruction of a warp touches all 32 banks twice (2 wavefronts per 256 B).
+template <int BK, int MT>
+__device__ __forceinline__ void preact_stage(uint32_t a, const float* tab_scale, const float* tab_shift, int c0, int relu) {
+  constexpr int kChunks = BK / 8;
+  constexpr int kRowsPerPass = kMmaThreads / kChunks;
+  const int c = threadIdx.x % kChunks;
+  const int r0 = threadIdx.x / kChunks;
+  // two passes of 4 channels (8 bytes) per chunk: 8 table values live next to the 128 accumulators of the widest tile without spilling
+#pragma unroll 1
+  for (int pass = 0; pass < 2; ++pass) {
+    const int half = pass ^ ((r0 / (64 / BK)) & 1);
+    const int ch = c0 + c * 8 + half * 4;
+    const float4 sc = *reinterpret_cast<const float4*>(tab_scale + ch);
+    const float4 sh = *reinterpret_cast<const float4*>(tab_shift + ch);
+#pragma unroll 1
+    for (int i = 0; i < MT * BM / kRowsPerPass; ++i) {
+      const int r = r0 + i * kRowsPerPass;
+      const int pc = (BK == 64) ? (c ^ (r & 7)) : (c ^ ((r >> 1) & 3));
+      const uint32_t addr = a + r * (BK * 2) + pc * 16 + half * 8;
+      uint32_t v0, v1;
+      asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v0), "=r"(v1) : "r"(addr) : "memory");
+      const float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&v0));
+      const float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&v1));
+      float y0 = __fmaf_rn(sc.x, f0.x, sh.x), y1 = __fmaf_rn(sc.y, f0.y, sh.y);
+      float y2 = __fmaf_rn(sc.z, f1.x, sh.z), y3 = __fmaf_rn(sc.w, f1.y, sh.w);
+      if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); y2 = fmaxf(y2, 0.f); y3 = fmaxf(y3, 0.f); }
+      __half2 h0 = __floats2half2_rn(y0, y1), h1 = __floats2half2_rn(y2, y3);
+      asm volatile("st.shared.v2.b32 [%0], {%1, %2};" :: "r"(addr), "r"(*reinterpret_cast<uint32_t*>(&h0)), "r"(*reinterpret_cast<uint32_t*>(&h1))
+                   : "memory");
+    }
+  }
+}
+
+// The body of both implicit-GEMM kernels of this family.  kPre = false is conv_igemm_kernel; kPre = true (1x1 only) is
+// conv_preact_kernel, whose MMA warpgroup applies `pre` to every A stage in shared memory before issuing the unchanged
+// shared-memory wgmma.
+template <int BN, int BK, int MT, bool kPre>
+__device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap& tmap_y,
+                                                const ConvParams p, const PreAct pre) {
+  using Cfg = ConvCfg<BN, BK, MT, kPre ? kPreMaxCh : 0>;
   constexpr int kStages = Cfg::kStages;
   constexpr bool kMergedA = Cfg::kMergedA;
   extern __shared__ uint8_t smem_raw[];
@@ -261,12 +311,25 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     uint32_t phase = 0;
     uint32_t acc_phase = 0;
     int tr_m = 0;
+    float* pre_scale = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);     // [kPreMaxCh] (kPre only)
+    float* pre_shift = pre_scale + kPreMaxCh;
+    if constexpr (kPre) {
+      for (int i = threadIdx.x; i < p.cin; i += kMmaThreads) { pre_scale[i] = __ldg(pre.scale + i); pre_shift[i] = __ldg(pre.shift + i); }
+      asm volatile("bar.sync 2, %0;" :: "n"(kMmaThreads) : "memory");
+    }
     for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
       const int kb_first = it.kb0, kb_last = it.kb1 - 1;
       int prev = -1;
       for (int kb = kb_first; kb <= kb_last; ++kb) {
         mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x300 | stage);
         if (threadIdx.x == 0) { YB_TRACE(1, tr_m); ++tr_m; }
+        if constexpr (kPre) {
+          // 1x1: K-block kb is channels [kb * BK, kb * BK + BK).  The generic-proxy writes are made visible to the wgmma (async
+          // proxy) by the fence, and the whole tile is transformed before any warp issues its MMAs.
+          preact_stage<BK, MT>(smem_a + stage * Cfg::kABytes, pre_scale, pre_shift, kb * BK, pre.relu);
+          fence_proxy_async_smem();
+          asm volatile("bar.sync 2, %0;" :: "n"(kMmaThreads) : "memory");
+        }
         if (!(p.skip & 4)) {
           const uint64_t bdesc = make_kmajor_desc<Cfg::kSwizzle>(smem_b + stage * Cfg::kBBytes);
           wgmma_fence();
@@ -589,6 +652,20 @@ conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
     if (p.tma_store && lane == 0) tma_store_wait<0>();     // every bulk store of this warp has landed before the CTA's shared memory goes away
   }
+}
+
+template <int BN, int BK, int MT>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
+  conv_igemm_body<BN, BK, MT, false>(tmap_a, tmap_b, tmap_y, p, PreAct{nullptr, nullptr, 0});
+}
+
+template <int BN, int BK, int MT>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_preact_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                   const __grid_constant__ CUtensorMap tmap_y, const ConvParams p, const PreAct pre) {
+  conv_igemm_body<BN, BK, MT, true>(tmap_a, tmap_b, tmap_y, p, pre);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1125,12 +1202,18 @@ static int get_encoders(EncodeTiledFn* tiled, EncodeIm2colFn* im2col) {
 int get_tensor_map_encoders(EncodeTiledFn* tiled, EncodeIm2colFn* im2col) { return get_encoders(tiled, im2col); }
 
 template <int BN, int BK, int MT>
-static int launch_conv(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, cudaStream_t stream) {
+static int launch_conv(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, const PreAct* pre,
+                       cudaStream_t stream) {
   using Cfg = ConvCfg<BN, BK, MT>;
-  static bool attr_set = false;
-  if (!attr_set) {
+  using PreCfg = ConvCfg<BN, BK, MT, kPreMaxCh>;
+  static bool attr_set = false, pre_attr_set = false;
+  if (pre == nullptr && !attr_set) {
     YB_CUDA(cudaFuncSetAttribute(conv_igemm_kernel<BN, BK, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
+  }
+  if (pre != nullptr && !pre_attr_set) {
+    YB_CUDA(cudaFuncSetAttribute(conv_preact_kernel<BN, BK, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, PreCfg::kSmemBytes));
+    pre_attr_set = true;
   }
   const int tiles = p.m_tiles * p.n_tiles;
   cudaLaunchConfig_t cfg;
@@ -1149,9 +1232,13 @@ static int launch_conv(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   if (p.streamk) cfg.gridDim = dim3(sm_count());          // sk_base / sk_rem were computed for exactly this many CTAs
   else cfg.gridDim = dim3(tiles < sm_count() ? tiles : sm_count());
   cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.dynamicSmemBytes = pre != nullptr ? PreCfg::kSmemBytes : Cfg::kSmemBytes;
   cfg.stream = stream;
   cfg.attrs = attr; cfg.numAttrs = nattr;
+  if (pre != nullptr) {
+    YB_CUDA(cudaLaunchKernelEx(&cfg, conv_preact_kernel<BN, BK, MT>, ta, tb, ty, p, *pre));
+    return check_launch("conv_preact_kernel");
+  }
   YB_CUDA(cudaLaunchKernelEx(&cfg, conv_igemm_kernel<BN, BK, MT>, ta, tb, ty, p));
   return check_launch("conv_igemm_kernel");
 }
@@ -1185,13 +1272,14 @@ static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
 
 // CTA tile shapes (BLOCK_N, M-subtiles): the one-warpgroup kernel keeps MT * BLOCK_N <= 128 accumulators per thread; 128 x 2 is
 // the two-consumer kernel
+// the two-consumer shape has no pre-activation form (conv_choose never picks it when `pre` is set)
 template <int BK>
 static int dispatch_conv(int bn, int mt, int grid, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p,
-                         cudaStream_t stream) {
+                         const PreAct* pre, cudaStream_t stream) {
   if (mt == 2 && bn == 128) return launch_wide<BK>(ta, tb, ty, p, grid, stream);
-  if (mt == 2) return launch_conv<64, BK, 2>(ta, tb, ty, p, stream);
-  if (bn == 64) return launch_conv<64, BK, 1>(ta, tb, ty, p, stream);
-  return launch_conv<128, BK, 1>(ta, tb, ty, p, stream);
+  if (mt == 2) return launch_conv<64, BK, 2>(ta, tb, ty, p, pre, stream);
+  if (bn == 64) return launch_conv<64, BK, 1>(ta, tb, ty, p, pre, stream);
+  return launch_conv<128, BK, 1>(ta, tb, ty, p, pre, stream);
 }
 
 static int conv_c32_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -1275,7 +1363,7 @@ constexpr double kWideEpiNsPerOut = 0.08; // two-consumer register epilogue, ns 
 constexpr double kSkNs = 16000.0;         // stream-K partial dump + collect, one-warpgroup kernel
 constexpr double kSkNsWide = 9000.0;      // the same from registers, two-consumer kernel
 int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, int a_channels, int out_mode, int flags, bool workspace_ok,
-                bool stats, bool lo, ConvChoice* out) {
+                bool stats, bool lo, bool pre, ConvChoice* out) {
   ConvChoice c;
   memset(&c, 0, sizeof(c));
   const int sms = sm_count();
@@ -1293,7 +1381,8 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, 
   const bool sk_possible = !stats && workspace_ok && (flags & 8) == 0;
   const bool sk_force = sk_possible && ((flags >> 30) & 1);
   // the two-consumer kernel: fp16 NHWC through the TMA store, no residual output, statistics or profiling ablation
-  const bool wide_ok = out_mode == 0 && !lo && !stats && ((flags >> 24) & 0xF) == 0 && ((flags >> 29) & 1) == 0;
+  // (the pre-activation form exists only for the one-warpgroup kernel)
+  const bool wide_ok = out_mode == 0 && !lo && !stats && !pre && ((flags >> 24) & 0xF) == 0 && ((flags >> 29) & 1) == 0;
   const int force_bn = (flags >> 8) & 0x3FF;
   const int force_mt = (flags >> 20) & 0x3;
   const int force_pair = (flags >> 22) & 0x3;      // 0 = auto, 1 = single-CTA tiles (the only form), 2 = CTA pair (not on sm_90)
@@ -1352,7 +1441,7 @@ int conv_choice(int batch, int height, int width, int cin, int cout, int ksize, 
   YB_REQUIRE(out != nullptr && batch > 0 && height > 0 && width > 0 && cin % 32 == 0 && cout > 0 && (ksize == 1 || ksize == 3),
              "conv_choice: bad shape");
   ConvChoice c;
-  const int rc = conv_choose(batch, height, width, cin, cout, ksize, cin, out_mode, flags, with_workspace != 0, false, false, &c);
+  const int rc = conv_choose(batch, height, width, cin, cout, ksize, cin, out_mode, flags, with_workspace != 0, false, false, false, &c);
   if (rc) return rc;
   out[0] = c.kernel; out[1] = c.bk; out[2] = c.bn; out[3] = c.kernel == kKernelC32 ? C32Cfg::TH * C32Cfg::TW : BM * c.mt;
   out[4] = c.streamk; out[5] = c.grid;
@@ -1361,8 +1450,19 @@ int conv_choice(int batch, int height, int width, int cin, int cout, int ksize, 
 
 int conv_igemm_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                        int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
-                       int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off, cudaStream_t stream) {
+                       int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off,
+                       const float* pre_scale, const float* pre_shift, int pre_relu, cudaStream_t stream) {
   YB_REQUIRE(x && w && scale && shift && y, "conv: null pointer");
+  // pre-activation form (pre_scale != NULL): 1x1, plain fp16 operands, no statistics
+  const bool pre = pre_scale != nullptr;
+  if (pre) {
+    YB_REQUIRE(pre_shift != nullptr && (pre_relu == 0 || pre_relu == 1), "conv_preact: pre_shift must be given, pre_relu 0 or 1");
+    YB_REQUIRE(ksize == 1, "conv_preact: k=%d, the pre-activation form is 1x1 only", ksize);
+    YB_REQUIRE(a_channels <= 0 || a_channels == cin, "conv_preact: split-precision operands are not supported");
+    YB_REQUIRE(lo_ch_off < 0 && stats == nullptr, "conv_preact: no residual output and no fused statistics");
+    YB_REQUIRE(cin <= kPreMaxCh, "conv_preact: Cin=%d exceeds the %d-channel pre-activation table", cin, kPreMaxCh);
+  }
+  const PreAct pre_act{pre_scale, pre_shift, pre_relu};
   // split-precision operands (see ConvParams::a_wrap): cin is the concatenated reduction width, a_channels what x really holds
   if (a_channels <= 0) a_channels = cin;
   YB_REQUIRE(a_channels <= cin && a_channels % 32 == 0 && cin - a_channels <= a_channels, "conv: a_channels=%d does not fit cin=%d", a_channels, cin);
@@ -1384,15 +1484,16 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
   // stream-K needs the caller's workspace (one per stream: partial sums + flags)
   const bool ws_ok = workspace != nullptr && workspace_bytes >= conv_workspace_bytes() && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0;
   ConvChoice ch;
-  int rc = conv_choose(batch, height, width, cin, cout, ksize, a_channels, out_mode, flags, ws_ok, stats != nullptr, lo_ch_off >= 0, &ch);
+  int rc = conv_choose(batch, height, width, cin, cout, ksize, a_channels, out_mode, flags, ws_ok, stats != nullptr, lo_ch_off >= 0, pre, &ch);
   if (rc) return rc;
+  YB_REQUIRE(!pre || ch.kernel == kKernelIgemm, "conv_preact: no pre-activation form of kernel %d", ch.kernel);
   if (ch.kernel == kKernelC32)
     return conv_c32_forward(x, w, scale, shift, slope, y, batch, height, width, cout, x_ld, y_ld, y_ch_off, (flags >> 4) & 1, flags, stats, stream);
   const int bk = ch.bk, bn = ch.bn, mt = ch.mt, streamk = ch.streamk;
   // 1x1 layers read A as a plain [pixels, Cin] matrix (2-D tiled TMA: cheaper per instruction than im2col mode);
   // YB_CONV_1X1_IM2COL=1 switches back for A/B runs
   static const int k1x1_im2col = getenv("YB_CONV_1X1_IM2COL") ? atoi(getenv("YB_CONV_1X1_IM2COL")) : 0;
-  const int a_im2col = (ksize == 3) ? 1 : ((k1x1_im2col && !(flags & 1)) ? 1 : 0);
+  const int a_im2col = (ksize == 3) ? 1 : ((k1x1_im2col && !(flags & 1) && !pre) ? 1 : 0);
 
   EncodeTiledFn enc_tiled;
   EncodeIm2colFn enc_im2col;
@@ -1485,8 +1586,8 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
   }
-  if (bk == 64) return dispatch_conv<64>(bn, mt, ch.grid, ta, tb, ty, p, stream);
-  return dispatch_conv<32>(bn, mt, ch.grid, ta, tb, ty, p, stream);
+  if (bk == 64) return dispatch_conv<64>(bn, mt, ch.grid, ta, tb, ty, p, pre ? &pre_act : nullptr, stream);
+  return dispatch_conv<32>(bn, mt, ch.grid, ta, tb, ty, p, pre ? &pre_act : nullptr, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -8,6 +8,7 @@
 //   add_relu    out += residual; relu (:58-59, :100-101); residual_bwd is the gradient at a block boundary.
 // The 3x3 / 1x1 convs themselves (with folded BN and ReLU or identity) are yb_conv_bn_act_fwd.
 #include "yb_common.h"
+#include "yb_pool.cuh"
 #include <cuda_fp16.h>
 #include <stdint.h>
 
@@ -151,16 +152,6 @@ int stem7x7_wgrad(const float* x, const void* dz, float* dw, int batch, int heig
   return check_launch("stem7x7_wgrad_kernel");
 }
 
-__device__ __forceinline__ uint4 hmax8_(uint4 a, uint4 b) {
-  uint4 r;
-  const __half2* pa = reinterpret_cast<const __half2*>(&a);
-  const __half2* pb = reinterpret_cast<const __half2*>(&b);
-  __half2* pr = reinterpret_cast<__half2*>(&r);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) pr[i] = __hmax2(pa[i], pb[i]);
-  return r;
-}
-
 // nn.MaxPool2d(kernel_size=3, stride=2, padding=1): out[oy, ox] = max over the in-range pixels of rows 2oy-1..2oy+1, columns 2ox-1..2ox+1
 __global__ void maxpool3x3_s2_kernel(const __half* __restrict__ x, __half* __restrict__ y, int batch, int height, int width, int channels) {
   const int c8 = channels >> 3;
@@ -173,21 +164,7 @@ __global__ void maxpool3x3_s2_kernel(const __half* __restrict__ x, __half* __res
   const int px = static_cast<int>(t % ow); t /= ow;
   const int py = static_cast<int>(t % oh);
   const long long img = t / oh;
-  bool any = false;
-  uint4 m = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-  for (int r = 0; r < 3; ++r) {
-    const int iy = 2 * py - 1 + r;
-    if (iy < 0 || iy >= height) continue;
-#pragma unroll
-    for (int s = 0; s < 3; ++s) {
-      const int ix = 2 * px - 1 + s;
-      if (ix < 0 || ix >= width) continue;
-      const uint4 v = __ldg(reinterpret_cast<const uint4*>(x + ((img * height + iy) * width + ix) * channels + cg * 8));
-      m = any ? hmax8_(m, v) : v;
-      any = true;
-    }
-  }
+  const uint4 m = maxpool3x3_s2_window(x, img, py, px, cg, height, width, channels);
   reinterpret_cast<uint4*>(y)[idx] = m;
 }
 
