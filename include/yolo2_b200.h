@@ -143,7 +143,9 @@ int yb_reorg_f32_nchw(const float* x, float* y, int batch, int channels, int hei
 /* ---- head: model.Inference.forward (model/__init__.py:117-135) + F.softmax (detect.py:152) ---- */
 /* feature fp32 [B, A*(5+C), rows, cols]; anchors fp32 [A,2] (height,width).  Outputs: iou [B,cells,A],
  * center_offset/size_norm/yx_min/yx_max [B,cells,A,2], logits/prob [B,cells,A,C] (prob may be NULL;
- * logits may be NULL when num_cls == 1). */
+ * logits may be NULL when num_cls == 1).  Cell k of the grid decodes at (k / rows, k % rows), the reference's meshgrid
+ * (model/__init__.py:53-56), which is the (row, col) grid only when rows == cols.  Limits, refused with an error before any launch:
+ * the shared-memory slab A*(5+C) * 33 floats must fit 200 KB (A*(5+C) <= 1551 channels); batch <= 65535. */
 int yb_decode_fwd(const float* feature, const float* anchors_hw, float* iou, float* center_offset, float* size_norm, float* yx_min,
                   float* yx_max, float* logits, float* prob, int batch, int rows, int cols, int num_anchors, int num_cls,
                   yb_stream_t stream);
@@ -157,7 +159,11 @@ int yb_decode_fwd(const float* feature, const float* anchors_hw, float* iou, flo
  * iou*prob > threshold_cls in mask.nonzero() order: det_keep (rank in the keep list), det_cls,
  * det_score, each [B,det_cap]; n_det[B].  Optional (NULL to skip): filt_box[B,n] = input box of each
  * filtered rank (ascending, the order detect.filter_visible returns), best_cls/best_prob[B,n] =
- * torch.max(prob, -1) per input box (detect.py:52). */
+ * torch.max(prob, -1) per input box (detect.py:52).
+ * Limits, refused with an error before any launch: n <= 16384 boxes per image; limit <= 1024; the scratch of one image,
+ * 12 * n_pad + limit * (28 + 4 * ceil(limit / 32)) + 64 bytes with n_pad = the power of two >= max(n, limit + 1, 32), must fit 220 KB
+ * of shared memory (so n = 16384 runs with limit <= 200 but not with limit = 1024).  When det_cap is smaller than the number of
+ * (box, class) pairs, n_det == det_cap and the arrays hold the first det_cap pairs; nothing is written past det_cap. */
 int yb_filter_nms(const float* score, const float* yx_min, const float* yx_max, const float* prob, int batch, int n, int num_cls,
                   int mode, float threshold, float threshold_cls, float overlap, int limit, int* n_filtered, int* n_keep,
                   int* keep_idx, int* keep_box, int* n_det, int* det_keep, int* det_cls, float* det_score, int det_cap,
@@ -172,7 +178,12 @@ int yb_iou_matrix(const float* yx_min1, const float* yx_max1, const float* yx_mi
  * Outputs: losses[5] = (foreground, background, center, size, cls), each already / (B*cells*A); positive /
  * negative uint8 [B,cells,A]; best_iou [B,cells,A]; and the UNWEIGHTED per-term gradients w.r.t. feature
  * (grad_terms: feature layout, grad_bg [B,A,cells]) consumed by yb_region_loss_bwd.  pos_count[B] and
- * partial[B*5] are scratch.  cross_entropy: train/cross_entropy (config.ini:77). */
+ * partial[B*5] are scratch.  cross_entropy: train/cross_entropy (config.ini:77).
+ * Limit, refused with an error before any launch: G <= 128 ground-truth slots per image.  The predicted boxes sit on the
+ * reference's meshgrid (cell k at (k / rows, k % rows)) while positives are marked at the true cell i * cols + j, exactly as the
+ * reference does at rows != cols.  A ground truth whose centre lies outside the grid marks nothing; class ids outside [0, C) are
+ * clamped into range; with no positive in the batch the class term and its gradient are 0 (the reference's mean over zero rows
+ * is NaN); pos_count[b] is the number of positive (cell, anchor) pairs of image b. */
 int yb_region_loss_fwd(const float* feature, const float* anchors_hw, const float* gt_yx_min, const float* gt_yx_max,
                        const long long* gt_cls, int batch, int rows, int cols, int num_anchors, int num_cls, int num_gt, float threshold,
                        int cross_entropy, float* losses, unsigned char* positive, unsigned char* negative, float* best_iou, int* pos_count,
@@ -297,7 +308,9 @@ int yb_photometric_batch_u8(const void* src, void* dst, int batch, int height, i
  * Segmented batch: image i owns detections [det_off[i], det_off[i+1]) (descending score within the image, as postprocess returns
  * them) and ground-truth boxes [gt_off[i], gt_off[i+1]); boxes are (y, x) float pairs, classes int32.  tp[d] = 1 iff detection d's
  * best-IoU ground truth of its own class (ties: lowest index) has IoU > threshold and was not claimed by an earlier detection of
- * the image.  IoU uses the reference's operation order (utils/iou/torch.py:24-61) with min_union = float32 eps. */
+ * the image.  IoU uses the reference's operation order (utils/iou/torch.py:24-61) with min_union = float32 eps.
+ * Limit, refused with an error before any launch: max_gt (the largest ground-truth count of one image) <= 1024.  Detections whose
+ * class is outside [0, num_cls) are not written: pass tp zero-filled. */
 int yb_eval_match(const float* det_yx_min, const float* det_yx_max, const int* det_cls, const int* det_off, const float* gt_yx_min,
                   const float* gt_yx_max, const int* gt_cls, const int* gt_off, int batch, int num_cls, int max_gt, float threshold, float min_union,
                   unsigned char* tp, yb_stream_t stream);

@@ -438,10 +438,79 @@ def synth_images(batch, height=416, width=416, seed=0):
     return torch.rand(batch, 3, height, width, generator=g)
 
 
-def synth_feature(batch, size, seed):
-    """Head feature map [B, 125, S, S] the region-loss fixtures start from (tests/golden/make_golden_loss.py), regenerated from its seed."""
+def synth_feature(batch, size, seed, channels=125, cols=None):
+    """Head feature map [B, channels, size, cols or size] the region-loss fixtures start from (tests/golden/make_golden_loss.py,
+    make_golden_head.py), regenerated from its seed."""
     g = torch.Generator().manual_seed(100 + seed)
-    return torch.randn(batch, 125, size, size, generator=g) * 1.5
+    return torch.randn(batch, channels, size, size if cols is None else cols, generator=g) * 1.5
+
+
+def synth_anchors(num_anchors):
+    """[A,2] (height, width) anchors: yolo-voc's five, or for any other count a ladder of distinct aspect ratios."""
+    if num_anchors == 5:
+        return anchors_yolo_voc()
+    k = torch.arange(num_anchors, dtype=torch.float32)
+    return torch.stack([1.0 + 1.75 * k, 0.75 + 1.25 * k + (k % 2) * 1.5], 1)
+
+
+# Cases of tests/golden/head.npz (the head and tail executed by the reference off the square 20-class 5-anchor family):
+# tag -> rows, cols, anchors, classes, batch, ground-truth slots, seed, one-hot class branch, empty images
+# ('one': image 1 has only padding slots, 'all': no image has a ground-truth box).
+HEAD_CASES = dict(
+    wide=dict(rows=10, cols=19, a=5, c=20, batch=2, slots=12, seed=40),
+    tall=dict(rows=19, cols=10, a=5, c=20, batch=2, slots=12, seed=41, one_hot=True),
+    strip_h=dict(rows=1, cols=13, a=5, c=20, batch=2, slots=4, seed=42),
+    strip_v=dict(rows=13, cols=1, a=5, c=20, batch=2, slots=4, seed=43),
+    coco=dict(rows=13, cols=13, a=5, c=80, batch=1, slots=16, seed=44),
+    c3a3=dict(rows=13, cols=17, a=3, c=3, batch=2, slots=8, seed=45),
+    c1a9=dict(rows=11, cols=13, a=9, c=1, batch=2, slots=8, seed=46),
+    nopos_one=dict(rows=13, cols=13, a=5, c=20, batch=3, slots=6, seed=47, empty='one'),
+    nopos_all=dict(rows=13, cols=13, a=5, c=20, batch=2, slots=6, seed=48, empty='all'),
+)
+
+
+def head_case_inputs(tag):
+    """(feature [B, A*(5+C), rows, cols], anchors [A,2], data in grid units) of one HEAD_CASES entry, from its seed."""
+    k = HEAD_CASES[tag]
+    rows, cols, a, c = k['rows'], k['cols'], k['a'], k['c']
+    channels = a * (5 + c) if c > 1 else a * 5
+    feature = synth_feature(k['batch'], rows, k['seed'], channels, cols)
+    height, width = rows * 32, cols * 32
+    tgt = synth_targets(k['batch'], height, width, slots=k['slots'], num_cls=c, seed=20 + k['seed'])
+    empty = k.get('empty')
+    if empty:
+        for key in tgt:
+            if empty == 'all':
+                tgt[key].zero_()
+            else:
+                tgt[key][1].zero_()
+    return feature, synth_anchors(a), norm_data(tgt, height, width, rows, cols)
+
+
+def synth_detections(n, num_cls, seed, extent=13.0):
+    """Post-filter input (iou [n], yx_min / yx_max [n,2], prob [n,C]) made with exactly rounded elementwise operations only, so
+    that every machine regenerates it bit for bit: boxes jittered around 24 cluster centres (so NMS suppresses), objectness
+    uniform, class scores a product of three uniforms (most are small, a few per box pass 0.005)."""
+    g = torch.Generator().manual_seed(seed)
+    centres = torch.rand(24, 2, generator=g) * extent
+    c = centres[torch.randint(0, 24, (n,), generator=g)] + (torch.rand(n, 2, generator=g) - 0.5) * 1.5
+    s = torch.rand(n, 2, generator=g) * (extent / 4) + 0.25
+    iou = torch.rand(n, generator=g)
+    if num_cls > 1:
+        prob = torch.rand(n, num_cls, generator=g) * torch.rand(n, num_cls, generator=g) * torch.rand(n, num_cls, generator=g)
+    else:
+        prob = torch.ones(n, 1)
+    return iou, c - s / 2, c + s / 2, prob
+
+
+def synth_lattice_boxes(n, seed, extent=6):
+    """NMS input on an integer lattice: corners and sizes are small integers, so coordinates repeat and many pairwise IoUs are
+    exactly 1/2, 1/4 or 1 in fp32 -- the `iou <= overlap` boundary is hit when overlap is one of those.  Distinct scores."""
+    g = torch.Generator().manual_seed(seed)
+    lo = torch.randint(0, extent, (n, 2), generator=g).float()
+    size = torch.randint(1, 4, (n, 2), generator=g).float()
+    score = (torch.randperm(n, generator=g).float() + 0.5) / n
+    return score, lo, lo + size
 
 
 # Fixture activations larger than SAMPLE_MIN_ELEMS are stored as a seeded sample of SAMPLE_FRACTION of their elements (name + '_sample'),
@@ -769,6 +838,25 @@ def synth_eval_case(seed, n_det=60, n_gt=12, num_cls=4, extent=13.0):
     det_cls = torch.where(torch.rand(n_det, generator=g) < 0.8, gt_cls[src], torch.randint(0, num_cls, (n_det,), generator=g))
     score = torch.sort(torch.rand(n_det, generator=g), descending=True)[0]
     return dict(gt_min=gt_min, gt_max=gt_max, gt_cls=gt_cls, det_min=det_min, det_max=det_max, det_cls=det_cls, score=score)
+
+
+# head.npz: post-filter, lattice-NMS and evaluation-matching cases (tests/golden/make_golden_head.py)
+HEAD_POST_MODES = dict(wide=(1,), tall=(1,), coco=(1, 0), c3a3=(1, 0), c1a9=(0,))     # detect/fix values run per case
+HEAD_NMS_CASES = dict(half=(300, 50, 0.5, 200), quarter=(300, 51, 0.25, 200), one=(120, 52, 1.0, 200), zero=(120, 53, 0.0, 200),
+                 limit33=(400, 54, 0.5, 33))                                     # tag -> n, seed, overlap, limit (lattice boxes)
+HEAD_EVAL_CASES = dict(c80=(60, 200, 40, 80, False), one_cls=(61, 120, 40, 80, True), dup=(62, 90, 24, 20, True))
+#                                                      tag -> seed, detections, ground truth, classes, all of one class + duplicated boxes
+
+
+def head_eval_case(tag):
+    seed, n_det, n_gt, num_cls, crowd = HEAD_EVAL_CASES[tag]
+    case = synth_eval_case(seed, n_det, n_gt, num_cls)
+    if crowd:                                        # > 32 boxes of one class, every other one a copy of its neighbour
+        case['gt_cls'] = torch.full_like(case['gt_cls'], 3)
+        case['det_cls'] = torch.full_like(case['det_cls'], 3)
+        case['gt_min'][1::2] = case['gt_min'][0::2]
+        case['gt_max'][1::2] = case['gt_max'][0::2]
+    return case, num_cls
 
 
 # ----------------------------------------------------------------------------------------------

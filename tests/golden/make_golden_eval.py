@@ -22,14 +22,20 @@ from oracle import yolo2_oracle as O  # noqa: E402
 REF = '/root/reference'
 
 
-def main():
-    model, utils, detect = G.import_reference()
+def reference_eval_fns(utils):
+    """The reference's four pure evaluation functions, extracted from eval.py and exec'd."""
     np.bool, np.float = bool, float                  # aliases removed in numpy >= 1.24, used at eval.py:59,73,111
     tree = ast.parse(open(os.path.join(REF, 'eval.py')).read())
     names = ('_matching', 'matching', 'voc_ap', 'average_precision')
     wanted = [n for n in tree.body if isinstance(n, ast.FunctionDef) and n.name in names]
     ns = dict(np=np, torch=torch, utils=utils)
     exec(compile(ast.Module(body=wanted, type_ignores=[]), os.path.join(REF, 'eval.py'), 'exec'), ns)
+    return ns
+
+
+def main():
+    model, utils, detect = G.import_reference()
+    ns = reference_eval_fns(utils)
     out = {}
     cases = [(1, 60, 12, 4), (2, 200, 40, 20), (3, 5, 1, 1), (4, 30, 0, 3), (5, 0, 6, 3)]
     all_tp, all_score, all_num = {}, {}, {}
