@@ -967,8 +967,8 @@ def test_training_per_layer_on_oracle_inputs(ops):
             inp = prev
         u = units[key]
         b, _, h, w = inp.shape
-        z = tr._raw_conv(u, inp.to(DEV).permute(0, 2, 3, 1).contiguous().half(), key=key)
-        mean, invstd = tr._bn_forward(key, u, z, b * h * w)
+        z, stats_done = tr._raw_conv(u, inp.to(DEV).permute(0, 2, 3, 1).contiguous().half(), key=key)
+        mean, invstd = tr._bn_forward(key, u, z, b * h * w, stats_done)
         a = tr._apply(u, z, mean, invstd, b, h, w, False)
         m_ref, v_ref = stats[key]
         e_m = ((mean.cpu() - m_ref).abs().max() / v_ref.sqrt().max()).item()          # mean error relative to the channel spread

@@ -1,4 +1,4 @@
-"""Training-mode forward and backward of the Darknet-19 backbone on the CUDA kernels.
+"""Training-mode forward and backward of the backbones (Darknet-19, Tiny, MobileNet, ResNet) on the CUDA kernels.
 
 What the reference gets from torch autograd over nn.Conv2d / BatchNorm2d(train) / LeakyReLU / MaxPool2d /
 reorg / cat (model/yolo2.py:49-65,125-130; train.py:344-351) is issued here as an explicit kernel chain:
@@ -12,6 +12,9 @@ reorg / cat (model/yolo2.py:49-65,125-130; train.py:344-351) is issued here as a
 Gradients travel in fp16 multiplied by `grad_scale` (static loss scaling; parameter gradients are un-scaled in fp32).
 BatchNorm statistics are per process (per GPU), exactly like the per-replica statistics of the reference's
 nn.DataParallel.
+
+`TrainerBase` holds everything that does not depend on a network's topology; each trainer class describes only its
+own: unit order, `grad_order()`, first layer or stem, joins, pools, reorg.
 """
 import os
 
@@ -72,23 +75,29 @@ class PackPlan(object):
         ops.call('yb_pack_weights_batch', self.table, self.count, self.blocks)
 
 
-class DarknetTrainer(object):
-    def __init__(self, engine, grad_scale=16384.0):
-        self.engine = engine
+class TrainerBase(object):
+    """What every training chain shares, whatever its topology: the step state (gradient arena, data-parallel reducer, overflow flag,
+    BatchNorm accumulators, weight-gradient stream), the forward and backward pieces of a conv + BatchNorm unit, the head's gradient, and
+    the start and end of a step.  A subclass names the network (`NAME`), lists its parameters in the order its backward produces their
+    gradients (`grad_order()`) and, to use the shared `_head_backward`, its head (`_head_unit()`)."""
+    NAME = 'network'
+
+    def __init__(self, dnn, grad_scale=16384.0, slope=SLOPE):
+        self.dnn = dnn
         self.grad_scale = float(grad_scale)
-        self.sums = {}       # per-unit double[2C] accumulators (self-cleaning)
-        self.wd_cache = {}   # dgrad weight buffers per unit (contents re-packed every step)
+        self.slope = slope       # negative slope of the activation (LeakyReLU(0.1) for the yolo2 backbones, 0 = ReLU for MobileNet / ResNet)
+        self.sums = {}           # per-unit double[2C] accumulators (self-cleaning)
+        self._ones_cache = {}    # fp32 (ones, zeros) per channel count and device: identity scale / shift of raw convs
+        self.wd_cache = {}       # dgrad weight buffers per unit (contents re-packed every step)
         # data parallel: b200.ddp.GradientAllReducer attached by train.iterate; every gradient kernel writes into the reducer-visible
         # arena and reports it (`_emit`) so the bucket's all-reduce starts while the rest of the backward chain is still running
-        self.slope = SLOPE     # negative slope of the activation (LeakyReLU(0.1) for the yolo2 backbones, 0 = ReLU for MobileNet)
         self.reducer = None
         self.arena = None
-        self.found_inf = None  # device float[1]: 1 when the last backward produced a non-finite gradient (then zeroed), see backward()
+        self.found_inf = None  # device float[1]: 1 when the last backward produced a non-finite gradient (then zeroed), see _finish_backward()
         self._arenas = {}      # one per (device, parameter set, reducer): CUDA graphs keep writing the arena they were captured with
         self._main = None
         # BN batch statistics in the conv epilogue (yb_conv_bn_act_stats_fwd) instead of yb_bn_stats; YB_FUSE_STATS=0 for A/B runs
         self.fuse_stats = os.environ.get('YB_FUSE_STATS', '1') != '0'
-        self._fused_stats = False
         # weight gradients on a second stream (overlap with the BatchNorm backward chain); YB_WGRAD_STREAM=0 for A/B runs
         self.wgrad_stream = os.environ.get('YB_WGRAD_STREAM', '1') != '0'
         self._side_streams = {}
@@ -96,13 +105,90 @@ class DarknetTrainer(object):
         self._pack_plan = None
         self._tracked = []
 
+    # ---- step state ----------------------------------------------------------------------------------
+    def _start_forward(self, x):
+        """Start of a training step: no BatchNorm counted yet; returns the image as contiguous fp32."""
+        self._tracked = []
+        if not x.is_cuda:
+            raise RuntimeError('%s training: input must be a CUDA tensor' % self.NAME)
+        return x.contiguous().float()
+
     def _bump_tracked(self):
         """`num_batches_tracked += 1` of every BatchNorm of the step as ONE multi-tensor kernel instead of one tiny launch per layer."""
         if self._tracked:
             torch._foreach_add_(self._tracked, 1)
             self._tracked = []
 
-    # ---- helpers -------------------------------------------------------------------------------------
+    def _start_backward(self, dev):
+        """Start of the backward chain: the gradient arena of this parameter set, and the stream the chain runs on."""
+        self._ensure_arena(self.dnn, dev)
+        self._main = torch.cuda.current_stream(dev)
+
+    def _finish_backward(self, dev):
+        """End of the backward chain: the main stream waits for the weight-gradient stream and for every bucket's all-reduce (no host
+        wait), then the fp16 gradient overflow guard runs (after the exchange, so every rank takes the same decision): `found_inf` is raised
+        and the gradients are zeroed instead of poisoning the optimizer state; train.iterate hands the flag to optimizers that can skip."""
+        self._join(dev)
+        if self.reducer is not None:
+            self.reducer.finish()
+        if self.found_inf is None or self.found_inf.device != dev:
+            self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)      # 0-dim like GradScaler's (fused optimizers subtract it from their step counters)
+        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+
+    def _ensure_arena(self, dnn, device):
+        """Persistent flat fp32 gradient buffer (b200.ddp.GradArena) for the parameters of `dnn` (the trainer's module): gradient
+        kernels write straight into their slots, `.grad` of every parameter is a view of it, buckets of it are all-reduced in place."""
+        params = dict(dnn.named_parameters())
+        key = (str(device), tuple((n, tuple(p.shape)) for n, p in params.items()), id(self.reducer))
+        self.arena = self._arenas.get(key)
+        if self.arena is None:
+            order = [n for n in self.grad_order() if n in params]
+            if set(order) != set(params):
+                raise RuntimeError('%s trainer: unexpected parameter set %s' % (self.NAME, sorted(set(params) ^ set(order))[:4]))
+            bucket_bytes = self.reducer.bucket_bytes if self.reducer is not None else (32 << 20)
+            self.arena = self._arenas[key] = _ddp.GradArena([(n, tuple(params[n].shape)) for n in order], device, bucket_bytes)
+            if self.reducer is not None:
+                self.reducer.attach(self.arena)
+        return self.arena
+
+    def _emit(self, name, grads):
+        if self.reducer is not None:
+            dev = grads[name].device
+            side = self._side_streams.get(dev) if self._side_busy else None
+            self.reducer.on_grad(name, grads[name], streams=(self._main, side))
+
+    @property
+    def _unscale(self):
+        """Inverse loss scale, with the 1 / world of the data-parallel gradient average folded in."""
+        return 1.0 / (self.grad_scale * (self.reducer.grad_divisor if self.reducer is not None else 1.0))
+
+    def _pack(self, entries, device):
+        """Forward and data-gradient fp16 operands of the units `entries` = [(key, unit, cout_pad)] in ONE batched launch (PackPlan); the
+        plan is rebuilt when a weight moved."""
+        plan = self._pack_plan
+        if plan is None or plan.key != tuple(u.conv.weight.data_ptr() for _, u, _ in entries) or plan.table.device != device:
+            plan = self._pack_plan = PackPlan([(key, u.conv.weight.detach(), True, True, cp) for key, u, cp in entries], device)
+        plan.run()
+        for key, u, _ in entries:
+            u.w16 = plan.fwd[key]
+            self.wd_cache[key] = plan.dgrad[key]
+
+    def _sums(self, key, channels, device):
+        t = self.sums.get(key)
+        if t is None or t.numel() != 2 * channels or t.device != device:
+            t = torch.zeros(2 * channels, dtype=torch.float64, device=device)
+            self.sums[key] = t
+        return t
+
+    def _ones(self, c, device):
+        key = (c, str(device))
+        t = self._ones_cache.get(key)
+        if t is None:
+            t = (torch.ones(c, dtype=torch.float32, device=device), torch.zeros(c, dtype=torch.float32, device=device))
+            self._ones_cache[key] = t
+        return t
+
+    # ---- unit helpers --------------------------------------------------------------------------------
     def _slope(self, u):
         """Activation slope of a unit's train-mode BatchNorm + activation: its own `train_slope` (ResNet units: 0 = ReLU, 1 = identity),
         else the trainer's."""
@@ -113,104 +199,37 @@ class DarknetTrainer(object):
         """State-dict names of a unit's (conv weight, BN weight, BN bias): `key.conv.weight`, `key.bn.*` unless the unit carries `pnames`."""
         return getattr(u, 'pnames', None) or (key + '.conv.weight', key + '.bn.weight', key + '.bn.bias')
 
-    def _emit(self, name, grads):
-        if self.reducer is not None:
-            dev = grads[name].device
-            side = self._side_streams.get(dev) if self._side_busy else None
-            self.reducer.on_grad(name, grads[name], streams=(self._main, side))
+    @staticmethod
+    def _saved_unit(u, ain, z, mean, invstd, hh, ww, pooled=False, **extra):
+        """What the backward of a unit reads: the unit, its input activation (None: the image), z and the batch statistics, the output
+        size and whether the output is max-pooled, plus whatever the topology needs (`extra`)."""
+        s = _Saved()
+        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w, s.pooled = u, ain, z, mean, invstd, hh, ww, pooled
+        s.__dict__.update(extra)
+        return s
 
-    def grad_order(self):
-        """State-dict names of all parameters in the order the backward chain produces their gradients."""
-        eng = self.engine
-        names = ['layers3.1.conv.bias', 'layers3.1.conv.weight']
-        for key in ['layers3.0'] + list(reversed(eng._k2)) + ['passthrough'] + list(reversed(eng._k1)):
-            names += [key + '.bn.weight', key + '.bn.bias', key + '.conv.weight']
-        return names
-
-    def _ensure_arena(self, dnn, device):
-        """Persistent flat fp32 gradient buffer (b200.ddp.GradArena): gradient kernels write straight into their slots, `.grad`
-        of every parameter is a view of it, buckets of it are all-reduced in place."""
-        params = dict(dnn.named_parameters())
-        key = (str(device), tuple((n, tuple(p.shape)) for n, p in params.items()), id(self.reducer))
-        self.arena = self._arenas.get(key)
-        if self.arena is None:
-            order = [n for n in self.grad_order() if n in params]
-            if set(order) != set(params):
-                raise RuntimeError('Darknet trainer: unexpected parameter set %s' % sorted(set(params) ^ set(order))[:4])
-            bucket_bytes = self.reducer.bucket_bytes if self.reducer is not None else (32 << 20)
-            self.arena = self._arenas[key] = _ddp.GradArena([(n, tuple(params[n].shape)) for n in order], device, bucket_bytes)
-            if self.reducer is not None:
-                self.reducer.attach(self.arena)
-        return self.arena
-
-    @property
-    def _unscale(self):
-        """Inverse loss scale, with the 1 / world of the data-parallel gradient average folded in."""
-        return 1.0 / (self.grad_scale * (self.reducer.grad_divisor if self.reducer is not None else 1.0))
-
-    def _repack(self, device):
-        """All kernel operands that depend on the parameters, re-derived for this step: one batched pack launch for the fp16 weight
-        operands (forward + data gradient); the first layer reads its fp32 weights and the head its fp32 bias in place.  The eval-mode
-        BatchNorm fold is NOT refreshed here (training uses batch statistics); `Darknet.train(False)` invalidates it."""
-        eng = self.engine
-        units, keys = eng.all_units(), eng.unit_keys()
-        ptrs = tuple(u.conv.weight.data_ptr() for u in units[1:])
-        plan = self._pack_plan
-        if plan is None or plan.key != ptrs or plan.table.device != device:
-            entries = []
-            for u, key in zip(units[1:], keys[1:]):
-                cpad = (u.cout + 31) // 32 * 32 if u.bn is None else 0          # the head's filters are padded to the dz buffer's width
-                entries.append((key, u.conv.weight.detach(), True, True, cpad))
-            plan = self._pack_plan = PackPlan(entries, device)
-        plan.run()
-        units[0].w16 = units[0].conv.weight.detach().contiguous()
-        for u, key in zip(units[1:], keys[1:]):
-            u.w16 = plan.fwd[key]
-            u._wver = None                      # the eval path re-checks (and may re-pack into its own buffer)
-            self.wd_cache[key] = plan.dgrad[key]
-        head = units[-1]
-        if head.bn is None:
-            one, _ = self._ones(head.cout, device)
-            head.scale = one
-            head.shift = head.conv.bias.detach() if head.conv.bias is not None else self._ones(head.cout, device)[1]
-            head._bver = None
-
-    def _sums(self, key, channels, device):
-        t = self.sums.get(key)
-        if t is None or t.numel() != 2 * channels or t.device != device:
-            t = torch.zeros(2 * channels, dtype=torch.float64, device=device)
-            self.sums[key] = t
-        return t
-
-    def _ones(self, c, device):
-        key = ('ones', c, str(device))
-        t = self.sums.get(key)
-        if t is None:
-            t = (torch.ones(c, dtype=torch.float32, device=device), torch.zeros(c, dtype=torch.float32, device=device))
-            self.sums[key] = t
-        return t
-
-    def _raw_conv(self, u, src, out=None, key=None, **kw):
-        """Raw conv output z.  With `key` (a BN unit of the generic kernel) the batch statistics are accumulated in the
-        conv epilogue into the unit's double accumulators, so `_bn_forward` does not read z again."""
+    # ---- forward -------------------------------------------------------------------------------------
+    def _raw_conv(self, u, src, key=None):
+        """Raw conv output z, and whether its batch statistics were accumulated.  With `key` (a BN unit of the generic kernel) they are
+        accumulated in the conv epilogue into the unit's double accumulators when the shape allows, so `_bn_forward` does not read z
+        again.  Returns (z, stats_done)."""
         one, zero = self._ones(u.cout, src.device)
-        self._fused_stats = False
         c32 = u.cin == 32 and u.ksize == 3 and u.cout <= 64          # the halo-tile kernel: fused statistics need exact 16 x 8 tiling
         if key is not None and self.fuse_stats and not (c32 and (src.shape[1] % 16 or src.shape[2] % 8)):
-            self._fused_stats = True
-            return ops.conv_bn_act_stats(src, u.w16, one, zero, 1.0, self._sums(('f', key), u.cout, src.device), out=out)
-        return ops.conv_bn_act(src, u.w16, one, zero, 1.0, out=out, **kw)
+            return ops.conv_bn_act_stats(src, u.w16, one, zero, 1.0, self._sums(('f', key), u.cout, src.device)), True
+        return ops.conv_bn_act(src, u.w16, one, zero, 1.0), False
 
-    def _bn_forward(self, key, u, z, rows):
+    def _bn_forward(self, key, u, z, rows, stats_done):
+        """Batch statistics of z (accumulated here by yb_bn_stats unless the conv that wrote z already did: `stats_done`) -> mean, invstd and
+        the running-statistics update."""
         bn = u.bn
         c = u.cout
         dev = z.device
         sums = self._sums(('f', key), c, dev)
         mean = torch.empty(c, dtype=torch.float32, device=dev)
         invstd = torch.empty(c, dtype=torch.float32, device=dev)
-        if not getattr(self, '_fused_stats', False):
+        if not stats_done:
             ops.call('yb_bn_stats', z, z.shape[-1], rows, c, sums)
-        self._fused_stats = False
         ops.call('yb_bn_finalize', sums, rows, c, float(bn.eps), float(bn.momentum), bn.running_mean, bn.running_var, mean, invstd)
         if bn.num_batches_tracked is not None:
             self._tracked.append(bn.num_batches_tracked)      # incremented together at the end of the forward pass (_bump_tracked)
@@ -225,11 +244,165 @@ class DarknetTrainer(object):
                  b, h, w, c, int(pool))
         return out
 
-    @staticmethod
-    def _saved_unit(u, ain, z, mean, invstd, hh, ww, pooled):
-        s = _Saved()
-        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w, s.pooled = u, ain, z, mean, invstd, hh, ww, pooled
-        return s
+    # ---- backward ------------------------------------------------------------------------------------
+    def _bn_act_backward(self, key, s, b, da=None, da_off=0, dap=None, dap_off=0, dz=None):
+        """BatchNorm + activation (+ 2x2 max-pool) backward of a saved unit from the gradient of its output: `da` unpooled (read at channel
+        `da_off`), `dap` through the unit's max-pool (at channel `dap_off`).  The reduce pass accumulates into the unit's double
+        accumulators; with `dz` the apply pass then writes the gradient of z.  Returns the accumulators."""
+        u = s.u
+        sums = self._sums(('b', key), u.cout, s.z.device)
+        args = (s.z, s.z.shape[-1], s.mean, s.invstd, u.bn.weight.detach(), u.bn.bias.detach(), self._slope(u), da, 0 if da is None else da.shape[-1],
+                da_off, dap, 0 if dap is None else dap.shape[-1], dap_off, b, s.h, s.w, u.cout, int(dap is not None), sums)
+        ops.call('yb_bn_act_bwd', 0, *args, None, 0, 1)
+        if dz is not None:
+            ops.call('yb_bn_act_bwd', 1, *args, dz, dz.shape[-1], 1)
+        return sums
+
+    def _bn_param_grad(self, key, u, sums, grads):
+        """dgamma, dbeta of a unit from its backward accumulators into the arena (un-scaled, / world), then the accumulators are cleared."""
+        _, gname, bname = self._pnames(key, u)
+        dgamma, dbeta = self.arena.views[gname], self.arena.views[bname]
+        ops.call('yb_bn_param_grad', sums, u.cout, dgamma, dbeta, 1, self._unscale)
+        grads[gname], grads[bname] = dgamma, dbeta
+        self._emit(gname, grads)
+        self._emit(bname, grads)
+
+    def _bn_backward(self, key, s, b, grads, dz, da=None, da_off=0, dap=None, dap_off=0):
+        """Both passes of the BatchNorm + activation backward into dz, then dgamma and dbeta."""
+        self._bn_param_grad(key, s.u, self._bn_act_backward(key, s, b, da, da_off, dap, dap_off, dz), grads)
+
+    def _wd(self, key, u, cout_pad=0):
+        """Data-gradient operand of a unit (rotated, transposed fp16 weights), re-packed every step into a reused buffer."""
+        w = u.conv.weight
+        cout, cin, k, _ = w.shape
+        cp = max(cout, cout_pad)
+        wd = self.wd_cache.get(key)
+        plan = self._pack_plan
+        if plan is not None and wd is not None and plan.dgrad.get(key) is wd and wd.shape == (cin, k, k, cp):
+            return wd                         # packed by this step's batched launch (_pack)
+        if wd is None or wd.shape != (cin, k, k, cp) or wd.device != w.device:
+            wd = torch.empty(cin, k, k, cp, dtype=torch.float16, device=w.device)
+            self.wd_cache[key] = wd
+        ops.call('yb_pack_weight_dgrad_f16', w.detach().contiguous(), wd, cout, cin, k, cp)
+        return wd
+
+    def _dgrad(self, key, u, dz, cout_pad=0):
+        """Gradient at a unit's input: the forward conv kernel on dz with the unit's data-gradient operand."""
+        one, zero = self._ones(u.cin, dz.device)
+        return ops.conv_bn_act(dz, self._wd(key, u, cout_pad), one, zero, 1.0)
+
+    def _wgrad(self, u, ain, dz, b, hh, ww, grads, name):
+        """Weight gradient of one unit.  It depends only on (ain, dz) and nothing downstream depends on it before the
+        optimizer, so it is issued on a second stream: the tensor-bound wgrad kernel then overlaps the HBM-bound
+        BatchNorm backward of the next unit (and its data gradient) instead of queueing in front of them.  The fork /
+        join is plain stream-event ordering, so it is captured as parallel branches of the step's CUDA graph."""
+        cout, cin, k = u.cout, u.cin, u.ksize
+        dev = dz.device
+        side = self._side(dev)
+        if side is not None:
+            main = torch.cuda.current_stream(dev)
+            try:
+                fork = torch.cuda.Event()
+                fork.record(main)
+                side.wait_event(fork)
+            except Exception as ex:
+                raise RuntimeError('weight-gradient fork for %s failed (main %r, side %r): %s' % (name, main, side, ex)) from ex
+            dz.record_stream(side)          # dz / ain are main-stream allocations still read by the side stream
+            ain.record_stream(side)
+            self._side_busy = True
+        with torch.cuda.stream(side) if side is not None else _NullCtx():
+            dw_krsc = torch.empty(cout, k, k, cin, dtype=torch.float32, device=dev)
+            ops.call('yb_conv_wgrad', ain, dz, dw_krsc, b, hh, ww, cin, cout, k, ain.shape[-1], dz.shape[-1])
+            wname = self._pnames(name, u)[0]
+            dw = self.arena.views[wname]                                                     # [cout, cin, k, k] slot of the gradient arena
+            ops.call('yb_unpack_wgrad', dw_krsc, dw, cout, cin, k, self._unscale)            # layout change + inverse loss scale (/ world)
+            grads[wname] = dw
+            self._emit(wname, grads)
+
+    def _side(self, dev):
+        # only while the step is being captured into a CUDA graph: in eager mode the step is host-bound and the extra
+        # event / stream bookkeeping costs more (measured +2.6 ms) than the overlap gains (0.1 ms)
+        if not self.wgrad_stream or not torch.cuda.is_current_stream_capturing():
+            return None
+        st = self._side_streams.get(dev)
+        if st is None:
+            st = torch.cuda.Stream(device=dev)
+            self._side_streams[dev] = st
+        return st
+
+    def _join(self, dev):
+        """Main stream waits for everything issued on the wgrad stream (end of backward: the optimizer reads the grads)."""
+        if self._side_busy:
+            torch.cuda.current_stream(dev).wait_stream(self._side_streams[dev])
+            self._side_busy = False
+
+    def _unit_backward(self, key, s, b, grads, da=None, da_off=0, dap=None, dap_off=0):
+        """Backward of one BN unit; returns the gradient w.r.t. the unit's input activation, or dz when the unit reads the image."""
+        u = s.u
+        dz = torch.empty(b, s.h, s.w, u.cout, dtype=torch.float16, device=s.z.device)
+        self._bn_backward(key, s, b, grads, dz, da, da_off, dap, dap_off)
+        if s.ain is None:
+            return dz
+        self._wgrad(u, s.ain, dz, b, s.h, s.w, grads, key)
+        return self._dgrad(key, u, dz)
+
+    def _head_grad(self, bias, chead, a_last, hh, ww, dfeature, grads):
+        """Head (1x1 conv with bias) from dfeature, the fp32 NCHW gradient of the loss w.r.t. its output: the bias gradient from the unscaled
+        fp32 gradient, and dz scaled into fp16 and padded to a multiple of 32 channels (returned)."""
+        b, dev = a_last.shape[0], a_last.device
+        cpad = (chead + 31) // 32 * 32
+        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
+        dbias = self.arena.views[bias]
+        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
+        grads[bias] = dbias.mul_(self._unscale)
+        self._emit(bias, grads)
+        return dzh
+
+    def _head_backward(self, a_last, hh, ww, dfeature, grads):
+        """Head: bias gradient and padded dz (`_head_grad`), weight gradient, and the data gradient at the head's input."""
+        key, u, bias = self._head_unit()
+        dzh = self._head_grad(bias, u.cout, a_last, hh, ww, dfeature, grads)
+        self._wgrad(u, a_last, dzh, a_last.shape[0], hh, ww, grads, key)
+        return self._dgrad(key, u, dzh, dzh.shape[-1])
+
+
+class DarknetTrainer(TrainerBase):
+    """Training-mode forward / backward of `model.yolo2.Darknet` (Darknet-19 with the passthrough, reorg and concat) on the units of its
+    inference engine (`dnn.engine`)."""
+    NAME = 'Darknet'
+
+    @property
+    def engine(self):
+        return self.dnn.engine
+
+    def grad_order(self):
+        """State-dict names of all parameters in the order the backward chain produces their gradients."""
+        eng = self.engine
+        names = ['layers3.1.conv.bias', 'layers3.1.conv.weight']
+        for key in ['layers3.0'] + list(reversed(eng._k2)) + ['passthrough'] + list(reversed(eng._k1)):
+            names += [key + '.bn.weight', key + '.bn.bias', key + '.conv.weight']
+        return names
+
+    def _head_unit(self):
+        return 'layers3.1', self.engine.units3[1], 'layers3.1.conv.bias'
+
+    def _repack(self, device):
+        """All kernel operands that depend on the parameters, re-derived for this step: one batched pack launch for the fp16 weight
+        operands (forward + data gradient); the first layer reads its fp32 weights and the head its fp32 bias in place.  The eval-mode
+        BatchNorm fold is NOT refreshed here (training uses batch statistics); `Darknet.train(False)` invalidates it."""
+        eng = self.engine
+        units, keys = eng.all_units(), eng.unit_keys()
+        # the head's filters are padded to the dz buffer's width
+        self._pack([(key, u, (u.cout + 31) // 32 * 32 if u.bn is None else 0) for u, key in zip(units[1:], keys[1:])], device)
+        units[0].w16 = units[0].conv.weight.detach().contiguous()
+        for u in units[1:]:
+            u._wver = None                      # the eval path re-checks (and may re-pack into its own buffer)
+        head = units[-1]
+        if head.bn is None:
+            one, zero = self._ones(head.cout, device)
+            head.scale = one
+            head.shift = head.conv.bias.detach() if head.conv.bias is not None else zero
+            head._bver = None
 
     def _first_forward(self, x):
         """layers1.0 on the fp32 image: raw conv (batch statistics in its copy-out loop when the shape allows) -> BN -> leaky + 2x2 max-pool.
@@ -238,13 +411,13 @@ class DarknetTrainer(object):
         b, _, h, w = x.shape
         dev = x.device
         z = torch.empty(b, h, w, u0.cout, dtype=torch.float16, device=dev)
-        if self.fuse_stats and h % 32 == 0 and w % 16 == 0:
+        stats_done = self.fuse_stats and h % 32 == 0 and w % 16 == 0
+        if stats_done:
             # batch statistics accumulated by the conv kernel's copy-out loop: z is not read again for them
             ops.call('yb_conv0_raw_stats_fwd', x, u0.w16, z, self._sums(('f', 'layers1.0'), u0.cout, dev), b, h, w, u0.cout)
-            self._fused_stats = True
         else:
             ops.call('yb_conv0_raw_fwd', x, u0.w16, z, b, h, w, u0.cout)
-        mean, invstd = self._bn_forward('layers1.0', u0, z, b * h * w)
+        mean, invstd = self._bn_forward('layers1.0', u0, z, b * h * w, stats_done)
         a = self._apply(u0, z, mean, invstd, b, h, w, True)
         return self._saved_unit(u0, None, z, mean, invstd, h, w, True), a
 
@@ -252,8 +425,8 @@ class DarknetTrainer(object):
         """One BN unit on its input src [B,hh,ww,*]: raw conv -> batch statistics -> normalise + leaky (+ 2x2 max-pool), the activation
         written into `out` at channel `a_off` when given.  `pooled` (default: `pool`) is what the backward chain is told about the unit's
         output.  Returns (activation, saved unit)."""
-        z = self._raw_conv(u, src, key=key)
-        mean, invstd = self._bn_forward(key, u, z, b * hh * ww)
+        z, stats_done = self._raw_conv(u, src, key=key)
+        mean, invstd = self._bn_forward(key, u, z, b * hh * ww, stats_done)
         a = self._apply(u, z, mean, invstd, b, hh, ww, pool, out=out, a_off=a_off)
         return a, self._saved_unit(u, src, z, mean, invstd, hh, ww, pool if pooled is None else pooled)
 
@@ -269,30 +442,10 @@ class DarknetTrainer(object):
         ops.call('yb_reorg_bwd_f16', dcat, dcat.shape[-1], 0, d_apt, b, h, w, c)
         return d_apt
 
-    def _bn_backward(self, key, s, b, grads, da, dap, dz, ld_dz):
-        u = s.u
-        c = u.cout
-        dev = s.z.device
-        sums = self._sums(('b', key), c, dev)
-        args = (s.z, s.z.shape[-1], s.mean, s.invstd, u.bn.weight.detach(), u.bn.bias.detach(), self._slope(u), da, 0 if da is None else da.shape[-1], 0, dap,
-                0 if dap is None else dap.shape[-1], 0, b, s.h, s.w, c, 1 if dap is not None else 0, sums)
-        ops.call('yb_bn_act_bwd', 0, *args, None, 0, 1)
-        ops.call('yb_bn_act_bwd', 1, *args, dz, ld_dz, 1)
-        _, gname, bname = self._pnames(key, u)
-        dgamma, dbeta = self.arena.views[gname], self.arena.views[bname]
-        ops.call('yb_bn_param_grad', sums, c, dgamma, dbeta, 1, self._unscale)
-        grads[gname], grads[bname] = dgamma, dbeta
-        self._emit(gname, grads)
-        self._emit(bname, grads)
-
-    # ---- forward -------------------------------------------------------------------------------------
     def forward(self, x):
-        self._tracked = []
+        x = self._start_forward(x)
         eng = self.engine
-        if not x.is_cuda:
-            raise RuntimeError('Darknet training: input must be a CUDA tensor')
         b, _, h, w = x.shape
-        x = x.contiguous().float()
         if eng.precision != 'fast':
             raise RuntimeError("Darknet training uses fp16 operands with fp32 accumulation; precision='strict' is an inference mode "
                                "(call dnn.engine.set_precision('fast') before train())")
@@ -335,149 +488,33 @@ class DarknetTrainer(object):
         self._bump_tracked()
         return feature, saved
 
-    # ---- backward ------------------------------------------------------------------------------------
-    def _wd(self, key, u, cout_pad=0):
-        """Data-gradient operand of a unit (rotated, transposed fp16 weights), re-packed every step into a reused buffer."""
-        w = u.conv.weight
-        cout, cin, k, _ = w.shape
-        cp = max(cout, cout_pad)
-        wd = self.wd_cache.get(key)
-        plan = self._pack_plan
-        if plan is not None and wd is not None and plan.dgrad.get(key) is wd and wd.shape == (cin, k, k, cp):
-            return wd                         # packed by this step's batched launch (_repack)
-        if wd is None or wd.shape != (cin, k, k, cp) or wd.device != w.device:
-            wd = torch.empty(cin, k, k, cp, dtype=torch.float16, device=w.device)
-            self.wd_cache[key] = wd
-        ops.call('yb_pack_weight_dgrad_f16', w.detach().contiguous(), wd, cout, cin, k, cp)
-        return wd
-
-    def _wgrad(self, u, ain, dz, b, hh, ww, grads, name, cout=None):
-        """Weight gradient of one unit.  It depends only on (ain, dz) and nothing downstream depends on it before the
-        optimizer, so it is issued on a second stream: the tensor-bound wgrad kernel then overlaps the HBM-bound
-        BatchNorm backward of the next unit (and its data gradient) instead of queueing in front of them.  The fork /
-        join is plain stream-event ordering, so it is captured as parallel branches of the step's CUDA graph."""
-        cout = u.cout if cout is None else cout
-        cin, k = u.cin, u.ksize
-        dev = dz.device
-        side = self._side(dev)
-        if side is not None:
-            main = torch.cuda.current_stream(dev)
-            try:
-                fork = torch.cuda.Event()
-                fork.record(main)
-                side.wait_event(fork)
-            except Exception as ex:
-                raise RuntimeError('weight-gradient fork for %s failed (main %r, side %r): %s' % (name, main, side, ex)) from ex
-            dz.record_stream(side)          # dz / ain are main-stream allocations still read by the side stream
-            ain.record_stream(side)
-            self._side_busy = True
-        with torch.cuda.stream(side) if side is not None else _NullCtx():
-            dw_krsc = torch.empty(cout, k, k, cin, dtype=torch.float32, device=dev)
-            ops.call('yb_conv_wgrad', ain, dz, dw_krsc, b, hh, ww, cin, cout, k, ain.shape[-1], dz.shape[-1])
-            wname = self._pnames(name, u)[0]
-            dw = self.arena.views[wname]                                                     # [cout, cin, k, k] slot of the gradient arena
-            ops.call('yb_unpack_wgrad', dw_krsc, dw, cout, cin, k, self._unscale)            # layout change + inverse loss scale (/ world)
-            grads[wname] = dw
-            self._emit(wname, grads)
-
-    def _side(self, dev):
-        # only while the step is being captured into a CUDA graph: in eager mode the step is host-bound and the extra
-        # event / stream bookkeeping costs more (measured +2.6 ms) than the overlap gains (0.1 ms)
-        if not self.wgrad_stream or not torch.cuda.is_current_stream_capturing():
-            return None
-        st = self._side_streams.get(dev)
-        if st is None:
-            st = torch.cuda.Stream(device=dev)
-            self._side_streams[dev] = st
-        return st
-
-    def _join(self, dev):
-        """Main stream waits for everything issued on the wgrad stream (end of backward: the optimizer reads the grads)."""
-        if self._side_busy:
-            torch.cuda.current_stream(dev).wait_stream(self._side_streams[dev])
-            self._side_busy = False
-
-    def _unit_backward(self, key, s, b, grads, da=None, da_off=0, dap=None, dap_off=0, need_dgrad=True):
-        """Backward of one BN unit; returns the gradient w.r.t. the unit's input activation (or None)."""
-        u = s.u
-        c = u.cout
-        dev = s.z.device
-        window = 1 if (dap is not None) else 0
-        sums = self._sums(('b', key), c, dev)
-        bnw, bnb = u.bn.weight.detach(), u.bn.bias.detach()
-        args = (s.z, s.z.shape[-1], s.mean, s.invstd, bnw, bnb, self._slope(u), da, 0 if da is None else da.shape[-1], da_off, dap,
-                0 if dap is None else dap.shape[-1], dap_off, b, s.h, s.w, c, window, sums)
-        ops.call('yb_bn_act_bwd', 0, *args, None, 0, 1)
-        _, gname, bname = self._pnames(key, u)
-        dgamma = self.arena.views[gname]
-        dbeta = self.arena.views[bname]
-        dz = torch.empty(b, s.h, s.w, c, dtype=torch.float16, device=dev)
-        ops.call('yb_bn_act_bwd', 1, *args, dz, c, 1)
-        ops.call('yb_bn_param_grad', sums, c, dgamma, dbeta, 1, self._unscale)     # un-scales (/ world), then clears the accumulators
-        grads[gname] = dgamma
-        grads[bname] = dbeta
-        self._emit(gname, grads)
-        self._emit(bname, grads)
-        if s.ain is None:
-            return dz
-        self._wgrad(u, s.ain, dz, b, s.h, s.w, grads, key)
-        if not need_dgrad:
-            return None
-        one, zero = self._ones(u.cin, dev)
-        return ops.conv_bn_act(dz, self._wd(key, u), one, zero, 1.0)
-
-    def _head_backward(self, a_last, hh, ww, dfeature, grads):
-        """Head (layers3.1, 1x1 conv with bias): bias gradient from the unscaled fp32 gradient, dz scaled into fp16 and padded to a multiple of
-        32 channels, weight gradient, and the data gradient at the head's input."""
-        u31 = self.engine.units3[1]
-        b, dev = a_last.shape[0], a_last.device
-        chead = u31.cout
-        cpad = (chead + 31) // 32 * 32
-        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views['layers3.1.conv.bias']
-        scaled = (dfeature.contiguous().float() * self.grad_scale)
-        ops.call('yb_head_grad_prepare', scaled, dzh, dbias, b, chead, cpad, hh * ww)
-        grads['layers3.1.conv.bias'] = dbias.mul_(self._unscale)
-        self._emit('layers3.1.conv.bias', grads)
-        self._wgrad(u31, a_last, dzh, b, hh, ww, grads, 'layers3.1', cout=chead)
-        one, zero = self._ones(u31.cin, dev)
-        return ops.conv_bn_act(dzh, self._wd('layers3.1', u31, cpad), one, zero, 1.0)
-
     def _first_backward(self, x, s0, g_da, g_dap, grads):
         """layers1.0 backward from the gradient of its activation (g_da unpooled, g_dap through its max-pool): BN + leaky (+ pool) backward
         and the weight gradient from the fp32 image x."""
         b, _, h, w = x.shape
-        dev = s0.z.device
         dw0 = self.arena.views['layers1.0.conv.weight']
         if g_da is None and g_dap is not None and h % 8 == 0 and w % 32 == 0 and os.environ.get('YB_CONV0_WGRAD_FUSED', '1') != '0':
             # reduce pass of the BatchNorm backward, then the weight-gradient kernel forms dz itself (in shared memory, from z and the pooled
             # gradient): the 2 x 708 MB (B = 64 @ 416) write + read of dz and one launch disappear
             u0 = s0.u
-            sums = self._sums(('b', 'layers1.0'), u0.cout, dev)
-            bnw, bnb = u0.bn.weight.detach(), u0.bn.bias.detach()
-            ops.call('yb_bn_act_bwd', 0, s0.z, s0.z.shape[-1], s0.mean, s0.invstd, bnw, bnb, self.slope, None, 0, 0, g_dap, g_dap.shape[-1], 0,
-                     b, s0.h, s0.w, u0.cout, 1, sums, None, 0, 1)
-            ops.call('yb_conv0_wgrad_bn', x, s0.z, g_dap, g_dap.shape[-1], 0, s0.mean, s0.invstd, bnw, bnb, self.slope, sums, dw0, b, h, w)
-            dgamma, dbeta = self.arena.views['layers1.0.bn.weight'], self.arena.views['layers1.0.bn.bias']
-            ops.call('yb_bn_param_grad', sums, u0.cout, dgamma, dbeta, 1, self._unscale)          # also clears the accumulators (after their last reader)
-            grads['layers1.0.bn.weight'], grads['layers1.0.bn.bias'] = dgamma, dbeta
-            self._emit('layers1.0.bn.weight', grads)
-            self._emit('layers1.0.bn.bias', grads)
+            sums = self._bn_act_backward('layers1.0', s0, b, dap=g_dap)
+            ops.call('yb_conv0_wgrad_bn', x, s0.z, g_dap, g_dap.shape[-1], 0, s0.mean, s0.invstd, u0.bn.weight.detach(), u0.bn.bias.detach(),
+                     self._slope(u0), sums, dw0, b, h, w)
+            self._bn_param_grad('layers1.0', u0, sums, grads)          # also clears the accumulators (after their last reader)
         else:
             dz0 = self._unit_backward('layers1.0', s0, b, grads, da=g_da, dap=g_dap)
             ops.call('yb_conv0_wgrad', x, dz0, dw0, b, h, w)
         grads['layers1.0.conv.weight'] = dw0.mul_(self._unscale)
         self._emit('layers1.0.conv.weight', grads)
 
-    def backward(self, saved, dfeature, dnn=None):
+    def backward(self, saved, dfeature):
         """dfeature: fp32 NCHW gradient of the loss w.r.t. the head output.  Returns {state_dict key: fp32 grad}: views of the
         persistent gradient arena, already averaged over the data-parallel ranks when a reducer is attached."""
         eng = self.engine
         b = saved.b
         grads = {}
         dev = dfeature.device
-        self._ensure_arena(dnn if dnn is not None else self._dnn, dev)
-        self._main = torch.cuda.current_stream(dev)
+        self._start_backward(dev)
         da = self._head_backward(saved.a30, saved.h32, saved.w32, dfeature, grads)
         # layers3.0 -> gradient of the concat buffer
         dcat = self._unit_backward('layers3.0', saved.units['layers3.0'], b, grads, da=da)
@@ -502,28 +539,21 @@ class DarknetTrainer(object):
             g_da, g_dap = (None, g) if prev_pooled else (g, None)
         # layers1.0: weight gradient straight from the fp32 image
         self._first_backward(saved.x, saved.units['layers1.0'], g_da, g_dap, grads)
-        self._join(dev)
-        if self.reducer is not None:
-            self.reducer.finish()          # main stream waits for every bucket's all-reduce (no host wait)
-        # fp16 gradient overflow guard (after the exchange, so every rank takes the same decision): `found_inf` is raised and the
-        # gradients are zeroed instead of poisoning the optimizer state; train.iterate hands the flag to optimizers that can skip
-        if self.found_inf is None or self.found_inf.device != dev:
-            self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)      # 0-dim like GradScaler's (fused optimizers subtract it from their step counters)
-        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+        self._finish_backward(dev)
         return grads
 
 
-class TinyTrainer(DarknetTrainer):
+class TinyTrainer(TrainerBase):
     """Training-mode forward / backward of `model.yolo2.Tiny` (reference model/yolo2.py:140-173) on the same kernels: a plain chain of
     conv units, five of them followed by MaxPool2d(2) (fused into the normalise kernel), the sixth by ConstantPad2d + MaxPool2d(2, stride 1).
 
     The 16-channel first layer rides on the 32-filter first-layer kernels: its weights are zero-padded to 32 outputs, BatchNorm runs over the
     16 real channels of the 32-wide buffers (the kernels take the channel count and the pixel pitch separately), the padding channels stay
     exactly zero, and the second unit's weights are zero-padded on the input side to match (its weight gradient is cut back to 16 inputs)."""
+    NAME = 'Tiny'
 
     def __init__(self, dnn, grad_scale=16384.0):
-        DarknetTrainer.__init__(self, _TinyEngineView(dnn), grad_scale)
-        self.dnn = dnn
+        TrainerBase.__init__(self, dnn, grad_scale)
         self._zero_bufs = {}
 
     def grad_order(self):
@@ -532,6 +562,10 @@ class TinyTrainer(DarknetTrainer):
         for key in reversed(keys[:-1]):
             names += [key + '.bn.weight', key + '.bn.bias', key + '.conv.weight']
         return names
+
+    def _head_unit(self):
+        key_h, u_h, _ = self.dnn.unit_keys()[-1]
+        return key_h, u_h, key_h + '.conv.bias'
 
     def _zeros(self, tag, shape, device):
         """Persistent zero-initialised fp16 buffer whose padding channels are never written."""
@@ -542,12 +576,8 @@ class TinyTrainer(DarknetTrainer):
         return t
 
     def forward(self, x):
-        self._tracked = []
-        if not x.is_cuda:
-            raise RuntimeError('Tiny training: input must be a CUDA tensor')
+        x = self._start_forward(x)
         b, _, h, w = x.shape
-        x = x.contiguous().float()
-        dev = x.device
         plan = self.dnn.unit_keys()
         units = [u for _, u, _ in plan]
         for i, u in enumerate(units):
@@ -585,10 +615,10 @@ class TinyTrainer(DarknetTrainer):
         w0[:c0].copy_(u0.conv.weight.detach())
         z = self._zeros(('z0', b, h, w), (b, h, w, 32), dev)
         ops.call('yb_conv0_raw_fwd', x, w0, z, b, h, w, 32)
-        mean, invstd = self._bn_forward(key0, u0, z, b * h * w)
+        mean, invstd = self._bn_forward(key0, u0, z, b * h * w, False)
         cur = self._zeros(('a0', b, h, w), (b, h // 2, w // 2, 32), dev)
         self._apply(u0, z, mean, invstd, b, h, w, True, out=cur)
-        return self._saved_unit(u0, None, z, mean, invstd, h, w, True), cur
+        return self._saved_unit(u0, None, z, mean, invstd, h, w, True, x=x), cur      # the weight gradient reads the image
 
     def _chain_unit_forward(self, key, u, after, cur, b, hh, ww):
         """One chain unit on its input cur [B,hh,ww,chan]: raw conv (weights zero-padded on the input side when chan > Cin) -> BN -> leaky,
@@ -604,44 +634,24 @@ class TinyTrainer(DarknetTrainer):
         else:
             w16 = u.w16
         one, zero = self._ones(u.cout, dev)
-        if self.fuse_stats and not (chan == 32 and u.ksize == 3 and u.cout <= 64):
+        stats_done = self.fuse_stats and not (chan == 32 and u.ksize == 3 and u.cout <= 64)
+        if stats_done:
             z = ops.conv_bn_act_stats(cur, w16, one, zero, 1.0, self._sums(('f', key), u.cout, dev))
-            self._fused_stats = True
         else:
             z = ops.conv_bn_act(cur, w16, one, zero, 1.0)
-            self._fused_stats = False
-        mean, invstd = self._bn_forward(key, u, z, b * hh * ww)
+        mean, invstd = self._bn_forward(key, u, z, b * hh * ww, stats_done)
         a = self._apply(u, z, mean, invstd, b, hh, ww, after == 'pool')
-        s = self._saved_unit(u, cur, z, mean, invstd, hh, ww, after == 'pool')
-        s.cin_pad = chan
+        s = self._saved_unit(u, cur, z, mean, invstd, hh, ww, after == 'pool', cin_pad=chan)
         if after == 'pool_s1':
             s.a_unpooled = a
             a = ops.maxpool2x2_s1(a)
         return a, s
 
-    def _head_backward(self, a_last, hh, ww, dfeature, grads):
-        """Head (1x1 conv with bias): bias gradient, dz scaled into fp16 and padded to a multiple of 32 channels, weight gradient, and the data
-        gradient at the head's input."""
-        key_h, u_h, _ = self.dnn.unit_keys()[-1]
-        b, dev = a_last.shape[0], a_last.device
-        chead = u_h.cout
-        cpad = (chead + 31) // 32 * 32
-        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views[key_h + '.conv.bias']
-        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
-        grads[key_h + '.conv.bias'] = dbias.mul_(self._unscale)
-        self._emit(key_h + '.conv.bias', grads)
-        self._wgrad(u_h, a_last, dzh, b, hh, ww, grads, key_h, cout=chead)
-        one, zero = self._ones(u_h.cin, dev)
-        return ops.conv_bn_act(dzh, self._wd(key_h, u_h, cpad), one, zero, 1.0)
-
-    def backward(self, saved, dfeature, dnn=None):
+    def backward(self, saved, dfeature):
         b = saved.b
         grads = {}
         dev = dfeature.device
-        self._ensure_arena(self.dnn, dev)
-        self._main = torch.cuda.current_stream(dev)
-        self._x = saved.x
+        self._start_backward(dev)
         g = self._head_backward(saved.a_last, saved.hh, saved.ww, dfeature, grads)
         for key, after in reversed(saved.order):
             s = saved.units[key]
@@ -653,38 +663,34 @@ class TinyTrainer(DarknetTrainer):
             pooled = after == 'pool'
             if s.ain is None:
                 # first layer: dz into the 32-wide zero-padded buffer the first-layer weight-gradient kernel reads
-                g = self._tiny_unit0_backward(key, s, b, grads, g)
+                self._tiny_unit0_backward(key, s, b, grads, g)
                 break
-            if getattr(s, 'cin_pad', u.cin) != u.cin:
+            if s.cin_pad != u.cin:
                 g = self._tiny_padded_unit_backward(key, s, b, grads, g, pooled)
             else:
                 g = self._unit_backward(key, s, b, grads, da=None if pooled else g, dap=g if pooled else None)
-        self._join(dev)
-        if self.reducer is not None:
-            self.reducer.finish()
-        if self.found_inf is None or self.found_inf.device != dev:
-            self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
-        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+        self._finish_backward(dev)
         return grads
 
     def _tiny_unit0_backward(self, key, s, b, grads, g):
+        """Unit 0 from the gradient g through its max-pool: dz into a 32-wide buffer whose padding channels stay zero, then the 32-filter
+        first-layer weight gradient from the fp32 image the unit saved (s.x), cut back to the C0 real filters."""
         dev = s.z.device
         dz = self._zeros(('dz0', b, s.h, s.w), (b, s.h, s.w, 32), dev)          # channels >= cout stay zero
-        self._bn_backward(key, s, b, grads, None, g, dz, 32)
+        self._bn_backward(key, s, b, grads, dz, dap=g)
         dw32 = torch.empty(32, 3, 3, 3, dtype=torch.float32, device=dev)
-        ops.call('yb_conv0_wgrad', self._x, dz, dw32, b, s.h, s.w)
+        ops.call('yb_conv0_wgrad', s.x, dz, dw32, b, s.h, s.w)
         dw = self.arena.views[key + '.conv.weight']
         dw.copy_(dw32[:s.u.cout]).mul_(self._unscale)
         grads[key + '.conv.weight'] = dw
         self._emit(key + '.conv.weight', grads)
-        return None
 
     def _tiny_padded_unit_backward(self, key, s, b, grads, g, pooled):
         """Unit whose input buffer is wider than its Cin (zero-padded): the weight gradient is computed over the padded width and cut back."""
         u = s.u
         dev = s.z.device
         dz = torch.empty(b, s.h, s.w, u.cout, dtype=torch.float16, device=dev)
-        self._bn_backward(key, s, b, grads, None if pooled else g, g if pooled else None, dz, u.cout)
+        self._bn_backward(key, s, b, grads, dz, da=None if pooled else g, dap=g if pooled else None)
         k, cp = u.ksize, s.cin_pad
         dw_krsc = torch.empty(u.cout, k, k, cp, dtype=torch.float32, device=dev)
         ops.call('yb_conv_wgrad', s.ain, dz, dw_krsc, b, s.h, s.w, cp, u.cout, k, s.ain.shape[-1], dz.shape[-1])
@@ -694,16 +700,7 @@ class TinyTrainer(DarknetTrainer):
         dw.copy_(full[:, :u.cin])
         grads[key + '.conv.weight'] = dw
         self._emit(key + '.conv.weight', grads)
-        one, zero = self._ones(u.cin, dev)
-        return ops.conv_bn_act(dz, self._wd(key, u), one, zero, 1.0)      # [B, h, w, Cin]: the producer's real channels
-
-
-class _TinyEngineView(object):
-    """The two things DarknetTrainer reads from an engine, for a plain chain."""
-    precision = 'fast'
-
-    def __init__(self, dnn):
-        self._dnn = dnn
+        return self._dgrad(key, u, dz)      # [B, h, w, Cin]: the producer's real channels
 
 
 class _BNUnit(object):
@@ -714,16 +711,15 @@ class _BNUnit(object):
         self._bver = None
 
 
-class MobileNetTrainer(DarknetTrainer):
+class MobileNetTrainer(TrainerBase):
     """Training-mode forward / backward of `model.mobilenet.MobileNet` (reference model/mobilenet.py:25-85): conv_bn(3, 32, stride 2), thirteen
     [depthwise 3x3 (stride 1 or 2) + BN + ReLU, pointwise 1x1 + BN + ReLU] units, a 1x1 head with bias.  Pointwise convs, their weight /
     data gradients and the head run on the wgmma kernels of the Darknet path; the depthwise and first-layer kernels are HBM-bound CUDA-core
     kernels (csrc/mobilenet_ops.cu).  BatchNorm momentum is the PyTorch default 0.1 here (read from the modules), the activation ReLU."""
+    NAME = 'MobileNet'
 
     def __init__(self, dnn, grad_scale=16384.0):
-        DarknetTrainer.__init__(self, _TinyEngineView(dnn), grad_scale)
-        self.dnn = dnn
-        self.slope = 0.0
+        TrainerBase.__init__(self, dnn, grad_scale, slope=0.0)
         self._units = None
 
     def _plan(self):
@@ -747,11 +743,8 @@ class MobileNetTrainer(DarknetTrainer):
         return names + ['layers.0.bn.weight', 'layers.0.bn.bias', 'layers.0.conv.weight']
 
     def forward(self, x):
-        self._tracked = []
-        if not x.is_cuda:
-            raise RuntimeError('MobileNet training: input must be a CUDA tensor')
+        x = self._start_forward(x)
         b, _, h, w = x.shape
-        x = x.contiguous().float()
         dev = x.device
         plan = self._plan()
         saved = _Saved()
@@ -782,11 +775,9 @@ class MobileNetTrainer(DarknetTrainer):
         z = torch.empty(b, hh, ww, 32, dtype=torch.float16, device=x.device)
         ops.call('yb_mb_conv0_raw_fwd', x, self.dnn.layers[0].conv.weight.detach().contiguous(), z, b, h, w)
         u0 = self._plan()['first']
-        mean, invstd = self._bn_forward('layers.0', u0, z, b * hh * ww)
+        mean, invstd = self._bn_forward('layers.0', u0, z, b * hh * ww, False)
         a = self._apply(u0, z, mean, invstd, b, hh, ww, False)
-        s0 = _Saved()
-        s0.u, s0.z, s0.mean, s0.invstd, s0.h, s0.w = u0, z, mean, invstd, hh, ww
-        return s0, a
+        return self._saved_unit(u0, None, z, mean, invstd, hh, ww), a
 
     def _dw_forward(self, rec, cur, b, hh, ww):
         """Depthwise 3x3 unit (stride 1 or 2) on its input cur [B,hh,ww,C]: raw conv -> BN -> ReLU.  Returns (activation, saved unit)."""
@@ -796,23 +787,19 @@ class MobileNetTrainer(DarknetTrainer):
         zd = torch.empty(b, oh, ow, ch, dtype=torch.float16, device=cur.device)
         wd = rec['dw_conv'].weight.detach().contiguous().view(ch, 9)
         ops.call('yb_dwconv3x3_raw_fwd', cur, wd, zd, b, hh, ww, ch, stride)
-        mean, invstd = self._bn_forward(key + '.dw', rec['dw'], zd, b * oh * ow)
+        mean, invstd = self._bn_forward(key + '.dw', rec['dw'], zd, b * oh * ow, False)
         ad = self._apply(rec['dw'], zd, mean, invstd, b, oh, ow, False)
-        sd = _Saved()
-        sd.u, sd.ain, sd.z, sd.mean, sd.invstd, sd.h, sd.w, sd.in_h, sd.in_w, sd.stride, sd.wd = rec['dw'], cur, zd, mean, invstd, oh, ow, hh, ww, stride, wd
-        return ad, sd
+        return ad, self._saved_unit(rec['dw'], cur, zd, mean, invstd, oh, ow, in_h=hh, in_w=ww, stride=stride, wd=wd)
 
     def _pw_forward(self, rec, ad, b, oh, ow):
         """Pointwise 1x1 unit on the wgmma conv: raw conv (statistics in its epilogue) -> BN -> ReLU.  Returns (activation, saved unit)."""
         key = rec['key']
         up = rec['pw']
         up.refresh(force=True)
-        zp = self._raw_conv(up, ad, key=key + '.pw')
-        mean, invstd = self._bn_forward(key + '.pw', up, zp, b * oh * ow)
+        zp, stats_done = self._raw_conv(up, ad, key=key + '.pw')
+        mean, invstd = self._bn_forward(key + '.pw', up, zp, b * oh * ow, stats_done)
         ap = self._apply(up, zp, mean, invstd, b, oh, ow, False)
-        sp = _Saved()
-        sp.u, sp.ain, sp.z, sp.mean, sp.invstd, sp.h, sp.w, sp.pooled = up, ad, zp, mean, invstd, oh, ow, False
-        return ap, sp
+        return ap, self._saved_unit(up, ad, zp, mean, invstd, oh, ow)
 
     def _dw_backward(self, key, sd, b, grads, g):
         """Depthwise unit backward from the gradient g of its activation: BN + ReLU backward, depthwise weight and data gradients.  Returns the
@@ -820,7 +807,7 @@ class MobileNetTrainer(DarknetTrainer):
         ch = sd.u.cout
         dev = g.device
         dz = torch.empty(b, sd.h, sd.w, ch, dtype=torch.float16, device=dev)
-        self._bn_backward(key + '.dw', sd, b, grads, g, None, dz, ch)
+        self._bn_backward(key + '.dw', sd, b, grads, dz, da=g)
         dwd = self.arena.views[key + '.dw.conv.weight']
         ops.call('yb_dwconv3x3_wgrad', sd.ain, dz, dwd, b, sd.in_h, sd.in_w, ch, sd.stride)
         grads[key + '.dw.conv.weight'] = dwd.mul_(self._unscale)
@@ -833,25 +820,20 @@ class MobileNetTrainer(DarknetTrainer):
         """First layer backward from the gradient g of its activation: BN + ReLU backward, then the weight gradient from the fp32 image."""
         b, _, h, w = x.shape
         dz0 = torch.empty(b, s0.h, s0.w, 32, dtype=torch.float16, device=g.device)
-        self._bn_backward('layers.0', s0, b, grads, g, None, dz0, 32)
+        self._bn_backward('layers.0', s0, b, grads, dz0, da=g)
         dw0 = self.arena.views['layers.0.conv.weight']
         ops.call('yb_mb_conv0_wgrad', x, dz0, dw0, b, h, w)
         grads['layers.0.conv.weight'] = dw0.mul_(self._unscale)
         self._emit('layers.0.conv.weight', grads)
 
     def _head_backward(self, a_last, hh, ww, dfeature, grads):
-        """Head (1x1 conv with bias): bias gradient, dz scaled into fp16 and padded to 128 channels, weight gradient, and the data gradient at
-        the head's input."""
+        """Head (1x1 conv with bias): bias gradient and padded dz (`_head_grad`), then the weight gradient and the data gradient at the head's
+        input, both on the main stream."""
         b, dev = a_last.shape[0], a_last.device
         head = self._plan()['head']
         chead, cin = head.weight.shape[0], head.weight.shape[1]
-        cpad = (chead + 31) // 32 * 32
-        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views['layers.14.bias']
-        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
-        grads['layers.14.bias'] = dbias.mul_(self._unscale)
-        self._emit('layers.14.bias', grads)
-        # head weight gradient / data gradient (1x1)
+        dzh = self._head_grad('layers.14.bias', chead, a_last, hh, ww, dfeature, grads)
+        cpad = dzh.shape[-1]
         dw_krsc = torch.empty(chead, 1, 1, cin, dtype=torch.float32, device=dev)
         ops.call('yb_conv_wgrad', a_last, dzh, dw_krsc, b, hh, ww, cin, chead, 1, a_last.shape[-1], dzh.shape[-1])
         dwh = self.arena.views['layers.14.weight']
@@ -863,24 +845,18 @@ class MobileNetTrainer(DarknetTrainer):
         one, zero = self._ones(cin, dev)
         return ops.conv_bn_act(dzh, wdh, one, zero, 1.0)
 
-    def backward(self, saved, dfeature, dnn=None):
+    def backward(self, saved, dfeature):
         b = saved.b
         grads = {}
         dev = dfeature.device
-        self._ensure_arena(self.dnn, dev)
-        self._main = torch.cuda.current_stream(dev)
+        self._start_backward(dev)
         g = self._head_backward(saved.a_last, saved.hh, saved.ww, dfeature, grads)
         for key, sd, sp in reversed(saved.units):
             # pointwise unit: generic BN backward + wgmma weight / data gradient (state-dict names layers.N.pw.*)
             g = self._unit_backward(key + '.pw', sp, b, grads, da=g)
             g = self._dw_backward(key, sd, b, grads, g)
         self._first_backward(saved.x, saved.first, g, grads)
-        self._join(dev)
-        if self.reducer is not None:
-            self.reducer.finish()
-        if self.found_inf is None or self.found_inf.device != dev:
-            self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
-        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+        self._finish_backward(dev)
         return grads
 
 
@@ -896,7 +872,7 @@ class _ResUnit(object):
         self._bver = None
 
 
-class ResNetTrainer(DarknetTrainer):
+class ResNetTrainer(TrainerBase):
     """Training-mode forward / backward of `model.resnet.ResNet` (reference model/resnet.py:28-142): stem conv 7x7 stride 2 + BN + ReLU,
     MaxPool2d(3, 2, 1), BasicBlock / Bottleneck stacks, a 1x1 head with bias.
 
@@ -907,11 +883,10 @@ class ResNetTrainer(DarknetTrainer):
     stride-1 weight and data gradients.  At each block boundary yb_residual_bwd_f16 sums the main path's data gradient and the skip path's and
     applies the previous block's ReLU mask in one pass.  The stem's gradient runs through the max-pool backward (first maximum of each window),
     the BN + ReLU backward and a CUDA-core weight-gradient kernel on the fp32 image."""
+    NAME = 'ResNet'
 
     def __init__(self, dnn, grad_scale=16384.0):
-        DarknetTrainer.__init__(self, _TinyEngineView(dnn), grad_scale)
-        self.dnn = dnn
-        self.slope = 0.0
+        TrainerBase.__init__(self, dnn, grad_scale, slope=0.0)
         self._blocks = None
 
     def _plan(self):
@@ -945,19 +920,14 @@ class ResNetTrainer(DarknetTrainer):
                 names += [u.pnames[1], u.pnames[2], u.pnames[0]]
         return names + ['bn1.weight', 'bn1.bias', 'conv1.weight']
 
+    def _head_unit(self):
+        return self._head.key, self._head, 'conv.bias'
+
     def _repack(self, device):
         """Forward and data-gradient fp16 operands of every 1x1 / 3x3 conv and the head in ONE batched launch (the stem reads its fp32
         weights in place)."""
-        units = self._conv_units() + [self._head]
-        ptrs = tuple(u.conv.weight.data_ptr() for u in units)
-        plan = self._pack_plan
-        if plan is None or plan.key != ptrs or plan.table.device != device:
-            cpad = (self._head.cout + 31) // 32 * 32          # the head's filters are padded to the dz buffer's width
-            plan = self._pack_plan = PackPlan([(u.key, u.conv.weight.detach(), True, True, cpad if u is self._head else 0) for u in units], device)
-        plan.run()
-        for u in units:
-            u.w16 = plan.fwd[u.key]
-            self.wd_cache[u.key] = plan.dgrad[u.key]
+        cpad = (self._head.cout + 31) // 32 * 32          # the head's filters are padded to the dz buffer's width
+        self._pack([(u.key, u, 0) for u in self._conv_units()] + [(self._head.key, self._head, cpad)], device)
 
     def _subsample(self, x):
         b, h, w, c = x.shape
@@ -966,34 +936,30 @@ class ResNetTrainer(DarknetTrainer):
         return out
 
     def _unit_forward(self, u, src, b, hh, ww):
-        s = _Saved()
         if u.stride == 2 and u.ksize == 1:
             src = self._subsample(src)                     # kept: the weight gradient reads it
             hh, ww = src.shape[1], src.shape[2]
-        s.u, s.ain, s.in_h, s.in_w = u, src, hh, ww
         if u.stride == 2 and u.ksize == 3:
             # statistics over the selected (stride-2) pixels only: not from the full-resolution conv epilogue
-            z = self._subsample(self._raw_conv(u, src))
+            z, _ = self._raw_conv(u, src)
+            z = self._subsample(z)
+            stats_done = False
             oh, ow = z.shape[1], z.shape[2]
         else:
-            z = self._raw_conv(u, src, key=u.key)
+            z, stats_done = self._raw_conv(u, src, key=u.key)
             oh, ow = hh, ww
-        mean, invstd = self._bn_forward(u.key, u, z, b * oh * ow)
+        mean, invstd = self._bn_forward(u.key, u, z, b * oh * ow, stats_done)
         a = self._apply(u, z, mean, invstd, b, oh, ow, False)
-        s.z, s.mean, s.invstd, s.h, s.w = z, mean, invstd, oh, ow
-        return a, s
+        return a, self._saved_unit(u, src, z, mean, invstd, oh, ow, in_h=hh, in_w=ww)
 
     def forward(self, x):
-        self._tracked = []
-        if not x.is_cuda:
-            raise RuntimeError('ResNet training: input must be a CUDA tensor')
+        x = self._start_forward(x)
         b, c, h, w = x.shape
         if c != 3 or h % 32 or w % 32:
             raise ValueError('ResNet expects [B,3,H,W] with H, W multiples of 32')
         net = self.dnn
         if tuple(net.conv1.weight.shape) != (64, 3, 7, 7):
             raise ValueError('ResNet: the stem must be a 7x7 conv with 64 output channels')
-        x = x.contiguous().float()
         dev = x.device
         blocks = self._plan()
         self._repack(dev)
@@ -1032,13 +998,11 @@ class ResNetTrainer(DarknetTrainer):
         hh, ww = h // 2, w // 2
         z = torch.empty(b, hh, ww, 64, dtype=torch.float16, device=dev)
         ops.call('yb_stem7x7_raw_fwd', x, st.conv.weight.detach(), z, b, h, w)
-        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww)
+        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww, False)
         a = self._apply(st, z, mean, invstd, b, hh, ww, False)
-        s = _Saved()
-        s.u, s.ain, s.z, s.mean, s.invstd, s.h, s.w = st, None, z, mean, invstd, hh, ww
         pooled = torch.empty(b, hh // 2, ww // 2, 64, dtype=torch.float16, device=dev)
         ops.call('yb_maxpool3x3_s2_f16', a, pooled, b, hh, ww, 64)
-        return s, a, pooled
+        return self._saved_unit(st, None, z, mean, invstd, hh, ww), a, pooled
 
     @staticmethod
     def _join_forward(cur, res):
@@ -1055,22 +1019,6 @@ class ResNetTrainer(DarknetTrainer):
         ops.call('yb_residual_bwd_f16', mask, gm, gb, stride_b, g, b, h, w, gm.shape[-1])
         return g
 
-    def _head_backward(self, a_last, hh, ww, dfeature, grads):
-        """Head (1x1 conv with bias): bias gradient from the fp32 gradient, dz scaled into fp16 and padded to 128 channels, weight gradient,
-        and the data gradient at the head's input (before the last block's ReLU mask)."""
-        b, dev = a_last.shape[0], a_last.device
-        head = self._head
-        chead, cin = head.cout, head.cin
-        cpad = (chead + 31) // 32 * 32
-        dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
-        dbias = self.arena.views['conv.bias']
-        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
-        grads['conv.bias'] = dbias.mul_(self._unscale)
-        self._emit('conv.bias', grads)
-        self._wgrad(head, a_last, dzh, b, hh, ww, grads, head.key, cout=chead)
-        one, zero = self._ones(cin, dev)
-        return ops.conv_bn_act(dzh, self._wd(head.key, head, cpad), one, zero, 1.0)
-
     def _stem_backward(self, x, st, stem_a, g, grads):
         """Stem backward from the gradient g at the max-pool output: max-pool backward -> BN + ReLU backward -> weight gradient from the fp32
         image.  Returns the gradient at the stem's activation (the max-pool's input)."""
@@ -1079,7 +1027,7 @@ class ResNetTrainer(DarknetTrainer):
         da = torch.empty_like(stem_a)
         ops.call('yb_maxpool3x3_s2_bwd_f16', stem_a, g, da, b, st.h, st.w, 64)
         dz = torch.empty(b, st.h, st.w, 64, dtype=torch.float16, device=dev)
-        self._bn_backward(st.u.key, st, b, grads, da, None, dz, 64)
+        self._bn_backward(st.u.key, st, b, grads, dz, da=da)
         dw = self.arena.views['conv1.weight']
         ops.call('yb_stem7x7_wgrad', x, dz, dw, b, h, w)
         grads['conv1.weight'] = dw.mul_(self._unscale)
@@ -1093,19 +1041,17 @@ class ResNetTrainer(DarknetTrainer):
             return self._unit_backward(u.key, s, b, grads, da=da)
         dev = s.z.device
         dz = torch.empty(b, s.h, s.w, u.cout, dtype=torch.float16, device=dev)
-        self._bn_backward(u.key, s, b, grads, da, None, dz, u.cout)
+        self._bn_backward(u.key, s, b, grads, dz, da=da)
         dzf = torch.empty(b, s.in_h, s.in_w, u.cout, dtype=torch.float16, device=dev)
         ops.call('yb_upsample2_zero_f16', dz, dzf, b, s.in_h, s.in_w, u.cout)
         self._wgrad(u, s.ain, dzf, b, s.in_h, s.in_w, grads, u.key)
-        one, zero = self._ones(u.cin, dev)
-        return ops.conv_bn_act(dzf, self._wd(u.key, u), one, zero, 1.0)
+        return self._dgrad(u.key, u, dzf)
 
-    def backward(self, saved, dfeature, dnn=None):
+    def backward(self, saved, dfeature):
         b = saved.b
         grads = {}
         dev = dfeature.device
-        self._ensure_arena(self.dnn, dev)
-        self._main = torch.cuda.current_stream(dev)
+        self._start_backward(dev)
         hh, ww = saved.hh, saved.ww
         gh = self._head_backward(saved.a_last, hh, ww, dfeature, grads)
         g = self._join_backward(saved.a_last, gh, None, 1, b, hh, ww)        # through the last block's ReLU
@@ -1121,10 +1067,5 @@ class ResNetTrainer(DarknetTrainer):
             mask = None if xin is saved.pool else xin           # layer1.0's input is the max-pool output: no ReLU in between
             g = self._join_backward(mask, gm, gb, stride_b, b, in_h, in_w)
         self._stem_backward(saved.x, saved.stem, saved.stem_a, g, grads)
-        self._join(dev)
-        if self.reducer is not None:
-            self.reducer.finish()
-        if self.found_inf is None or self.found_inf.device != dev:
-            self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
-        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+        self._finish_backward(dev)
         return grads

@@ -94,7 +94,7 @@ class _DarknetTrainFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dfeature):
         dnn = ctx.dnn
-        grads = dnn.trainer.backward(ctx.saved, dfeature, dnn)
+        grads = dnn.trainer.backward(ctx.saved, dfeature)
         ctx.saved = None
         # The gradients live in the trainer's persistent arena (b200.ddp.GradArena; in data-parallel runs its buckets are being
         # all-reduced in place right now).  `.grad` is bound to those views directly -- handing them to autograd instead would let
@@ -183,7 +183,7 @@ class Darknet(nn.Module):
     @property
     def trainer(self):
         if self._trainer is None:
-            self._trainer = _train.DarknetTrainer(self.engine)
+            self._trainer = _train.DarknetTrainer(self)
         return self._trainer
 
     def train(self, mode=True):
