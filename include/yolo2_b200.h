@@ -352,6 +352,31 @@ int yb_bn_relu_avgpool2x2_f16(const void* x, int x_ld, const float* scale, const
 /* yb_maxpool3x3_s2_f16 writing channels [y_ch_off, y_ch_off + C) of y [B,(H+1)/2,(W+1)/2,y_ld] (the stem pool into the first block's buffer). */
 int yb_maxpool3x3_s2_ld_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
 
+/* ---- Inception-v3 plugin (model/inception3.py:29-118 over torchvision's BasicConv2d / InceptionA-E), inference ------------------------
+ * yb_conv2d_bn_act_fwd: the implicit-GEMM conv of yb_conv_bn_act_fwd_ws with a general geometry -- kh x kw filters (1..7 each), stride 1 or 2,
+ * zero padding pad_h < kh, pad_w < kw -- on x fp16 NHWC [B,in_h,in_w,Cin] (pixel pitch x_ld, Cin % 32 == 0) and w fp16 [Cout][kh][kw][Cin]
+ * (yb_pack_weight_khw_f16).  The output is [B,OH,OW,*] fp16 NHWC (pitch y_ld, first channel y_ch_off) or fp32 NCHW [B,Cout,OH,OW] with
+ * OH = (in_h + 2 pad_h - kh) / stride + 1, OW likewise; epilogue, flags and workspace as yb_conv_bn_act_fwd_ws.  Any other geometry, an empty
+ * output or Cin % 32 != 0 is refused with YB_ERR_BAD_ARG before any launch.  (k, k, 1, (k-1)/2) for k in {1, 3} gives the bits of
+ * yb_conv_bn_act_fwd_ws.  yb_conv2d_choice is yb_conv_choice for this geometry (height / width are the INPUT dims). */
+int yb_conv2d_bn_act_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch, int in_h, int in_w,
+                         int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int x_ld, long long y_ld, int y_ch_off, int out_mode,
+                         int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);
+int yb_conv2d_choice(int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int out_mode, int flags,
+                     int with_workspace, int out[6]);
+/* nn.Conv2d weight fp32 [Cout,Cin,kh,kw] -> fp16 [cout_pad][kh][kw][cin_pad], zero where co >= Cout or ci >= Cin (Inception's 80- and 48-channel
+ * layers run as 96 / 64 channels: zero filters with scale 1 / shift 0 give exact zeros after the ReLU, and zero input channels add nothing). */
+int yb_pack_weight_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, int kh, int kw, int cout_pad, int cin_pad, yb_stream_t stream);
+/* Conv2d_1a_3x3: nn.Conv2d(3, 32, 3, stride 2, padding pad) + folded BatchNorm + ReLU, x fp32 NCHW [B,3,H,W] -> y fp16 NHWC
+ * [B,(H+2pad-3)/2+1,(W+2pad-3)/2+1,32]; pad 0 (Inception) or 1 (the bits of yb_mb_conv0_bn_relu_fwd). */
+int yb_stem3x3_s2_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height,
+                              int width, int pad, yb_stream_t stream);
+/* F.max_pool2d(x, 3, stride=2) (no padding, floor): x [B,H,W,C] -> channels [y_ch_off, y_ch_off + C) of y [B,(H-3)/2+1,(W-3)/2+1,y_ld].
+ * H, W >= 3; C, y_ld, y_ch_off multiples of 8. */
+int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
+/* F.avg_pool2d(x, 3, stride=1, padding=1, count_include_pad=True): x, y [B,H,W,C]; y = fp16(fp32 sum of the in-range window / 9). */
+int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
+
 /* Training of the ResNet plugin: what torch autograd does for the stem, the max-pool, the stride-2 selection and the residual join.  BatchNorm and
  * the activations are the generic train-mode kernels above (slope 0 = ReLU, slope 1 = identity); the 3x3 / 1x1 convs and their gradients are the
  * wgmma kernels, a stride-2 conv's backward being the stride-1 gradients of the zero-inserted dz (yb_upsample2_zero_f16).

@@ -91,6 +91,13 @@ SIGNATURES = {
                               c_longlong, P],
     'yb_bn_relu_avgpool2x2_f16': [P, c_int, P, P, P, c_int, c_int, c_int, c_int, P],
     'yb_maxpool3x3_s2_ld_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_conv2d_bn_act_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int,
+                             c_int, c_int, P, c_longlong, P],
+    'yb_conv2d_choice': [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int * 6)],
+    'yb_pack_weight_khw_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_stem3x3_s2_bn_relu_fwd': [P, P, P, P, P, c_int, c_int, c_int, c_int, P],
+    'yb_maxpool3x3_s2_valid_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_avgpool3x3_s1_f16': [P, P, c_int, c_int, c_int, c_int, P],
 }
 
 _lib = None

@@ -176,6 +176,87 @@ def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch
     return out
 
 
+def conv2d_out_size(size, k, stride, pad):
+    return (size + 2 * pad - k) // stride + 1
+
+
+def conv2d_choice(batch, height, width, cin, cout, kh, kw, stride=1, pad=(0, 0), out_mode=OUT_F16_NHWC, flags=0, workspace=True):
+    """conv_choice for the general geometry (yb_conv2d_choice); height / width are the input dims, pad = (pad_h, pad_w)."""
+    out = (ctypes.c_int * 6)()
+    _l.check(_l.load().yb_conv2d_choice(batch, height, width, cin, cout, kh, kw, stride, pad[0], pad[1], out_mode, flags, int(bool(workspace)),
+                                        ctypes.byref(out)), 'yb_conv2d_choice')
+    return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5])
+
+
+def conv2d_bn_act(x, w, scale, shift, slope, stride=1, pad=(0, 0), out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, workspace=None):
+    """yb_conv2d_bn_act_fwd: the conv_bn_act unit with kh x kw filters, stride 1 or 2 and zero padding pad = (pad_h, pad_w).
+    x: fp16 [B,H,W,x_ld] (the first `cin` channels, default the weight's); w: fp16 [Cout,kh,kw,Cin] (pack_weight_khw_f16);
+    out (fp16): [B,OH,OW,y_ld] written at channels [y_ch_off, y_ch_off+Cout); out (fp32): [B,Cout,OH,OW]."""
+    _req(x, torch.float16, 'x'); _req(w, torch.float16, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    b, h, wd, x_ld = x.shape
+    cout, kh, kw, wcin = w.shape
+    cin = wcin if cin is None else cin
+    if cin != wcin:
+        raise ValueError('weight Cin %d != %d' % (wcin, cin))
+    oh, ow = conv2d_out_size(h, kh, stride, pad[0]), conv2d_out_size(wd, kw, stride, pad[1])
+    if out is None:
+        out = (torch.empty(b, oh, ow, cout, dtype=torch.float16, device=x.device) if out_mode == OUT_F16_NHWC
+               else torch.empty(b, cout, oh, ow, dtype=torch.float32, device=x.device))
+    if out_mode == OUT_F16_NHWC:
+        _req(out, torch.float16, 'out')
+        y_ld = out.shape[-1]
+    else:
+        _req(out, torch.float32, 'out')
+        y_ld = 0
+    ws_ptr, ws_bytes = (None, 0) if workspace is None else (_p(_req(workspace, torch.uint8, 'workspace')), workspace.numel())
+    _ck(_l.load().yb_conv2d_bn_act_fwd(_p(x), _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, cin, cout, kh, kw, stride, pad[0], pad[1],
+                                       x_ld, y_ld, y_ch_off, out_mode, flags, ws_ptr, ws_bytes, _s()), 'yb_conv2d_bn_act_fwd')
+    return out
+
+
+def pack_weight_khw_f16(w, cout_pad=None, cin_pad=None):
+    """[Cout,Cin,kh,kw] fp32 -> fp16 [cout_pad,kh,kw,cin_pad], zero in the padded filters and channels."""
+    _req(w, torch.float32, 'weight')
+    cout, cin, kh, kw = w.shape
+    cout_pad = cout if cout_pad is None else cout_pad
+    cin_pad = cin if cin_pad is None else cin_pad
+    out = torch.empty(cout_pad, kh, kw, cin_pad, dtype=torch.float16, device=w.device)
+    _ck(_l.load().yb_pack_weight_khw_f16(_p(w), _p(out), cout, cin, kh, kw, cout_pad, cin_pad, _s()), 'yb_pack_weight_khw_f16')
+    return out
+
+
+def stem3x3_s2(x, w, scale, shift, pad=0):
+    """nn.Conv2d(3, 32, 3, stride 2, pad) + folded BatchNorm + ReLU: x fp32 NCHW [B,3,H,W] -> fp16 NHWC [B,OH,OW,32]."""
+    _req(x, torch.float32, 'x'); _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    b, c, h, wd = x.shape
+    if c != 3 or tuple(w.shape) != (32, 3, 3, 3):
+        raise ValueError('stem3x3_s2: x [B,3,H,W] and w [32,3,3,3] expected')
+    out = torch.empty(b, conv2d_out_size(h, 3, 2, pad), conv2d_out_size(wd, 3, 2, pad), 32, dtype=torch.float16, device=x.device)
+    _ck(_l.load().yb_stem3x3_s2_bn_relu_fwd(_p(x), _p(w), _p(scale), _p(shift), _p(out), b, h, wd, pad, _s()), 'yb_stem3x3_s2_bn_relu_fwd')
+    return out
+
+
+def maxpool3x3_s2_valid(x, out=None, y_ch_off=0):
+    """F.max_pool2d(x, 3, stride=2) on fp16 NHWC x [B,H,W,C] into channels [y_ch_off, y_ch_off + C) of out [B,OH,OW,y_ld]."""
+    _req(x, torch.float16, 'x')
+    b, h, w, c = x.shape
+    if out is None:
+        out = torch.empty(b, conv2d_out_size(h, 3, 2, 0), conv2d_out_size(w, 3, 2, 0), c, dtype=torch.float16, device=x.device)
+    _req(out, torch.float16, 'out')
+    _ck(_l.load().yb_maxpool3x3_s2_valid_f16(_p(x), _p(out), out.shape[-1], y_ch_off, b, h, w, c, _s()), 'yb_maxpool3x3_s2_valid_f16')
+    return out
+
+
+def avgpool3x3_s1(x, out=None):
+    """F.avg_pool2d(x, 3, stride=1, padding=1) (count_include_pad=True) on fp16 NHWC x [B,H,W,C]."""
+    _req(x, torch.float16, 'x')
+    b, h, w, c = x.shape
+    out = torch.empty_like(x) if out is None else out
+    _req(out, torch.float16, 'out')
+    _ck(_l.load().yb_avgpool3x3_s1_f16(_p(x), _p(out), b, h, w, c, _s()), 'yb_avgpool3x3_s1_f16')
+    return out
+
+
 def conv1x1_preact(x, w, pre_scale, pre_shift, pre_relu, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0,
                    workspace=None):
     """DenseNet's norm -> relu -> 1x1 conv (yb_conv1x1_preact_fwd): the conv reads a = fp16(act(fmaf(pre_scale, x, pre_shift))) with act = ReLU

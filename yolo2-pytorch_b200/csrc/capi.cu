@@ -131,6 +131,13 @@ int dwconv3x3(const void*, const float*, const float*, const float*, void*, int,
 int dw_dgrad(const void*, const float*, void*, int, int, int, int, int, cudaStream_t);
 int dw_wgrad(const void*, const void*, float*, int, int, int, int, int, cudaStream_t);
 int mb_conv0_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
+int conv2d_choice(int, int, int, int, int, int, int, int, int, int, int, int, int, int*);
+int conv2d_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, int, int, int, int,
+                   long long, int, int, int, void*, long long, double*, int, int, const float*, const float*, int, cudaStream_t);
+int pack_weight_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
+int stem3x3_s2(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
+int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
+int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
 
 }  // namespace yb
 
@@ -477,6 +484,35 @@ int yb_upsample2_zero_f16(const void* x, void* y, int batch, int height, int wid
 int yb_residual_bwd_f16(const void* y, const void* g_a, const void* g_b, int stride_b, void* out, int batch, int height, int width, int channels,
                         yb_stream_t stream) {
   return yb::residual_bwd(y, g_a, g_b, stride_b, out, batch, height, width, channels, S(stream));
+}
+
+int yb_conv2d_bn_act_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch, int in_h, int in_w,
+                         int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int x_ld, long long y_ld, int y_ch_off, int out_mode,
+                         int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
+  return yb::conv2d_forward(x, w, scale, shift, slope, y, batch, in_h, in_w, cin, cout, kh, kw, stride, pad_h, pad_w, x_ld, y_ld, y_ch_off, out_mode,
+                            flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, S(stream));
+}
+
+int yb_conv2d_choice(int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int out_mode, int flags,
+                     int with_workspace, int out[6]) {
+  return yb::conv2d_choice(batch, in_h, in_w, cin, cout, kh, kw, stride, pad_h, pad_w, out_mode, flags, with_workspace, out);
+}
+
+int yb_pack_weight_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, int kh, int kw, int cout_pad, int cin_pad, yb_stream_t stream) {
+  return yb::pack_weight_khw(w_oihw, w_f16, cout, cin, kh, kw, cout_pad, cin_pad, S(stream));
+}
+
+int yb_stem3x3_s2_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height,
+                              int width, int pad, yb_stream_t stream) {
+  return yb::stem3x3_s2(x_nchw, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, pad, S(stream));
+}
+
+int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::maxpool3x3_s2_valid(x, y, y_ld, y_ch_off, batch, height, width, channels, S(stream));
+}
+
+int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::avgpool3x3_s1(x, y, batch, height, width, channels, S(stream));
 }
 
 int yb_comm_version(int* nccl_version) { return yb::comm_version(nccl_version); }

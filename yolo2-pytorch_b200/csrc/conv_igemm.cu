@@ -1,9 +1,10 @@
 // K1: convolution as an implicit GEMM on the Hopper tensor cores (wgmma), sm_90a.
 //
 // Replaces the reference's  nn.Conv2d -> nn.BatchNorm2d(eval) -> nn.LeakyReLU(0.1)  unit
-// (reference model/yolo2.py:49-65) for k in {1,3}, stride 1, pad (k-1)/2.
+// (reference model/yolo2.py:49-65) for k in {1,3}, stride 1, pad (k-1)/2, and the general geometry of Inception-v3
+// (kh x kw filters up to 7 x 7, stride 1 or 2, any padding below the filter size; yb_conv2d_bn_act_fwd).
 //
-//   D[M = B*H*W pixels, N = Cout] = A[M, K = k*k*Cin] * W[N, K]^T
+//   D[M = B*OH*OW output pixels, N = Cout] = A[M, K = kh*kw*Cin] * W[N, K]^T
 //
 //   * A is never materialised: each K-block (one filter tap, BK input channels) of a 128-pixel
 //     M-tile is fetched by ONE im2col-mode TMA (cp.async.bulk.tensor.4d...im2col) straight from
@@ -25,14 +26,15 @@
 namespace yb {
 
 struct ConvParams {
-  int m_total;      // B*H*W
-  int height, width;
+  int m_total;      // B*OH*OW
+  int height, width;  // OUTPUT rows / columns: they drive the M enumeration and the fp32 NCHW epilogue
   int cin, cout;
-  int ksize, pad;
+  int kh, kw, pad_h, pad_w, stride;
+  int in_h, in_w;   // input rows / columns
   int kb_per_tap;   // Cin / BK
-  int num_kb;       // ksize*ksize*kb_per_tap
+  int num_kb;       // kh*kw*kb_per_tap
   int m_tiles, n_tiles;
-  int a_im2col;     // 1: im2col TMA, 0: plain 2D tiled TMA over [M, Cin] (1x1 only)
+  int a_im2col;     // 1: im2col TMA, 0: plain 2D tiled TMA over [M, Cin] (1x1, stride 1 only)
   const float* scale;
   const float* shift;
   float slope;
@@ -257,7 +259,7 @@ __device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmap_a, const
         const int n_tile = tile % p.n_tiles;
         const int m_tile = tile / p.n_tiles;
         const int m_cta = m_tile * Cfg::kRowsPerTile;
-        int img[MT], h0[MT], w0[MT];
+        int img[MT], h0[MT], w0[MT];       // input coordinates of the first output pixel's window corner, per subtile
         int nsub = 0;                      // subtiles that start inside the tensor (the rest are skipped)
 #pragma unroll
         for (int t = 0; t < MT; ++t) {
@@ -265,8 +267,9 @@ __device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmap_a, const
           if (ms < p.m_total) nsub = t + 1;
           img[t] = ms / p.hw;
           const int rem = ms - img[t] * p.hw;
-          h0[t] = rem / p.width;
-          w0[t] = rem - h0[t] * p.width;
+          const int oh = rem / p.width;
+          h0[t] = oh * p.stride - p.pad_h;
+          w0[t] = (rem - oh * p.width) * p.stride - p.pad_w;
         }
         if (p.skip & 1) nsub = 0;
         if (kMergedA && nsub) nsub = MT;      // the merged box always transfers (and zero-fills) both subtiles
@@ -275,8 +278,8 @@ __device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmap_a, const
           const int tap = kb / p.kb_per_tap;
           const int c0 = (kb - tap * p.kb_per_tap) * BK;    // offset inside the (possibly concatenated) weight row of this tap
           const int ca = c0 >= p.a_wrap ? c0 - p.a_wrap : c0;   // activation channel (split mode: the hi part is read twice)
-          const int r = tap / p.ksize;
-          const int s = tap - r * p.ksize;
+          const int r = tap / p.kw;
+          const int s = tap - r * p.kw;
           mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x100 | stage);
           YB_TRACE(0, tr_p); ++tr_p;
           const uint32_t full = bar_full + 8 * stage;
@@ -286,7 +289,7 @@ __device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmap_a, const
             // a large per-instruction cost, rows past the tensor end are zero-filled
             if (!(p.skip & 1)) {
               const uint32_t dst = smem_a + stage * Cfg::kABytes;
-              if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[0] - p.pad, h0[0] - p.pad, img[0], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+              if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[0], h0[0], img[0], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
               else tma_load_2d(dst, &tmap_a, full, ca, m_cta);
             }
           } else {
@@ -294,7 +297,7 @@ __device__ __forceinline__ void conv_igemm_body(const CUtensorMap& tmap_a, const
           for (int t = 0; t < MT; ++t) {
             if (t < nsub) {
               const uint32_t dst = smem_a + stage * Cfg::kABytes + t * Cfg::kASubBytes;
-              if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[t] - p.pad, h0[t] - p.pad, img[t], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+              if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0[t], h0[t], img[t], static_cast<uint16_t>(s), static_cast<uint16_t>(r));
               else tma_load_2d(dst, &tmap_a, full, ca, m_cta + t * BM);
             }
           }
@@ -739,19 +742,20 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         const int m_cta = (it.tile / p.n_tiles) * kWideRows;
         const int img = m_cta / p.hw;
         const int rem = m_cta - img * p.hw;
-        const int h0 = rem / p.width;
-        const int w0 = rem - h0 * p.width;
+        const int oh = rem / p.width;
+        const int h0 = oh * p.stride - p.pad_h;                // input coordinates of the first output pixel's window corner
+        const int w0 = (rem - oh * p.width) * p.stride - p.pad_w;
         for (int kb = it.kb0; kb < it.kb1; ++kb) {
           const int tap = kb / p.kb_per_tap;
           const int c0 = (kb - tap * p.kb_per_tap) * BK;
           const int ca = c0 >= p.a_wrap ? c0 - p.a_wrap : c0;
-          const int r = tap / p.ksize;
-          const int s = tap - r * p.ksize;
+          const int r = tap / p.kw;
+          const int s = tap - r * p.kw;
           mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x600 | stage);
           const uint32_t full = bar_full + 8 * stage;
           mbar_arrive_expect_tx(full, Cfg::kStageBytes);      // the A box always transfers (and zero-fills) all 256 rows
           const uint32_t dst = smem_a + stage * Cfg::kABytes;
-          if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0 - p.pad, h0 - p.pad, img, static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+          if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0, h0, img, static_cast<uint16_t>(s), static_cast<uint16_t>(r));
           else tma_load_2d(dst, &tmap_a, full, ca, m_cta);
           tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, full, tap * p.cin + c0, n_tile * kWideBN);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
@@ -1355,21 +1359,24 @@ static int conv_c32_forward(const void* x, const void* w, const float* scale, co
 // more than plain tiled ones) plus its operand bytes at a per-SM L2->SM rate; the one-warpgroup kernel's epilogue overlaps the
 // next main loop (a tile costs the larger of the two), the two-consumer kernel's register epilogue does not (they add).  With
 // these constants the model picks, on each of those 21 launches, a shape within 3 % of the fastest one measured.
-constexpr double kKbNsIm2col = 240.0;     // ns per K-block, 3x3 layers (im2col-mode A box)
-constexpr double kKbNsTiled = 100.0;      // ns per K-block, 1x1 layers (plain 2-D tiled A box)
+constexpr double kKbNsIm2col = 240.0;     // ns per K-block, every conv but 1x1 stride 1 (im2col-mode A box)
+constexpr double kKbNsTiled = 100.0;      // ns per K-block, 1x1 stride-1 layers (plain 2-D tiled A box)
 constexpr double kFeedBytesPerNs = 130.0; // L2 -> SM operand bytes per ns per SM
 constexpr double kEpiNsPerOut = 0.15;     // one-warpgroup epilogue, ns per output element (overlapped with the main loop)
 constexpr double kWideEpiNsPerOut = 0.08; // two-consumer register epilogue, ns per output element (not overlapped)
 constexpr double kSkNs = 16000.0;         // stream-K partial dump + collect, one-warpgroup kernel
 constexpr double kSkNsWide = 9000.0;      // the same from registers, two-consumer kernel
-int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, int a_channels, int out_mode, int flags, bool workspace_ok,
-                bool stats, bool lo, bool pre, ConvChoice* out) {
+// height / width are the OUTPUT dims (M counts output pixels); a K-block of every conv but 1x1 stride 1 pays the im2col box cost.
+int conv_choose(int batch, int height, int width, int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int a_channels, int out_mode,
+                int flags, bool workspace_ok, bool stats, bool lo, bool pre, ConvChoice* out) {
   ConvChoice c;
   memset(&c, 0, sizeof(c));
   const int sms = sm_count();
   const bool split = a_channels != cin || lo;
-  // 3x3, Cin = 32, Cout <= 64 (layers1.2): halo-tile kernel unless a test asks for one of the im2col kernels
-  if (!split && cin == 32 && ksize == 3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 8) & 0xFFFF) == 0) {
+  const bool same3x3 = kh == 3 && kw == 3 && stride == 1 && pad_h == 1 && pad_w == 1;
+  const bool im2col_cost = !(kh == 1 && kw == 1 && stride == 1);
+  // 3x3 same-padded stride 1, Cin = 32, Cout <= 64 (layers1.2): halo-tile kernel unless a test asks for one of the im2col kernels
+  if (!split && cin == 32 && same3x3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 8) & 0xFFFF) == 0) {
     const long long tiles = static_cast<long long>(batch) * ((width + C32Cfg::TW - 1) / C32Cfg::TW) * ((height + C32Cfg::TH - 1) / C32Cfg::TH);
     c.kernel = kKernelC32; c.bk = 32; c.bn = C32Cfg::BN; c.mt = 1;
     c.grid = static_cast<int>(tiles < sms ? tiles : sms);
@@ -1391,7 +1398,7 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, 
              "conv: BLOCK_N=%d x %d M-subtiles is not a tile shape of this launch (64 x 1, 128 x 1, 64 x 2; 128 x 2 for fp16 NHWC "
              "outputs without residual or statistics)", force_bn, force_mt ? force_mt : 1);
   const long long m_total = static_cast<long long>(batch) * height * width;
-  const int num_kb = ksize * ksize * (cin / bk);
+  const int num_kb = kh * kw * (cin / bk);
   double best = 1e300;
   for (int cbn = 64; cbn <= 128; cbn *= 2) {
     if (force_bn && cbn != force_bn) continue;
@@ -1403,7 +1410,7 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, 
       const int rows_tile = BM * cmt;
       const double tiles = static_cast<double>((m_total + rows_tile - 1) / rows_tile) * ((cout + cbn - 1) / cbn);
       const double rounds = static_cast<double>((static_cast<long long>(tiles) + sms - 1) / sms);
-      const double kb_ns = (ksize == 3 ? kKbNsIm2col : kKbNsTiled) + (cmt * BM + cbn) * bk * 2.0 / kFeedBytesPerNs;
+      const double kb_ns = (im2col_cost ? kKbNsIm2col : kKbNsTiled) + (cmt * BM + cbn) * bk * 2.0 / kFeedBytesPerNs;
       const double main_ns = num_kb * kb_ns;
       const double outs = static_cast<double>(rows_tile) * cbn;
       const double tile_ns = cwide ? main_ns + outs * kWideEpiNsPerOut : (main_ns > outs * kEpiNsPerOut ? main_ns : outs * kEpiNsPerOut);
@@ -1436,28 +1443,55 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int ksize, 
   return 0;
 }
 
-// out = {kernel (kKernel*), BK, BLOCK_N, rows per CTA tile, stream-K, grid} of a yb_conv_bn_act_fwd(_ws) launch
-int conv_choice(int batch, int height, int width, int cin, int cout, int ksize, int out_mode, int flags, int with_workspace, int* out) {
-  YB_REQUIRE(out != nullptr && batch > 0 && height > 0 && width > 0 && cin % 32 == 0 && cout > 0 && (ksize == 1 || ksize == 3),
-             "conv_choice: bad shape");
+// The general geometry accepted by yb_conv2d_bn_act_fwd / yb_conv2d_choice; writes the output dims.
+static int conv_geometry(int in_h, int in_w, int kh, int kw, int stride, int pad_h, int pad_w, int* out_h, int* out_w) {
+  YB_REQUIRE(kh >= 1 && kh <= 7 && kw >= 1 && kw <= 7, "conv2d: kernel %d x %d (1..7 on each axis)", kh, kw);
+  YB_REQUIRE(stride == 1 || stride == 2, "conv2d: stride %d (1 or 2)", stride);
+  YB_REQUIRE(pad_h >= 0 && pad_h < kh && pad_w >= 0 && pad_w < kw, "conv2d: padding (%d, %d) for a %d x %d kernel (0 <= pad < k)", pad_h, pad_w, kh,
+             kw);
+  YB_REQUIRE(in_h > 0 && in_w > 0 && in_h + 2 * pad_h >= kh && in_w + 2 * pad_w >= kw, "conv2d: %d x %d input gives an empty output", in_h, in_w);
+  *out_h = (in_h + 2 * pad_h - kh) / stride + 1;
+  *out_w = (in_w + 2 * pad_w - kw) / stride + 1;
+  return 0;
+}
+
+// out = {kernel (kKernel*), BK, BLOCK_N, rows per CTA tile, stream-K, grid} of a yb_conv2d_bn_act_fwd launch
+int conv2d_choice(int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int out_mode, int flags,
+                  int with_workspace, int* out) {
+  YB_REQUIRE(out != nullptr && batch > 0 && cin > 0 && cin % 32 == 0 && cout > 0, "conv_choice: bad shape");
+  int oh = 0, ow = 0;
+  int rc = conv_geometry(in_h, in_w, kh, kw, stride, pad_h, pad_w, &oh, &ow);
+  if (rc) return rc;
   ConvChoice c;
-  const int rc = conv_choose(batch, height, width, cin, cout, ksize, cin, out_mode, flags, with_workspace != 0, false, false, false, &c);
+  rc = conv_choose(batch, oh, ow, cin, cout, kh, kw, stride, pad_h, pad_w, cin, out_mode, flags, with_workspace != 0, false, false, false, &c);
   if (rc) return rc;
   out[0] = c.kernel; out[1] = c.bk; out[2] = c.bn; out[3] = c.kernel == kKernelC32 ? C32Cfg::TH * C32Cfg::TW : BM * c.mt;
   out[4] = c.streamk; out[5] = c.grid;
   return 0;
 }
 
-int conv_igemm_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
-                       int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
-                       int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off,
-                       const float* pre_scale, const float* pre_shift, int pre_relu, cudaStream_t stream) {
+// the same for a yb_conv_bn_act_fwd(_ws) launch: k x k, stride 1, pad (k-1)/2
+int conv_choice(int batch, int height, int width, int cin, int cout, int ksize, int out_mode, int flags, int with_workspace, int* out) {
+  YB_REQUIRE(out != nullptr && batch > 0 && height > 0 && width > 0 && cin % 32 == 0 && cout > 0 && (ksize == 1 || ksize == 3),
+             "conv_choice: bad shape");
+  return conv2d_choice(batch, height, width, cin, cout, ksize, ksize, 1, (ksize - 1) / 2, (ksize - 1) / 2, out_mode, flags, with_workspace, out);
+}
+
+int conv2d_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch, int in_h, int in_w,
+                   int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int x_ld, long long y_ld, int y_ch_off, int out_mode,
+                   int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off,
+                   const float* pre_scale, const float* pre_shift, int pre_relu, cudaStream_t stream) {
   YB_REQUIRE(x && w && scale && shift && y, "conv: null pointer");
+  YB_REQUIRE(batch > 0, "conv: bad shape");
+  int height = 0, width = 0;      // output dims
+  int rc = conv_geometry(in_h, in_w, kh, kw, stride, pad_h, pad_w, &height, &width);
+  if (rc) return rc;
+  const bool plain_1x1 = kh == 1 && kw == 1 && stride == 1;
   // pre-activation form (pre_scale != NULL): 1x1, plain fp16 operands, no statistics
   const bool pre = pre_scale != nullptr;
   if (pre) {
     YB_REQUIRE(pre_shift != nullptr && (pre_relu == 0 || pre_relu == 1), "conv_preact: pre_shift must be given, pre_relu 0 or 1");
-    YB_REQUIRE(ksize == 1, "conv_preact: k=%d, the pre-activation form is 1x1 only", ksize);
+    YB_REQUIRE(plain_1x1, "conv_preact: k=%d x %d, stride %d: the pre-activation form is 1x1 stride 1 only", kh, kw, stride);
     YB_REQUIRE(a_channels <= 0 || a_channels == cin, "conv_preact: split-precision operands are not supported");
     YB_REQUIRE(lo_ch_off < 0 && stats == nullptr, "conv_preact: no residual output and no fused statistics");
     YB_REQUIRE(cin <= kPreMaxCh, "conv_preact: Cin=%d exceeds the %d-channel pre-activation table", cin, kPreMaxCh);
@@ -1469,9 +1503,7 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
   YB_REQUIRE(lo_ch_off < 0 || (out_mode == 0 && stats == nullptr && lo_ch_off % 8 == 0 && lo_ch_off >= y_ch_off + cout && lo_ch_off + cout <= y_ld),
              "conv: lo_ch_off=%d (needs fp16 NHWC output with room for a second Cout-wide slice)", lo_ch_off);
   YB_REQUIRE(stats == nullptr || out_mode == 0, "conv: fused statistics need the fp16 NHWC output");
-  YB_REQUIRE(ksize == 1 || ksize == 3, "conv: ksize %d unsupported (1 or 3)", ksize);
-  YB_REQUIRE(batch > 0 && height > 0 && width > 0, "conv: bad shape");
-  YB_REQUIRE(cin % 32 == 0, "conv: Cin=%d must be a multiple of 32 (layer 0 uses yb_conv0_*)", cin);
+  YB_REQUIRE(cin > 0 && cin % 32 == 0, "conv: Cin=%d must be a multiple of 32 (layer 0 uses yb_conv0_*)", cin);
   YB_REQUIRE(x_ld >= a_channels && x_ld % 8 == 0, "conv: x_ld=%d", x_ld);
   YB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0, "conv: x/w must be 16B aligned");
   YB_REQUIRE(out_mode == 0 || out_mode == 1, "conv: out_mode");
@@ -1480,20 +1512,21 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
                "conv: fp16 NHWC output needs Cout, y_ld, y_ch_off multiples of 8 and a 16B aligned pointer");
   }
   const long long m_total_ll = static_cast<long long>(batch) * height * width;
-  YB_REQUIRE(m_total_ll < (1ll << 31) - kWideRows, "conv: too many pixels");
+  YB_REQUIRE(m_total_ll < (1ll << 31) - kWideRows && static_cast<long long>(batch) * in_h * in_w < (1ll << 31), "conv: too many pixels");
   // stream-K needs the caller's workspace (one per stream: partial sums + flags)
   const bool ws_ok = workspace != nullptr && workspace_bytes >= conv_workspace_bytes() && (reinterpret_cast<uintptr_t>(workspace) & 255) == 0;
   ConvChoice ch;
-  int rc = conv_choose(batch, height, width, cin, cout, ksize, a_channels, out_mode, flags, ws_ok, stats != nullptr, lo_ch_off >= 0, pre, &ch);
+  rc = conv_choose(batch, height, width, cin, cout, kh, kw, stride, pad_h, pad_w, a_channels, out_mode, flags, ws_ok, stats != nullptr, lo_ch_off >= 0,
+                   pre, &ch);
   if (rc) return rc;
   YB_REQUIRE(!pre || ch.kernel == kKernelIgemm, "conv_preact: no pre-activation form of kernel %d", ch.kernel);
   if (ch.kernel == kKernelC32)
     return conv_c32_forward(x, w, scale, shift, slope, y, batch, height, width, cout, x_ld, y_ld, y_ch_off, (flags >> 4) & 1, flags, stats, stream);
   const int bk = ch.bk, bn = ch.bn, mt = ch.mt, streamk = ch.streamk;
-  // 1x1 layers read A as a plain [pixels, Cin] matrix (2-D tiled TMA: cheaper per instruction than im2col mode);
+  // 1x1 stride-1 layers read A as a plain [pixels, Cin] matrix (2-D tiled TMA: cheaper per instruction than im2col mode);
   // YB_CONV_1X1_IM2COL=1 switches back for A/B runs
   static const int k1x1_im2col = getenv("YB_CONV_1X1_IM2COL") ? atoi(getenv("YB_CONV_1X1_IM2COL")) : 0;
-  const int a_im2col = (ksize == 3) ? 1 : ((k1x1_im2col && !(flags & 1) && !pre) ? 1 : 0);
+  const int a_im2col = !plain_1x1 ? 1 : ((k1x1_im2col && !(flags & 1) && !pre) ? 1 : 0);
 
   EncodeTiledFn enc_tiled;
   EncodeIm2colFn enc_im2col;
@@ -1502,9 +1535,10 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
 
   ConvParams p;
   p.m_total = static_cast<int>(m_total_ll);
-  p.height = height; p.width = width; p.cin = cin; p.cout = cout; p.ksize = ksize; p.pad = (ksize - 1) / 2;
+  p.height = height; p.width = width; p.cin = cin; p.cout = cout;
+  p.kh = kh; p.kw = kw; p.pad_h = pad_h; p.pad_w = pad_w; p.stride = stride; p.in_h = in_h; p.in_w = in_w;
   p.kb_per_tap = cin / bk;
-  p.num_kb = ksize * ksize * p.kb_per_tap;
+  p.num_kb = kh * kw * p.kb_per_tap;
   const int rows_tile = BM * mt;
   p.m_tiles = (p.m_total + rows_tile - 1) / rows_tile;
   p.n_tiles = (cout + bn - 1) / bn;
@@ -1535,13 +1569,15 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
   CUresult cr;
   const int a_rows = BM * mt;     // pixels per A box (ConvCfg::kMergedA)
   if (a_im2col) {
-    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(a_channels), static_cast<cuuint64_t>(width), static_cast<cuuint64_t>(height),
+    // the input tensor; the bounding box of window corners is [-pad, in + pad - k] on each axis, walked with the conv's stride, so
+    // consecutive box pixels are consecutive output pixels (row-major, then the next image)
+    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(a_channels), static_cast<cuuint64_t>(in_w), static_cast<cuuint64_t>(in_h),
                                 static_cast<cuuint64_t>(batch)};
-    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * width,
-                                   static_cast<cuuint64_t>(x_ld) * 2 * width * height};
-    const int lower[2] = {-p.pad, -p.pad};                    // {W, H}
-    const int upper[2] = {p.pad - (ksize - 1), p.pad - (ksize - 1)};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * in_w,
+                                   static_cast<cuuint64_t>(x_ld) * 2 * in_w * in_h};
+    const int lower[2] = {-pad_w, -pad_h};                    // {W, H}
+    const int upper[2] = {pad_w - (kw - 1), pad_h - (kh - 1)};
+    const cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
     cr = enc_im2col(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x), dims, strides, lower, upper,
                     static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(a_rows), estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -1550,7 +1586,7 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
     // tensors smaller than 128 KiB drivers <= 13.1 set a descriptor bit that breaks im2col loads.
     int drv = 0;
     cudaDriverGetVersion(&drv);
-    const unsigned long long span_bytes = static_cast<unsigned long long>(x_ld) * 2ull * width * height * batch;
+    const unsigned long long span_bytes = static_cast<unsigned long long>(x_ld) * 2ull * in_w * in_h * batch;
     if (drv <= 13010 && span_bytes < 131072ull) reinterpret_cast<uint64_t*>(&ta)[1] &= ~(1ull << 21);
   } else {
     const cuuint64_t dims[2] = {static_cast<cuuint64_t>(a_channels), static_cast<cuuint64_t>(p.m_total)};
@@ -1562,7 +1598,7 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(A) failed (%d)", static_cast<int>(cr));
   }
   {
-    const cuuint64_t k_total = static_cast<cuuint64_t>(ksize) * ksize * cin;
+    const cuuint64_t k_total = static_cast<cuuint64_t>(kh) * kw * cin;
     const cuuint64_t dims[2] = {k_total, static_cast<cuuint64_t>(cout)};
     const cuuint64_t strides[1] = {k_total * 2};
     const cuuint32_t box[2] = {static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(bn)};
@@ -1590,6 +1626,16 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
   return dispatch_conv<32>(bn, mt, ch.grid, ta, tb, ty, p, pre ? &pre_act : nullptr, stream);
 }
 
+// k x k, stride 1, pad (k-1)/2: yb_conv_bn_act_fwd(_ws) and its statistics, split and pre-activation forms
+int conv_igemm_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
+                       int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
+                       int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off,
+                       const float* pre_scale, const float* pre_shift, int pre_relu, cudaStream_t stream) {
+  YB_REQUIRE(ksize == 1 || ksize == 3, "conv: ksize %d unsupported (1 or 3)", ksize);
+  return conv2d_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, ksize, 1, (ksize - 1) / 2, (ksize - 1) / 2, x_ld, y_ld,
+                        y_ch_off, out_mode, flags, workspace, workspace_bytes, stats, a_channels, lo_ch_off, pre_scale, pre_shift, pre_relu, stream);
+}
+
 // ---------------------------------------------------------------------------------------------
 // CUDA-core reference of the same unit: test / bisect utility only (never on the product path).
 // One thread per (pixel, cout); fp16 inputs, fp32 accumulate, identical epilogue and outputs.
@@ -1605,14 +1651,14 @@ __global__ void conv_ref_kernel(const __half* __restrict__ x, const __half* __re
   const int h = pix / p.width;
   const int wq = pix - h * p.width;
   float acc = 0.f;
-  for (int r = 0; r < p.ksize; ++r) {
-    const int hi = h + r - p.pad;
-    if (hi < 0 || hi >= p.height) continue;
-    for (int s = 0; s < p.ksize; ++s) {
-      const int wi = wq + s - p.pad;
-      if (wi < 0 || wi >= p.width) continue;
-      const __half* xp = x + (static_cast<long long>(img) * p.hw + static_cast<long long>(hi) * p.width + wi) * x_ld;
-      const __half* wp = w + (static_cast<long long>(co) * p.ksize * p.ksize + r * p.ksize + s) * p.cin;
+  for (int r = 0; r < p.kh; ++r) {
+    const int hi = h * p.stride + r - p.pad_h;
+    if (hi < 0 || hi >= p.in_h) continue;
+    for (int s = 0; s < p.kw; ++s) {
+      const int wi = wq * p.stride + s - p.pad_w;
+      if (wi < 0 || wi >= p.in_w) continue;
+      const __half* xp = x + ((static_cast<long long>(img) * p.in_h + hi) * p.in_w + wi) * x_ld;
+      const __half* wp = w + (static_cast<long long>(co) * p.kh * p.kw + r * p.kw + s) * p.cin;
       for (int c = 0; c < p.cin; ++c) acc += __half2float(xp[c]) * __half2float(wp[c]);
     }
   }
@@ -1632,7 +1678,8 @@ int conv_ref_forward(const void* x, const void* w, const float* scale, const flo
   ConvParams p;
   memset(&p, 0, sizeof(p));
   p.m_total = batch * height * width;
-  p.height = height; p.width = width; p.cin = cin; p.cout = cout; p.ksize = ksize; p.pad = (ksize - 1) / 2;
+  p.height = height; p.width = width; p.cin = cin; p.cout = cout;
+  p.kh = ksize; p.kw = ksize; p.pad_h = (ksize - 1) / 2; p.pad_w = (ksize - 1) / 2; p.stride = 1; p.in_h = height; p.in_w = width;
   p.scale = scale; p.shift = shift; p.slope = slope; p.y = y; p.y_ld = y_ld; p.y_ch_off = y_ch_off; p.out_mode = out_mode;
   p.hw = height * width;
   const long long total = static_cast<long long>(p.m_total) * cout;

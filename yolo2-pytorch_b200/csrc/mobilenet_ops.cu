@@ -1,6 +1,7 @@
 // MobileNet plugin kernels (BASELINE configs[4], "C5"; /root/reference model/mobilenet.py:25-85), inference only.
 //   mb_conv0   conv_bn(3, 32, stride 2): nn.Conv2d(3,32,3,2,1) + BatchNorm2d + ReLU  (:25-30), fp32 NCHW image in,
-//              fp16 NHWC out -- the layout boundary of this backbone.
+//              fp16 NHWC out -- the layout boundary of this backbone.  kPad = 0 is Inception-v3's Conv2d_1a_3x3 (the same conv without
+//              padding, any H, W >= 3).
 //   dwconv3x3  conv_dw: depthwise nn.Conv2d(C,C,3,stride,1,groups=C) + BatchNorm2d + ReLU (:33-38) on fp16 NHWC.
 //              HBM-bound: one thread = 8 channels (16 B) of one output pixel, 9 vector loads, fp32 FMA, 16 B store.
 // The pointwise convs (conv_pw, :41-46) and the 1x1 head reuse the wgmma implicit-GEMM kernel (slope = 0 -> ReLU).
@@ -10,6 +11,7 @@
 
 namespace yb {
 
+template <int kPad>
 __global__ void __launch_bounds__(256) mb_conv0_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ scale,
                                                        const float* __restrict__ shift, __half* __restrict__ y, int batch, int height, int width, int raw,
                                                        int split) {
@@ -18,7 +20,7 @@ __global__ void __launch_bounds__(256) mb_conv0_kernel(const float* __restrict__
   for (int i = threadIdx.x; i < 27 * 32; i += blockDim.x) ws[i / 32][i % 32] = w[(i % 32) * 27 + i / 32];
   if (threadIdx.x < 32) { sc[threadIdx.x] = raw ? 1.f : scale[threadIdx.x]; sh[threadIdx.x] = raw ? 0.f : shift[threadIdx.x]; }
   __syncthreads();
-  const int oh = height >> 1, ow = width >> 1;
+  const int oh = (height + 2 * kPad - 3) / 2 + 1, ow = (width + 2 * kPad - 3) / 2 + 1;
   const long long total = static_cast<long long>(batch) * oh * ow;
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -33,10 +35,10 @@ __global__ void __launch_bounds__(256) mb_conv0_kernel(const float* __restrict__
   for (int c = 0; c < 3; ++c)
 #pragma unroll
     for (int r = 0; r < 3; ++r) {
-      const int iy = 2 * py - 1 + r;
+      const int iy = 2 * py - kPad + r;
 #pragma unroll
       for (int s = 0; s < 3; ++s) {
-        const int ix = 2 * px - 1 + s;
+        const int ix = 2 * px - kPad + s;
         const float v = (iy >= 0 && iy < height && ix >= 0 && ix < width) ? __ldg(x + ((static_cast<long long>(img) * 3 + c) * height + iy) * width + ix) : 0.f;
         const float4* wp = reinterpret_cast<const float4*>(&ws[c * 9 + r * 3 + s][0]);
 #pragma unroll
@@ -72,8 +74,22 @@ int mb_conv0(const float* x, const float* w, const float* scale, const float* sh
              cudaStream_t stream) {
   YB_REQUIRE(x && w && (raw || (scale && shift)) && y && batch > 0 && height % 2 == 0 && width % 2 == 0 && !(raw && split), "mb_conv0: bad argument");
   const long long total = static_cast<long long>(batch) * (height / 2) * (width / 2);
-  mb_conv0_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(x, w, raw ? w : scale, raw ? w : shift, reinterpret_cast<__half*>(y), batch, height, width, raw,
-                                                                                 split);
+  mb_conv0_kernel<1><<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(x, w, raw ? w : scale, raw ? w : shift, reinterpret_cast<__half*>(y), batch, height, width,
+                                                                                    raw, split);
+  return check_launch("mb_conv0_kernel");
+}
+
+// Inception-v3 Conv2d_1a_3x3: nn.Conv2d(3, 32, 3, stride 2, pad `pad`) + folded BatchNorm + ReLU, x fp32 NCHW [B,3,H,W] -> y fp16 NHWC
+// [B,(H+2pad-3)/2+1,(W+2pad-3)/2+1,32].  pad = 1 is the MobileNet instantiation (same bits as mb_conv0 at even H, W).
+int stem3x3_s2(const float* x, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width, int pad,
+               cudaStream_t stream) {
+  YB_REQUIRE(x && w && scale && shift && y && batch > 0 && (pad == 0 || pad == 1), "stem3x3_s2: bad argument (pad 0 or 1)");
+  YB_REQUIRE(height + 2 * pad >= 3 && width + 2 * pad >= 3, "stem3x3_s2: %d x %d input gives an empty output", height, width);
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(y) & 15) == 0, "stem3x3_s2: y must be 16B aligned");
+  const long long total = static_cast<long long>(batch) * ((height + 2 * pad - 3) / 2 + 1) * ((width + 2 * pad - 3) / 2 + 1);
+  const unsigned grid = static_cast<unsigned>((total + 255) / 256);
+  if (pad == 0) mb_conv0_kernel<0><<<grid, 256, 0, stream>>>(x, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, 0, 0);
+  else mb_conv0_kernel<1><<<grid, 256, 0, stream>>>(x, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, 0, 0);
   return check_launch("mb_conv0_kernel");
 }
 
