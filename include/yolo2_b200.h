@@ -377,6 +377,13 @@ int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, i
 /* F.avg_pool2d(x, 3, stride=1, padding=1, count_include_pad=True): x, y [B,H,W,C]; y = fp16(fp32 sum of the in-range window / 9). */
 int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
 
+/* ---- Inception-v4 plugin (model/inception4.py), inference: the convs, the stem and the max-pools are the Inception-v3 entry points above ---
+ * nn.AvgPool2d(3, stride=1, padding=1, count_include_pad=False), the pool of every Inception_A / B / C `branch3` (model/inception4.py:126, 190,
+ * 256): x, y [B,H,W,C] fp16 NHWC; y = fp16(fp32 sum of the in-range 3x3 window in row-major order / n), one round-to-nearest division, with n
+ * the number of in-range pixels (4 in a corner, 6 on an edge, 9 inside; 1 x N and N x 1 images count likewise).  Interior pixels are the bits
+ * of yb_avgpool3x3_s1_f16.  C a multiple of 8, x / y 16-byte aligned. */
+int yb_avgpool3x3_s1_excl_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
+
 /* Training of the ResNet plugin: what torch autograd does for the stem, the max-pool, the stride-2 selection and the residual join.  BatchNorm and
  * the activations are the generic train-mode kernels above (slope 0 = ReLU, slope 1 = identity); the 3x3 / 1x1 convs and their gradients are the
  * wgmma kernels, a stride-2 conv's backward being the stride-1 gradients of the zero-inserted dz (yb_upsample2_zero_f16).

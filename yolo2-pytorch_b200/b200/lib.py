@@ -98,6 +98,7 @@ SIGNATURES = {
     'yb_stem3x3_s2_bn_relu_fwd': [P, P, P, P, P, c_int, c_int, c_int, c_int, P],
     'yb_maxpool3x3_s2_valid_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_avgpool3x3_s1_f16': [P, P, c_int, c_int, c_int, c_int, P],
+    'yb_avgpool3x3_s1_excl_f16': [P, P, c_int, c_int, c_int, c_int, P],
 }
 
 _lib = None

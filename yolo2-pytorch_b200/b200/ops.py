@@ -257,6 +257,16 @@ def avgpool3x3_s1(x, out=None):
     return out
 
 
+def avgpool3x3_s1_excl(x, out=None):
+    """nn.AvgPool2d(3, stride=1, padding=1, count_include_pad=False) on fp16 NHWC x [B,H,W,C]: the divisor is the number of in-range pixels."""
+    _req(x, torch.float16, 'x')
+    b, h, w, c = x.shape
+    out = torch.empty_like(x) if out is None else out
+    _req(out, torch.float16, 'out')
+    _ck(_l.load().yb_avgpool3x3_s1_excl_f16(_p(x), _p(out), b, h, w, c, _s()), 'yb_avgpool3x3_s1_excl_f16')
+    return out
+
+
 def conv1x1_preact(x, w, pre_scale, pre_shift, pre_relu, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0,
                    workspace=None):
     """DenseNet's norm -> relu -> 1x1 conv (yb_conv1x1_preact_fwd): the conv reads a = fp16(act(fmaf(pre_scale, x, pre_shift))) with act = ReLU

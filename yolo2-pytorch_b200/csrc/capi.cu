@@ -138,6 +138,7 @@ int pack_weight_khw(const float*, void*, int, int, int, int, int, int, cudaStrea
 int stem3x3_s2(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
 int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
+int avgpool3x3_s1_excl(const void*, void*, int, int, int, int, cudaStream_t);
 
 }  // namespace yb
 
@@ -513,6 +514,10 @@ int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, i
 
 int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
   return yb::avgpool3x3_s1(x, y, batch, height, width, channels, S(stream));
+}
+
+int yb_avgpool3x3_s1_excl_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::avgpool3x3_s1_excl(x, y, batch, height, width, channels, S(stream));
 }
 
 int yb_comm_version(int* nccl_version) { return yb::comm_version(nccl_version); }

@@ -1,4 +1,5 @@
-// Inception-v3 plugin kernels (model/inception3.py of the reference over torchvision's BasicConv2d / InceptionA-E), inference.
+// Inception-v3 and Inception-v4 plugin kernels (model/inception3.py of the reference over torchvision's BasicConv2d / InceptionA-E, and
+// model/inception4.py), inference.
 //   pack_weight_khw       fp32 OIHW [Cout][Cin][kh][kw] -> fp16 [cout_pad][kh][kw][cin_pad], zeros in the padding: the B operand of the
 //                         general-geometry conv (yb_conv2d_bn_act_fwd), with Cout / Cin rounded up to what the tensor-core conv needs
 //                         (Inception's 80- and 48-channel layers run as 96 / 64 channels whose extra filters and inputs are zero).
@@ -6,6 +7,10 @@
 //                         Mixed_6a / Mixed_7a lands directly in its block's concatenation buffer.
 //   avgpool3x3_s1         F.avg_pool2d(x, 3, stride=1, padding=1) with count_include_pad=True (torchvision's Inception blocks): the
 //                         divisor is 9 at every pixel, borders included.  The branch's 1x1 conv then runs on the pooled tensor.
+//   avgpool3x3_s1_excl    nn.AvgPool2d(3, stride=1, padding=1, count_include_pad=False) (the branch3 pools of model/inception4.py's
+//                         Inception_A / B / C): the divisor is the number of in-range taps, 4 in a corner, 6 on an edge, 9 inside.
+//                         Same kernel as avgpool3x3_s1 with the divisor chosen by a template parameter, so interior pixels are
+//                         bit-identical between the two.
 // The first conv (3 -> 32, 3x3, stride 2, pad 0) is mb_conv0_kernel<0> (mobilenet_ops.cu); every other conv is the implicit GEMM.
 #include "yb_common.h"
 #include "yb_pool.cuh"
@@ -75,7 +80,9 @@ int maxpool3x3_s2_valid(const void* x, void* y, int y_ld, int y_ch_off, int batc
   return check_launch("maxpool3x3_s2_valid_kernel");
 }
 
-// y[b, oy, ox, c] = fp16((sum of the in-range pixels of rows oy-1..oy+1, columns ox-1..ox+1 in fp32, row-major order) / 9)
+// y[b, oy, ox, c] = fp16((sum of the in-range pixels of rows oy-1..oy+1, columns ox-1..ox+1 in fp32, row-major order) / n), one division
+// rounded to nearest; n = 9 (kExclPad false: count_include_pad) or the number of in-range pixels (kExclPad true)
+template <bool kExclPad>
 __global__ void avgpool3x3_s1_kernel(const __half* __restrict__ x, __half* __restrict__ y, int batch, int height, int width, int channels) {
   const int c8 = channels >> 3;
   const long long total = static_cast<long long>(batch) * height * width * c8;
@@ -104,20 +111,35 @@ __global__ void avgpool3x3_s1_kernel(const __half* __restrict__ x, __half* __res
       for (int e = 0; e < 8; ++e) acc[e] += __half2float(hv[e]);
     }
   }
+  float n = 9.f;
+  if (kExclPad) {
+    const int rows = 3 - (py == 0) - (py == height - 1), cols = 3 - (px == 0) - (px == width - 1);
+    n = static_cast<float>(rows * cols);
+  }
   uint4 out;
   __half2* ho = reinterpret_cast<__half2*>(&out);
 #pragma unroll
-  for (int e = 0; e < 4; ++e) ho[e] = __floats2half2_rn(__fdiv_rn(acc[2 * e], 9.f), __fdiv_rn(acc[2 * e + 1], 9.f));
+  for (int e = 0; e < 4; ++e) ho[e] = __floats2half2_rn(__fdiv_rn(acc[2 * e], n), __fdiv_rn(acc[2 * e + 1], n));
   reinterpret_cast<uint4*>(y)[idx] = out;
 }
 
-int avgpool3x3_s1(const void* x, void* y, int batch, int height, int width, int channels, cudaStream_t stream) {
-  YB_REQUIRE(x && y && batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 8 == 0, "avgpool3x3_s1: bad argument (C a multiple of 8)");
-  YB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "avgpool3x3_s1: x / y must be 16B aligned");
+template <bool kExclPad>
+static int avgpool3x3_s1_launch(const void* x, void* y, int batch, int height, int width, int channels, cudaStream_t stream, const char* name) {
+  YB_REQUIRE(x && y && batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 8 == 0, "%s: bad argument (C a multiple of 8)", name);
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0, "%s: x / y must be 16B aligned", name);
   const long long total = static_cast<long long>(batch) * height * width * (channels / 8);
-  avgpool3x3_s1_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const __half*>(x), reinterpret_cast<__half*>(y),
-                                                                                      batch, height, width, channels);
-  return check_launch("avgpool3x3_s1_kernel");
+  avgpool3x3_s1_kernel<kExclPad><<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const __half*>(x),
+                                                                                                 reinterpret_cast<__half*>(y), batch, height,
+                                                                                                 width, channels);
+  return check_launch(kExclPad ? "avgpool3x3_s1_kernel<excl>" : "avgpool3x3_s1_kernel");
+}
+
+int avgpool3x3_s1(const void* x, void* y, int batch, int height, int width, int channels, cudaStream_t stream) {
+  return avgpool3x3_s1_launch<false>(x, y, batch, height, width, channels, stream, "avgpool3x3_s1");
+}
+
+int avgpool3x3_s1_excl(const void* x, void* y, int batch, int height, int width, int channels, cudaStream_t stream) {
+  return avgpool3x3_s1_launch<true>(x, y, batch, height, width, channels, stream, "avgpool3x3_s1_excl");
 }
 
 }  // namespace yb
