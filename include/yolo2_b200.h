@@ -77,6 +77,12 @@ int yb_conv0_bn_leaky_pool_fwd(const float* x_nchw, const float* w_oihw, const f
  * transform/__init__.py) and cuts the host->device copy 4x. */
 int yb_conv0_u8_bn_leaky_pool_fwd(const unsigned char* x_nhwc_u8, const float* w_oihw, const float* scale, const float* shift,
                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream);
+/* VGG's features.0 (model/vgg.py:41-50, make_layers: Conv2d(3, v, 3, padding=1) -> [BatchNorm2d] -> ReLU [-> MaxPool2d(2, 2)]) with 64 filters:
+ * x fp32 NCHW [B,3,H,W] -> y fp16 NHWC [B,H,W,64], or [B,H/2,W/2,64] with pool = 1 (the 2x2 max of the activated values).
+ * w fp32 OIHW [64,3,3,3]; y = act(conv * scale + shift) with act(t) = t > 0 ? t : slope * t.  H % 32 == 0, W % 16 == 0.
+ * A layer with fewer filters runs padded to 64 with zero weights, scale 1 and shift 0. */
+int yb_conv0_c64_bn_act_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, float slope, void* y_nhwc_f16,
+                            int batch, int height, int width, int pool, yb_stream_t stream);
 /* k in {1,3}, stride 1, pad (k-1)/2 conv + per-channel scale/shift + leaky(slope) as a wgmma
  * implicit GEMM.  x: fp16 NHWC [B,H,W,Cin] with pixel pitch x_ld; w: fp16 [Cout][k][k][Cin];
  * y: fp16 NHWC (pixel pitch y_ld, first channel y_ch_off) or fp32 NCHW [B,Cout,H,W].
@@ -250,6 +256,9 @@ int yb_conv0_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw,
 int yb_conv0_wgrad_bn(const float* x_nchw, const void* z_nhwc_f16, const void* dap, long long ld_dap, int dap_off, const float* mean, const float* invstd,
                       const float* gamma, const float* beta, float slope, const double* sums, float* dw_oihw, int batch, int height, int width,
                       yb_stream_t stream);
+/* VGG's features.0 weight gradient [64,3,3,3] (model/vgg.py:41-50, 64 filters) from the fp32 NCHW image and dz fp16 NHWC [B,H,W,64] (the
+ * gradient of the conv output, loss-scaled); dw is overwritten.  H % 8 == 0, W % 32 == 0. */
+int yb_conv0_c64_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream);
 /* wgmma weight gradient: dw_krsc fp32 [Cout][k][k][Cin] (overwritten) from x fp16 NHWC [B,H,W,x_ld] and dz fp16 [B,H,W,dz_ld]. */
 int yb_conv_wgrad(const void* x, const void* dz, float* dw_krsc, int batch, int height, int width, int cin, int cout, int ksize, int x_ld,
                   int dz_ld, yb_stream_t stream);

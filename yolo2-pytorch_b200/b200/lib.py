@@ -19,6 +19,7 @@ SIGNATURES = {
     'yb_bn_fold': [P, P, P, P, c_float, P, P, c_int, P],
     'yb_conv0_bn_leaky_pool_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
     'yb_conv0_u8_bn_leaky_pool_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
+    'yb_conv0_c64_bn_act_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
     'yb_conv_bn_act_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int, P],
     'yb_conv_bn_act_stats_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, P, P],
     'yb_conv_workspace_bytes': [],
@@ -53,6 +54,7 @@ SIGNATURES = {
     'yb_reorg_bwd_f16': [P, c_longlong, c_int, P, c_int, c_int, c_int, c_int, P],
     'yb_head_grad_prepare': [P, P, P, c_int, c_int, c_int, c_int, P],
     'yb_conv0_wgrad': [P, P, P, c_int, c_int, c_int, P],
+    'yb_conv0_c64_wgrad': [P, P, P, c_int, c_int, c_int, P],
     'yb_conv0_wgrad_bn': [P, P, P, c_longlong, c_int, P, P, P, P, c_float, P, P, c_int, c_int, c_int, P],
     'yb_conv_wgrad': [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_unpack_wgrad': [P, P, c_int, c_int, c_int, c_float, P],

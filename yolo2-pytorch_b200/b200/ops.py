@@ -121,6 +121,24 @@ def conv0_u8_bn_leaky_pool(x, w, scale, shift, slope, out=None):
     return out
 
 
+def conv0_c64_bn_act(x, w, scale, shift, slope, pool=False, out=None):
+    """Conv2d(3, 64, 3, padding 1) + scale/shift + activation (+ 2x2 max-pool) of VGG's features.0 (yb_conv0_c64_bn_act_fwd):
+    x fp32 NCHW [B,3,H,W], w fp32 [64,3,3,3], scale / shift fp32 [64] -> fp16 NHWC [B,H,W,64], or [B,H/2,W/2,64] with `pool`."""
+    _req(x, torch.float32, 'x'); _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    b, c, h, wd = x.shape
+    if c != 3 or tuple(w.shape) != (64, 3, 3, 3) or scale.numel() != 64 or shift.numel() != 64:
+        raise ValueError('conv0_c64: x [B,3,H,W], w [64,3,3,3] and 64 scales / shifts expected')
+    oh, ow = (h // 2, wd // 2) if pool else (h, wd)
+    if out is None:
+        out = torch.empty(b, oh, ow, 64, dtype=torch.float16, device=x.device)
+    _req(out, torch.float16, 'out')
+    if tuple(out.shape) != (b, oh, ow, 64):
+        raise ValueError('conv0_c64: out must be [%d,%d,%d,64]' % (b, oh, ow))
+    _ck(_l.load().yb_conv0_c64_bn_act_fwd(_p(x), _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, int(bool(pool)), _s()),
+        'yb_conv0_c64_bn_act_fwd')
+    return out
+
+
 def _conv_common(fn_name, x, w, scale, shift, slope, out, batch, height, width, cin, cout, k, x_ld, y_ld, y_ch_off, out_mode, flags,
                  workspace=None):
     if workspace is not None and fn_name == 'yb_conv_bn_act_fwd':

@@ -1069,3 +1069,167 @@ class ResNetTrainer(TrainerBase):
         self._stem_backward(saved.x, saved.stem, saved.stem_a, g, grads)
         self._finish_backward(dev)
         return grads
+
+
+class VGGTrainer(TrainerBase):
+    """Training-mode forward / backward of `model.vgg.VGG` (reference model/vgg.py): a chain of 3x3 conv units, each conv (with bias) -> BatchNorm2d
+    -> ReLU (`_bn` constructors) or conv -> ReLU, some followed by MaxPool2d(2, 2), then the 1x1 head with bias.
+
+    BatchNorm units are the shared unit: raw conv (bias in the shift, so the running mean sees it; batch statistics in the conv epilogue) ->
+    batch statistics -> running-stat update (momentum and eps from the module) -> normalise + ReLU, with the following max-pool fused into the
+    normalise pass; their backward routes through the pool.  The conv bias before a BatchNorm has an exactly zero gradient (the normalisation
+    removes any per-channel constant), so its arena slot is zero.  Plain units run the inference epilogue (scale 1, shift = bias, ReLU) and
+    keep the unpooled activation a; a following max-pool is a separate yb_maxpool2x2_f16.  Their backward is yb_bn_act_bwd with has_bn = 0
+    and slope 0 on a (for ReLU, a > 0 exactly where the conv output is), routed through the pool to the first maximum of each window; the
+    reduce pass's per-channel sum is the bias gradient.  features.0 reads the fp32 image (yb_conv0_c64_bn_act_fwd: raw with scale 1, shift =
+    bias and slope 1 for a BatchNorm unit, else activated) and its weight gradient is yb_conv0_c64_wgrad; it needs no data gradient."""
+    NAME = 'VGG'
+
+    def __init__(self, dnn, grad_scale=16384.0):
+        TrainerBase.__init__(self, dnn, grad_scale, slope=0.0)
+        self._units = None
+        self._scratch = {}
+
+    def _plan(self):
+        if self._units is None:
+            names = {m: n for n, m in self.dnn.named_modules()}
+            units = []
+            for i, mu in enumerate(self.dnn.units):
+                key = names[mu.conv]
+                bn = names[mu.bn] if mu.bn is not None else None
+                u = _ResUnit(key, mu.conv, mu.bn, 0.0, (key + '.weight', bn and bn + '.weight', bn and bn + '.bias'))
+                u.bias_name, u.pool = key + '.bias', mu.pool
+                units.append(u)
+            self._units = units
+            self._head = _ResUnit('conv', self.dnn.conv, None, 1.0, ('conv.weight', None, None))
+        return self._units
+
+    def grad_order(self):
+        names = ['conv.bias', 'conv.weight']
+        for u in reversed(self._plan()):
+            if u.bn is not None:
+                names += [u.pnames[1], u.pnames[2]]
+            names += [u.bias_name, u.pnames[0]]
+        return names
+
+    def _head_unit(self):
+        return self._head.key, self._head, 'conv.bias'
+
+    def _check(self):
+        units = self._plan()
+        if units[0].cout != 64:
+            raise ValueError('VGG training: features.0 must have 64 filters (has %d)' % units[0].cout)
+        for u in units[1:]:
+            if u.cout % 32:
+                raise ValueError('VGG training: %s has %d filters; training needs multiples of 32' % (u.key, u.cout))
+
+    def _repack(self, device):
+        """Forward and data-gradient fp16 operands of every conv after the first and of the head in ONE batched launch."""
+        cpad = (self._head.cout + 31) // 32 * 32          # the head's filters are padded to the dz buffer's width
+        self._pack([(u.key, u, 0) for u in self._plan()[1:]] + [(self._head.key, self._head, cpad)], device)
+
+    def _buf(self, tag, c, device):
+        t = self._scratch.get((tag, c, str(device)))
+        if t is None:
+            t = self._scratch[(tag, c, str(device))] = torch.empty(c, dtype=torch.float32, device=device)
+        return t
+
+    def forward(self, x):
+        x = self._start_forward(x)
+        b, c, h, w = x.shape
+        if c != 3 or h % 32 or w % 32:
+            raise ValueError('VGG expects [B,3,H,W] with H, W multiples of 32')
+        self._check()
+        dev = x.device
+        units = self._plan()
+        self._repack(dev)
+        saved = _Saved()
+        saved.x, saved.b, saved.units = x, b, []
+        hh, ww = h, w
+        cur = None
+        for i, u in enumerate(units):
+            cur, s = self._unit_forward(u, x if i == 0 else cur, b, hh, ww)
+            saved.units.append(s)
+            if u.pool:
+                hh, ww = hh // 2, ww // 2
+        head = self._head
+        one, _ = self._ones(head.cout, dev)
+        feature = ops.conv_bn_act(cur, head.w16, one, head.conv.bias.detach(), 1.0, out_mode=ops.OUT_F32_NCHW)
+        saved.a_last, saved.hh, saved.ww = cur, hh, ww
+        self._bump_tracked()
+        return feature, saved
+
+    def _unit_forward(self, u, src, b, hh, ww):
+        """One unit on its input (the fp32 image for features.0): returns (its output, pooled when a MaxPool2d follows; saved unit)."""
+        dev = src.device
+        bias = u.conv.bias.detach()
+        first = src.dim() == 4 and src.dtype == torch.float32
+        if u.bn is not None:
+            one, _ = self._ones(u.cout, dev)
+            if first:
+                z = ops.conv0_c64_bn_act(src, u.conv.weight.detach().contiguous(), one, bias, 1.0)
+                stats_done = False
+            elif self.fuse_stats:
+                z, stats_done = ops.conv_bn_act_stats(src, u.w16, one, bias, 1.0, self._sums(('f', u.key), u.cout, dev)), True
+            else:
+                z, stats_done = ops.conv_bn_act(src, u.w16, one, bias, 1.0), False
+            mean, invstd = self._bn_forward(u.key, u, z, b * hh * ww, stats_done)
+            a = self._apply(u, z, mean, invstd, b, hh, ww, u.pool)
+            return a, self._saved_unit(u, None if first else src, z, mean, invstd, hh, ww, u.pool)
+        one, _ = self._ones(u.cout, dev)
+        if first:
+            a = ops.conv0_c64_bn_act(src, u.conv.weight.detach().contiguous(), one, bias, 0.0)
+        else:
+            a = ops.conv_bn_act(src, u.w16, one, bias, 0.0)
+        out = ops.maxpool2x2(a) if u.pool else a
+        return out, self._saved_unit(u, None if first else src, a, None, None, hh, ww, u.pool)
+
+    def _plain_backward(self, s, b, grads, g):
+        """Plain unit: ReLU (+ max-pool) backward on the stored activation into dz, and the bias gradient from the reduce pass's sums."""
+        u = s.u
+        dev = s.z.device
+        da, dap = (None, g) if s.pooled else (g, None)
+        dz = torch.empty(b, s.h, s.w, u.cout, dtype=torch.float16, device=dev)
+        sums = self._sums(('b', u.key), u.cout, dev)
+        args = (s.z, u.cout, None, None, None, None, 0.0, da, 0 if da is None else da.shape[-1], 0, dap, 0 if dap is None else dap.shape[-1], 0,
+                b, s.h, s.w, u.cout, int(dap is not None), sums)
+        ops.call('yb_bn_act_bwd', 0, *args, None, 0, 0)
+        ops.call('yb_bn_act_bwd', 1, *args, dz, u.cout, 0)
+        dbias = self.arena.views[u.bias_name]
+        ops.call('yb_bn_param_grad', sums, u.cout, self._buf('dgamma', u.cout, dev), dbias, 1, self._unscale)
+        grads[u.bias_name] = dbias
+        self._emit(u.bias_name, grads)
+        return dz
+
+    def _bn_unit_backward(self, s, b, grads, g):
+        """BatchNorm unit: the shared BN + ReLU (+ pool) backward into dz, dgamma and dbeta; the conv bias before it gets its zero gradient."""
+        u = s.u
+        da, dap = (None, g) if s.pooled else (g, None)
+        dz = torch.empty(b, s.h, s.w, u.cout, dtype=torch.float16, device=s.z.device)
+        self._bn_backward(u.key, s, b, grads, dz, da=da, dap=dap)
+        dbias = self.arena.views[u.bias_name]
+        dbias.zero_()
+        grads[u.bias_name] = dbias
+        self._emit(u.bias_name, grads)
+        return dz
+
+    def backward(self, saved, dfeature):
+        b = saved.b
+        grads = {}
+        dev = dfeature.device
+        self._start_backward(dev)
+        g = self._head_backward(saved.a_last, saved.hh, saved.ww, dfeature, grads)
+        for s in reversed(saved.units):
+            u = s.u
+            dz = self._bn_unit_backward(s, b, grads, g) if u.bn is not None else self._plain_backward(s, b, grads, g)
+            if s.ain is not None:
+                self._wgrad(u, s.ain, dz, b, s.h, s.w, grads, u.key)
+                g = self._dgrad(u.key, u, dz)
+                continue
+            x = saved.x
+            dw = self.arena.views[u.pnames[0]]
+            ops.call('yb_conv0_c64_wgrad', x, dz, dw, b, x.shape[2], x.shape[3])
+            grads[u.pnames[0]] = dw.mul_(self._unscale)
+            self._emit(u.pnames[0], grads)
+        self._finish_backward(dev)
+        return grads

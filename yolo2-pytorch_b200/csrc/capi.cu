@@ -75,6 +75,8 @@ int pack_weights_batch(const void*, int, int, cudaStream_t);
 void conv_set_trace(void*);
 int bn_fold(const float*, const float*, const float*, const float*, float, float*, float*, int, cudaStream_t);
 int conv0_tc_forward(const void*, int, const float*, const float*, const float*, float, void*, int, int, int, int, int, double*, cudaStream_t);
+int conv0_c64_forward(const float*, const float*, const float*, const float*, float, void*, int, int, int, int, cudaStream_t);
+int conv0_c64_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
 int maxpool2x2(const void*, void*, int, int, int, int, int, cudaStream_t);
 int maxpool2x2_s1(const void*, void*, int, int, int, int, int, cudaStream_t);
 int maxpool2x2_s1_bwd(const void*, const void*, void*, int, int, int, int, cudaStream_t);
@@ -176,6 +178,11 @@ int yb_conv0_bn_leaky_pool_fwd(const float* x_nchw, const float* w_oihw, const f
 int yb_conv0_u8_bn_leaky_pool_fwd(const unsigned char* x_nhwc_u8, const float* w_oihw, const float* scale, const float* shift,
                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream) {
   return yb::conv0_tc_forward(x_nhwc_u8, 1, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, cout, 0, nullptr, S(stream));
+}
+
+int yb_conv0_c64_bn_act_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, float slope, void* y_nhwc_f16,
+                            int batch, int height, int width, int pool, yb_stream_t stream) {
+  return yb::conv0_c64_forward(x_nchw, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, pool, S(stream));
 }
 
 int yb_conv_bn_act_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -355,6 +362,10 @@ int yb_reorg_bwd_f16(const void* dy, long long ld_dy, int dy_off, void* dx, int 
 int yb_head_grad_prepare(const float* dfeature, void* dz_nhwc_f16, float* dbias, int batch, int channels, int channels_pad, int cells,
                          yb_stream_t stream) {
   return yb::head_grad_prepare(dfeature, dz_nhwc_f16, dbias, batch, channels, channels_pad, cells, S(stream));
+}
+
+int yb_conv0_c64_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream) {
+  return yb::conv0_c64_wgrad(x_nchw, dz_nhwc_f16, dw_oihw, batch, height, width, S(stream));
 }
 
 int yb_conv0_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream) {

@@ -488,4 +488,256 @@ int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* sc
   return check_launch("conv0_tc_kernel");
 }
 
+// ---------------------------------------------------------------------------------------------
+// 64-filter form of conv0_k16_kernel: VGG's features.0, Conv2d(3, 64, 3, padding 1) + bias or folded BatchNorm + ReLU, optionally followed by
+// MaxPool2d(2, 2) (model/vgg.py make_layers).  Same 32 x 16 tiles and operands read in place (patch_e / patch_o, per-filter-row B), N = 64.
+// A whole tile's accumulators at N = 64 would be 4 x 2 x 32 = 256 registers per thread, so the tile runs as two passes over accumulator
+// rows 0..63 (window rows 0..7, pixel rows 0..15) and 64..127: per pass 4 x 3 wgmma (M 64, N 64, K 16) into 4 x 32 registers, then that
+// pass's epilogue.  kPool: scale/shift + activation on the four pixels of each window, their max stored from registers as the 32-filter form.
+// Otherwise the pass's 16 x 16 pixels x 64 channels are staged in shared memory (32 KB; pixel col at slot col / 2 + (col & 1) * 8 of its row,
+// 16-byte chunk jj at jj ^ (col / 2)) and leave as 2 KB contiguous rows.  scale / shift are read through the L1 (the static shared memory is
+// at its 48 KB limit).
+constexpr int kC64Out = 64;
+constexpr int kC64StageBytes = (kV2Rows / 2) * kV2Cols * kC64Out * 2;   // 32 KB
+
+template <bool kPool>
+__global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_c64_kernel(const Conv0Params p) {
+  __shared__ __align__(128) uint8_t stage[kPool ? 16 : kC64StageBytes];
+  __shared__ __align__(128) uint8_t patch_e[kV2Copy + 48];
+  __shared__ __align__(128) uint8_t patch_o[kV2Copy + 48];
+  __shared__ __align__(128) uint8_t b_smem[3 * 2048];           // per filter row: [n / 8][k / 8][n % 8][k % 8] fp16 (64 x 16)
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t e_base = smem_u32(patch_e), o_base = smem_u32(patch_o), b_base = smem_u32(b_smem);
+
+  if (tid < 12) {
+    reinterpret_cast<uint32_t*>(patch_e + kV2Copy)[tid] = 0u;
+    reinterpret_cast<uint32_t*>(patch_o + kV2Copy)[tid] = 0u;
+  }
+  if (tid < 2) reinterpret_cast<uint32_t*>(patch_o)[tid] = 0u;
+#pragma unroll
+  for (int n0 = 0; n0 < kC64Out; n0 += 32) {
+    // B operand, filter row r: element (n, k = s * 4 + c) = w[n][c][r][s] for s, c < 3, else 0
+    const int n = n0 + (tid >> 2), s4 = tid & 3;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      float v[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) v[c] = (s4 < 3 && c < 3) ? __ldg(p.w + n * 27 + c * 9 + r * 3 + s4) : 0.f;
+      const uint2 pk = make_uint2(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]));
+      *reinterpret_cast<uint2*>(b_smem + r * 2048 + (n >> 3) * 256 + (s4 >> 1) * 128 + (n & 7) * 16 + (s4 & 1) * 8) = pk;
+    }
+  }
+  __syncthreads();
+  pdl_trigger();
+
+  const int oh = p.height >> 1, ow = p.width >> 1;
+  auto prefetch = [&](int t, float (&v)[kV2Iters][3]) {
+    const int ptx = t % p.tiles_x;
+    const int pt2 = t / p.tiles_x;
+    const int pty = pt2 % p.tiles_y;
+    const int pimg = pt2 / p.tiles_y;
+    const int y0 = pty * kV2Rows - 1, x0 = ptx * kV2Cols - 1;
+#pragma unroll
+    for (int k = 0; k < kV2Iters; ++k) {
+      const int i = tid + k * 128;
+      const int r = i / kV2PC, c = i - r * kV2PC;
+      const int iy = y0 + r, ix = x0 + c;
+      const bool ok = i < kV2Pixels && iy >= 0 && iy < p.height && ix >= 0 && ix < p.width;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch)
+        v[k][ch] = ok ? __ldg(reinterpret_cast<const float*>(p.x) + ((static_cast<long long>(pimg) * 3 + ch) * p.height + iy) * p.width + ix) : 0.f;
+    }
+  };
+  float pre[kV2Iters][3];
+  if (static_cast<int>(blockIdx.x) < p.num_tiles) prefetch(blockIdx.x, pre);
+
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int tx = tile % p.tiles_x;
+    const int t2 = tile / p.tiles_x;
+    const int ty = t2 % p.tiles_y;
+    const int img = t2 / p.tiles_y;
+    __syncthreads();                                // the previous tile's wgmma and copy-out are done with the patch and the stage
+#pragma unroll
+    for (int k = 0; k < kV2Iters; ++k) {
+      const int i = tid + k * 128;
+      if (i < kV2Pixels) {
+        const uint2 pk = make_uint2(pack_h2(pre[k][0], pre[k][1]), pack_h2(pre[k][2], 0.f));
+        *reinterpret_cast<uint2*>(patch_e + i * 8) = pk;
+        *reinterpret_cast<uint2*>(patch_o + 8 + i * 8) = pk;
+      }
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      float acc[4][32];
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int dy = j >> 1, dx = j & 1;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+          const uint32_t a_addr = (dx ? o_base + 8 : e_base) + ((dy + r) * kV2PC + dx) * 8 + h * 8 * (2 * kV2Pitch);
+          wgmma_f16<kC64Out>(acc[j], make_kmajor_desc_noswz(a_addr, 16, 2 * kV2Pitch), make_kmajor_desc_noswz(b_base + r * 2048, 128, 256), r != 0);
+        }
+      }
+      wgmma_commit();
+      if (h == 0) {
+        const int next = tile + gridDim.x;
+        if (next < p.num_tiles) prefetch(next, pre);
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) fence_regs(acc[j]);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = 64 * h + 16 * warp + (lane >> 2) + 8 * hh;
+        const int wy = m >> 3, wx = m & 7;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int c = 8 * jj + 2 * (lane & 3);
+          const float s0 = __ldg(p.scale + c), s1 = __ldg(p.scale + c + 1), b0 = __ldg(p.shift + c), b1 = __ldg(p.shift + c + 1);
+          if constexpr (kPool) {
+            float best0 = -INFINITY, best1 = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              float t0 = acc[j][4 * jj + 2 * hh] * s0 + b0, t1 = acc[j][4 * jj + 2 * hh + 1] * s1 + b1;
+              t0 = t0 > 0.f ? t0 : t0 * p.slope;
+              t1 = t1 > 0.f ? t1 : t1 * p.slope;
+              best0 = fmaxf(best0, t0);
+              best1 = fmaxf(best1, t1);
+            }
+            const int py = ty * (kV2Rows / 2) + wy, px = tx * (kV2Cols / 2) + wx;
+            *reinterpret_cast<uint32_t*>(p.y + ((static_cast<long long>(img) * oh + py) * ow + px) * kC64Out + c) = pack_h2(best0, best1);
+          } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              float t0 = acc[j][4 * jj + 2 * hh] * s0 + b0, t1 = acc[j][4 * jj + 2 * hh + 1] * s1 + b1;
+              t0 = t0 > 0.f ? t0 : t0 * p.slope;
+              t1 = t1 > 0.f ? t1 : t1 * p.slope;
+              const int row = 2 * (wy - 8 * h) + (j >> 1), slot = wx + (j & 1) * 8;
+              *reinterpret_cast<uint32_t*>(stage + (row * kV2Cols + slot) * (kC64Out * 2) + ((jj ^ wx) << 4) + (lane & 3) * 4) = pack_h2(t0, t1);
+            }
+          }
+        }
+      }
+      if constexpr (!kPool) {
+        __syncthreads();                            // the pass is staged
+        // 16 rows x 128 chunks of 16 B: on every trip thread tid copies chunk g = tid % 8 of pixel col = tid / 8 of one row
+        const int col = tid >> 3, g = tid & 7;
+        const int src_off = ((col >> 1) + (col & 1) * 8) * (kC64Out * 2) + ((g ^ (col >> 1)) << 4);
+        __half* dst = p.y + ((static_cast<long long>(img) * p.height + ty * kV2Rows + 16 * h) * p.width + tx * kV2Cols + col) * kC64Out + g * 8;
+#pragma unroll 4
+        for (int row = 0; row < kV2Rows / 2; ++row) {
+          const uint4 q = *reinterpret_cast<const uint4*>(stage + row * (kV2Cols * kC64Out * 2) + src_off);
+          *reinterpret_cast<uint4*>(dst + static_cast<long long>(row) * p.width * kC64Out) = q;
+        }
+        __syncthreads();                            // copied out before the next pass stages over it
+      }
+    }
+  }
+}
+
+int conv0_c64_forward(const float* x, const float* w, const float* scale, const float* shift, float slope, void* y, int batch, int height,
+                      int width, int pool, cudaStream_t stream) {
+  YB_REQUIRE(x && w && scale && shift && y, "conv0_c64: null pointer");
+  YB_REQUIRE(batch > 0 && height > 0 && width > 0 && height % kV2Rows == 0 && width % kV2Cols == 0,
+             "conv0_c64: H must be a multiple of %d and W of %d (got %dx%d)", kV2Rows, kV2Cols, height, width);
+  Conv0Params p;
+  p.x = x; p.w = w; p.scale = scale; p.shift = shift; p.slope = slope; p.y = reinterpret_cast<__half*>(y);
+  p.batch = batch; p.height = height; p.width = width;
+  p.tiles_x = width / kV2Cols;
+  p.tiles_y = height / kV2Rows;
+  const long long tiles = static_cast<long long>(p.tiles_x) * p.tiles_y * batch;
+  YB_REQUIRE(tiles < (1ll << 31), "conv0_c64: too many tiles");
+  p.num_tiles = static_cast<int>(tiles);
+  p.raw = 0;
+  p.stats = nullptr;
+  p.dbg = debug_word_device();
+  const int max_ctas = sm_count() * kC0CtasPerSm;
+  const int grid = p.num_tiles < max_ctas ? p.num_tiles : max_ctas;
+  if (pool) conv0_c64_kernel<true><<<grid, 128, 0, stream>>>(p);
+  else conv0_c64_kernel<false><<<grid, 128, 0, stream>>>(p);
+  return check_launch("conv0_c64_kernel");
+}
+
+// ---------------------------------------------------------------------------------------------
+// Weight gradient of the 64-filter first layer: dw[co][ci][r][s] = sum over (b, y, x) of x[b][ci][y + r - 1][x + s - 1] * dz[b][y][x][co], from
+// the caller's fp32 NCHW image and the fp16 NHWC gradient of the layer's conv output.  The reduction runs over B*H*W pixels in 8 x 32 pixel
+// tiles spread over persistent CTAs (4 per SM).  A CTA stages the haloed fp32 patch and the tile's dz (32 KB) in shared memory; thread
+// (co = tid % 64, tap group tid / 64) owns the taps g, g + 4, ... (7 or 6 of the 27) of filter co and accumulates them in fp32 registers
+// over all its tiles: per pixel one dz load (a warp reads 32 consecutive channels) and one broadcast patch load per tap.  The 27 x 64
+// partial sums of every CTA are added into dw (zeroed first) with atomics.
+constexpr int kCW0Rows = 8, kCW0Cols = 32, kCW0Pix = kCW0Rows * kCW0Cols;
+constexpr int kCW0PR = kCW0Rows + 2, kCW0PC = kCW0Cols + 2;
+constexpr int kCW0CtasPerSm = 4;
+
+__global__ void __launch_bounds__(256, kCW0CtasPerSm) conv0_c64_wgrad_kernel(const float* __restrict__ x, const __half* __restrict__ dz,
+                                                                            float* __restrict__ dw, int height, int width, int tiles_x,
+                                                                            int tiles_y, int num_tiles) {
+  __shared__ __align__(16) __half dzs[kCW0Pix * kC64Out];
+  __shared__ float patch[3 * kCW0PR * kCW0PC];
+  const int tid = threadIdx.x, co = tid & 63, tg = tid >> 6;
+  int off[7];
+#pragma unroll
+  for (int j = 0; j < 7; ++j) {
+    const int tap = tg + 4 * j < 27 ? tg + 4 * j : 0;
+    off[j] = ((tap / 9) * kCW0PR + (tap % 9) / 3) * kCW0PC + tap % 3;
+  }
+  float acc[7];
+#pragma unroll
+  for (int j = 0; j < 7; ++j) acc[j] = 0.f;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int tx = tile % tiles_x;
+    const int t2 = tile / tiles_x;
+    const int ty = t2 % tiles_y;
+    const int img = t2 / tiles_y;
+    const int y0 = ty * kCW0Rows, x0 = tx * kCW0Cols;
+    __syncthreads();                              // the previous tile's reads are done
+    for (int i = tid; i < 3 * kCW0PR * kCW0PC; i += 256) {
+      const int c = i / (kCW0PR * kCW0PC);
+      const int rem = i - c * (kCW0PR * kCW0PC);
+      const int r = rem / kCW0PC, col = rem - r * kCW0PC;
+      const int iy = y0 - 1 + r, ix = x0 - 1 + col;
+      patch[i] = (iy >= 0 && iy < height && ix >= 0 && ix < width)
+                     ? __ldg(x + ((static_cast<long long>(img) * 3 + c) * height + iy) * width + ix) : 0.f;
+    }
+    // dz tile: 8 rows of 32 pixels x 128 B, each row contiguous in memory
+#pragma unroll
+    for (int k = 0; k < kCW0Pix * kC64Out / 8 / 256; ++k) {
+      const int i = tid + k * 256;                // 16-byte chunk: row i / 256, chunk i % 256 of that row
+      const int r = i >> 8, q = i & 255;
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(dz + ((static_cast<long long>(img) * height + y0 + r) * width + x0) * kC64Out) + q);
+      reinterpret_cast<uint4*>(dzs)[i] = v;
+    }
+    __syncthreads();
+#pragma unroll 2
+    for (int p = 0; p < kCW0Pix; ++p) {
+      const float d = __half2float(dzs[p * kC64Out + co]);
+      const int po = (p >> 5) * kCW0PC + (p & 31);
+#pragma unroll
+      for (int j = 0; j < 7; ++j) acc[j] = fmaf(patch[off[j] + po], d, acc[j]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 7; ++j)
+    if (tg + 4 * j < 27) atomicAdd(dw + co * 27 + tg + 4 * j, acc[j]);
+}
+
+int conv0_c64_wgrad(const float* x, const void* dz, float* dw, int batch, int height, int width, cudaStream_t stream) {
+  YB_REQUIRE(x && dz && dw, "conv0_c64_wgrad: null pointer");
+  YB_REQUIRE(batch > 0 && height > 0 && width > 0 && height % kCW0Rows == 0 && width % kCW0Cols == 0,
+             "conv0_c64_wgrad: H must be a multiple of %d and W of %d (got %dx%d)", kCW0Rows, kCW0Cols, height, width);
+  YB_CUDA(cudaMemsetAsync(dw, 0, 64 * 27 * sizeof(float), stream));
+  const int tiles_x = width / kCW0Cols, tiles_y = height / kCW0Rows;
+  const long long tiles = static_cast<long long>(tiles_x) * tiles_y * batch;
+  YB_REQUIRE(tiles < (1ll << 31), "conv0_c64_wgrad: too many tiles");
+  const int cap = sm_count() * kCW0CtasPerSm;
+  const int grid = tiles < cap ? static_cast<int>(tiles) : cap;
+  conv0_c64_wgrad_kernel<<<grid, 256, 0, stream>>>(x, reinterpret_cast<const __half*>(dz), dw, height, width, tiles_x, tiles_y,
+                                                   static_cast<int>(tiles));
+  return check_launch("conv0_c64_wgrad_kernel");
+}
+
 }  // namespace yb
