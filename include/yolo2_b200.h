@@ -393,6 +393,44 @@ int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int widt
  * of yb_avgpool3x3_s1_f16.  C a multiple of 8, x / y 16-byte aligned. */
 int yb_avgpool3x3_s1_excl_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
 
+/* Training of the Inception-v3 plugin (model/inception3.py): the gradients of the general-geometry conv and of the stem, the pools and the joins.
+ *   conv2d_wgrad        dw fp32 [Cout][kh][kw][Cin] (overwritten, not scaled) of the yb_conv2d_bn_act_fwd geometry: kh, kw in 1..7, pad < k,
+ *                       stride 1 or 2, Cin a multiple of 32 up to 2048; x fp16 [B,in_h,in_w,x_ld] (channels [0, Cin) read), dz fp16
+ *                       [B,OH,OW,dz_ld] at the conv's output grid (channels [0, Cout) read).  For (k, k, 1, (k-1)/2) it is yb_conv_wgrad, bit for
+ *                       bit.  YB_WGRAD_SPLITS overrides the split count of the pixel range, as for yb_conv_wgrad.
+ *   unpack_wgrad_khw    fp32 [Cout][kh][kw][krsc_cin] -> the reference's OIHW [Cout][Cin][kh][kw], times `scale` (krsc_cin >= Cin: the
+ *                       activation carried zero channels beyond the module's Cin).
+ *   pack_weight_dgrad_khw  fp32 OIHW [Cout][Cin][kh][kw] -> fp16 [cin_pad][kh][kw][cout_pad], rotated by 180 degrees and transposed, zeros in the
+ *                       padding: the data gradient is yb_conv2d_bn_act_fwd on dz at padding (kh-1-pad_h, kw-1-pad_w), stride 1 (on the
+ *                       zero-inserted dz, yb_upsample2_zero_f16, for a stride-2 conv).
+ *   stem3x3_s2_raw      Conv2d_1a_3x3's raw output z fp16 NHWC [B,(H+2pad-3)/2+1,(W+2pad-3)/2+1,32] (no BatchNorm, no ReLU); pad 0 or 1;
+ *   stem3x3_s2_wgrad    its weight gradient dw fp32 OIHW [32,3,3,3] (overwritten) from the fp32 NCHW image and dz of that shape;
+ *   maxpool3x3_s2_valid_bwd  dx [B,H,W,C] from the pool's input x [B,H,W,C] and dy = channels [dy_ch_off, dy_ch_off + C) of
+ *                       [B,(H-3)/2+1,(W-3)/2+1,dy_ld]: each output's gradient goes to the first maximum of its window in scan order; a
+ *                       gather, deterministic.  C, dy_ld, dy_ch_off multiples of 8;
+ *   join_f16            out = a + b (+ c (+ d)), count fp16 elements summed in fp32 and rounded once (c / d may be NULL). */
+int yb_conv2d_wgrad(const void* x, const void* dz, float* dw_krsc, int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride,
+                    int pad_h, int pad_w, int x_ld, int dz_ld, yb_stream_t stream);
+int yb_unpack_wgrad_khw(const float* dw_krsc, float* dw_oihw, int cout, int cin, int kh, int kw, int krsc_cin, float scale, yb_stream_t stream);
+int yb_pack_weight_dgrad_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, int kh, int kw, int cout_pad, int cin_pad, yb_stream_t stream);
+int yb_stem3x3_s2_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, int pad, yb_stream_t stream);
+int yb_stem3x3_s2_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, int pad, yb_stream_t stream);
+int yb_maxpool3x3_s2_valid_bwd_f16(const void* x, const void* dy, int dy_ld, int dy_ch_off, void* dx, int batch, int height, int width, int channels,
+                                   yb_stream_t stream);
+int yb_join_f16(const void* a, const void* b, const void* c, const void* d, void* out, long long count, yb_stream_t stream);
+/* Both operands of many kh x kw units in ONE launch (the training step re-packs every weight).  `units_dev` is a DEVICE array of at most 256
+ * units; unit i owns the flat element range [elem0, elem0 + 2n), n = cout_pad * kh * kw * cin_pad, with elem0 ascending from 0 and
+ * total_elems = the end of the last range.  out_fwd = the yb_pack_weight_khw_f16 layout, out_dgrad = the yb_pack_weight_dgrad_khw_f16 layout,
+ * bit for bit; either may be NULL. */
+typedef struct yb_pack_khw_unit {
+  const float* w_oihw;
+  void* out_fwd;
+  void* out_dgrad;
+  long long elem0;
+  int cout, cin, kh, kw, cout_pad, cin_pad;
+} yb_pack_khw_unit;
+int yb_pack_weights_khw_batch(const yb_pack_khw_unit* units_dev, int num_units, long long total_elems, yb_stream_t stream);
+
 /* Training of the ResNet plugin: what torch autograd does for the stem, the max-pool, the stride-2 selection and the residual join.  BatchNorm and
  * the activations are the generic train-mode kernels above (slope 0 = ReLU, slope 1 = identity); the 3x3 / 1x1 convs and their gradients are the
  * wgmma kernels, a stride-2 conv's backward being the stride-1 gradients of the zero-inserted dz (yb_upsample2_zero_f16).

@@ -101,6 +101,14 @@ SIGNATURES = {
     'yb_maxpool3x3_s2_valid_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_avgpool3x3_s1_f16': [P, P, c_int, c_int, c_int, c_int, P],
     'yb_avgpool3x3_s1_excl_f16': [P, P, c_int, c_int, c_int, c_int, P],
+    'yb_conv2d_wgrad': [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_unpack_wgrad_khw': [P, P, c_int, c_int, c_int, c_int, c_int, c_float, P],
+    'yb_pack_weight_dgrad_khw_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_stem3x3_s2_raw_fwd': [P, P, P, c_int, c_int, c_int, c_int, P],
+    'yb_stem3x3_s2_wgrad': [P, P, P, c_int, c_int, c_int, c_int, P],
+    'yb_maxpool3x3_s2_valid_bwd_f16': [P, P, c_int, c_int, P, c_int, c_int, c_int, c_int, P],
+    'yb_join_f16': [P, P, P, P, P, c_longlong, P],
+    'yb_pack_weights_khw_batch': [P, c_int, c_longlong, P],
 }
 
 _lib = None

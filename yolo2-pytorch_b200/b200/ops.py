@@ -285,6 +285,77 @@ def avgpool3x3_s1_excl(x, out=None):
     return out
 
 
+def conv2d_wgrad(x, dz, kh, kw, stride=1, pad=(0, 0), cin=None, cout=None, out=None):
+    """yb_conv2d_wgrad: fp32 [Cout,kh,kw,Cin] (not scaled) of the yb_conv2d_bn_act_fwd geometry, from x fp16 [B,H,W,x_ld] (channels [0, cin))
+    and dz fp16 [B,OH,OW,dz_ld] (channels [0, cout)) at the conv's output grid."""
+    _req(x, torch.float16, 'x'); _req(dz, torch.float16, 'dz')
+    b, h, wd, x_ld = x.shape
+    cin = x_ld if cin is None else cin
+    cout = dz.shape[-1] if cout is None else cout
+    if tuple(dz.shape[:3]) != (b, conv2d_out_size(h, kh, stride, pad[0]), conv2d_out_size(wd, kw, stride, pad[1])):
+        raise ValueError('conv2d_wgrad: dz %s is not the output grid of x %s' % (tuple(dz.shape), tuple(x.shape)))
+    out = torch.empty(cout, kh, kw, cin, dtype=torch.float32, device=x.device) if out is None else _req(out, torch.float32, 'out')
+    _ck(_l.load().yb_conv2d_wgrad(_p(x), _p(dz), _p(out), b, h, wd, cin, cout, kh, kw, stride, pad[0], pad[1], x_ld, dz.shape[-1], _s()),
+        'yb_conv2d_wgrad')
+    return out
+
+
+def pack_weight_dgrad_khw_f16(w, cout_pad=None, cin_pad=None, out=None):
+    """[Cout,Cin,kh,kw] fp32 -> fp16 [cin_pad,kh,kw,cout_pad]: rotated by 180 degrees, transposed, zero in the padding (the data-gradient operand)."""
+    _req(w, torch.float32, 'weight')
+    cout, cin, kh, kw = w.shape
+    cout_pad = cout if cout_pad is None else cout_pad
+    cin_pad = cin if cin_pad is None else cin_pad
+    out = torch.empty(cin_pad, kh, kw, cout_pad, dtype=torch.float16, device=w.device) if out is None else out
+    _ck(_l.load().yb_pack_weight_dgrad_khw_f16(_p(w), _p(out), cout, cin, kh, kw, cout_pad, cin_pad, _s()), 'yb_pack_weight_dgrad_khw_f16')
+    return out
+
+
+def stem3x3_s2_raw(x, w, pad=0):
+    """Raw nn.Conv2d(3, 32, 3, stride 2, pad) (no BatchNorm, no ReLU): x fp32 NCHW [B,3,H,W] -> z fp16 NHWC [B,OH,OW,32]."""
+    _req(x, torch.float32, 'x'); _req(w, torch.float32, 'w')
+    b, c, h, wd = x.shape
+    if c != 3 or tuple(w.shape) != (32, 3, 3, 3):
+        raise ValueError('stem3x3_s2_raw: x [B,3,H,W] and w [32,3,3,3] expected')
+    out = torch.empty(b, conv2d_out_size(h, 3, 2, pad), conv2d_out_size(wd, 3, 2, pad), 32, dtype=torch.float16, device=x.device)
+    _ck(_l.load().yb_stem3x3_s2_raw_fwd(_p(x), _p(w), _p(out), b, h, wd, pad, _s()), 'yb_stem3x3_s2_raw_fwd')
+    return out
+
+
+def stem3x3_s2_wgrad(x, dz, pad=0, out=None):
+    """Weight gradient of the stride-2 3 -> 32 stem: fp32 OIHW [32,3,3,3] from the fp32 NCHW image and dz fp16 NHWC [B,OH,OW,32]."""
+    _req(x, torch.float32, 'x'); _req(dz, torch.float16, 'dz')
+    b, _, h, wd = x.shape
+    if tuple(dz.shape) != (b, conv2d_out_size(h, 3, 2, pad), conv2d_out_size(wd, 3, 2, pad), 32):
+        raise ValueError('stem3x3_s2_wgrad: dz %s does not match x %s' % (tuple(dz.shape), tuple(x.shape)))
+    out = torch.empty(32, 3, 3, 3, dtype=torch.float32, device=x.device) if out is None else out
+    _ck(_l.load().yb_stem3x3_s2_wgrad(_p(x), _p(dz), _p(out), b, h, wd, pad, _s()), 'yb_stem3x3_s2_wgrad')
+    return out
+
+
+def maxpool3x3_s2_valid_bwd(x, dy, dy_ch_off=0, out=None):
+    """Backward of maxpool3x3_s2_valid: dx [B,H,W,C] from its input x and dy = channels [dy_ch_off, dy_ch_off + C) of [B,OH,OW,dy_ld]."""
+    _req(x, torch.float16, 'x'); _req(dy, torch.float16, 'dy')
+    b, h, w, c = x.shape
+    out = torch.empty_like(x) if out is None else out
+    _ck(_l.load().yb_maxpool3x3_s2_valid_bwd_f16(_p(x), _p(dy), dy.shape[-1], dy_ch_off, _p(out), b, h, w, c, _s()), 'yb_maxpool3x3_s2_valid_bwd_f16')
+    return out
+
+
+def join(terms, out=None):
+    """The sum of 2..4 fp16 tensors of one shape, in fp32, rounded once (yb_join_f16)."""
+    if not 2 <= len(terms) <= 4:
+        raise ValueError('join: 2 to 4 terms, got %d' % len(terms))
+    for t in terms:
+        _req(t, torch.float16, 'term')
+        if t.shape != terms[0].shape:
+            raise ValueError('join: shapes %s and %s differ' % (tuple(terms[0].shape), tuple(t.shape)))
+    out = torch.empty_like(terms[0]) if out is None else out
+    ts = list(terms) + [None] * (4 - len(terms))
+    _ck(_l.load().yb_join_f16(*[_p(t) for t in ts], _p(out), out.numel(), _s()), 'yb_join_f16')
+    return out
+
+
 def conv1x1_preact(x, w, pre_scale, pre_shift, pre_relu, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0,
                    workspace=None):
     """DenseNet's norm -> relu -> 1x1 conv (yb_conv1x1_preact_fwd): the conv reads a = fp16(act(fmaf(pre_scale, x, pre_shift))) with act = ReLU

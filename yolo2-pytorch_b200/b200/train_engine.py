@@ -1233,3 +1233,380 @@ class VGGTrainer(TrainerBase):
             self._emit(u.pnames[0], grads)
         self._finish_backward(dev)
         return grads
+
+
+class _IncUnit(object):
+    """One torchvision BasicConv2d of Inception-v3 (conv without bias -> BatchNorm2d(eps 1e-3) -> ReLU) as the Inception trainer reads it:
+    its geometry, its filter count rounded up to a multiple of 32 (the 80- and 48-filter convs run with zero filters) and the width of the
+    buffer it reads (`cin_pad`: zero channels beyond the module's Cin get zero weights)."""
+
+    def __init__(self, key, unit, cin_pad):
+        conv = unit.conv
+        self.key, self.conv, self.bn = key, conv, unit.bn
+        self.kh, self.kw = conv.kernel_size
+        self.stride, self.pad = conv.stride[0], tuple(conv.padding)
+        self.cout, self.cin = conv.weight.shape[0], conv.weight.shape[1]
+        self.cout_pad, self.cin_pad = (self.cout + 31) // 32 * 32, cin_pad
+        self.pnames = (key + '.conv.weight', key + '.bn.weight', key + '.bn.bias')
+        self.w16 = self.wd = None
+
+
+class KhwPackPlan(object):
+    """Every kh x kw unit's forward operand [cout_pad,kh,kw,cin_pad] and data-gradient operand [cin_pad,kh,kw,cout_pad] (fp16) re-derived from
+    the fp32 weights by ONE launch (yb_pack_weights_khw_batch), into persistent buffers whose addresses the device table holds; the plan is
+    rebuilt when a weight moves.  The table is `yb_pack_khw_unit` (include/yolo2_b200.h)."""
+    DTYPE = np.dtype([('w', '<u8'), ('f', '<u8'), ('d', '<u8'), ('e0', '<i8'), ('cout', '<i4'), ('cin', '<i4'), ('kh', '<i4'), ('kw', '<i4'),
+                      ('cp', '<i4'), ('cip', '<i4')])
+
+    def __init__(self, entries, device):
+        """entries: [(key, weight [Cout,Cin,kh,kw] fp32 contiguous, cout_pad, cin_pad)]"""
+        assert self.DTYPE.itemsize == 56
+        table = np.zeros(len(entries), dtype=self.DTYPE)
+        self.key = tuple(w.data_ptr() for _, w, _, _ in entries)
+        self.fwd, self.dgrad = {}, {}
+        e0 = 0
+        for i, (key, w, cp, cip) in enumerate(entries):
+            cout, cin, kh, kw = w.shape
+            if w.dtype != torch.float32 or not w.is_contiguous() or cp < cout or cip < cin:
+                raise ValueError('KhwPackPlan: unsupported weight %s %s' % (key, tuple(w.shape)))
+            f = self.fwd[key] = torch.empty(cp, kh, kw, cip, dtype=torch.float16, device=device)
+            d = self.dgrad[key] = torch.empty(cip, kh, kw, cp, dtype=torch.float16, device=device)
+            table[i] = (w.data_ptr(), f.data_ptr(), d.data_ptr(), e0, cout, cin, kh, kw, cp, cip)
+            e0 += 2 * f.numel()
+        self.total = e0
+        self.count = len(entries)
+        self.table = torch.from_numpy(table.view(np.uint8).copy()).to(device)
+
+    def run(self):
+        ops.call('yb_pack_weights_khw_batch', self.table, self.count, self.total)
+
+
+def _bn_chunks(c):
+    """Channel ranges of a BatchNorm of c channels (a multiple of 16) that the train-mode BatchNorm kernels take one at a time: those kernels need
+    C / 8 to divide 256, so 80 runs as 64 + 16, 192 as 128 + 64, 448 as 256 + 128 + 64."""
+    out, off = [], 0
+    for n in (2048, 1024, 512, 256, 128, 64, 32, 16, 8):
+        while c - off >= n:
+            out.append((off, n))
+            off += n
+    if off != c:
+        raise ValueError('BatchNorm of %d channels: not a multiple of 8' % c)
+    return out
+
+
+# Mixed block layouts: (BasicConv2d, what it reads, first channel of the block output it writes or None for an intermediate).  'x' is the block
+# input, 'pool' its 3x3 average pool (count_include_pad), any other name a unit of the same block.  Consumers follow their producers.
+_INCEPTION_BLOCKS = {
+    'A': (('branch1x1', 'x', 0), ('branch5x5_1', 'x', None), ('branch5x5_2', 'branch5x5_1', 64), ('branch3x3dbl_1', 'x', None),
+          ('branch3x3dbl_2', 'branch3x3dbl_1', None), ('branch3x3dbl_3', 'branch3x3dbl_2', 128), ('branch_pool', 'pool', 224)),
+    'B': (('branch3x3', 'x', 0), ('branch3x3dbl_1', 'x', None), ('branch3x3dbl_2', 'branch3x3dbl_1', None), ('branch3x3dbl_3', 'branch3x3dbl_2', 384)),
+    'C': (('branch1x1', 'x', 0), ('branch7x7_1', 'x', None), ('branch7x7_2', 'branch7x7_1', None), ('branch7x7_3', 'branch7x7_2', 192),
+          ('branch7x7dbl_1', 'x', None), ('branch7x7dbl_2', 'branch7x7dbl_1', None), ('branch7x7dbl_3', 'branch7x7dbl_2', None),
+          ('branch7x7dbl_4', 'branch7x7dbl_3', None), ('branch7x7dbl_5', 'branch7x7dbl_4', 384), ('branch_pool', 'pool', 576)),
+    'D': (('branch3x3_1', 'x', None), ('branch3x3_2', 'branch3x3_1', 0), ('branch7x7x3_1', 'x', None), ('branch7x7x3_2', 'branch7x7x3_1', None),
+          ('branch7x7x3_3', 'branch7x7x3_2', None), ('branch7x7x3_4', 'branch7x7x3_3', 320)),
+    'E': (('branch1x1', 'x', 0), ('branch3x3_1', 'x', None), ('branch3x3_2a', 'branch3x3_1', 320), ('branch3x3_2b', 'branch3x3_1', 704),
+          ('branch3x3dbl_1', 'x', None), ('branch3x3dbl_2', 'branch3x3dbl_1', None), ('branch3x3dbl_3a', 'branch3x3dbl_2', 1088),
+          ('branch3x3dbl_3b', 'branch3x3dbl_2', 1472), ('branch_pool', 'pool', 1856)),
+}
+# the pool branch of Mixed_6a / Mixed_7a: F.max_pool2d(x, 3, stride=2) into these channels onwards
+_INCEPTION_MAXPOOL = {'B': 480, 'D': 512}
+_INCEPTION_KIND = {'Mixed_5b': 'A', 'Mixed_5c': 'A', 'Mixed_5d': 'A', 'Mixed_6a': 'B', 'Mixed_6b': 'C', 'Mixed_6c': 'C', 'Mixed_6d': 'C',
+                   'Mixed_6e': 'C', 'Mixed_7a': 'D', 'Mixed_7b': 'E', 'Mixed_7c': 'E'}
+_INCEPTION_STEM = ('Conv2d_1a_3x3', 'Conv2d_2a_3x3', 'Conv2d_2b_3x3', 'Conv2d_3b_1x1', 'Conv2d_4a_3x3')
+
+
+class InceptionTrainer(TrainerBase):
+    """Training-mode forward / backward of `model.inception3.Inception3` (reference model/inception3.py over torchvision's BasicConv2d and
+    InceptionA..E), for any input side >= 75.
+
+    Forward per BasicConv2d: raw yb_conv2d_bn_act_fwd (scale 1, shift 0, slope 1) with the module's kh x kw, stride and padding -> batch
+    statistics (yb_bn_stats) -> running-statistics update with the module's eps (1e-3) and momentum (0.1) -> normalise + ReLU into the unit's
+    channel range of its block's buffer (no concatenation).  The stem conv is the raw form of the stride-2 first-layer kernel on the fp32 image.
+
+    Backward of a block runs its units in reverse: BatchNorm + ReLU backward from the unit's channel slice of the block gradient (or from the
+    joined gradient of its consumers) -> weight gradient (yb_conv2d_wgrad; stride 2 walks the strided im2col box natively) -> data gradient
+    (the forward conv on dz with the rotated, transposed weights; a stride-2 conv on the zero-inserted dz).  The gradient at a tensor read by
+    several units is their sum (yb_join_f16: fp32, one rounding); the pool branch's contribution is the average pool of its gradient (that pool,
+    with a constant divisor and a symmetric window, is its own transpose), the max-pool branch's is yb_maxpool3x3_s2_valid_bwd_f16.  The stem
+    runs last: max-pool backward, BatchNorm backward, and the first conv's weight gradient from the fp32 image.
+
+    The static loss scale is 1024, not the other chains' 16384: through 11 Mixed blocks and the stem the largest activation gradient grows
+    about 50-fold from the head to the stem (measured on the synthetic step of the tests), so 16384 overflows fp16 in the stem and the
+    gradient guard would zero every step."""
+    NAME = 'Inception3'
+
+    def __init__(self, dnn, grad_scale=1024.0):
+        TrainerBase.__init__(self, dnn, grad_scale, slope=0.0)
+        self._units = None
+
+    # ---- plan --------------------------------------------------------------------------------------------
+    def _plan(self):
+        if self._units is None:
+            net = self.dnn
+            units = {}
+            width = 3
+            for name in _INCEPTION_STEM:
+                u = units[name] = _IncUnit(name, getattr(net, name), width)
+                width = u.cout_pad
+            width = units['Conv2d_4a_3x3'].cout_pad
+            for name, kind in _INCEPTION_KIND.items():
+                m = getattr(net, name)
+                for attr, src, _ in _INCEPTION_BLOCKS[kind]:
+                    key = '%s.%s' % (name, attr)
+                    units[key] = _IncUnit(key, getattr(m, attr), width if src in ('x', 'pool') else units['%s.%s' % (name, src)].cout_pad)
+                width = self._block_width(kind, m, width)
+            self._head = _ResUnit('conv', net.conv, None, 1.0, ('conv.weight', None, None))
+            self._units = units
+        return self._units
+
+    @staticmethod
+    def _block_width(kind, m, cin):
+        return {'A': lambda: 224 + m.branch_pool.conv.out_channels, 'B': lambda: 480 + cin, 'C': lambda: 768, 'D': lambda: 512 + cin,
+                'E': lambda: 2048}[kind]()
+
+    def block_units(self, name):
+        """The units of block `name` (a Mixed_* name or 'stem') in forward order."""
+        units = self._plan()
+        if name == 'stem':
+            return [units[n] for n in _INCEPTION_STEM]
+        return [units['%s.%s' % (name, attr)] for attr, _, _ in _INCEPTION_BLOCKS[_INCEPTION_KIND[name]]]
+
+    def grad_order(self):
+        names = ['conv.bias', 'conv.weight']
+        for name in list(reversed(list(_INCEPTION_KIND))) + ['stem']:
+            for u in reversed(self.block_units(name)):
+                names += [u.pnames[1], u.pnames[2], u.pnames[0]]
+        return names
+
+    def _head_unit(self):
+        return self._head.key, self._head, 'conv.bias'
+
+    def _repack(self, device):
+        """Forward and data-gradient fp16 operands of every conv after the stem's first and of the head, re-derived from the fp32 weights in
+        ONE launch (KhwPackPlan; the optimizer just changed the weights).  The stem conv reads its fp32 weights in place."""
+        units = [u for name, u in self._plan().items() if name != 'Conv2d_1a_3x3']
+        head = self._head
+        cpad = (head.cout + 31) // 32 * 32            # the head's filters are padded to the width of its dz buffer
+        entries = [(u.key, u.conv.weight.detach(), u.cout_pad, u.cin_pad) for u in units] + [(head.key, head.conv.weight.detach(), cpad, head.cin)]
+        plan = self._pack_plan
+        wdev = entries[0][1].device                    # the weights' device, with its index ('cuda' alone would never compare equal)
+        if plan is None or plan.key != tuple(w.data_ptr() for _, w, _, _ in entries) or plan.table.device != wdev:
+            plan = self._pack_plan = KhwPackPlan(entries, wdev)
+        plan.run()
+        for u in units:
+            u.w16, u.wd = plan.fwd[u.key], plan.dgrad[u.key]
+        head.w16 = plan.fwd[head.key][:head.cout]      # the forward writes fp32 NCHW with the module's own filter count
+        self.wd_cache[head.key] = plan.dgrad[head.key]
+
+    def _wd(self, key, u, cout_pad=0):
+        """The head's data-gradient operand, from this step's batched pack (the 1 x 1 layout of yb_pack_weight_dgrad_f16)."""
+        return self.wd_cache[key]
+
+    def _check(self, x):
+        b, c, h, w = x.shape
+        if c != 3:
+            raise ValueError('Inception3 expects [B,3,H,W]')
+        from model.inception3 import MIN_SIZE
+        if h < MIN_SIZE or w < MIN_SIZE:
+            raise ValueError('Inception3: a %d x %d input leaves a stage empty (H and W must be >= %d)' % (h, w, MIN_SIZE))
+        for u in self._plan().values():
+            if u.bn.momentum is None or not u.bn.track_running_stats:
+                raise ValueError('Inception3 training: %s needs a BatchNorm with running statistics and a momentum' % u.key)
+
+    # ---- forward -----------------------------------------------------------------------------------------
+    def _bn_unit_forward(self, u, z, ain, out=None, a_off=0, **extra):
+        """Train-mode BatchNorm + ReLU of a unit's raw output z [B,OH,OW,cout_pad]: batch statistics, running-statistics update, and the
+        activation into channels [a_off, a_off + cout) of `out` (default: a new buffer of cout_pad channels, exact zeros beyond cout)."""
+        b, oh, ow, ld = z.shape
+        dev = z.device
+        rows = b * oh * ow
+        if out is None:
+            out = (torch.zeros if u.cout_pad != u.cout else torch.empty)(b, oh, ow, u.cout_pad, dtype=torch.float16, device=dev)
+        bn = u.bn
+        mean = torch.empty(u.cout, dtype=torch.float32, device=dev)
+        invstd = torch.empty(u.cout, dtype=torch.float32, device=dev)
+        gamma, beta = bn.weight.detach(), bn.bias.detach()
+        for off, n in _bn_chunks(u.cout):
+            sums = self._sums(('f', u.key, off), n, dev)
+            ops.call('yb_bn_stats', z[..., off:], ld, rows, n, sums)
+            ops.call('yb_bn_finalize', sums, rows, n, float(bn.eps), float(bn.momentum), bn.running_mean[off:], bn.running_var[off:], mean[off:],
+                     invstd[off:])
+            ops.call('yb_bn_act_apply', z[..., off:], ld, mean[off:], invstd[off:], gamma[off:], beta[off:], 0.0, out, out.shape[-1], a_off + off,
+                     b, oh, ow, n, 0)
+        if bn.num_batches_tracked is not None:
+            self._tracked.append(bn.num_batches_tracked)
+        return out, self._saved_unit(u, ain, z, mean, invstd, oh, ow, a_off=a_off, **extra)
+
+    def _unit_forward(self, u, src, out=None, a_off=0):
+        one, zero = self._ones(u.cout_pad, src.device)
+        z = ops.conv2d_bn_act(src, u.w16, one, zero, 1.0, stride=u.stride, pad=u.pad)
+        return self._bn_unit_forward(u, z, src, out, a_off, in_h=src.shape[1], in_w=src.shape[2])
+
+    def stem_forward(self, x):
+        """Conv2d_1a_3x3 .. the second max-pool on the fp32 image x [B,3,H,W]: (Mixed_5b's input [B,H5,W5,192], saved stem)."""
+        u1, u2a, u2b, u3b, u4a = self.block_units('stem')
+        z = ops.stem3x3_s2_raw(x, u1.conv.weight.detach().contiguous(), pad=0)
+        a, s1 = self._bn_unit_forward(u1, z, None)
+        a, s2a = self._unit_forward(u2a, a)
+        a3, s2b = self._unit_forward(u2b, a)
+        p1 = ops.maxpool3x3_s2_valid(a3)
+        a, s3b = self._unit_forward(u3b, p1)
+        a5, s4a = self._unit_forward(u4a, a)
+        p2 = ops.maxpool3x3_s2_valid(a5)
+        st = _Saved()
+        st.x, st.units, st.a3, st.a5 = x, [s1, s2a, s2b, s3b, s4a], a3, a5
+        return p2, st
+
+    def block_forward(self, name, x):
+        """Mixed block `name` on x (fp16 NHWC): (its concatenated output, saved block)."""
+        kind = _INCEPTION_KIND[name]
+        m = getattr(self.dnn, name)
+        b, h, w, c = x.shape
+        oh, ow = ((h - 3) // 2 + 1, (w - 3) // 2 + 1) if kind in _INCEPTION_MAXPOOL else (h, w)
+        out = torch.empty(b, oh, ow, self._block_width(kind, m, c), dtype=torch.float16, device=x.device)
+        vals = {'x': x}
+        if kind in ('A', 'C', 'E'):
+            vals['pool'] = ops.avgpool3x3_s1(x)          # kept: the branch_pool weight gradient reads it
+        recs = []
+        for (attr, src, off), u in zip(_INCEPTION_BLOCKS[kind], self.block_units(name)):
+            a, s = self._unit_forward(u, vals[src], out if off is not None else None, off or 0)
+            s.src, s.name, s.to_out = src, attr, off is not None
+            vals[attr] = a
+            recs.append(s)
+        if kind in _INCEPTION_MAXPOOL:
+            ops.maxpool3x3_s2_valid(x, out, _INCEPTION_MAXPOOL[kind])
+        blk = _Saved()
+        blk.name, blk.kind, blk.x, blk.units = name, kind, x, recs
+        return out, blk
+
+    def forward(self, x):
+        x = self._start_forward(x)
+        self._check(x)
+        if self.dnn.transform_input:
+            raise NotImplementedError('Inception3: transform_input=True has no kernel path (the reference never sets it)')
+        dev = x.device
+        self._plan()
+        self._repack(dev)
+        saved = _Saved()
+        saved.b = x.shape[0]
+        cur, saved.stem = self.stem_forward(x)
+        saved.blocks = []
+        for name in _INCEPTION_KIND:
+            cur, blk = self.block_forward(name, cur)
+            saved.blocks.append(blk)
+        head = self._head
+        one, _ = self._ones(head.cout, dev)
+        feature = ops.conv2d_bn_act(cur, head.w16, one, head.conv.bias.detach(), 1.0, out_mode=ops.OUT_F32_NCHW)
+        saved.a_last, saved.hh, saved.ww = cur, cur.shape[1], cur.shape[2]
+        self._bump_tracked()
+        return feature, saved
+
+    # ---- backward ----------------------------------------------------------------------------------------
+    def _bn_unit_backward(self, s, da, da_off, grads):
+        """BatchNorm + ReLU backward of a saved unit from channels [da_off, da_off + cout) of da: dz [B,OH,OW,cout_pad] (exact zeros beyond
+        cout), dgamma and dbeta."""
+        u = s.u
+        b = s.z.shape[0]
+        dev = s.z.device
+        dz = (torch.zeros if u.cout_pad != u.cout else torch.empty)(b, s.h, s.w, u.cout_pad, dtype=torch.float16, device=dev)
+        _, gname, bname = u.pnames
+        dgamma, dbeta = self.arena.views[gname], self.arena.views[bname]
+        gamma, beta = u.bn.weight.detach(), u.bn.bias.detach()
+        for off, n in _bn_chunks(u.cout):
+            sums = self._sums(('b', u.key, off), n, dev)
+            args = (s.z[..., off:], s.z.shape[-1], s.mean[off:], s.invstd[off:], gamma[off:], beta[off:], 0.0, da, da.shape[-1], da_off + off,
+                    None, 0, 0, b, s.h, s.w, n, 0, sums)
+            ops.call('yb_bn_act_bwd', 0, *args, None, 0, 1)
+            ops.call('yb_bn_act_bwd', 1, *args, dz[..., off:], dz.shape[-1], 1)
+            ops.call('yb_bn_param_grad', sums, n, dgamma[off:], dbeta[off:], 1, self._unscale)
+        grads[gname], grads[bname] = dgamma, dbeta
+        self._emit(gname, grads)
+        self._emit(bname, grads)
+        return dz
+
+    def _wgrad_khw(self, s, dz, grads):
+        """Weight gradient of a unit from its input and dz, on the weight-gradient stream while a graph is captured (as TrainerBase._wgrad)."""
+        u, ain = s.u, s.ain
+        dev = dz.device
+        side = self._side(dev)
+        if side is not None:
+            fork = torch.cuda.Event()
+            fork.record(torch.cuda.current_stream(dev))
+            side.wait_event(fork)
+            dz.record_stream(side)
+            ain.record_stream(side)
+            self._side_busy = True
+        with torch.cuda.stream(side) if side is not None else _NullCtx():
+            b, h, w, ld = ain.shape
+            dw_krsc = torch.empty(u.cout, u.kh, u.kw, ld, dtype=torch.float32, device=dev)
+            ops.call('yb_conv2d_wgrad', ain, dz, dw_krsc, b, h, w, ld, u.cout, u.kh, u.kw, u.stride, u.pad[0], u.pad[1], ld, dz.shape[-1])
+            wname = u.pnames[0]
+            dw = self.arena.views[wname]
+            ops.call('yb_unpack_wgrad_khw', dw_krsc, dw, u.cout, u.cin, u.kh, u.kw, ld, self._unscale)
+            grads[wname] = dw
+            self._emit(wname, grads)
+
+    def _dgrad_khw(self, s, dz):
+        """Gradient at a unit's input [B,H,W,cin_pad]: the forward conv on dz (zero-inserted for stride 2) with the rotated, transposed
+        weights at padding (k - 1 - pad); zero channels beyond Cin."""
+        u = s.u
+        if u.stride == 2:
+            fh, fw = s.in_h + 2 * u.pad[0] - u.kh + 1, s.in_w + 2 * u.pad[1] - u.kw + 1      # the stride-1 output grid
+            dzf = torch.empty(dz.shape[0], fh, fw, dz.shape[-1], dtype=torch.float16, device=dz.device)
+            ops.call('yb_upsample2_zero_f16', dz, dzf, dz.shape[0], fh, fw, dz.shape[-1])
+            dz = dzf
+        one, zero = self._ones(u.cin_pad, dz.device)
+        return ops.conv2d_bn_act(dz, u.wd, one, zero, 1.0, pad=(u.kh - 1 - u.pad[0], u.kw - 1 - u.pad[1]))
+
+    def _unit_backward(self, s, da, da_off, grads, need_dgrad=True):
+        dz = self._bn_unit_backward(s, da, da_off, grads)
+        self._wgrad_khw(s, dz, grads)
+        return self._dgrad_khw(s, dz) if need_dgrad else None
+
+    @staticmethod
+    def _sum(terms):
+        return terms[0] if len(terms) == 1 else ops.join(terms)
+
+    def block_backward(self, blk, g, grads):
+        """Backward of a saved Mixed block from g, the gradient of its output: the parameter gradients of its units, and the gradient at its
+        input.  Every branch's data gradient at a shared tensor is collected and joined once."""
+        terms = {}
+        for s in reversed(blk.units):
+            if s.to_out:
+                gi = self._unit_backward(s, g, s.a_off, grads)
+            else:
+                gi = self._unit_backward(s, self._sum(terms.pop(s.name)), 0, grads)
+            terms.setdefault(s.src, []).append(gi)
+        if 'pool' in terms:
+            terms['x'].append(ops.avgpool3x3_s1(self._sum(terms.pop('pool'))))
+        if blk.kind in _INCEPTION_MAXPOOL:
+            terms['x'].append(ops.maxpool3x3_s2_valid_bwd(blk.x, g, _INCEPTION_MAXPOOL[blk.kind]))
+        return self._sum(terms['x'])
+
+    def stem_backward(self, st, g, grads):
+        """Stem backward from g, the gradient at Mixed_5b's input: returns the gradient at Conv2d_1a_3x3's activation."""
+        s1, s2a, s2b, s3b, s4a = st.units
+        g = self._unit_backward(s4a, ops.maxpool3x3_s2_valid_bwd(st.a5, g), 0, grads)
+        g = self._unit_backward(s3b, g, 0, grads)
+        g = self._unit_backward(s2b, ops.maxpool3x3_s2_valid_bwd(st.a3, g), 0, grads)
+        g = self._unit_backward(s2a, g, 0, grads)
+        dz = self._bn_unit_backward(s1, g, 0, grads)
+        x = st.x
+        wname = s1.u.pnames[0]
+        dw = self.arena.views[wname]
+        ops.call('yb_stem3x3_s2_wgrad', x, dz, dw, x.shape[0], x.shape[2], x.shape[3], 0)
+        grads[wname] = dw.mul_(self._unscale)
+        self._emit(wname, grads)
+        return g
+
+    def backward(self, saved, dfeature):
+        grads = {}
+        dev = dfeature.device
+        self._start_backward(dev)
+        g = self._head_backward(saved.a_last, saved.hh, saved.ww, dfeature, grads)
+        for blk in reversed(saved.blocks):
+            g = self.block_backward(blk, g, grads)
+        self.stem_backward(saved.stem, g, grads)
+        self._finish_backward(dev)
+        return grads

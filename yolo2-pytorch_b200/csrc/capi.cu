@@ -141,6 +141,14 @@ int stem3x3_s2(const float*, const float*, const float*, const float*, void*, in
 int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1_excl(const void*, void*, int, int, int, int, cudaStream_t);
+int conv2d_wgrad_forward(const void*, const void*, float*, int, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
+int unpack_wgrad_khw(const float*, float*, int, int, int, int, int, float, cudaStream_t);
+int pack_weight_dgrad_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
+int stem3x3_s2_raw(const float*, const float*, void*, int, int, int, int, cudaStream_t);
+int stem3x3_s2_wgrad(const float*, const void*, float*, int, int, int, int, cudaStream_t);
+int maxpool3x3_s2_valid_bwd(const void*, const void*, int, int, void*, int, int, int, int, cudaStream_t);
+int join_f16(const void*, const void*, const void*, const void*, void*, long long, cudaStream_t);
+int pack_weights_khw_batch(const void*, int, long long, cudaStream_t);
 
 }  // namespace yb
 
@@ -529,6 +537,40 @@ int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int widt
 
 int yb_avgpool3x3_s1_excl_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
   return yb::avgpool3x3_s1_excl(x, y, batch, height, width, channels, S(stream));
+}
+
+int yb_conv2d_wgrad(const void* x, const void* dz, float* dw_krsc, int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride,
+                    int pad_h, int pad_w, int x_ld, int dz_ld, yb_stream_t stream) {
+  return yb::conv2d_wgrad_forward(x, dz, dw_krsc, batch, in_h, in_w, cin, cout, kh, kw, stride, pad_h, pad_w, x_ld, dz_ld, S(stream));
+}
+
+int yb_unpack_wgrad_khw(const float* dw_krsc, float* dw_oihw, int cout, int cin, int kh, int kw, int krsc_cin, float scale, yb_stream_t stream) {
+  return yb::unpack_wgrad_khw(dw_krsc, dw_oihw, cout, cin, kh, kw, krsc_cin, scale, S(stream));
+}
+
+int yb_pack_weight_dgrad_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, int kh, int kw, int cout_pad, int cin_pad, yb_stream_t stream) {
+  return yb::pack_weight_dgrad_khw(w_oihw, w_f16, cout, cin, kh, kw, cout_pad, cin_pad, S(stream));
+}
+
+int yb_stem3x3_s2_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, int pad, yb_stream_t stream) {
+  return yb::stem3x3_s2_raw(x_nchw, w_oihw, z_nhwc_f16, batch, height, width, pad, S(stream));
+}
+
+int yb_stem3x3_s2_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, int pad, yb_stream_t stream) {
+  return yb::stem3x3_s2_wgrad(x_nchw, dz_nhwc_f16, dw_oihw, batch, height, width, pad, S(stream));
+}
+
+int yb_maxpool3x3_s2_valid_bwd_f16(const void* x, const void* dy, int dy_ld, int dy_ch_off, void* dx, int batch, int height, int width, int channels,
+                                   yb_stream_t stream) {
+  return yb::maxpool3x3_s2_valid_bwd(x, dy, dy_ld, dy_ch_off, dx, batch, height, width, channels, S(stream));
+}
+
+int yb_join_f16(const void* a, const void* b, const void* c, const void* d, void* out, long long count, yb_stream_t stream) {
+  return yb::join_f16(a, b, c, d, out, count, S(stream));
+}
+
+int yb_pack_weights_khw_batch(const yb_pack_khw_unit* units_dev, int num_units, long long total_elems, yb_stream_t stream) {
+  return yb::pack_weights_khw_batch(units_dev, num_units, total_elems, S(stream));
 }
 
 int yb_comm_version(int* nccl_version) { return yb::comm_version(nccl_version); }

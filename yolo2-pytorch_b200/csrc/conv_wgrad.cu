@@ -2,7 +2,7 @@
 // Replaces what torch autograd runs for nn.Conv2d.weight.grad (reference model/yolo2.py:57,
 // train.py:351 loss_total.backward()).
 //
-//   dW[co][r][s][ci] = sum over output pixels p of  dz[p, co] * x[p + (r-1, s-1), ci]        (zero outside the image)
+//   dW[co][r][s][ci] = sum over output pixels p of  dz[p, co] * x[stride * p + (r - pad_h, s - pad_w), ci]   (zero outside the image)
 //
 // As a GEMM the reduction runs over PIXELS:  D[M = 128 co, N = ci-chunk] += A[M, K = pixels] * B[N, K]^T with
 // A(m, k) = dz[p0 + k][co0 + m] and B(n, k) = x[shift(p0 + k)][ci0 + n].  Both tensors are NHWC (channel
@@ -15,6 +15,11 @@
 // groups, so the dz tile is fetched once per K-block and reused by all G groups; the pixel range is split across CTAs
 // (split-K) and the fp32 partial sums are added into a zero-initialised [Cout][k][k][Cin] buffer with 8-byte vector
 // atomics.
+//
+// The geometry is that of yb_conv2d_bn_act_fwd: kh x kw filters (1..7), stride 1 or 2, padding below the filter size.  The pixel walk
+// follows the OUTPUT grid (dz's rows): the producer splits a K-block's first pixel on the output dims, and the im2col box is walked on
+// the input tensor with element strides equal to the conv stride, exactly as the forward kernel's A operand is, so a stride-2 conv
+// costs the MMAs of its own output pixels (no zero-inserted dz).  yb_conv_wgrad is the (k, k, 1, (k-1)/2) case of the same code.
 #include "yb_common.h"
 #include "yb_ptx.cuh"
 #include <stdlib.h>
@@ -26,8 +31,8 @@ constexpr int WG_THREADS = WG_MMA_THREADS + 32;     // + the TMA producer warp
 constexpr int WG_MAX_GROUPS = 9;
 
 struct WgradParams {
-  int m_total, hw, width;
-  int cin, cout, ksize, pad;
+  int m_total, hw, width;   // output pixels, output H * W, output W
+  int cin, cout, kh, kw, pad_h, pad_w, stride;
   int n_per_group;      // N of one (tap, ci-chunk) group (32, 64, 128, 192 or 256)
   int groups_per_cta;   // G
   int col_tiles;        // taps * ceil(cin / n_per_group)
@@ -119,7 +124,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
         const int p0 = kb * WG_KP;
         const int img = p0 / p.hw;
         const int rem = p0 - img * p.hw;
-        const int h0 = rem / p.width, w0 = rem - h0 * p.width;
+        const int oh0 = rem / p.width, ow0 = rem - oh0 * p.width;
+        const int h0 = oh0 * p.stride - p.pad_h, w0 = ow0 * p.stride - p.pad_w;    // input corner of the first pixel's window
         mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x600 | stage);
         mbar_arrive_expect_tx(bar_full + 8 * stage, tx_bytes);
         const uint32_t sa = smem_base + stage * kStageBytes;
@@ -132,9 +138,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
           const int t = first_tile + g;
           const int tap = t / p.chunks_per_tap;
           const int ci0 = (t - tap * p.chunks_per_tap) * p.n_per_group;
-          const int r = tap / p.ksize, s = tap - r * p.ksize;
+          const int r = tap / p.kw, s = tap - r * p.kw;
           for (int j = 0; j < boxes_per_group; ++j) {
-            tma_load_im2col_4d(sb, &tmap_x, bar_full + 8 * stage, ci0 + j * kBCh, w0 - p.pad, h0 - p.pad, img, static_cast<uint16_t>(s),
+            tma_load_im2col_4d(sb, &tmap_x, bar_full + 8 * stage, ci0 + j * kBCh, w0, h0, img, static_cast<uint16_t>(s),
                                static_cast<uint16_t>(r));
             sb += kBBox;
           }
@@ -170,7 +176,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   wgmma_wait<0>();
   fence_regs(acc);
   // epilogue straight from the fragment: rows = output channels, column pairs = two consecutive input channels of one group
-  const long long ktot = static_cast<long long>(p.ksize) * p.ksize * p.cin;
+  const long long ktot = static_cast<long long>(p.kh) * p.kw * p.cin;
   const int w4 = warp & 3;
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
@@ -218,14 +224,18 @@ static int launch_wgrad(const CUtensorMap& tdz, const CUtensorMap& tx, const Wgr
 // pixels per stage (one TMA box) and pipeline depth: 128-pixel boxes, two stages
 constexpr int kWgKP = 128, kWgStages = 2;
 constexpr int kWgNmaxWide = 256;    // Cin >= 64: 64-channel boxes
-constexpr int kWgNmaxNarrow = 96;   // Cin = 32: three taps of 32 channels per CTA
+constexpr int kWgNmaxNarrow = 96;   // Cin % 64 != 0: 32-channel boxes, three taps of 32 channels or one 96-channel group per CTA
 
-int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch, int height, int width, int cin, int cout, int ksize, int x_ld,
-                       int dz_ld, cudaStream_t stream) {
+// Both entries below: the geometry checks, then the launch.  Cin is any multiple of 32 here; yb_conv2d_wgrad documents its own range.
+static int wgrad_run(const void* x, const void* dz, float* dw_krsc, int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride,
+                     int pad_h, int pad_w, int x_ld, int dz_ld, cudaStream_t stream) {
   YB_REQUIRE(x && dz && dw_krsc, "wgrad: null pointer");
-  YB_REQUIRE(ksize == 1 || ksize == 3, "wgrad: ksize");
-  YB_REQUIRE(cin % 32 == 0 && (cin == 32 || cin % 64 == 0), "wgrad: Cin=%d unsupported", cin);
+  YB_REQUIRE(kh >= 1 && kh <= 7 && kw >= 1 && kw <= 7 && pad_h >= 0 && pad_h < kh && pad_w >= 0 && pad_w < kw && (stride == 1 || stride == 2),
+             "wgrad: kernel %d x %d, stride %d, padding (%d, %d) unsupported", kh, kw, stride, pad_h, pad_w);
+  YB_REQUIRE(cin > 0 && cin % 32 == 0, "wgrad: Cin=%d unsupported (a multiple of 32)", cin);
   YB_REQUIRE(cout > 0 && x_ld % 8 == 0 && dz_ld % 8 == 0 && x_ld >= cin && dz_ld >= cout, "wgrad: bad leading dimensions");
+  YB_REQUIRE(batch > 0 && in_h + 2 * pad_h >= kh && in_w + 2 * pad_w >= kw, "wgrad: %d x %d input gives an empty output", in_h, in_w);
+  const int height = (in_h + 2 * pad_h - kh) / stride + 1, width = (in_w + 2 * pad_w - kw) / stride + 1;   // the output grid
   const long long m_total = static_cast<long long>(batch) * height * width;
   YB_REQUIRE(m_total > 0 && m_total < (1ll << 31) - 256, "wgrad: bad pixel count");
   EncodeTiledFn enc_tiled;
@@ -233,15 +243,16 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
   int rc = get_tensor_map_encoders(&enc_tiled, &enc_im2col);
   if (rc) return rc;
 
-  const bool narrow = (cin == 32);
+  const bool narrow = (cin % 64 != 0);         // 32-channel activation boxes
   const int KP = kWgKP;
   const int nmax = narrow ? kWgNmaxNarrow : kWgNmaxWide;
 
   WgradParams p;
   p.m_total = static_cast<int>(m_total); p.hw = height * width; p.width = width;
-  p.cin = cin; p.cout = cout; p.ksize = ksize; p.pad = (ksize - 1) / 2;
-  const int taps = ksize * ksize;
-  p.n_per_group = cin >= 256 ? 256 : cin;                       // 32, 64, 128 or 256
+  p.cin = cin; p.cout = cout; p.kh = kh; p.kw = kw; p.pad_h = pad_h; p.pad_w = pad_w; p.stride = stride;
+  const int taps = kh * kw;
+  // wide: 64, 128, 192 or 256 channels per group; narrow: 96 (Cin = 96, 288, ...) or 32 (Cin = 32, 160, ...)
+  p.n_per_group = narrow ? (cin % 96 == 0 ? 96 : 32) : (cin >= 256 ? 256 : cin);
   if (p.n_per_group > nmax) p.n_per_group = nmax;
   p.chunks_per_tap = (cin + p.n_per_group - 1) / p.n_per_group;
   p.col_tiles = taps * p.chunks_per_tap;
@@ -294,20 +305,21 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "wgrad: cuTensorMapEncodeTiled(dz) failed (%d)", static_cast<int>(cr));
   }
   {
-    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(cin), static_cast<cuuint64_t>(width), static_cast<cuuint64_t>(height),
+    // the input tensor; window corners span [-pad, in + pad - k] on each axis, walked with the conv's stride (the output grid)
+    const cuuint64_t dims[4] = {static_cast<cuuint64_t>(cin), static_cast<cuuint64_t>(in_w), static_cast<cuuint64_t>(in_h),
                                 static_cast<cuuint64_t>(batch)};
-    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * width,
-                                   static_cast<cuuint64_t>(x_ld) * 2 * width * height};
-    const int lower[2] = {-p.pad, -p.pad};
-    const int upper[2] = {p.pad - (ksize - 1), p.pad - (ksize - 1)};
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    const cuuint64_t strides[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * in_w,
+                                   static_cast<cuuint64_t>(x_ld) * 2 * in_w * in_h};
+    const int lower[2] = {-pad_w, -pad_h};                    // {W, H}
+    const int upper[2] = {pad_w - (kw - 1), pad_h - (kh - 1)};
+    const cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
     const CUresult cr = enc_im2col(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x), dims, strides, lower, upper, narrow ? 32 : 64,
                                    KP, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, narrow ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "wgrad: cuTensorMapEncodeIm2col failed (%d)", static_cast<int>(cr));
     int drv = 0;
     cudaDriverGetVersion(&drv);
-    const unsigned long long span_bytes = static_cast<unsigned long long>(x_ld) * 2ull * width * height * batch;
+    const unsigned long long span_bytes = static_cast<unsigned long long>(x_ld) * 2ull * in_w * in_h * batch;
     if (drv <= 13010 && span_bytes < 131072ull) reinterpret_cast<uint64_t*>(&tx)[1] &= ~(1ull << 21);
   }
   const int grid = p.co_tiles * p.col_groups * p.splits;
@@ -322,7 +334,43 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
     if (n == 192) return launch_wgrad<128, kWgKP, kWgStages, kWgNmaxWide, 192>(tdz, tx, p, grid, stream);
     if (n == 256) return launch_wgrad<128, kWgKP, kWgStages, kWgNmaxWide, 256>(tdz, tx, p, grid, stream);
   }
-  return fail(YB_ERR_UNSUPPORTED, "wgrad: %d accumulator columns per CTA (Cin=%d, k=%d) has no kernel", n, cin, ksize);
+  return fail(YB_ERR_UNSUPPORTED, "wgrad: %d accumulator columns per CTA (Cin=%d, %d x %d) has no kernel", n, cin, kh, kw);
+}
+
+// The general geometry (Inception-v3): Cin a multiple of 32 up to 2048.
+int conv2d_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride,
+                         int pad_h, int pad_w, int x_ld, int dz_ld, cudaStream_t stream) {
+  YB_REQUIRE(cin <= 2048, "wgrad: Cin=%d unsupported (a multiple of 32 up to 2048)", cin);
+  return wgrad_run(x, dz, dw_krsc, batch, in_h, in_w, cin, cout, kh, kw, stride, pad_h, pad_w, x_ld, dz_ld, stream);
+}
+
+// The square same-padded form (Darknet, ResNet, VGG): k in {1, 3}, Cin = 32 or a multiple of 64, no upper limit.
+int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch, int height, int width, int cin, int cout, int ksize, int x_ld,
+                       int dz_ld, cudaStream_t stream) {
+  YB_REQUIRE(x && dz && dw_krsc, "wgrad: null pointer");
+  YB_REQUIRE(ksize == 1 || ksize == 3, "wgrad: ksize");
+  YB_REQUIRE(cin % 32 == 0 && (cin == 32 || cin % 64 == 0), "wgrad: Cin=%d unsupported", cin);
+  return wgrad_run(x, dz, dw_krsc, batch, height, width, cin, cout, ksize, ksize, 1, (ksize - 1) / 2, (ksize - 1) / 2, x_ld, dz_ld, stream);
+}
+
+// fp32 [Cout][kh][kw][krsc_cin] (the wgrad layout; krsc_cin >= cin when the activation carried zero channels) -> fp32 OIHW [Cout][Cin][kh][kw],
+// times `scale`.  One thread per output element.
+__global__ void unpack_wgrad_khw_kernel(const float* __restrict__ g, float* __restrict__ out, int cout, int cin, int taps, int krsc_cin, float scale) {
+  const long long total = static_cast<long long>(cout) * cin * taps;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int tap = static_cast<int>(idx % taps);
+  const long long t = idx / taps;
+  const int ci = static_cast<int>(t % cin);
+  const long long co = t / cin;
+  out[idx] = g[(co * taps + tap) * krsc_cin + ci] * scale;
+}
+
+int unpack_wgrad_khw(const float* g_krsc, float* out_oihw, int cout, int cin, int kh, int kw, int krsc_cin, float scale, cudaStream_t stream) {
+  YB_REQUIRE(g_krsc && out_oihw && cout > 0 && cin > 0 && krsc_cin >= cin && kh >= 1 && kh <= 7 && kw >= 1 && kw <= 7, "unpack_wgrad_khw: bad argument");
+  const long long total = static_cast<long long>(cout) * cin * kh * kw;
+  unpack_wgrad_khw_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(g_krsc, out_oihw, cout, cin, kh * kw, krsc_cin, scale);
+  return check_launch("unpack_wgrad_khw_kernel");
 }
 
 }  // namespace yb

@@ -419,15 +419,16 @@ int dw_wgrad(const void* a, const void* dz, float* dw, int batch, int height, in
   return check_launch("dw_wgrad_kernel");
 }
 
-// Weight gradient of the stride-2 first layer: dw[co][ci][r][s] = sum x[b, ci, 2*oy - 1 + r, 2*ox - 1 + s] * dz[b, oy, ox, co]  (fp32 OIHW [32,3,3,3],
-// ADDED to dw, zeroed by the host first).  256 threads = 32 output channels x 8 pixel lanes; a thread keeps its channel's 27 sums in registers.
+// Weight gradient of the stride-2 first layer: dw[co][ci][r][s] = sum x[b, ci, 2*oy - kPad + r, 2*ox - kPad + s] * dz[b, oy, ox, co]  (fp32 OIHW
+// [32,3,3,3], ADDED to dw, zeroed by the host first).  kPad = 1: MobileNet (even H, W); kPad = 0: Inception-v3's Conv2d_1a_3x3 (any H, W >= 3).  256 threads = 32 output channels x 8 pixel lanes; a thread keeps its channel's 27 sums in registers.
+template <int kPad>
 __global__ void __launch_bounds__(256) mb_conv0_wgrad_kernel(const float* __restrict__ x, const __half* __restrict__ dz, float* __restrict__ dw, int batch,
                                                              int height, int width) {
   __shared__ float s_dw[32 * 27];
   for (int i = threadIdx.x; i < 32 * 27; i += blockDim.x) s_dw[i] = 0.f;
   __syncthreads();
   const int co = threadIdx.x & 31, lane = threadIdx.x >> 5;
-  const int oh = height >> 1, ow = width >> 1;
+  const int oh = (height + 2 * kPad - 3) / 2 + 1, ow = (width + 2 * kPad - 3) / 2 + 1;
   const long long pixels = static_cast<long long>(batch) * oh * ow;
   float acc[27];
 #pragma unroll
@@ -442,10 +443,10 @@ __global__ void __launch_bounds__(256) mb_conv0_wgrad_kernel(const float* __rest
     for (int ci = 0; ci < 3; ++ci)
 #pragma unroll
       for (int r = 0; r < 3; ++r) {
-        const int iy = 2 * oy - 1 + r;
+        const int iy = 2 * oy - kPad + r;
 #pragma unroll
         for (int s2 = 0; s2 < 3; ++s2) {
-          const int ix = 2 * ox - 1 + s2;
+          const int ix = 2 * ox - kPad + s2;
           const float v = (iy >= 0 && iy < height && ix >= 0 && ix < width) ? __ldg(x + ((img * 3 + ci) * height + iy) * width + ix) : 0.f;
           acc[ci * 9 + r * 3 + s2] = fmaf(v, g, acc[ci * 9 + r * 3 + s2]);
         }
@@ -464,7 +465,33 @@ int mb_conv0_wgrad(const float* x, const void* dz, float* dw, int batch, int hei
   long long blocks = (pixels + 8 * 32 - 1) / (8 * 32);
   const int cap = sm_count() * 6;
   const int grid = static_cast<int>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
-  mb_conv0_wgrad_kernel<<<grid, 256, 0, stream>>>(x, reinterpret_cast<const __half*>(dz), dw, batch, height, width);
+  mb_conv0_wgrad_kernel<1><<<grid, 256, 0, stream>>>(x, reinterpret_cast<const __half*>(dz), dw, batch, height, width);
+  return check_launch("mb_conv0_wgrad_kernel");
+}
+
+// Inception-v3's Conv2d_1a_3x3 in training: the raw conv output z (no BatchNorm, no ReLU) and the weight gradient from the fp32 image, at
+// padding `pad` (0 for Inception; 1 gives the bits of the MobileNet forms).
+int stem3x3_s2_raw(const float* x, const float* w, void* z, int batch, int height, int width, int pad, cudaStream_t stream) {
+  YB_REQUIRE(x && w && z && batch > 0 && (pad == 0 || pad == 1), "stem3x3_s2_raw: bad argument (pad 0 or 1)");
+  YB_REQUIRE(height + 2 * pad >= 3 && width + 2 * pad >= 3, "stem3x3_s2_raw: %d x %d input gives an empty output", height, width);
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(z) & 15) == 0, "stem3x3_s2_raw: z must be 16B aligned");
+  const long long total = static_cast<long long>(batch) * ((height + 2 * pad - 3) / 2 + 1) * ((width + 2 * pad - 3) / 2 + 1);
+  const unsigned grid = static_cast<unsigned>((total + 255) / 256);
+  if (pad == 0) mb_conv0_kernel<0><<<grid, 256, 0, stream>>>(x, w, w, w, reinterpret_cast<__half*>(z), batch, height, width, 1, 0);
+  else mb_conv0_kernel<1><<<grid, 256, 0, stream>>>(x, w, w, w, reinterpret_cast<__half*>(z), batch, height, width, 1, 0);
+  return check_launch("mb_conv0_kernel");
+}
+
+int stem3x3_s2_wgrad(const float* x, const void* dz, float* dw, int batch, int height, int width, int pad, cudaStream_t stream) {
+  YB_REQUIRE(x && dz && dw && batch > 0 && (pad == 0 || pad == 1), "stem3x3_s2_wgrad: bad argument (pad 0 or 1)");
+  YB_REQUIRE(height + 2 * pad >= 3 && width + 2 * pad >= 3, "stem3x3_s2_wgrad: %d x %d input gives an empty output", height, width);
+  YB_CUDA(cudaMemsetAsync(dw, 0, 32 * 27 * sizeof(float), stream));
+  const long long pixels = static_cast<long long>(batch) * ((height + 2 * pad - 3) / 2 + 1) * ((width + 2 * pad - 3) / 2 + 1);
+  long long blocks = (pixels + 8 * 32 - 1) / (8 * 32);
+  const int cap = sm_count() * 6;
+  const int grid = static_cast<int>(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
+  if (pad == 0) mb_conv0_wgrad_kernel<0><<<grid, 256, 0, stream>>>(x, reinterpret_cast<const __half*>(dz), dw, batch, height, width);
+  else mb_conv0_wgrad_kernel<1><<<grid, 256, 0, stream>>>(x, reinterpret_cast<const __half*>(dz), dw, batch, height, width);
   return check_launch("mb_conv0_wgrad_kernel");
 }
 

@@ -1,4 +1,4 @@
-"""model.inception3 -- Inception-v3 backbone plugin on the CUDA kernels (inference).
+"""model.inception3 -- Inception-v3 backbone plugin on the CUDA kernels (inference and training).
 
 Drop-in for the reference's `model/inception3.py` (:29-118): `Inception3(config_channels, anchors, num_cls, transform_input=False)`, selectable
 with `[model] dnn = model.inception3.Inception3`, with the module tree and state_dict keys of the reference (torchvision's `BasicConv2d` =
@@ -14,14 +14,18 @@ head `conv` (:52).  Forward x[B,3,H,W] fp32 -> [B, A*(5+C), OH, OW] fp32, where 
   conv (+ bias)                         -> yb_conv2d_bn_act_fwd, fp32 NCHW out.
 The tensor-core conv needs Cin % 32 == 0: Conv2d_3b_1x1 (80 filters) and branch5x5_1 (48) run with 96 / 64 filters whose extra rows are zero
 (scale 1, shift 0: ReLU stores exact zeros) and their consumers read those channels with zero weights -- exact, no kernel change.
-The folded BatchNorms and packed weights are cached per parameter version; switching train() / eval() drops the cache.  There is no CPU
-path and no training path.
+The folded BatchNorms and packed weights are cached per parameter version; switching train() / eval() drops the cache.
+In train() mode on a CUDA tensor the forward is one autograd node (model.yolo2._DarknetTrainFunction) over
+b200.train_engine.InceptionTrainer: batch-statistics BatchNorm (eps 1e-3, momentum from the module), the running-statistics update, and an
+explicit backward chain that gives every parameter its fp32 gradient.  There is no CPU path: a train-mode forward on a CPU tensor raises
+NotImplementedError, an eval-mode one RuntimeError.
 """
 import torch
 import torch.nn as nn
 
 import model
 from b200 import ops as _ops
+from b200 import train_engine as _train
 
 MIN_SIZE = 75      # the smallest input side whose every stage is non-empty (Mixed_7a's output is 1 x 1)
 
@@ -134,7 +138,14 @@ class Inception3(nn.Module):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
         self._cache = {}
+        self._trainer = None
         _pretrained(self, config_channels)
+
+    @property
+    def trainer(self):
+        if self._trainer is None:
+            self._trainer = _train.InceptionTrainer(self)
+        return self._trainer
 
     def train(self, mode=True):
         """nn.Module.train + drop cached kernel operands."""
@@ -282,10 +293,14 @@ class Inception3(nn.Module):
         return _ops.conv2d_bn_act(a, w16, one, bias, 1.0, out_mode=_ops.OUT_F32_NCHW)
 
     def forward(self, x):
-        if self.training:
-            raise NotImplementedError('Inception3: training is not implemented on the kernels; call .eval() for inference')
         if self.transform_input:
             raise NotImplementedError('Inception3: transform_input=True has no kernel path (the reference never sets it)')
+        if self.training:
+            if not x.is_cuda:
+                raise NotImplementedError('Inception3: training runs on the CUDA kernels only; the input is a CPU tensor')
+            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.InceptionTrainer)
+            from model.yolo2 import _DarknetTrainFunction
+            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
         return self.run(x)
 
 
