@@ -56,7 +56,9 @@ const char* yb_last_error(void);
 int yb_debug_read(int out[4]);
 /* Profiling aid (tools/conv_trace.py): when dev_buf (768 x uint64, device memory) is non-NULL, block 0 of the
  * wgmma conv kernels records clock64() per pipeline event: [0,256) TMA producer, [256,512) MMA issuer,
- * [512,768) epilogue.  NULL switches it off (the default). */
+ * [512,768) epilogue.  The two-consumer kernel records per tile i of block 0: [256 + 2i] its last full-barrier
+ * wait, [257 + 2i] its first wgmma issue, [512 + 2i] its K-loop end, [513 + 2i] its epilogue end.  NULL switches it
+ * off (the default). */
 int yb_conv_set_trace(void* dev_buf);
 
 /* ---- parameter preparation ---------------------------------------------------------------- */

@@ -672,14 +672,24 @@ conv_preact_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 }
 
 // ---------------------------------------------------------------------------------------------
-// Wide family: a 256 x 128 CTA tile on two consumer warpgroups.  Warpgroup 0 is the producer (one thread issues the TMAs,
-// the group gives its registers back), warpgroups 1 and 2 each accumulate 128 pixels x 128 channels in registers
-// (128 fp32 per thread) from the same stage: A is one 256-pixel box, B is read by both.  Per FLOP that moves 2/3 of the
-// operand bytes of the 128 x 128 tile.  The epilogue runs from the registers (scale / shift, leaky, fp16, a 128B-swizzled
-// staging slice, TMA store), so there is no accumulator park; stream-K partials go to and come from `ws` out of the
-// registers.  Each accumulator sees the same K-blocks and k16 steps in the same order as in the 128 x 128 kernel, so a
-// launch without stream-K is bit-identical to it.  fp16 NHWC output only: the head, the residual (lo) output and the
-// training statistics stay on conv_igemm_kernel.
+// Wide family: a 256 x 128 CTA tile on two consumer warpgroups.  Warpgroup 0 is the producer (one thread issues the TMA loads,
+// one thread per consumer issues that consumer's TMA stores; the group gives its registers back), warpgroups 1 and 2 each
+// accumulate 128 pixels x 128 channels in registers (128 fp32 per thread) from the same stage: A is one 256-pixel box, B is read
+// by both.  Per FLOP that moves 2/3 of the operand bytes of the 128 x 128 tile.  The epilogue runs from the registers (scale /
+// shift, leaky, fp16, a 128B-swizzled staging slice, TMA store), so there is no accumulator park; stream-K partials go to and
+// come from `ws` out of the registers.  Each accumulator sees the same K-blocks and k16 steps in the same order as in the
+// 128 x 128 kernel, so a launch without stream-K is bit-identical to it.  fp16 NHWC output only: the head, the residual (lo)
+// output and the training statistics stay on conv_igemm_kernel.
+//
+// Epilogue overlap.  The tensor cores idle from a tile's last MMA to the next tile's first one, so the consumers keep that
+// stretch down to the conversion arithmetic:
+//   * the last K-block is committed as two groups, and rows 0..63 of a consumer's tile are converted while the MMAs into rows
+//     64..127 still run;
+//   * the tile's scale / shift sit in a shared-memory table (one float per consumer thread, loaded when the tile starts and
+//     stored there at its end), so the conversion reads one 16-byte word per column pair instead of waiting on global loads;
+//   * each 64-row half goes through the consumer's 16 KB staging slice, and a thread of the producer warpgroup issues its TMA
+//     stores and waits for them to read the slice (mbarriers slice_full / slice_empty): the consumer converts the second half
+//     into registers while the first half's stores drain, and starts the next tile as soon as the second half is staged.
 // ---------------------------------------------------------------------------------------------
 constexpr int kWideThreads = 384;
 constexpr int kWideRows = 256;
@@ -691,12 +701,13 @@ struct WideCfg {
   static constexpr int kABytes = kWideRows * BK * 2;
   static constexpr int kBBytes = kWideBN * BK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kOutBytes = 128 * 128;                   // per consumer: 128 rows x 64 channels fp16, 128B-swizzled
-  static constexpr int kFixedBytes = 2 * kOutBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kOutBytes = 128 * 128;                   // per consumer: 64 rows x 128 channels fp16 as two [64][128 B] blocks, 128B-swizzled
+  static constexpr int kTableBytes = kWideBN * 2 * 4;           // the tile's scale / shift: float4 {sc[2i], sc[2i + 1], sh[2i], sh[2i + 1]} per column pair
+  static constexpr int kFixedBytes = 2 * kOutBytes + kTableBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static constexpr int kStages = ((kSmemLimit - kFixedBytes) / kStageBytes) > 8 ? 8 : ((kSmemLimit - kFixedBytes) / kStageBytes);
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static constexpr int kWsFloats = kWideRows * kWideBN;         // one CTA's stream-K partial tile
-  static_assert(kStages >= 3, "shared memory budget");
+  static_assert(kStages >= (BK == 64 ? 4 : 8), "shared memory budget: the epilogue's slices and table must not cost a pipeline stage");
 };
 
 template <int BK>
@@ -710,8 +721,11 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const uint32_t smem_a = smem_base;
   const uint32_t smem_b = smem_base + kStages * Cfg::kABytes;
   const uint32_t smem_o = smem_base + kStages * Cfg::kStageBytes;         // [2 consumers][kOutBytes]
-  const uint32_t bar_full = smem_o + 2 * Cfg::kOutBytes;                 // [kStages]
-  const uint32_t bar_empty = bar_full + 8 * kStages;                     // [kStages]
+  const uint32_t table = smem_o + 2 * Cfg::kOutBytes;                     // [kWideBN / 2] float4
+  const uint32_t bar_full = table + Cfg::kTableBytes;                     // [kStages]
+  const uint32_t bar_empty = bar_full + 8 * kStages;                      // [kStages]
+  const uint32_t bar_slice_full = bar_empty + 8 * kStages;                // [2 consumers]: a 64-row half is staged
+  const uint32_t bar_slice_empty = bar_slice_full + 16;                   // [2 consumers]: its stores have read the slice
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int unit_id = static_cast<int>(blockIdx.x);
   const int num_units = static_cast<int>(gridDim.x);
@@ -720,6 +734,10 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar_full + 8 * i, 1);
       mbar_init(bar_empty + 8 * i, 8);                     // one arrival per consumer warp
+    }
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(bar_slice_full + 8 * c, 4);                // one arrival per warp of consumer c
+      mbar_init(bar_slice_empty + 8 * c, 1);               // its store thread
     }
     fence_mbar_init();
     fence_proxy_async_smem();
@@ -737,6 +755,7 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
+      int tr_p = 0;
       for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
         const int n_tile = it.tile % p.n_tiles;
         const int m_cta = (it.tile / p.n_tiles) * kWideRows;
@@ -752,6 +771,7 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           const int r = tap / p.kw;
           const int s = tap - r * p.kw;
           mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0x600 | stage);
+          YB_TRACE(0, tr_p); ++tr_p;
           const uint32_t full = bar_full + 8 * stage;
           mbar_arrive_expect_tx(full, Cfg::kStageBytes);      // the A box always transfers (and zero-fills) all 256 rows
           const uint32_t dst = smem_a + stage * Cfg::kABytes;
@@ -761,6 +781,34 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
+    } else if (threadIdx.x == 32 || threadIdx.x == 64) {
+      // store thread of consumer c: ships each staged 64-row half (rows >= M and channels >= Cout are clipped by the tensor map)
+      const int c = (threadIdx.x >> 5) - 1;
+      const uint32_t slice = smem_o + c * Cfg::kOutBytes;
+      uint32_t sph = 0;
+      for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
+        if (it.kb1 < p.num_kb) continue;                      // stream-K dump: nothing to store
+        const int n0 = (it.tile % p.n_tiles) * kWideBN;
+        const int m_base = (it.tile / p.n_tiles) * kWideRows + c * 128;
+        for (int h = 0; h < 2; ++h) {
+          mbar_wait(bar_slice_full + 8 * c, sph, p.dbg, 0x900 | c);
+#pragma unroll
+          for (int c2 = 0; c2 < 2; ++c2) {
+            if (n0 + c2 * 64 < p.cout) {
+#pragma unroll
+              for (int g = 0; g < 2; ++g) {
+                const int row = m_base + h * 64 + g * 32;
+                if (row < p.m_total) tma_store_2d(&tmap_y, slice + c2 * 8192 + g * 4096, n0 + c2 * 64, row);
+              }
+            }
+          }
+          tma_store_commit();
+          tma_store_wait_read<0>();
+          mbar_arrive(bar_slice_empty + 8 * c);
+          sph ^= 1;
+        }
+      }
+      tma_store_wait<0>();     // every bulk store has landed before the CTA's shared memory goes away
     }
     return;
   }
@@ -771,52 +819,74 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int warp = t >> 5;
   const int lane = t & 31;
   const bool leader = threadIdx.x == 128;
-  const uint32_t stage_o = smem_o + cw * Cfg::kOutBytes;
+  const uint32_t slice = smem_o + cw * Cfg::kOutBytes;
+  const int te = cw * 128 + t;                 // this thread's entry of the scale / shift table
+  const float4* tab4 = reinterpret_cast<const float4*>(smem_raw + (table - smem_u32(smem_raw)));
   float acc[2][64];
   int stage = 0;
   uint32_t phase = 0;
-  for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
+  uint32_t sph = 0;                            // staging slice phase
+  // trace (yb_conv_set_trace; block 0, consumer 0's first thread), tile i of the CTA: role 1 slot 2i = its last full-barrier wait,
+  // 2i + 1 = its first wgmma issue; role 2 slot 2i = its K-loop end (every MMA retired), 2i + 1 = its epilogue end.  tr_t = 2i
+  int tr_t = 0;
+  for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next(), tr_t += 2) {
     const int kb_first = it.kb0, kb_last = it.kb1 - 1;
-    int prev = -1;
-    for (int kb = kb_first; kb <= kb_last; ++kb) {
-      mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x700 | stage);
-      const uint64_t bdesc = make_kmajor_desc<Cfg::kSwizzle>(smem_b + stage * Cfg::kBBytes);
-      wgmma_fence();
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint64_t adesc = make_kmajor_desc<Cfg::kSwizzle>(smem_a + stage * Cfg::kABytes + (cw * 128 + h * 64) * Cfg::kSwizzle);
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k)
-          wgmma_f16<kWideBN>(acc[h], adesc + 2 * k, bdesc + 2 * k, ((kb - kb_first) | k) != 0);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar_empty + 8 * prev); }
-      prev = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
-    }
-    wgmma_wait<0>();
-    fence_regs(acc[0]);
-    fence_regs(acc[1]);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
-
     const int tile = it.tile;
     const int n0 = (tile % p.n_tiles) * kWideBN;
-    const int m_base = (tile / p.n_tiles) * kWideRows + cw * 128;
+    // stream-K roles of this segment: it stops short of the tile's last K-block (dump the partial sums), or finishes a tile whose
+    // first K-blocks were summed by lower-numbered CTAs (collect their partials first)
     const bool sk_dump = it.kb1 < p.num_kb;
     const bool sk_collect = !sk_dump && it.kb0 > 0;
-    // per-thread partial layout: float4 g of thread t of consumer cw at ((cw * 32 + g) * 128 + t) * 4 -- coalesced both ways
-    if (sk_dump) {
-      float4* dst = reinterpret_cast<float4*>(p.ws + static_cast<size_t>(blockIdx.x) * Cfg::kWsFloats) + cw * 32 * 128 + t;
-#pragma unroll
-      for (int g = 0; g < 32; ++g)
-        dst[g * 128] = make_float4(acc[g >> 4][4 * (g & 15)], acc[g >> 4][4 * (g & 15) + 1], acc[g >> 4][4 * (g & 15) + 2], acc[g >> 4][4 * (g & 15) + 3]);
-      __threadfence();
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (leader) st_release_gpu(p.flags + blockIdx.x, 1u);
-      continue;
+    float tab = 0.f;                           // table entry te: column pair te / 4, {scale, scale, shift, shift}[te % 4]
+    {
+      const int col = n0 + 2 * (te >> 2) + (te & 1);
+      if (!sk_dump && col < p.cout) tab = __ldg(((te & 2) ? p.shift : p.scale) + col);
     }
+    // waits for K-block kb's stage and returns its B descriptor
+    auto stage_ready = [&](int kb) {
+      mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x700 | stage);
+      if (leader) {
+        if (kb == kb_last) YB_TRACE(1, tr_t);
+        if (kb == kb_first) YB_TRACE(1, tr_t + 1);
+      }
+      wgmma_fence();
+      return make_kmajor_desc<Cfg::kSwizzle>(smem_b + stage * Cfg::kBBytes);
+    };
+    // one K-block of MMAs into the accumulator rows 64 h .. 64 h + 63
+    auto mma_rows = [&](float (&d)[64], int h, uint64_t bdesc, bool first_kb) {
+      const uint64_t adesc = make_kmajor_desc<Cfg::kSwizzle>(smem_a + stage * Cfg::kABytes + (cw * 128 + h * 64) * Cfg::kSwizzle);
+#pragma unroll
+      for (int k = 0; k < BK / UMMA_K; ++k) wgmma_f16<kWideBN>(d, adesc + 2 * k, bdesc + 2 * k, !first_kb || k != 0);
+    };
+    // the MMAs of the stage before `stage` have retired: hand it back to the producer
+    auto release_prev = [&]() {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * (stage == 0 ? kStages - 1 : stage - 1));
+    };
+    auto next_stage = [&](int kb) {
+      if (kb != kb_first) release_prev();
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    };
+    for (int kb = kb_first; kb < kb_last; ++kb) {
+      const uint64_t bdesc = stage_ready(kb);
+      mma_rows(acc[0], 0, bdesc, kb == kb_first);
+      mma_rows(acc[1], 1, bdesc, kb == kb_first);
+      wgmma_commit();
+      wgmma_wait<1>();      // one group in flight: the previous K-block's MMAs have retired, so its stage can be refilled
+      next_stage(kb);
+    }
+    {
+      // the last K-block, committed as two groups: rows 0..63 retire first
+      const uint64_t bdesc = stage_ready(kb_last);
+      mma_rows(acc[0], 0, bdesc, kb_last == kb_first);
+      wgmma_commit();
+      mma_rows(acc[1], 1, bdesc, kb_last == kb_first);
+      wgmma_commit();
+      wgmma_wait<1>();
+      fence_regs(acc[0]);
+      next_stage(kb_last);
+    }
+
     int sk_lo = 0;
     if (sk_collect) {
       const int u = tile * p.num_kb;
@@ -839,62 +909,87 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
-      for (int j = sk_lo; j < static_cast<int>(blockIdx.x); ++j) {
-        const float4* src = reinterpret_cast<const float4*>(p.ws + static_cast<size_t>(j) * Cfg::kWsFloats) + cw * 32 * 128 + t;
+    }
+    if (!sk_dump) {
+      // every consumer thread is done with the previous tile's table before it is overwritten, and reads this one after
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      asm volatile("st.shared.f32 [%0], %1;" :: "r"(table + 4 * te), "f"(tab) : "memory");
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+    // per-thread partial layout: float4 g of thread t of consumer cw at ((cw * 32 + g) * 128 + t) * 4 -- coalesced both ways;
+    // g / 16 is the accumulator row half h
 #pragma unroll
-        for (int g = 0; g < 32; ++g) {
+    for (int h = 0; h < 2; ++h) {
+      if (h == 1) {
+        wgmma_wait<0>();
+        fence_regs(acc[1]);
+        if (leader) YB_TRACE(2, tr_t);
+        release_prev();
+      }
+      if (sk_dump) {
+        float4* dst = reinterpret_cast<float4*>(p.ws + static_cast<size_t>(blockIdx.x) * Cfg::kWsFloats) + (cw * 32 + 16 * h) * 128 + t;
+#pragma unroll
+        for (int g = 0; g < 16; ++g) dst[g * 128] = make_float4(acc[h][4 * g], acc[h][4 * g + 1], acc[h][4 * g + 2], acc[h][4 * g + 3]);
+        continue;
+      }
+      for (int j = sk_lo; j < (sk_collect ? static_cast<int>(blockIdx.x) : 0); ++j) {
+        const float4* src = reinterpret_cast<const float4*>(p.ws + static_cast<size_t>(j) * Cfg::kWsFloats) + (cw * 32 + 16 * h) * 128 + t;
+#pragma unroll
+        for (int g = 0; g < 16; ++g) {
           const float4 a = __ldcg(src + g * 128);
-          float* d = &acc[g >> 4][4 * (g & 15)];
-          d[0] += a.x; d[1] += a.y; d[2] += a.z; d[3] += a.w;
+          acc[h][4 * g] += a.x; acc[h][4 * g + 1] += a.y; acc[h][4 * g + 2] += a.z; acc[h][4 * g + 3] += a.w;
         }
       }
-    }
-    // fragment of thread t: acc[h][4 j + 2 hh + e] is tile row 64 h + 16 warp + lane / 4 + 8 hh, column 8 j + 2 (lane % 4) + e
+      // scale / shift, leaky, fp16.  Fragment of thread t: acc[h][4 j + 2 hh + e] is tile row 64 h + 16 warp + lane / 4 + 8 hh,
+      // column 8 j + 2 (lane % 4) + e; pk[16 c2 + 2 jj + hh] holds the pair of j = 8 c2 + jj
+      uint32_t pk[32];
 #pragma unroll
-    for (int c2 = 0; c2 < 2; ++c2) {
-      if (n0 + c2 * 64 < p.cout) {                 // uniform over the CTA
-        // the previous bulk store of this consumer has read the staging slice
-        if (t == 0) tma_store_wait_read<0>();
-        asm volatile("bar.sync %0, 128;" :: "r"(2 + cw) : "memory");
+      for (int c2 = 0; c2 < 2; ++c2) {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
-          const int col = n0 + c2 * 64 + 8 * jj + 2 * (lane & 3);
-          const bool ok = col < p.cout;            // Cout % 8 == 0: both columns of the pair agree
-          const float sc0 = ok ? __ldg(p.scale + col) : 0.f, sc1 = ok ? __ldg(p.scale + col + 1) : 0.f;
-          const float sh0 = ok ? __ldg(p.shift + col) : 0.f, sh1 = ok ? __ldg(p.shift + col + 1) : 0.f;
+          const float4 ss = tab4[c2 * 32 + 4 * jj + (lane & 3)];
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const int j = c2 * 8 + jj;
-              float x0 = acc[h][4 * j + 2 * hh] * sc0 + sh0;
-              float x1 = acc[h][4 * j + 2 * hh + 1] * sc1 + sh1;
-              x0 = x0 > 0.f ? x0 : x0 * p.slope;
-              x1 = x1 > 0.f ? x1 : x1 * p.slope;
-              __half2 v = __floats2half2_rn(x0, x1);
-              const int r = h * 64 + warp * 16 + (lane >> 2) + hh * 8;
-              const uint32_t addr = stage_o + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
-              asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(*reinterpret_cast<uint32_t*>(&v)) : "memory");
-            }
+          for (int hh = 0; hh < 2; ++hh) {
+            const int j = c2 * 8 + jj;
+            float x0 = acc[h][4 * j + 2 * hh] * ss.x + ss.z;
+            float x1 = acc[h][4 * j + 2 * hh + 1] * ss.y + ss.w;
+            x0 = x0 > 0.f ? x0 : x0 * p.slope;
+            x1 = x1 > 0.f ? x1 : x1 * p.slope;
+            __half2 v = __floats2half2_rn(x0, x1);
+            pk[16 * c2 + 2 * jj + hh] = *reinterpret_cast<uint32_t*>(&v);
           }
         }
-        fence_proxy_async_smem();
-        asm volatile("bar.sync %0, 128;" :: "r"(2 + cw) : "memory");
-        if (t == 0) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g)     // rows >= M and channels >= Cout are clipped by the tensor map
-            if (m_base + 32 * g < p.m_total) tma_store_2d(&tmap_y, stage_o + g * 4096, n0 + c2 * 64, m_base + 32 * g);
-          tma_store_commit();
-        }
       }
+      // the slice is free once the store thread has seen the previous half's stores read it
+      mbar_wait(bar_slice_empty + 8 * cw, sph ^ 1, p.dbg, 0xA00 | cw);
+#pragma unroll
+      for (int c2 = 0; c2 < 2; ++c2)
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = warp * 16 + (lane >> 2) + hh * 8;       // row inside the half
+            const uint32_t addr = slice + c2 * 8192 + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
+            asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(pk[16 * c2 + 2 * jj + hh]) : "memory");
+          }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_slice_full + 8 * cw);
+      sph ^= 1;
     }
+    if (sk_dump) {
+      __threadfence();
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (leader) st_release_gpu(p.flags + blockIdx.x, 1u);
+      continue;
+    }
+    if (leader) YB_TRACE(2, tr_t + 1);
     if (sk_collect) {
       // every reader is done with the partials: hand the slots back (the next writer is a later launch)
       asm volatile("bar.sync 1, 256;" ::: "memory");
       for (int j = sk_lo + t + 128 * cw; j < static_cast<int>(blockIdx.x); j += 256) p.flags[j] = 0u;
     }
   }
-  if (t == 0) tma_store_wait<0>();
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1355,15 +1450,15 @@ static int conv_c32_forward(const void* x, const void* w, const float* scale, co
 // Kernel and tile shape of one conv launch.  flags may force BLOCK_N (bits 8..17) and the number of 128-row M-subtiles
 // (bits 20..21), forbid (bit 3) or force (bit 30) stream-K; otherwise the (BLOCK_N, M-subtiles, stream-K) triple with the lowest
 // modelled time wins.  Model (constants fitted to profiles/conv_layers_h100.json: every shape of the 21 implicit-GEMM launches of
-// C2 timed alone on an H100 SXM at a 700 W power limit): tiles run in ceil(tiles / SMs) rounds; a K-block costs a fixed issue latency (im2col boxes cost
+// C2 timed alone on an H100 SXM at a 700 W power limit, median of three runs): tiles run in ceil(tiles / SMs) rounds; a K-block costs a fixed issue latency (im2col boxes cost
 // more than plain tiled ones) plus its operand bytes at a per-SM L2->SM rate; the one-warpgroup kernel's epilogue overlaps the
-// next main loop (a tile costs the larger of the two), the two-consumer kernel's register epilogue does not (they add).  With
+// next main loop (a tile costs the larger of the two), the two-consumer kernel's register epilogue mostly does not (they add).  With
 // these constants the model picks, on each of those 21 launches, a shape within 3 % of the fastest one measured.
 constexpr double kKbNsIm2col = 240.0;     // ns per K-block, every conv but 1x1 stride 1 (im2col-mode A box)
 constexpr double kKbNsTiled = 100.0;      // ns per K-block, 1x1 stride-1 layers (plain 2-D tiled A box)
 constexpr double kFeedBytesPerNs = 130.0; // L2 -> SM operand bytes per ns per SM
 constexpr double kEpiNsPerOut = 0.15;     // one-warpgroup epilogue, ns per output element (overlapped with the main loop)
-constexpr double kWideEpiNsPerOut = 0.08; // two-consumer register epilogue, ns per output element (not overlapped)
+constexpr double kWideEpiNsPerOut = 0.04; // two-consumer register epilogue, ns per output element (what the next tile's MMAs do not hide)
 constexpr double kSkNs = 16000.0;         // stream-K partial dump + collect, one-warpgroup kernel
 constexpr double kSkNsWide = 9000.0;      // the same from registers, two-consumer kernel
 // height / width are the OUTPUT dims (M counts output pixels); a K-block of every conv but 1x1 stride 1 pays the im2col box cost.
