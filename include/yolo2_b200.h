@@ -394,6 +394,11 @@ int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int widt
  * the number of in-range pixels (4 in a corner, 6 on an edge, 9 inside; 1 x N and N x 1 images count likewise).  Interior pixels are the bits
  * of yb_avgpool3x3_s1_f16.  C a multiple of 8, x / y 16-byte aligned. */
 int yb_avgpool3x3_s1_excl_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
+/* Its backward (training of the Inception-v4 plugin): dy, dx [B,H,W,C] fp16 NHWC; for each input pixel i, dx[i] = fp16(sum over the in-range
+ * outputs o of i's 3x3 neighbourhood, row-major, of dy[o] / n(o)), n(o) the in-range count of o's own window (4 / 6 / 9; 1 x N and N x 1 alike),
+ * each term one round-to-nearest fp32 division, summed in fp32 and rounded once.  A gather: no atomics, deterministic.  C a multiple of 8,
+ * dy / dx 16-byte aligned. */
+int yb_avgpool3x3_s1_excl_bwd_f16(const void* dy, void* dx, int batch, int height, int width, int channels, yb_stream_t stream);
 
 /* Training of the Inception-v3 plugin (model/inception3.py): the gradients of the general-geometry conv and of the stem, the pools and the joins.
  *   conv2d_wgrad        dw fp32 [Cout][kh][kw][Cin] (overwritten, not scaled) of the yb_conv2d_bn_act_fwd geometry: kh, kw in 1..7, pad < k,

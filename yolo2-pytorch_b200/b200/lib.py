@@ -101,6 +101,7 @@ SIGNATURES = {
     'yb_maxpool3x3_s2_valid_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_avgpool3x3_s1_f16': [P, P, c_int, c_int, c_int, c_int, P],
     'yb_avgpool3x3_s1_excl_f16': [P, P, c_int, c_int, c_int, c_int, P],
+    'yb_avgpool3x3_s1_excl_bwd_f16': [P, P, c_int, c_int, c_int, c_int, P],
     'yb_conv2d_wgrad': [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_unpack_wgrad_khw': [P, P, c_int, c_int, c_int, c_int, c_int, c_float, P],
     'yb_pack_weight_dgrad_khw_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],

@@ -285,6 +285,17 @@ def avgpool3x3_s1_excl(x, out=None):
     return out
 
 
+def avgpool3x3_s1_excl_bwd(dy, out=None):
+    """Backward of avgpool3x3_s1_excl on fp16 NHWC dy [B,H,W,C]: each output's gradient divided by its own in-range count, gathered at the
+    inputs of its window (fp32 sum, one rounding)."""
+    _req(dy, torch.float16, 'dy')
+    b, h, w, c = dy.shape
+    out = torch.empty_like(dy) if out is None else out
+    _req(out, torch.float16, 'out')
+    _ck(_l.load().yb_avgpool3x3_s1_excl_bwd_f16(_p(dy), _p(out), b, h, w, c, _s()), 'yb_avgpool3x3_s1_excl_bwd_f16')
+    return out
+
+
 def conv2d_wgrad(x, dz, kh, kw, stride=1, pad=(0, 0), cin=None, cout=None, out=None):
     """yb_conv2d_wgrad: fp32 [Cout,kh,kw,Cin] (not scaled) of the yb_conv2d_bn_act_fwd geometry, from x fp16 [B,H,W,x_ld] (channels [0, cin))
     and dz fp16 [B,OH,OW,dz_ld] (channels [0, cout)) at the conv's output grid."""

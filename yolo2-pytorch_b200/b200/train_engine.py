@@ -1610,3 +1610,258 @@ class InceptionTrainer(TrainerBase):
         self.stem_backward(saved.stem, g, grads)
         self._finish_backward(dev)
         return grads
+
+
+class Inception4Trainer(InceptionTrainer):
+    """Training-mode forward / backward of the full-width `model.inception4.Inception4` (reference model/inception4.py), with BatchNorm on or
+    off, for any input side >= 75.  The blocks come from the model's own tables (`Block.UNITS / POOLS / CAT`, `Block.chain`, the plan of
+    `Inception4._plan`); at full width every width is a multiple of 32 and every channel layout the identity.
+
+    BatchNorm on: every unit is InceptionTrainer's (raw conv -> batch statistics in power-of-two channel chunks -> running-statistics update
+    with the module's eps 1e-3 and momentum 0.1 -> normalise + ReLU into the unit's channel range of its block's buffer); features.0 is the
+    raw stride-2 stem kernel on the fp32 image.  BatchNorm off (conv with bias -> ReLU): the inference epilogue (scale 1, shift = bias, ReLU)
+    writes the activation straight into the block buffer and is kept as the ReLU mask; its backward is yb_bn_act_bwd with has_bn = 0 in the
+    same channel chunks, and the reduce pass's per-channel sum is the bias gradient (as VGGTrainer's plain units).
+
+    Backward of a block runs its units in reverse; the gradient at a tensor read by several units (the block input: up to three branch heads
+    plus the pool term; Inception_C's branch1_0 and branch2_2, each read by two convs) is joined once (yb_join_f16).  The branch3 term is
+    yb_avgpool3x3_s1_excl_bwd_f16 of that conv's data gradient: the count-exclusive pool is not its own transpose (each output divides by
+    its own count, 4, 6 or 9); the max-pool term is yb_maxpool3x3_s2_valid_bwd_f16 from the block gradient's channel slice.  The stem runs
+    last: features.2 and features.1, then features.0's BatchNorm (or ReLU) backward and its weight gradient from the fp32 image.
+
+    The static loss scale is 32, not Inception-v3's 1024.  With BatchNorm the largest stored |gradient| grows 2100- to 3800-fold from the
+    last block to features.0's dz (measured on the synthetic steps of the tests: peaks of 4708 at 4 x 107 x 139 and 2934 at 2 x 416^2 at
+    scale 32); 1024 overflowed fp16 on the first step and 64 left less than 8-fold headroom below 65504.  Without BatchNorm the gradient
+    does not grow (peaks of 0.3 to 0.8 at scale 32) and part of the stem's gradient underflows; the same scale is used for both modes."""
+    NAME = 'Inception4'
+
+    def __init__(self, dnn, grad_scale=32.0):
+        InceptionTrainer.__init__(self, dnn, grad_scale)
+        self._blocks = None
+        self._scratch = {}
+
+    # ---- plan --------------------------------------------------------------------------------------------
+    def _plan(self):
+        """{unit key: _IncUnit} of every conv in forward order (the stem, then each block's units in `Block.UNITS` order), and the per-block
+        plan `self._blocks`: [(block index, module, [(unit key, path, source, output channel offset or None)], max-pool offset or None)].
+        `source` is 'x' (the block input), 'pool' (its count-exclusive average pool) or the path of the producing unit."""
+        if self._units is None:
+            net = self.dnn
+            f = net.features
+            names = {m: n for n, m in net.named_modules()}
+            units = {}
+            for i in range(3):
+                lay = net.layouts[f[i]]
+                units['features.%d' % i] = _IncUnit('features.%d' % i, f[i], 3 if lay is None else lay.width)
+            blocks = []
+            for m, segs, _ in net.blocks:
+                index = int(names[m].split('.')[1])
+                out_off = {seg_units[-1]: off for kind, seg_units, off in segs if kind != 'max'}
+                maxpool = [off for kind, _, off in segs if kind == 'max']
+                recs = []
+                for path, _, _, _, _, src in m.UNITS:
+                    mod = m.get_submodule(path)
+                    key = '%s.%s' % (names[m], path)
+                    units[key] = _IncUnit(key, mod, net.layouts[mod].width)
+                    recs.append((key, path, {None: 'x', 'avg': 'pool'}.get(src, src), out_off.get(mod)))
+                blocks.append((index, m, recs, maxpool[0] if maxpool else None))
+            for u in units.values():
+                u.bias_name = u.key + '.conv.bias' if u.bn is None else None
+            head = f[-1]
+            self._head = _ResUnit(names[head], head, None, 1.0, (names[head] + '.weight', None, None))
+            self._blocks = blocks
+            self._units = units
+        return self._units
+
+    def block_plan(self):
+        self._plan()
+        return self._blocks
+
+    def block_units(self, name):
+        """The units of the stem ('stem') or of block features.`name` (an index 3 .. 21) in forward order."""
+        units = self._plan()
+        if name == 'stem':
+            return [units['features.%d' % i] for i in range(3)]
+        recs = [r for i, _, r, _ in self._blocks if i == name][0]
+        return [units[key] for key, _, _, _ in recs]
+
+    def grad_order(self):
+        self._plan()
+        names = [self._head.key + '.bias', self._head.pnames[0]]
+        for name in [i for i, _, _, _ in reversed(self._blocks)] + ['stem']:
+            for u in reversed(self.block_units(name)):
+                names += [u.bias_name] if u.bn is None else [u.pnames[1], u.pnames[2]]
+                names.append(u.pnames[0])
+        return names
+
+    def _head_unit(self):
+        return self._head.key, self._head, self._head.key + '.bias'
+
+    def _repack(self, device):
+        """Forward and data-gradient fp16 operands of every conv after features.0 and of the head in ONE launch (KhwPackPlan); features.0
+        reads its fp32 weights in place."""
+        units = [u for key, u in self._plan().items() if key != 'features.0']
+        head = self._head
+        cpad = (head.cout + 31) // 32 * 32            # the head's filters are padded to the width of its dz buffer
+        entries = [(u.key, u.conv.weight.detach(), u.cout_pad, u.cin_pad) for u in units] + [(head.key, head.conv.weight.detach(), cpad, head.cin)]
+        plan = self._pack_plan
+        wdev = entries[0][1].device
+        if plan is None or plan.key != tuple(w.data_ptr() for _, w, _, _ in entries) or plan.table.device != wdev:
+            plan = self._pack_plan = KhwPackPlan(entries, wdev)
+        plan.run()
+        for u in units:
+            u.w16, u.wd = plan.fwd[u.key], plan.dgrad[u.key]
+        head.w16 = plan.fwd[head.key][:head.cout]
+        self.wd_cache[head.key] = plan.dgrad[head.key]
+
+    def _check(self, x):
+        """Refuse what the trainer cannot run: a channel-pruned or ratio != 1 model (its padded channel layout would need the gradient
+        gathered back out of the scattered channels), a bad shape, a BatchNorm without running statistics."""
+        from model.inception4 import MIN_SIZE, STEM_FILTERS
+        units = self._plan()
+        u0 = units['features.0']
+        if u0.cout != STEM_FILTERS:
+            raise ValueError('Inception4 training: features.0 has %d filters, the stem needs exactly %d; training needs the full-width model '
+                             '(no channel pruning, ratio 1)' % (u0.cout, STEM_FILTERS))
+        for u in units.values():          # every tensor is then a multiple of 32 channels wide, and every layout the identity
+            if u.cout % 32:
+                raise ValueError('Inception4 training: %s has %d filters, not a multiple of 32; training needs the full-width model '
+                                 '(no channel pruning, ratio 1)' % (u.key, u.cout))
+        b, c, h, w = x.shape
+        if c != 3:
+            raise ValueError('Inception4 expects [B,3,H,W]')
+        if h < MIN_SIZE or w < MIN_SIZE:
+            raise ValueError('Inception4: a %d x %d input leaves a stage empty (H and W must be >= %d)' % (h, w, MIN_SIZE))
+        for u in units.values():
+            if u.bn is not None and (u.bn.momentum is None or not u.bn.track_running_stats):
+                raise ValueError('Inception4 training: %s needs a BatchNorm with running statistics and a momentum' % u.key)
+
+    # ---- forward -----------------------------------------------------------------------------------------
+    def _unit_forward(self, u, src, out=None, a_off=0):
+        """One unit on src: BatchNorm on as InceptionTrainer's; off, conv + bias + ReLU into channels [a_off, a_off + cout) of `out` (or a
+        new buffer), that activation kept for the ReLU backward."""
+        if u.bn is not None:
+            return InceptionTrainer._unit_forward(self, u, src, out, a_off)
+        one, _ = self._ones(u.cout_pad, src.device)
+        a = ops.conv2d_bn_act(src, u.w16, one, u.conv.bias.detach(), 0.0, stride=u.stride, pad=u.pad, out=out, y_ch_off=a_off)
+        return a, self._saved_unit(u, src, None, None, None, a.shape[1], a.shape[2], act=a, a_off=a_off, in_h=src.shape[1], in_w=src.shape[2])
+
+    def stem_forward(self, x):
+        """features.0 .. features.2 on the fp32 image x [B,3,H,W]: (Mixed_3a's input [B,H3,W3,64], saved stem)."""
+        u0, u1, u2 = self.block_units('stem')
+        w0 = u0.conv.weight.detach().contiguous()
+        if u0.bn is not None:
+            a, s0 = self._bn_unit_forward(u0, ops.stem3x3_s2_raw(x, w0, pad=0), None)
+        else:
+            one, _ = self._ones(u0.cout, x.device)
+            a = ops.stem3x3_s2(x, w0, one, u0.conv.bias.detach(), pad=0)
+            s0 = self._saved_unit(u0, None, None, None, None, a.shape[1], a.shape[2], act=a, a_off=0)
+        a, s1 = self._unit_forward(u1, a)
+        a, s2 = self._unit_forward(u2, a)
+        st = _Saved()
+        st.x, st.units = x, [s0, s1, s2]
+        return a, st
+
+    def block_forward(self, index, x):
+        """Block features.`index` on x (fp16 NHWC): (its concatenated output, saved block)."""
+        from model.inception4 import Mixed_4a
+        _, m, recs, maxpool = [blk for blk in self._blocks if blk[0] == index][0]
+        b, h, w, c = x.shape
+        if m.POOLS:            # Mixed_3a / 5a, Reduction_A / B: every branch ends in a 3x3 valid stride-2 conv or pool
+            oh, ow = (h - 3) // 2 + 1, (w - 3) // 2 + 1
+        elif isinstance(m, Mixed_4a):      # two 3x3 valid convs in parallel branches
+            oh, ow = h - 2, w - 2
+        else:
+            oh, ow = h, w
+        width = self.dnn.blocks[index - 3][2].width
+        out = torch.empty(b, oh, ow, width, dtype=torch.float16, device=x.device)
+        vals = {'x': x}
+        if any(src == 'pool' for _, _, src, _ in recs):
+            vals['pool'] = ops.avgpool3x3_s1_excl(x)          # kept: the branch3 conv's weight gradient reads it
+        units = self._plan()
+        saved = []
+        for key, path, src, off in recs:
+            a, s = self._unit_forward(units[key], vals[src], out if off is not None else None, off or 0)
+            s.src, s.name, s.to_out = src, path, off is not None
+            vals[path] = a
+            saved.append(s)
+        if maxpool is not None:
+            ops.maxpool3x3_s2_valid(x, out, maxpool)
+        blk = _Saved()
+        blk.index, blk.x, blk.units, blk.maxpool = index, x, saved, maxpool
+        return out, blk
+
+    def forward(self, x):
+        x = self._start_forward(x)
+        self._check(x)
+        dev = x.device
+        self._repack(dev)
+        saved = _Saved()
+        saved.b = x.shape[0]
+        cur, saved.stem = self.stem_forward(x)
+        saved.blocks = []
+        for index, _, _, _ in self._blocks:
+            cur, blk = self.block_forward(index, cur)
+            saved.blocks.append(blk)
+        head = self._head
+        one, _ = self._ones(head.cout, dev)
+        feature = ops.conv2d_bn_act(cur, head.w16, one, head.conv.bias.detach(), 1.0, out_mode=ops.OUT_F32_NCHW)
+        saved.a_last, saved.hh, saved.ww = cur, cur.shape[1], cur.shape[2]
+        self._bump_tracked()
+        return feature, saved
+
+    # ---- backward ----------------------------------------------------------------------------------------
+    def _bn_unit_backward(self, s, da, da_off, grads):
+        """BatchNorm + ReLU backward as InceptionTrainer's; with BatchNorm off the ReLU backward on the kept activation (yb_bn_act_bwd,
+        has_bn = 0, in the BatchNorm's channel chunks) into dz, and the bias gradient from the reduce pass's per-channel sums."""
+        u = s.u
+        if u.bn is not None:
+            return InceptionTrainer._bn_unit_backward(self, s, da, da_off, grads)
+        a = s.act
+        b, dev = a.shape[0], a.device
+        dz = (torch.zeros if u.cout_pad != u.cout else torch.empty)(b, s.h, s.w, u.cout_pad, dtype=torch.float16, device=dev)
+        dbias = self.arena.views[u.bias_name]
+        dscratch = self._scratch.get((u.cout, dev))
+        if dscratch is None:
+            dscratch = self._scratch[(u.cout, dev)] = torch.empty(u.cout, dtype=torch.float32, device=dev)
+        for off, n in _bn_chunks(u.cout):
+            sums = self._sums(('b', u.key, off), n, dev)
+            args = (a[..., s.a_off + off:], a.shape[-1], None, None, None, None, 0.0, da, da.shape[-1], da_off + off, None, 0, 0, b, s.h, s.w, n, 0,
+                    sums)
+            ops.call('yb_bn_act_bwd', 0, *args, None, 0, 0)
+            ops.call('yb_bn_act_bwd', 1, *args, dz[..., off:], dz.shape[-1], 0)
+            ops.call('yb_bn_param_grad', sums, n, dscratch[off:], dbias[off:], 1, self._unscale)
+        grads[u.bias_name] = dbias
+        self._emit(u.bias_name, grads)
+        return dz
+
+    def block_backward(self, blk, g, grads):
+        """Backward of a saved block from g, the gradient of its output: the parameter gradients of its units and the gradient at its input,
+        every branch's contribution at a shared tensor joined once."""
+        terms = {}
+        for s in reversed(blk.units):
+            if s.to_out:
+                gi = self._unit_backward(s, g, s.a_off, grads)
+            else:
+                gi = self._unit_backward(s, self._sum(terms.pop(s.name)), 0, grads)
+            terms.setdefault(s.src, []).append(gi)
+        if 'pool' in terms:
+            terms['x'].append(ops.avgpool3x3_s1_excl_bwd(self._sum(terms.pop('pool'))))
+        if blk.maxpool is not None:
+            terms['x'].append(ops.maxpool3x3_s2_valid_bwd(blk.x, g, blk.maxpool))
+        return self._sum(terms['x'])
+
+    def stem_backward(self, st, g, grads):
+        """Stem backward from g, the gradient at Mixed_3a's input: features.2, features.1, then features.0's BatchNorm / ReLU backward and its
+        weight gradient from the fp32 image (no data gradient)."""
+        s0, s1, s2 = st.units
+        g = self._unit_backward(s2, g, 0, grads)
+        g = self._unit_backward(s1, g, 0, grads)
+        dz = self._bn_unit_backward(s0, g, 0, grads)
+        x = st.x
+        wname = s0.u.pnames[0]
+        dw = self.arena.views[wname]
+        ops.call('yb_stem3x3_s2_wgrad', x, dz, dw, x.shape[0], x.shape[2], x.shape[3], 0)
+        grads[wname] = dw.mul_(self._unscale)
+        self._emit(wname, grads)
+        return g

@@ -141,6 +141,7 @@ int stem3x3_s2(const float*, const float*, const float*, const float*, void*, in
 int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1_excl(const void*, void*, int, int, int, int, cudaStream_t);
+int avgpool3x3_s1_excl_bwd(const void*, void*, int, int, int, int, cudaStream_t);
 int conv2d_wgrad_forward(const void*, const void*, float*, int, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
 int unpack_wgrad_khw(const float*, float*, int, int, int, int, int, float, cudaStream_t);
 int pack_weight_dgrad_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
@@ -537,6 +538,10 @@ int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int widt
 
 int yb_avgpool3x3_s1_excl_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
   return yb::avgpool3x3_s1_excl(x, y, batch, height, width, channels, S(stream));
+}
+
+int yb_avgpool3x3_s1_excl_bwd_f16(const void* dy, void* dx, int batch, int height, int width, int channels, yb_stream_t stream) {
+  return yb::avgpool3x3_s1_excl_bwd(dy, dx, batch, height, width, channels, S(stream));
 }
 
 int yb_conv2d_wgrad(const void* x, const void* dz, float* dw_krsc, int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride,

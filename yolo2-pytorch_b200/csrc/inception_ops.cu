@@ -16,6 +16,8 @@
 //   pack_weight_dgrad_khw      the data-gradient operand: rotated by 180 degrees, transposed, zero-padded.
 //   maxpool3x3_s2_valid_bwd    the backward of maxpool3x3_s2_valid, dy read from a channel slice of a block's output gradient.
 //   join_f16                   the gradient at a tensor read by several units: the sum of up to four contributions.
+// Training (Inception-v4):
+//   avgpool3x3_s1_excl_bwd     the backward of avgpool3x3_s1_excl: each output's gradient divided by that output's own divisor.
 #include "yb_common.h"
 #include "yb_pool.cuh"
 #include <cuda_fp16.h>
@@ -331,6 +333,60 @@ int avgpool3x3_s1(const void* x, void* y, int batch, int height, int width, int 
 
 int avgpool3x3_s1_excl(const void* x, void* y, int batch, int height, int width, int channels, cudaStream_t stream) {
   return avgpool3x3_s1_launch<true>(x, y, batch, height, width, channels, stream, "avgpool3x3_s1_excl");
+}
+
+// Backward of avgpool3x3_s1_excl: dx[b, iy, ix, c] = fp16(sum over the in-range outputs (oy, ox) of rows iy-1..iy+1, columns ix-1..ix+1 in
+// row-major order of dy[b, oy, ox, c] / n(oy, ox)), each term one round-to-nearest fp32 division by that output's own in-range count, summed
+// in fp32 and rounded once.  The pool is not its own transpose: the divisor belongs to the output, not to the input pixel.  One thread per
+// pixel and 8 channels gathers; no atomics, deterministic.
+__global__ void avgpool3x3_s1_excl_bwd_kernel(const __half* __restrict__ dy, __half* __restrict__ dx, int batch, int height, int width,
+                                              int channels) {
+  const int c8 = channels >> 3;
+  const long long total = static_cast<long long>(batch) * height * width * c8;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int cg = static_cast<int>(idx % c8);
+  const long long pix = idx / c8;
+  const int px = static_cast<int>(pix % width);
+  const long long t = pix / width;
+  const int py = static_cast<int>(t % height);
+  const long long img = t / height;
+  float acc[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) acc[e] = 0.f;
+#pragma unroll
+  for (int r = -1; r <= 1; ++r) {
+    const int oy = py + r;
+    if (oy < 0 || oy >= height) continue;
+    const int rows = 3 - (oy == 0) - (oy == height - 1);
+#pragma unroll
+    for (int s = -1; s <= 1; ++s) {
+      const int ox = px + s;
+      if (ox < 0 || ox >= width) continue;
+      const float n = static_cast<float>(rows * (3 - (ox == 0) - (ox == width - 1)));
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(dy + ((img * height + oy) * width + ox) * channels + cg * 8));
+      const __half* hv = reinterpret_cast<const __half*>(&v);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[e] += __fdiv_rn(__half2float(hv[e]), n);
+    }
+  }
+  uint4 out;
+  __half2* ho = reinterpret_cast<__half2*>(&out);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) ho[e] = __floats2half2_rn(acc[2 * e], acc[2 * e + 1]);
+  reinterpret_cast<uint4*>(dx)[idx] = out;
+}
+
+int avgpool3x3_s1_excl_bwd(const void* dy, void* dx, int batch, int height, int width, int channels, cudaStream_t stream) {
+  YB_REQUIRE(dy && dx && batch > 0 && height > 0 && width > 0 && channels > 0 && channels % 8 == 0,
+             "avgpool3x3_s1_excl_bwd: bad argument (C a multiple of 8)");
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(dy) & 15) == 0 && (reinterpret_cast<uintptr_t>(dx) & 15) == 0,
+             "avgpool3x3_s1_excl_bwd: dy / dx must be 16B aligned");
+  const long long total = static_cast<long long>(batch) * height * width * (channels / 8);
+  avgpool3x3_s1_excl_bwd_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(reinterpret_cast<const __half*>(dy),
+                                                                                               reinterpret_cast<__half*>(dx), batch, height,
+                                                                                               width, channels);
+  return check_launch("avgpool3x3_s1_excl_bwd_kernel");
 }
 
 }  // namespace yb

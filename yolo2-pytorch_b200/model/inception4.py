@@ -1,4 +1,4 @@
-"""model.inception4 -- Inception-v4 backbone plugin on the CUDA kernels (inference).
+"""model.inception4 -- Inception-v4 backbone plugin on the CUDA kernels (inference and training).
 
 Drop-in for the reference's `model/inception4.py`: `Inception4(config_channels, anchors, num_cls, ratio=1)`, selectable with
 `[model] dnn = model.inception4.Inception4`, with the reference's module tree and state_dict keys: `features.0 .. features.2` the stem convs,
@@ -20,7 +20,12 @@ are zero with scale 1, shift 0: exact zeros after the ReLU), a block buffer is i
 order, and a max-pool branch carries its input's layout through.  Each tensor has a `Layout` (reference channel j -> buffer channel pos[j]);
 a consumer's weight is scattered onto its input's layout, zero elsewhere, before the pack.  With ratio 1 and an unpruned model every width is a
 multiple of 32 and every layout is the identity.  The scattered weights, folded BatchNorms and packs are cached per parameter version;
-switching train() / eval() drops the cache.  There is no CPU path and no training path.
+switching train() / eval() drops the cache.
+In train() mode on a CUDA tensor the forward is one autograd node (model.yolo2._DarknetTrainFunction) over
+b200.train_engine.Inception4Trainer: batch-statistics BatchNorm (eps 1e-3, momentum 0.1) with the running-statistics update, or conv + bias
++ ReLU with BatchNorm disabled, and an explicit backward chain that gives every parameter its fp32 gradient.  Training needs the full-width
+model: a channel-pruned or ratio != 1 model raises ValueError on a train-mode forward (its eval mode is unchanged).  There is no CPU path:
+a train-mode forward on a CPU tensor raises NotImplementedError, an eval-mode one RuntimeError.
 """
 import configparser
 
@@ -29,6 +34,7 @@ import torch.nn as nn
 
 import model
 from b200 import ops as _ops
+from b200 import train_engine as _train
 
 MIN_SIZE = 75      # the smallest input side whose every stage is non-empty (Reduction_B's output is 1 x 1)
 STEM_FILTERS = 32  # yb_stem3x3_s2_bn_relu_fwd computes exactly 32 filters
@@ -222,6 +228,7 @@ class Inception4(nn.Module):
         self._init(config)
         self._plan()
         self._cache = {}
+        self._trainer = None
         _pretrained(self, config)
 
     def _init(self, config):
@@ -262,6 +269,12 @@ class Inception4(nn.Module):
             lay = Layout.concat(parts)
             self.blocks.append((m, tuple(segs), lay))
         self.layouts[f[-1]] = lay
+
+    @property
+    def trainer(self):
+        if self._trainer is None:
+            self._trainer = _train.Inception4Trainer(self)
+        return self._trainer
 
     def train(self, mode=True):
         """nn.Module.train + drop cached kernel operands."""
@@ -391,7 +404,11 @@ class Inception4(nn.Module):
 
     def forward(self, x):
         if self.training:
-            raise NotImplementedError('Inception4: training is not implemented on the kernels; call .eval() for inference')
+            if not x.is_cuda:
+                raise NotImplementedError('Inception4: training runs on the CUDA kernels only; the input is a CPU tensor')
+            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.Inception4Trainer)
+            from model.yolo2 import _DarknetTrainFunction
+            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
         return self.run(x)
 
 
