@@ -363,6 +363,47 @@ int yb_bn_relu_avgpool2x2_f16(const void* x, int x_ld, const float* scale, const
 /* yb_maxpool3x3_s2_f16 writing channels [y_ch_off, y_ch_off + C) of y [B,(H+1)/2,(W+1)/2,y_ld] (the stem pool into the first block's buffer). */
 int yb_maxpool3x3_s2_ld_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
 
+/* ---- DenseNet plugin, training (b200.train_engine.DenseNetTrainer) ------------------------------------------------------------------
+ * Every train-mode norm that reads a block channel (each later dense layer's norm1, the transition's norm, norm5) uses that channel's
+ * batch statistics, computed once when the channel is written; each norm keeps its own gamma, beta and running statistics.
+ * yb_conv1x1_preact_stats_fwd: yb_conv1x1_preact_fwd (fp16 NHWC output, no workspace) that also adds the per-channel sum and sum of squares of
+ *   the stored fp16 outputs into sums[0..Cout) / sums[Cout..2Cout) (double, the contract of yb_conv_bn_act_stats_fwd).  With scale = 1,
+ *   shift = 0, slope = 1 its y is conv1's raw output z1, bit-identical to yb_conv1x1_preact_fwd with the same arguments. */
+int yb_conv1x1_preact_stats_fwd(const void* x, const void* w, const float* pre_scale, const float* pre_shift, int pre_relu, const float* scale,
+                                const float* shift, float slope, void* y, int batch, int height, int width, int cin, int cout, int x_ld, long long y_ld,
+                                int y_ch_off, double* sums, yb_stream_t stream);
+/* Weight gradient of the pre-activation 1x1 conv: dw_krsc fp32 [Cout][1][1][Cin] (yb_conv_wgrad's layout, overwritten) =
+ *   sum_p dz[p][co] * a[p][ci],  a = fp16_rn(act(fmaf(pre_scale[ci], x[p][ci], pre_shift[ci]))),  act = ReLU (pre_relu = 1) or identity (0),
+ * x fp16 NHWC [B,H,W,x_ld] (channels [0, cin) read), dz fp16 [B,H,W,dz_ld].  The transform runs on the shared-memory tile; a is never
+ * written.  Bit-identical to yb_conv_wgrad / yb_conv2d_wgrad on the materialised a with the same pixel split (YB_WGRAD_SPLITS as there).
+ * cin % 32 == 0, cin <= 1920; pre_scale / pre_shift 16-byte aligned. */
+int yb_conv1x1_preact_wgrad(const void* x, const float* pre_scale, const float* pre_shift, int pre_relu, const void* dz, float* dw_krsc, int batch,
+                            int height, int width, int cin, int cout, int x_ld, int dz_ld, yb_stream_t stream);
+/* (scale, shift) of a train-mode pre-activation norm: scale = gamma * invstd, shift = fmaf(-mean, scale, beta) (the values
+ * yb_bn_preact_bwd recomputes, so its ReLU mask is the forward's). */
+int yb_bn_batch_fold(const float* mean, const float* invstd, const float* gamma, const float* beta, float* scale, float* shift, int channels,
+                     yb_stream_t stream);
+/* Backward of a pre-activation norm a = act(fmaf(scale, x, shift)) (scale / shift as yb_bn_batch_fold) over channels [0, C) of the block
+ * buffer x [B,H,W,x_ld], from d(a) = da [B,H,W,da_ld] (pool = 0), or from da [B,H/2,W/2,da_ld] through a 2x2 average pool (pool = 1:
+ * d(a) = da / 4 at each window pixel).  mode 0: sums[0..C) += sum dy, sums[C..2C) += sum dy * xhat (yb_bn_act_bwd mode 0's accumulators,
+ * so yb_bn_param_grad gives dgamma / dbeta).  mode 1 (after mode 0): dx [B,H,W,dx_ld] fp32 += the gradient of x, channels [0, C) only; if
+ * dx16 != NULL, channels [dx16_ch0, C) are also stored as fp16 (after the addition) into dx16 [B,H,W,dx16_ld] from its channel 0.
+ * Any C % 8 == 0; pitches multiples of 8 (dx_ld of 4). */
+int yb_bn_preact_bwd(int mode, const void* x, long long x_ld, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                     int relu, const void* da, long long da_ld, int pool, int batch, int height, int width, int channels, double* sums, float* dx,
+                     long long dx_ld, void* dx16, long long dx16_ld, int dx16_ch0, yb_stream_t stream);
+/* Running statistics of every norm of a block from the shared batch statistics in ONE launch.  `norms_dev` is a DEVICE array of `count`
+ * entries; entry k: running = (1 - momentum) * running + momentum * batch over channels [0, channels) (in double, as yb_bn_finalize), with
+ * batch_mean / batch_var (unbiased) fp32 per block channel.  max_channels >= every entry's channels. */
+typedef struct yb_bn_running {
+  float* running_mean;
+  float* running_var;
+  int channels;
+  float momentum;
+} yb_bn_running;
+int yb_bn_running_update_batch(const float* batch_mean, const float* batch_var, const yb_bn_running* norms_dev, int count, int max_channels,
+                               yb_stream_t stream);
+
 /* ---- Inception-v3 plugin (model/inception3.py:29-118 over torchvision's BasicConv2d / InceptionA-E), inference ------------------------
  * yb_conv2d_bn_act_fwd: the implicit-GEMM conv of yb_conv_bn_act_fwd_ws with a general geometry -- kh x kw filters (1..7 each), stride 1 or 2,
  * zero padding pad_h < kh, pad_w < kw -- on x fp16 NHWC [B,in_h,in_w,Cin] (pixel pitch x_ld, Cin % 32 == 0) and w fp16 [Cout][kh][kw][Cin]

@@ -91,6 +91,12 @@ SIGNATURES = {
     'yb_dwconv3x3_bn_relu_fwd': [P, P, P, P, P, c_int, c_int, c_int, c_int, c_int, P],
     'yb_conv1x1_preact_fwd': [P, P, P, P, c_int, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int, P,
                               c_longlong, P],
+    'yb_conv1x1_preact_stats_fwd': [P, P, P, P, c_int, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, P, P],
+    'yb_conv1x1_preact_wgrad': [P, P, P, c_int, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P],
+    'yb_bn_batch_fold': [P, P, P, P, P, P, c_int, P],
+    'yb_bn_preact_bwd': [c_int, P, c_longlong, P, P, P, P, c_int, P, c_longlong, c_int, c_int, c_int, c_int, c_int, P, P, c_longlong, P, c_longlong,
+                         c_int, P],
+    'yb_bn_running_update_batch': [P, P, P, c_int, c_int, P],
     'yb_bn_relu_avgpool2x2_f16': [P, c_int, P, P, P, c_int, c_int, c_int, c_int, P],
     'yb_maxpool3x3_s2_ld_f16': [P, P, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_conv2d_bn_act_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int,

@@ -397,6 +397,52 @@ def conv1x1_preact(x, w, pre_scale, pre_shift, pre_relu, scale, shift, slope, ou
     return out
 
 
+def conv1x1_preact_stats(x, w, pre_scale, pre_shift, pre_relu, sums, cin=None):
+    """Training form of conv1x1_preact (yb_conv1x1_preact_stats_fwd): the raw output z = a . W^T (fp16 NHWC [B,H,W,Cout]) and, added into
+    `sums` (float64 [2*Cout]), the per-channel sum and sum of squares of the stored values."""
+    _req(x, torch.float16, 'x'); _req(w, torch.float16, 'w'); _req(pre_scale, torch.float32, 'pre_scale'); _req(pre_shift, torch.float32, 'pre_shift')
+    _req(sums, torch.float64, 'sums')
+    b, h, wd, x_ld = x.shape
+    cout, k, _, wcin = w.shape
+    cin = wcin if cin is None else cin
+    if cin != wcin or k != 1 or sums.numel() != 2 * cout or pre_scale.numel() < cin or pre_shift.numel() < cin:
+        raise ValueError('conv1x1_preact_stats: weight [%d,%d,%d,%d], %d input channels, %d sums' % (cout, k, k, wcin, cin, sums.numel()))
+    one = torch.ones(cout, dtype=torch.float32, device=x.device)
+    out = torch.empty(b, h, wd, cout, dtype=torch.float16, device=x.device)
+    _ck(_l.load().yb_conv1x1_preact_stats_fwd(_p(x), _p(w), _p(pre_scale), _p(pre_shift), int(bool(pre_relu)), _p(one), _p(one.new_zeros(cout)), 1.0,
+                                              _p(out), b, h, wd, cin, cout, x_ld, cout, 0, _p(sums), _s()), 'yb_conv1x1_preact_stats_fwd')
+    return out
+
+
+def conv1x1_preact_wgrad(x, pre_scale, pre_shift, pre_relu, dz, cin, cout):
+    """Weight gradient of the pre-activation 1x1 conv (yb_conv1x1_preact_wgrad): fp32 [Cout,1,1,Cin] (yb_conv_wgrad's layout) from x fp16
+    [B,H,W,x_ld] (channels [0, cin)) and dz fp16 [B,H,W,dz_ld]."""
+    _req(x, torch.float16, 'x'); _req(dz, torch.float16, 'dz'); _req(pre_scale, torch.float32, 'pre_scale'); _req(pre_shift, torch.float32, 'pre_shift')
+    b, h, wd, x_ld = x.shape
+    dw = torch.empty(cout, 1, 1, cin, dtype=torch.float32, device=x.device)
+    _ck(_l.load().yb_conv1x1_preact_wgrad(_p(x), _p(pre_scale), _p(pre_shift), int(bool(pre_relu)), _p(dz), _p(dw), b, h, wd, cin, cout, x_ld,
+                                          dz.shape[-1], _s()), 'yb_conv1x1_preact_wgrad')
+    return dw
+
+
+def bn_batch_fold(mean, invstd, gamma, beta):
+    """(scale, shift) of a train-mode pre-activation norm from the shared batch statistics (yb_bn_batch_fold)."""
+    c = gamma.numel()
+    scale = torch.empty(c, dtype=torch.float32, device=gamma.device)
+    shift = torch.empty_like(scale)
+    call('yb_bn_batch_fold', mean, invstd, gamma, beta, scale, shift, c)
+    return scale, shift
+
+
+def bn_preact_bwd(mode, x, mean, invstd, gamma, beta, relu, da, pool, sums, dx=None, dx16=None, dx16_ch0=0, channels=None):
+    """One pass of a pre-activation norm's backward (yb_bn_preact_bwd) over channels [0, C) of x fp16 [B,H,W,x_ld]: mode 0 adds into `sums`
+    (float64 [2C]); mode 1 adds dx into `dx` (fp32 [B,H,W,dx_ld]) and stores channels [dx16_ch0, C) of the result into `dx16` (fp16)."""
+    b, h, wd, x_ld = x.shape
+    c = gamma.numel() if channels is None else channels
+    call('yb_bn_preact_bwd', int(mode), x, x_ld, mean, invstd, gamma, beta, int(relu), da, da.shape[-1], int(pool), b, h, wd, c, sums,
+         dx, 0 if dx is None else dx.shape[-1], dx16, 0 if dx16 is None else dx16.shape[-1], int(dx16_ch0))
+
+
 def conv_bn_act_split(x, w, scale, shift, slope, out, a_channels, y_ch_off=0, lo_ch_off=-1, out_mode=OUT_F16_NHWC, flags=0, workspace=None):
     """Split-precision conv unit (yb_conv_bn_act_split_fwd).  x: fp16 [B,H,W,x_ld] holding `a_channels` usable channels
     (C, or 2C = [hi | lo]); w: fp16 [Cout,k,k,K'] from pack_weight_split_f16; out fp16 [B,H,W,y_ld]: hi at y_ch_off, and the fp16

@@ -1,4 +1,4 @@
-"""Training-mode forward and backward of the backbones (Darknet-19, Tiny, MobileNet, ResNet) on the CUDA kernels.
+"""Training-mode forward and backward of the backbones (Darknet-19, Tiny, MobileNet, ResNet, VGG, Inception, DenseNet) on the CUDA kernels.
 
 What the reference gets from torch autograd over nn.Conv2d / BatchNorm2d(train) / LeakyReLU / MaxPool2d /
 reorg / cat (model/yolo2.py:49-65,125-130; train.py:344-351) is issued here as an explicit kernel chain:
@@ -345,6 +345,43 @@ class TrainerBase(object):
             return dz
         self._wgrad(u, s.ain, dz, b, s.h, s.w, grads, key)
         return self._dgrad(key, u, dz)
+
+    # ---- the 7x7 stem of ResNet and DenseNet (`self._stem`: its conv + BatchNorm unit) -------------------------------------
+    def _stem_forward(self, x, out=None):
+        """Stem on the fp32 image x [B,3,H,W]: raw 7x7 stride-2 conv -> BN (batch statistics) -> ReLU -> 3x3 stride-2 max-pool, into a new
+        tensor or, with `out`, into channels [0, 64) of `out` (DenseNet's first block buffer).  Returns (saved unit, activation before the
+        pool, pooled output)."""
+        b, _, h, w = x.shape
+        dev = x.device
+        st = self._stem
+        hh, ww = h // 2, w // 2
+        z = torch.empty(b, hh, ww, 64, dtype=torch.float16, device=dev)
+        ops.call('yb_stem7x7_raw_fwd', x, st.conv.weight.detach(), z, b, h, w)
+        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww, False)
+        a = self._apply(st, z, mean, invstd, b, hh, ww, False)
+        if out is None:
+            pooled = torch.empty(b, hh // 2, ww // 2, 64, dtype=torch.float16, device=dev)
+            ops.call('yb_maxpool3x3_s2_f16', a, pooled, b, hh, ww, 64)
+        else:
+            pooled = out
+            ops.call('yb_maxpool3x3_s2_ld_f16', a, out, out.shape[-1], 0, b, hh, ww, 64)
+        return self._saved_unit(st, None, z, mean, invstd, hh, ww), a, pooled
+
+    def _stem_backward(self, x, st, stem_a, g, grads):
+        """Stem backward from the gradient g at the max-pool output: max-pool backward -> BN + ReLU backward -> weight gradient from the fp32
+        image.  Returns the gradient at the stem's activation (the max-pool's input)."""
+        b, _, h, w = x.shape
+        dev = g.device
+        da = torch.empty_like(stem_a)
+        ops.call('yb_maxpool3x3_s2_bwd_f16', stem_a, g, da, b, st.h, st.w, 64)
+        dz = torch.empty(b, st.h, st.w, 64, dtype=torch.float16, device=dev)
+        self._bn_backward(st.u.key, st, b, grads, dz, da=da)
+        wname = st.u.pnames[0]
+        dw = self.arena.views[wname]
+        ops.call('yb_stem7x7_wgrad', x, dz, dw, b, h, w)
+        grads[wname] = dw.mul_(self._unscale)
+        self._emit(wname, grads)
+        return da
 
     def _head_grad(self, bias, chead, a_last, hh, ww, dfeature, grads):
         """Head (1x1 conv with bias) from dfeature, the fp32 NCHW gradient of the loss w.r.t. its output: the bias gradient from the unscaled
@@ -989,21 +1026,6 @@ class ResNetTrainer(TrainerBase):
         self._bump_tracked()
         return feature, saved
 
-    def _stem_forward(self, x):
-        """Stem on the fp32 image x [B,3,H,W]: raw 7x7 stride-2 conv -> BN (batch statistics) -> ReLU -> 3x3 stride-2 max-pool.
-        Returns (saved unit, activation before the pool, pooled output)."""
-        b, _, h, w = x.shape
-        dev = x.device
-        st = self._stem
-        hh, ww = h // 2, w // 2
-        z = torch.empty(b, hh, ww, 64, dtype=torch.float16, device=dev)
-        ops.call('yb_stem7x7_raw_fwd', x, st.conv.weight.detach(), z, b, h, w)
-        mean, invstd = self._bn_forward(st.key, st, z, b * hh * ww, False)
-        a = self._apply(st, z, mean, invstd, b, hh, ww, False)
-        pooled = torch.empty(b, hh // 2, ww // 2, 64, dtype=torch.float16, device=dev)
-        ops.call('yb_maxpool3x3_s2_f16', a, pooled, b, hh, ww, 64)
-        return self._saved_unit(st, None, z, mean, invstd, hh, ww), a, pooled
-
     @staticmethod
     def _join_forward(cur, res):
         """Block join: cur = relu(cur + res), in place (the units keep z, not their output)."""
@@ -1018,21 +1040,6 @@ class ResNetTrainer(TrainerBase):
         g = torch.empty_like(gm)
         ops.call('yb_residual_bwd_f16', mask, gm, gb, stride_b, g, b, h, w, gm.shape[-1])
         return g
-
-    def _stem_backward(self, x, st, stem_a, g, grads):
-        """Stem backward from the gradient g at the max-pool output: max-pool backward -> BN + ReLU backward -> weight gradient from the fp32
-        image.  Returns the gradient at the stem's activation (the max-pool's input)."""
-        b, _, h, w = x.shape
-        dev = g.device
-        da = torch.empty_like(stem_a)
-        ops.call('yb_maxpool3x3_s2_bwd_f16', stem_a, g, da, b, st.h, st.w, 64)
-        dz = torch.empty(b, st.h, st.w, 64, dtype=torch.float16, device=dev)
-        self._bn_backward(st.u.key, st, b, grads, dz, da=da)
-        dw = self.arena.views['conv1.weight']
-        ops.call('yb_stem7x7_wgrad', x, dz, dw, b, h, w)
-        grads['conv1.weight'] = dw.mul_(self._unscale)
-        self._emit('conv1.weight', grads)
-        return da
 
     def _res_unit_backward(self, s, b, grads, da):
         """Backward of one block unit from the gradient of its output; returns the gradient of its input (s.ain's resolution)."""
@@ -1865,3 +1872,320 @@ class Inception4Trainer(InceptionTrainer):
         grads[wname] = dw.mul_(self._unscale)
         self._emit(wname, grads)
         return g
+
+
+class _DenseStats(object):
+    """Per-block batch statistics shared by every norm that reads a block channel: double accumulators (the writer of channels [s, s + n)
+    owns sums[2s, 2s + 2n) in the [sum | sum of squares] layout of yb_bn_stats), the batch mean / unbiased variance that feed the running
+    statistics (zero-initialised: yb_bn_finalize with momentum 1 stores them), and mean / invstd."""
+
+    def __init__(self, width, device):
+        self.sums = torch.zeros(2 * width, dtype=torch.float64, device=device)
+        self.bmean = torch.zeros(width, dtype=torch.float32, device=device)
+        self.bvar = torch.zeros(width, dtype=torch.float32, device=device)
+        self.mean = torch.zeros(width, dtype=torch.float32, device=device)
+        self.invstd = torch.zeros(width, dtype=torch.float32, device=device)
+        self.running = None       # (key, device table of yb_bn_running) of the block's norms
+
+    def seg(self, s, n):
+        return self.sums[2 * s:2 * s + 2 * n]
+
+
+class DenseNetTrainer(TrainerBase):
+    """Training-mode forward / backward of `model.densenet.DenseNet` (densenet121 / 169 / 201; reference model/densenet.py over torchvision's
+    _DenseLayer / _Transition).  Each dense block lives in one fp16 buffer as wide as its output, as in inference.
+
+    Forward: the stem is ResNet's (`TrainerBase._stem_forward`), pooling into channels [0, 64) of block 1's buffer.  A channel's batch
+    statistics are computed once, when it is written (yb_bn_stats on the stem's pool output, the conv2 and transition-conv epilogues), and
+    shared by every norm that reads it; each norm folds them with its own gamma / beta (yb_bn_batch_fold), and all norms of a block update
+    their running statistics in one launch (yb_bn_running_update_batch).  A dense layer is norm1 + relu1 + conv1 on the block's first Ci
+    channels (yb_conv1x1_preact_stats_fwd: raw z1 with norm2's statistics in its epilogue), norm2 + relu2 (the shared unit helpers), then the
+    3x3 conv2 writing its 32 channels at channel Ci with their statistics.  A transition pools before its 1x1 conv, as in inference, and keeps
+    the pooled activation for its weight gradient; norm5 feeds the head through the identity pre-activation.
+
+    Backward: the gradient of a block buffer is accumulated in fp32 ([B,H,W,C] per block): every pre-activation norm's backward
+    (yb_bn_preact_bwd; its reduce pass is yb_bn_act_bwd mode 0 when C / 8 divides 256 and the gradient is unpooled) adds its dx, and rounds to
+    fp16 the slice that its contribution completes -- layer j's 32 channels once layer j + 1 has added its part, the block input once layer
+    1 has -- which is the next dz: conv2's, the transition conv's (on the pooled grid) or the stem pool's.  The pre-activation convs' weight
+    gradients form a = act(norm(x)) on the shared-memory tile (yb_conv1x1_preact_wgrad)."""
+    NAME = 'DenseNet'
+    GROWTH = 32
+    GRAD_SCALE = 1024.0      # static loss scale, chosen on synthetic steps (DESIGN §6)
+
+    def __init__(self, dnn, grad_scale=GRAD_SCALE):
+        TrainerBase.__init__(self, dnn, grad_scale, slope=0.0)
+        self._blocks = None
+        self._stats = {}
+
+    # ---- plan ----------------------------------------------------------------------------------------
+    @staticmethod
+    def _norm_unit(key, bn, channels):
+        u = _BNUnit(bn, channels)
+        u.key, u.pnames = key, (None, key + '.weight', key + '.bias')
+        return u
+
+    def _plan(self):
+        if self._blocks is None:
+            net = self.dnn
+            f = net.features
+            self._stem = _ResUnit('features.conv0', f.conv0, f.norm0, 0.0, ('features.conv0.weight', 'features.norm0.weight', 'features.norm0.bias'))
+            self._head = _ResUnit('features.conv', f.conv, None, 1.0, ('features.conv.weight', None, None))
+            blocks = []
+            for i, n in enumerate(net.block_config):
+                name = 'features.denseblock%d' % (i + 1)
+                mod = getattr(f, 'denseblock%d' % (i + 1))
+                cin0, width = net.block_channels[i]
+                layers = []
+                for j in range(n):
+                    key = '%s.denselayer%d' % (name, j + 1)
+                    layer = getattr(mod, 'denselayer%d' % (j + 1))
+                    ci = cin0 + j * net.growth_rate
+                    layers.append(dict(cin=ci, norm1=self._norm_unit(key + '.norm1', layer.norm1, ci),
+                                       conv1=_ResUnit(key + '.conv1', layer.conv1, layer.norm2, 0.0,
+                                                      (key + '.conv1.weight', key + '.norm2.weight', key + '.norm2.bias')),
+                                       conv2=_ResUnit(key + '.conv2', layer.conv2, None, 1.0, (key + '.conv2.weight', None, None))))
+                if i + 1 < len(net.block_config):
+                    tname = 'features.transition%d' % (i + 1)
+                    t = getattr(f, 'transition%d' % (i + 1))
+                    tail = self._norm_unit(tname + '.norm', t.norm, width)
+                    tconv = _ResUnit(tname + '.conv', t.conv, None, 1.0, (tname + '.conv.weight', None, None))
+                else:
+                    tail, tconv = self._norm_unit('features.norm5', f.norm5, width), None
+                blocks.append(dict(index=i, cin=cin0, width=width, layers=layers, tail=tail, tconv=tconv))
+            self._blocks = blocks
+        return self._blocks
+
+    def grad_order(self):
+        names = ['features.conv.bias', 'features.conv.weight']
+        for blk in reversed(self._plan()):
+            if blk['tconv'] is not None:
+                names += [blk['tconv'].pnames[0]]
+            names += list(blk['tail'].pnames[1:])
+            for layer in reversed(blk['layers']):
+                c1, c2 = layer['conv1'], layer['conv2']
+                names += [c2.pnames[0], c1.pnames[1], c1.pnames[2], c1.pnames[0]] + list(layer['norm1'].pnames[1:])
+        return names + ['features.norm0.weight', 'features.norm0.bias', 'features.conv0.weight']
+
+    def _block_norm_settings(self, blk):
+        """(eps, momentum) shared by every norm reading the block's channels (each later norm1 and the tail all read channel 0)."""
+        norms = [layer['norm1'].bn for layer in blk['layers']] + [blk['tail'].bn]
+        eps = set(float(bn.eps) for bn in norms)
+        mom = set(bn.momentum for bn in norms)
+        if len(eps) != 1 or len(mom) != 1:
+            raise ValueError('DenseNet training: the norms reading %s disagree on eps %s or momentum %s; they share one set of batch '
+                             'statistics' % ('features.denseblock%d' % (blk['index'] + 1), sorted(eps), sorted(mom, key=str)))
+        m = mom.pop()
+        if m is None:
+            raise ValueError('DenseNet training: momentum=None (cumulative running average) is not supported')
+        return eps.pop(), float(m)
+
+    def _repack(self, device):
+        """Forward and data-gradient fp16 operands of every conv1, conv2, transition conv and the head in ONE batched launch (the stem reads
+        its fp32 weights in place)."""
+        entries = []
+        for blk in self._plan():
+            for layer in blk['layers']:
+                entries += [(layer['conv1'].key, layer['conv1'], 0), (layer['conv2'].key, layer['conv2'], 0)]
+            if blk['tconv'] is not None:
+                entries.append((blk['tconv'].key, blk['tconv'], 0))
+        entries.append((self._head.key, self._head, (self._head.cout + 31) // 32 * 32))      # padded to the dz buffer's width
+        self._pack(entries, device)
+
+    def _block_stats(self, blk, device):
+        key = (blk['index'], str(device))
+        st = self._stats.get(key)
+        if st is None or st.mean.numel() != blk['width']:
+            st = self._stats[key] = _DenseStats(blk['width'], device)
+        return st
+
+    # ---- forward -------------------------------------------------------------------------------------
+    def _finalize(self, st, s, n, rows, eps):
+        """Batch statistics of block channels [s, s + n) from their accumulators: mean / invstd, and the batch mean / unbiased variance for the
+        running statistics (yb_bn_finalize with momentum 1 writes exactly those into its running-stat outputs)."""
+        ops.call('yb_bn_finalize', st.seg(s, n), rows, n, eps, 1.0, st.bmean[s:s + n], st.bvar[s:s + n], st.mean[s:s + n], st.invstd[s:s + n])
+
+    @staticmethod
+    def _fold(st, nu):
+        c = nu.cout
+        scale = torch.empty(c, dtype=torch.float32, device=st.mean.device)
+        shift = torch.empty_like(scale)
+        ops.call('yb_bn_batch_fold', st.mean, st.invstd, nu.bn.weight.detach(), nu.bn.bias.detach(), scale, shift, c)
+        return scale, shift
+
+    def _running_update(self, blk, st, momentum):
+        """Running statistics of every norm of the block (each over its own channels [0, C)) in one launch; num_batches_tracked with the rest."""
+        norms = [layer['norm1'] for layer in blk['layers']] + [blk['tail']]
+        key = tuple((nu.bn.running_mean.data_ptr(), nu.bn.running_var.data_ptr()) for nu in norms)
+        if st.running is None or st.running[0] != key:
+            table = np.zeros(len(norms), dtype=np.dtype([('m', '<u8'), ('v', '<u8'), ('c', '<i4'), ('mom', '<f4')]))
+            for k, nu in enumerate(norms):
+                table[k] = (nu.bn.running_mean.data_ptr(), nu.bn.running_var.data_ptr(), nu.cout, momentum)
+            st.running = (key, torch.from_numpy(table.view(np.uint8).copy()).to(st.mean.device))
+        ops.call('yb_bn_running_update_batch', st.bmean, st.bvar, st.running[1], len(norms), blk['width'])
+        for nu in norms:
+            if nu.bn.num_batches_tracked is not None:
+                self._tracked.append(nu.bn.num_batches_tracked)
+            nu._bver = None
+
+    def _layer_forward(self, layer, buf, st, eps, b, hh, ww):
+        """One dense layer on channels [0, Ci) of the block buffer; its 32 new channels (and their statistics) land at channel Ci."""
+        ci, c1, c2 = layer['cin'], layer['conv1'], layer['conv2']
+        dev = buf.device
+        pre = self._fold(st, layer['norm1'])
+        one, zero = self._ones(c1.cout, dev)
+        z1 = torch.empty(b, hh, ww, c1.cout, dtype=torch.float16, device=dev)
+        ops.call('yb_conv1x1_preact_stats_fwd', buf, c1.w16, pre[0], pre[1], 1, one, zero, 1.0, z1, b, hh, ww, ci, c1.cout, buf.shape[-1], c1.cout, 0,
+                 self._sums(('f', c1.key), c1.cout, dev))
+        mean2, invstd2 = self._bn_forward(c1.key, c1, z1, b * hh * ww, True)
+        a2 = self._apply(c1, z1, mean2, invstd2, b, hh, ww, False)
+        one, zero = self._ones(c2.cout, dev)
+        ops.call('yb_conv_bn_act_stats_fwd', a2, c2.w16, one, zero, 1.0, buf, b, hh, ww, c2.cin, c2.cout, 3, a2.shape[-1], buf.shape[-1], ci, 0,
+                 st.seg(ci, c2.cout))
+        self._finalize(st, ci, c2.cout, b * hh * ww, eps)
+        return self._saved_unit(c1, None, z1, mean2, invstd2, hh, ww, a2=a2, pre=pre)
+
+    def _transition_forward(self, blk, rec, nblk, nst, eps, b):
+        """norm + relu + AvgPool2d(2) of the whole block buffer (rec.pre: the norm's fold), kept for the weight gradient, then the 1x1 conv into
+        channels [0, C/2) of the next block's new buffer with their statistics (into nst).  Returns (that buffer, nst)."""
+        width, hh, ww, dev = blk['width'], rec.h, rec.w, rec.buf.device
+        tc = blk['tconv']
+        rec.pooled = torch.empty(b, hh // 2, ww // 2, width, dtype=torch.float16, device=dev)
+        ops.call('yb_bn_relu_avgpool2x2_f16', rec.buf, width, rec.pre[0], rec.pre[1], rec.pooled, b, hh, ww, width)
+        hh, ww = hh // 2, ww // 2
+        nbuf = torch.empty(b, hh, ww, nblk['width'], dtype=torch.float16, device=dev)
+        one, zero = self._ones(tc.cout, dev)
+        ops.call('yb_conv_bn_act_stats_fwd', rec.pooled, tc.w16, one, zero, 1.0, nbuf, b, hh, ww, width, tc.cout, 1, width, nbuf.shape[-1], 0, 0,
+                 nst.seg(0, tc.cout))
+        self._finalize(nst, 0, tc.cout, b * hh * ww, eps)
+        return nbuf, nst
+
+    def _head_forward(self, rec):
+        """norm5 (rec.pre, identity activation) + the head conv with bias on the last block's buffer: the fp32 NCHW feature."""
+        head = self._head
+        one, _ = self._ones(head.cout, rec.buf.device)
+        return ops.conv1x1_preact(rec.buf, head.w16, rec.pre[0], rec.pre[1], False, one, head.conv.bias.detach(), 1.0, out_mode=ops.OUT_F32_NCHW)
+
+    def _check(self, x):
+        net = self.dnn
+        b, c, h, w = x.shape
+        if c != 3 or h % 32 or w % 32:
+            raise ValueError('DenseNet expects [B,3,H,W] with H, W multiples of 32')
+        why = net.unsupported()
+        if why is not None:
+            raise NotImplementedError('DenseNet: no kernel path for %s' % why)
+        if net.growth_rate != self.GROWTH or net.bn_size * net.growth_rate != 128:
+            raise NotImplementedError('DenseNet training: growth rate %d, bn_size %d (the training path is built for 32 and 4)'
+                                      % (net.growth_rate, net.bn_size))
+
+    def forward(self, x):
+        x = self._start_forward(x)
+        self._check(x)
+        b, _, h, w = x.shape
+        dev = x.device
+        blocks = self._plan()
+        settings = [self._block_norm_settings(blk) for blk in blocks]
+        self._repack(dev)
+        saved = _Saved()
+        saved.x, saved.b, saved.blocks = x, b, []
+        hh, ww = h // 4, w // 4
+        buf = torch.empty(b, hh, ww, blocks[0]['width'], dtype=torch.float16, device=dev)
+        saved.stem, saved.stem_a, _ = self._stem_forward(x, out=buf)
+        st = self._block_stats(blocks[0], dev)
+        ops.call('yb_bn_stats', buf, buf.shape[-1], b * hh * ww, 64, st.seg(0, 64))
+        self._finalize(st, 0, 64, b * hh * ww, settings[0][0])
+        feature = None
+        for blk, (eps, momentum) in zip(blocks, settings):
+            rec = _Saved()
+            rec.buf, rec.st, rec.h, rec.w = buf, st, hh, ww
+            rec.layers = [self._layer_forward(layer, buf, st, eps, b, hh, ww) for layer in blk['layers']]
+            self._running_update(blk, st, momentum)
+            rec.pre = self._fold(st, blk['tail'])
+            if blk['tconv'] is not None:
+                nblk = blocks[blk['index'] + 1]
+                buf, st = self._transition_forward(blk, rec, nblk, self._block_stats(nblk, dev), settings[blk['index'] + 1][0], b)
+                hh, ww = hh // 2, ww // 2
+            else:
+                feature = self._head_forward(rec)
+            saved.blocks.append(rec)
+        self._bump_tracked()
+        return feature, saved
+
+    # ---- backward ------------------------------------------------------------------------------------
+    def _preact_wgrad(self, u, x, pre, relu, dz, b, hh, ww, grads):
+        """Weight gradient of a pre-activation 1x1 conv (conv1, the head) into its arena slot."""
+        dev = dz.device
+        dw_krsc = torch.empty(u.cout, 1, 1, u.cin, dtype=torch.float32, device=dev)
+        ops.call('yb_conv1x1_preact_wgrad', x, pre[0], pre[1], int(relu), dz, dw_krsc, b, hh, ww, u.cin, u.cout, x.shape[-1], dz.shape[-1])
+        wname = u.pnames[0]
+        dw = self.arena.views[wname]
+        ops.call('yb_unpack_wgrad', dw_krsc, dw, u.cout, u.cin, 1, self._unscale)
+        grads[wname] = dw
+        self._emit(wname, grads)
+
+    def _preact_bn_backward(self, nu, rec, da, relu, pool, gbuf, out16, out16_ch0, b, grads):
+        """Backward of a pre-activation norm over channels [0, C) of the block buffer: reduce (dgamma, dbeta), then dx added into the fp32 block
+        gradient with channels [out16_ch0, C) also rounded into out16."""
+        c = nu.cout
+        buf, st = rec.buf, rec.st
+        sums = self._sums(('b', nu.key), c, buf.device)
+        gamma, beta = nu.bn.weight.detach(), nu.bn.bias.detach()
+        if not pool and 256 % (c // 8) == 0:         # yb_bn_act_bwd's kernels need C / 8 to divide their 256 threads
+            ops.call('yb_bn_act_bwd', 0, buf, buf.shape[-1], st.mean, st.invstd, gamma, beta, 0.0 if relu else 1.0, da, da.shape[-1], 0, None, 0, 0,
+                     b, rec.h, rec.w, c, 0, sums, None, 0, 1)
+        else:
+            ops.call('yb_bn_preact_bwd', 0, buf, buf.shape[-1], st.mean, st.invstd, gamma, beta, int(relu), da, da.shape[-1], int(pool), b, rec.h, rec.w, c,
+                     sums, None, 0, None, 0, 0)
+        ops.call('yb_bn_preact_bwd', 1, buf, buf.shape[-1], st.mean, st.invstd, gamma, beta, int(relu), da, da.shape[-1], int(pool), b, rec.h, rec.w, c,
+                 sums, gbuf, gbuf.shape[-1], out16, out16.shape[-1], out16_ch0)
+        self._bn_param_grad(nu.key, nu, sums, grads)
+
+    def _tail_backward(self, blk, rec, g, gbuf, b, grads):
+        """Backward of the block's tail into its fp32 gradient gbuf: norm5 + head from dfeature g (fp32 NCHW), or the transition from g, the
+        fp16 gradient of its conv's output.  Returns the fp16 gradient of the block's last 32 channels (the last conv2's dz)."""
+        hh, ww, width = rec.h, rec.w, blk['width']
+        dz2 = torch.empty(b, hh, ww, self.GROWTH, dtype=torch.float16, device=g.device)
+        if blk['tconv'] is None:
+            head = self._head
+            dzh = self._head_grad('features.conv.bias', head.cout, rec.buf, hh, ww, g, grads)
+            self._preact_wgrad(head, rec.buf, rec.pre, 0, dzh, b, hh, ww, grads)
+            da = self._dgrad(head.key, head, dzh, dzh.shape[-1])
+            self._preact_bn_backward(blk['tail'], rec, da, 0, 0, gbuf, dz2, width - self.GROWTH, b, grads)
+        else:
+            tc = blk['tconv']
+            self._wgrad(tc, rec.pooled, g, b, hh // 2, ww // 2, grads, tc.key)
+            dpool = self._dgrad(tc.key, tc, g)
+            self._preact_bn_backward(blk['tail'], rec, dpool, 1, 1, gbuf, dz2, width - self.GROWTH, b, grads)
+        return dz2
+
+    def _layer_backward(self, layer, rec, s, dz2, gbuf, b, grads, first):
+        """Backward of one dense layer from dz2, the fp16 gradient of its 32 channels: conv2, norm2 + relu2, conv1 and norm1 + relu1, whose dx
+        is added into gbuf.  Returns the fp16 slice that contribution completes: the previous layer's 32 channels, or the block input when
+        `first`."""
+        hh, ww, dev = rec.h, rec.w, dz2.device
+        ci, c1, c2 = layer['cin'], layer['conv1'], layer['conv2']
+        self._wgrad(c2, s.a2, dz2, b, hh, ww, grads, c2.key)
+        da2 = self._dgrad(c2.key, c2, dz2)
+        dz1 = torch.empty(b, hh, ww, c1.cout, dtype=torch.float16, device=dev)
+        self._bn_backward(c1.key, s, b, grads, dz1, da=da2)
+        self._preact_wgrad(c1, rec.buf, s.pre, 1, dz1, b, hh, ww, grads)
+        da1 = self._dgrad(c1.key, c1, dz1)
+        n16 = ci if first else self.GROWTH
+        out16 = torch.empty(b, hh, ww, n16, dtype=torch.float16, device=dev)
+        self._preact_bn_backward(layer['norm1'], rec, da1, 1, 0, gbuf, out16, ci - n16, b, grads)
+        return out16
+
+    def backward(self, saved, dfeature):
+        b = saved.b
+        grads = {}
+        dev = dfeature.device
+        self._start_backward(dev)
+        g = dfeature         # the gradient arriving at the current block's tail
+        for blk, rec in reversed(list(zip(self._plan(), saved.blocks))):
+            gbuf = torch.zeros(b, rec.h, rec.w, blk['width'], dtype=torch.float32, device=dev)
+            dz2 = self._tail_backward(blk, rec, g, gbuf, b, grads)
+            for j in reversed(range(len(blk['layers']))):
+                dz2 = self._layer_backward(blk['layers'][j], rec, rec.layers[j], dz2, gbuf, b, grads, j == 0)
+            g = dz2          # the block input's gradient: the previous transition conv's dz, or the stem pool's
+        self._stem_backward(saved.x, saved.stem, saved.stem_a, g, grads)
+        self._finish_backward(dev)
+        return grads

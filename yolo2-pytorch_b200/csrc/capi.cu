@@ -143,6 +143,11 @@ int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1_excl(const void*, void*, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1_excl_bwd(const void*, void*, int, int, int, int, cudaStream_t);
 int conv2d_wgrad_forward(const void*, const void*, float*, int, int, int, int, int, int, int, int, int, int, int, int, cudaStream_t);
+int conv1x1_preact_wgrad(const void*, const float*, const float*, int, const void*, float*, int, int, int, int, int, int, int, cudaStream_t);
+int bn_batch_fold(const float*, const float*, const float*, const float*, float*, float*, int, cudaStream_t);
+int bn_preact_bwd(int, const void*, long long, const float*, const float*, const float*, const float*, int, const void*, long long, int, int, int,
+                  int, int, double*, float*, long long, void*, long long, int, cudaStream_t);
+int bn_running_update(const float*, const float*, const void*, int, int, cudaStream_t);
 int unpack_wgrad_khw(const float*, float*, int, int, int, int, int, float, cudaStream_t);
 int pack_weight_dgrad_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
 int stem3x3_s2_raw(const float*, const float*, void*, int, int, int, int, cudaStream_t);
@@ -236,6 +241,36 @@ int yb_conv1x1_preact_fwd(const void* x, const void* w, const float* pre_scale, 
   if (pre_scale == nullptr) return yb::fail(YB_ERR_BAD_ARG, "conv_preact: null pre_scale");
   return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, 1, x_ld, y_ld, y_ch_off, out_mode, flags,
                                 workspace, workspace_bytes, nullptr, 0, -1, pre_scale, pre_shift, pre_relu, S(stream));
+}
+
+int yb_conv1x1_preact_stats_fwd(const void* x, const void* w, const float* pre_scale, const float* pre_shift, int pre_relu, const float* scale,
+                                const float* shift, float slope, void* y, int batch, int height, int width, int cin, int cout, int x_ld, long long y_ld,
+                                int y_ch_off, double* sums, yb_stream_t stream) {
+  if (pre_scale == nullptr || sums == nullptr) return yb::fail(YB_ERR_BAD_ARG, "conv_preact_stats: null pre_scale or sums");
+  return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, 1, x_ld, y_ld, y_ch_off, 0, 0, nullptr, 0, sums, 0, -1,
+                                pre_scale, pre_shift, pre_relu, S(stream));
+}
+
+int yb_conv1x1_preact_wgrad(const void* x, const float* pre_scale, const float* pre_shift, int pre_relu, const void* dz, float* dw_krsc, int batch,
+                            int height, int width, int cin, int cout, int x_ld, int dz_ld, yb_stream_t stream) {
+  return yb::conv1x1_preact_wgrad(x, pre_scale, pre_shift, pre_relu, dz, dw_krsc, batch, height, width, cin, cout, x_ld, dz_ld, S(stream));
+}
+
+int yb_bn_batch_fold(const float* mean, const float* invstd, const float* gamma, const float* beta, float* scale, float* shift, int channels,
+                     yb_stream_t stream) {
+  return yb::bn_batch_fold(mean, invstd, gamma, beta, scale, shift, channels, S(stream));
+}
+
+int yb_bn_preact_bwd(int mode, const void* x, long long x_ld, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                     int relu, const void* da, long long da_ld, int pool, int batch, int height, int width, int channels, double* sums, float* dx,
+                     long long dx_ld, void* dx16, long long dx16_ld, int dx16_ch0, yb_stream_t stream) {
+  return yb::bn_preact_bwd(mode, x, x_ld, mean, invstd, gamma, beta, relu, da, da_ld, pool, batch, height, width, channels, sums, dx, dx_ld, dx16,
+                           dx16_ld, dx16_ch0, S(stream));
+}
+
+int yb_bn_running_update_batch(const float* batch_mean, const float* batch_var, const yb_bn_running* norms_dev, int count, int max_channels,
+                               yb_stream_t stream) {
+  return yb::bn_running_update(batch_mean, batch_var, norms_dev, count, max_channels, S(stream));
 }
 
 int yb_bn_relu_avgpool2x2_f16(const void* x, int x_ld, const float* scale, const float* shift, void* y, int batch, int height, int width,

@@ -1582,13 +1582,13 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
   int rc = conv_geometry(in_h, in_w, kh, kw, stride, pad_h, pad_w, &height, &width);
   if (rc) return rc;
   const bool plain_1x1 = kh == 1 && kw == 1 && stride == 1;
-  // pre-activation form (pre_scale != NULL): 1x1, plain fp16 operands, no statistics
+  // pre-activation form (pre_scale != NULL): 1x1, plain fp16 operands; fused statistics are the training form (yb_conv1x1_preact_stats_fwd)
   const bool pre = pre_scale != nullptr;
   if (pre) {
     YB_REQUIRE(pre_shift != nullptr && (pre_relu == 0 || pre_relu == 1), "conv_preact: pre_shift must be given, pre_relu 0 or 1");
     YB_REQUIRE(plain_1x1, "conv_preact: k=%d x %d, stride %d: the pre-activation form is 1x1 stride 1 only", kh, kw, stride);
     YB_REQUIRE(a_channels <= 0 || a_channels == cin, "conv_preact: split-precision operands are not supported");
-    YB_REQUIRE(lo_ch_off < 0 && stats == nullptr, "conv_preact: no residual output and no fused statistics");
+    YB_REQUIRE(lo_ch_off < 0, "conv_preact: no residual output");
     YB_REQUIRE(cin <= kPreMaxCh, "conv_preact: Cin=%d exceeds the %d-channel pre-activation table", cin, kPreMaxCh);
   }
   const PreAct pre_act{pre_scale, pre_shift, pre_relu};

@@ -44,6 +44,9 @@ struct WgradParams {
   int use_atomics;
   int skip;             // profiling ablation (results are garbage): 1 = no x loads, 2 = no dz loads, 4 = no MMA, 8 = no stores
   int* dbg;
+  const float* pre_scale;   // conv1x1_preact_wgrad: the activation operand is fp16(act(fmaf(pre_scale, x, pre_shift)))
+  const float* pre_shift;
+  int pre_relu;
 };
 
 // K-major is the fprop case (yb_ptx.cuh); this is the MN-major flavour: rows = K (pixels), kRowBytes of channels
@@ -53,6 +56,47 @@ __device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32
   constexpr uint64_t layout = (kRowBytes == 128) ? 1ull : 2ull;
   constexpr uint64_t sbo = (8ull * kRowBytes) >> 4;
   return static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4) | (static_cast<uint64_t>(lbo_bytes >> 4) << 16) | (sbo << 32) | (layout << 62);
+}
+
+// Pre-activation of the B operand (yb_conv1x1_preact_wgrad; DenseNet's norm -> relu -> 1x1 conv), applied in place to the `nboxes`
+// activation boxes of one stage: box q holds channels [c_first + q * kBCh, + kBCh) of KP pixel rows, kBRow bytes per row, TMA-swizzled
+// (logical 16-byte chunk c of row r sits at c ^ (r % 8) for 128-byte rows, c ^ ((r / 2) % 4) for 64-byte rows).  The arithmetic is that of
+// conv_igemm.cu's preact_stage: a = fp16_rn(act(fmaf(scale[c], x, shift[c]))).  Chunks at or past Cin (zero-filled by the TMA, never
+// stored) are left alone.  A thread keeps one chunk column; its 4 scale / shift pairs per half-chunk come from L1.
+template <int kBRow, int KP>
+__device__ __forceinline__ void preact_wgrad_stage(uint32_t sb, int c_first, int nboxes, int cin, const float* __restrict__ scale,
+                                                   const float* __restrict__ shift, int relu) {
+  constexpr int kChunks = kBRow / 16;
+  constexpr int kBCh = kBRow / 2;
+  constexpr int kRowsPerPass = WG_MMA_THREADS / kChunks;
+  const int c = threadIdx.x % kChunks;
+  const int r0 = threadIdx.x / kChunks;
+#pragma unroll 1
+  for (int q = 0; q < nboxes; ++q) {
+    const int ch0 = c_first + q * kBCh + c * 8;
+    if (ch0 >= cin) continue;
+#pragma unroll 1
+    for (int half = 0; half < 2; ++half) {
+      const float4 sc = __ldg(reinterpret_cast<const float4*>(scale + ch0 + 4 * half));
+      const float4 sh = __ldg(reinterpret_cast<const float4*>(shift + ch0 + 4 * half));
+#pragma unroll 2
+      for (int i = 0; i < KP / kRowsPerPass; ++i) {
+        const int r = r0 + i * kRowsPerPass;
+        const int pc = (kBRow == 128) ? (c ^ (r & 7)) : (c ^ ((r >> 1) & 3));
+        const uint32_t addr = sb + q * (KP * kBRow) + r * kBRow + pc * 16 + half * 8;
+        uint32_t v0, v1;
+        asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(v0), "=r"(v1) : "r"(addr) : "memory");
+        const float2 f0 = __half22float2(*reinterpret_cast<__half2*>(&v0));
+        const float2 f1 = __half22float2(*reinterpret_cast<__half2*>(&v1));
+        float y0 = __fmaf_rn(sc.x, f0.x, sh.x), y1 = __fmaf_rn(sc.y, f0.y, sh.y);
+        float y2 = __fmaf_rn(sc.z, f1.x, sh.z), y3 = __fmaf_rn(sc.w, f1.y, sh.w);
+        if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); y2 = fmaxf(y2, 0.f); y3 = fmaxf(y3, 0.f); }
+        __half2 h0 = __floats2half2_rn(y0, y1), h1 = __floats2half2_rn(y2, y3);
+        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" :: "r"(addr), "r"(*reinterpret_cast<uint32_t*>(&h0)), "r"(*reinterpret_cast<uint32_t*>(&h1))
+                     : "memory");
+      }
+    }
+  }
 }
 
 // kBRow = bytes per pixel row of the activation (B) boxes: 128 (64 channels) or 64 (32 channels, Cin = 32)
@@ -74,8 +118,9 @@ struct WgradCfg {
 };
 
 // N = accumulator columns of every CTA of the launch (groups_per_cta x n_per_group); a CTA with fewer groups computes the
-// surplus columns from stale shared memory and never stores them
-template <int kBRow, int WG_KP, int WG_STAGES, int NMAX, int N>
+// surplus columns from stale shared memory and never stores them.  kPre: the 1x1 pre-activation form (preact_wgrad_stage on every
+// activation stage before the MMAs; the B tile is shared by both warpgroups, so both finish the transform before either issues).
+template <int kBRow, int WG_KP, int WG_STAGES, int NMAX, int N, bool kPre = false>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_constant__ CUtensorMap tmap_x, const WgradParams p) {
   using Cfg = WgradCfg<kBRow, WG_KP, WG_STAGES, NMAX>;
@@ -158,6 +203,12 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   int prev = -1;
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(bar_full + 8 * stage, phase, p.dbg, 0x700 | stage);
+    if constexpr (kPre) {
+      preact_wgrad_stage<kBRow, WG_KP>(smem_base + stage * kStageBytes + kABytes, first_tile * p.n_per_group, ngroups * boxes_per_group, p.cin,
+                                       p.pre_scale, p.pre_shift, p.pre_relu);
+      fence_proxy_async_smem();
+      asm volatile("bar.sync 1, %0;" :: "n"(WG_MMA_THREADS) : "memory");
+    }
     if (!(p.skip & 4)) {
       const uint32_t sa = smem_base + stage * kStageBytes;
       const uint64_t adesc = make_mnmajor_desc<128>(sa + wg * kABox, kABox);
@@ -209,16 +260,22 @@ typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t
                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 int get_tensor_map_encoders(EncodeTiledFn* tiled, EncodeIm2colFn* im2col);
 
-template <int kBRow, int KP, int STAGES, int NMAX, int N>
-static int launch_wgrad(const CUtensorMap& tdz, const CUtensorMap& tx, const WgradParams& p, int grid, cudaStream_t stream) {
+template <int kBRow, int KP, int STAGES, int NMAX, int N, bool kPre>
+static int launch_wgrad_as(const CUtensorMap& tdz, const CUtensorMap& tx, const WgradParams& p, int grid, cudaStream_t stream) {
   using Cfg = WgradCfg<kBRow, KP, STAGES, NMAX>;
   static bool set = false;
   if (!set) {
-    YB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<kBRow, KP, STAGES, NMAX, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    YB_CUDA(cudaFuncSetAttribute(conv_wgrad_kernel<kBRow, KP, STAGES, NMAX, N, kPre>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     set = true;
   }
-  conv_wgrad_kernel<kBRow, KP, STAGES, NMAX, N><<<grid, WG_THREADS, Cfg::kSmemBytes, stream>>>(tdz, tx, p);
-  return check_launch("conv_wgrad_kernel");
+  conv_wgrad_kernel<kBRow, KP, STAGES, NMAX, N, kPre><<<grid, WG_THREADS, Cfg::kSmemBytes, stream>>>(tdz, tx, p);
+  return check_launch(kPre ? "conv_wgrad_kernel (pre-activation)" : "conv_wgrad_kernel");
+}
+
+template <int kBRow, int KP, int STAGES, int NMAX, int N>
+static int launch_wgrad(const CUtensorMap& tdz, const CUtensorMap& tx, const WgradParams& p, int grid, cudaStream_t stream) {
+  if (p.pre_scale != nullptr) return launch_wgrad_as<kBRow, KP, STAGES, NMAX, N, true>(tdz, tx, p, grid, stream);
+  return launch_wgrad_as<kBRow, KP, STAGES, NMAX, N, false>(tdz, tx, p, grid, stream);
 }
 
 // pixels per stage (one TMA box) and pipeline depth: 128-pixel boxes, two stages
@@ -228,7 +285,8 @@ constexpr int kWgNmaxNarrow = 96;   // Cin % 64 != 0: 32-channel boxes, three ta
 
 // Both entries below: the geometry checks, then the launch.  Cin is any multiple of 32 here; yb_conv2d_wgrad documents its own range.
 static int wgrad_run(const void* x, const void* dz, float* dw_krsc, int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride,
-                     int pad_h, int pad_w, int x_ld, int dz_ld, cudaStream_t stream) {
+                     int pad_h, int pad_w, int x_ld, int dz_ld, cudaStream_t stream, const float* pre_scale = nullptr,
+                     const float* pre_shift = nullptr, int pre_relu = 0) {
   YB_REQUIRE(x && dz && dw_krsc, "wgrad: null pointer");
   YB_REQUIRE(kh >= 1 && kh <= 7 && kw >= 1 && kw <= 7 && pad_h >= 0 && pad_h < kh && pad_w >= 0 && pad_w < kw && (stride == 1 || stride == 2),
              "wgrad: kernel %d x %d, stride %d, padding (%d, %d) unsupported", kh, kw, stride, pad_h, pad_w);
@@ -290,6 +348,7 @@ static int wgrad_run(const void* x, const void* dz, float* dw_krsc, int batch, i
   if (const char* e = getenv("YB_WGRAD_SKIP")) p.skip = atoi(e);
   p.use_atomics = p.splits > 1;
   p.dbg = debug_word_device();
+  p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu;
   const size_t dw_bytes = static_cast<size_t>(cout) * taps * cin * sizeof(float);
   if (p.use_atomics) YB_CUDA(cudaMemsetAsync(dw_krsc, 0, dw_bytes, stream));
 
@@ -351,6 +410,18 @@ int conv_wgrad_forward(const void* x, const void* dz, float* dw_krsc, int batch,
   YB_REQUIRE(ksize == 1 || ksize == 3, "wgrad: ksize");
   YB_REQUIRE(cin % 32 == 0 && (cin == 32 || cin % 64 == 0), "wgrad: Cin=%d unsupported", cin);
   return wgrad_run(x, dz, dw_krsc, batch, height, width, cin, cout, ksize, ksize, 1, (ksize - 1) / 2, (ksize - 1) / 2, x_ld, dz_ld, stream);
+}
+
+// DenseNet's pre-activation 1x1 conv: dW[co][ci] = sum_p dz[p][co] * a[p][ci], a = fp16(act(fmaf(pre_scale, x, pre_shift))) formed on the
+// shared-memory tile.  Same launch plan as yb_conv_wgrad / yb_conv2d_wgrad for a 1x1 layer, so it equals them on the materialised a
+// with the same split.  Cin a multiple of 32 up to the widest DenseNet-201 block (1920).
+int conv1x1_preact_wgrad(const void* x, const float* pre_scale, const float* pre_shift, int pre_relu, const void* dz, float* dw_krsc, int batch,
+                         int height, int width, int cin, int cout, int x_ld, int dz_ld, cudaStream_t stream) {
+  YB_REQUIRE(pre_scale && pre_shift && (pre_relu == 0 || pre_relu == 1), "preact_wgrad: pre_scale / pre_shift must be given, pre_relu 0 or 1");
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(pre_scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(pre_shift) & 15) == 0,
+             "preact_wgrad: pre_scale / pre_shift must be 16B aligned");
+  YB_REQUIRE(cin <= 1920, "preact_wgrad: Cin=%d unsupported (a multiple of 32 up to 1920)", cin);
+  return wgrad_run(x, dz, dw_krsc, batch, height, width, cin, cout, 1, 1, 1, 0, 0, x_ld, dz_ld, stream, pre_scale, pre_shift, pre_relu);
 }
 
 // fp32 [Cout][kh][kw][krsc_cin] (the wgrad layout; krsc_cin >= cin when the activation carried zero channels) -> fp32 OIHW [Cout][Cin][kh][kw],

@@ -1,4 +1,4 @@
-"""model.densenet -- DenseNet backbone plugin on the CUDA kernels (inference).
+"""model.densenet -- DenseNet backbone plugin on the CUDA kernels (inference and training).
 
 Drop-in for the reference's `model/densenet.py`: same constructors `densenet121 / densenet169 / densenet201 / densenet161
 (config_channels, anchors, num_cls)` (:68-117), same module tree and state_dict keys as torchvision's DenseNet under `features`
@@ -16,7 +16,11 @@ the block's final channel count, so the concatenations of the reference are neve
                                         in exact arithmetic and cuts that conv's work 4x; only the fp32 rounding order differs from the reference.
   norm5 + head conv (+ bias)         -> yb_conv1x1_preact_fwd with norm5 as the (identity-activation) pre-transform, fp32 NCHW out.
 The folded BatchNorms and packed weights are cached per parameter version; switching train() / eval() drops the cache.  There is no CPU
-path and no training path.
+path.
+
+train() mode on a CUDA tensor runs one autograd node over b200.train_engine.DenseNetTrainer (batch-statistics BatchNorm shared by every
+norm that reads a block channel, running-statistics update, the explicit backward chain), so train.iterate and train.GraphedStep work as
+for the other backbones.  A CPU tensor, densenet161 and drop_rate > 0 raise NotImplementedError in train mode.
 """
 import re
 from collections import OrderedDict
@@ -100,6 +104,7 @@ class DenseNet(nn.Module):
                 nn.init.zeros_(m.bias)
         self._register_load_state_dict_pre_hook(self._remap_hook)
         self._cache = {}
+        self._trainer = None
 
     @staticmethod
     def _remap_hook(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
@@ -211,9 +216,25 @@ class DenseNet(nn.Module):
         return _ops.conv1x1_preact(buf, self._packed('head', f.conv.weight), s5, t5, False, self._const(1, cout, x.device),
                                    f.conv.bias.detach().float().contiguous(), 1.0, out_mode=_ops.OUT_F32_NCHW)
 
+    @property
+    def trainer(self):
+        if self._trainer is None:
+            from b200 import train_engine as _train
+            self._trainer = _train.DenseNetTrainer(self)
+        return self._trainer
+
     def forward(self, x):
         if self.training:
-            raise NotImplementedError('DenseNet: training is not implemented on the kernels; call .eval() for inference')
+            if not x.is_cuda:
+                raise NotImplementedError('DenseNet: training runs on the CUDA kernels only; the input is a CPU tensor')
+            why = self.unsupported()
+            if why is not None:
+                raise NotImplementedError('DenseNet: no kernel path for %s' % why)
+            if self.drop_rate > 0:
+                raise NotImplementedError('DenseNet: drop_rate=%g: dense-layer dropout is not implemented in training' % self.drop_rate)
+            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.DenseNetTrainer)
+            from model.yolo2 import _DarknetTrainFunction
+            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
         return self.run(x)
 
 
