@@ -25,6 +25,44 @@ STRICT_KEEP = {'layers1.0': 'aw', 'layers1.2': 'aw', 'layers1.4': 'a', 'passthro
 PRECISIONS = ('fast', 'strict')
 
 
+class OperandCache(dict):
+    """Kernel operands built from module tensors (packed weights, folded BatchNorms), one entry per key."""
+
+    def fetch(self, key, tensors, build, extra=()):
+        """The value stored under `key` while every tensor's (data_ptr, _version) and `extra` are unchanged, else `build()`, stored in its
+        place.  A hit returns the same object: CUDA graphs captured over a forward read the cached buffers by address.  `tensors=()` gives
+        a constant built once."""
+        ver = tuple((t.data_ptr(), t._version) for t in tensors) + tuple(extra)
+        hit = self.get(key)
+        if hit is None or hit[0] != ver:
+            hit = self[key] = (ver, build())
+        return hit[1]
+
+
+def epilogue_tensors(bn, bias=None):
+    """The tensors `fold_epilogue(bn, bias)` reads."""
+    ts = () if bias is None else (bias,)
+    return ts if bn is None else ts + (bn.weight, bn.bias, bn.running_mean, bn.running_var)
+
+
+def fold_epilogue(bn, bias, cout_pad=None):
+    """(scale, shift) of a conv's epilogue: BatchNorm `bn` folded (the conv's `bias`, if it has one, folded into the shift), or (1, bias)
+    without BatchNorm; padded to `cout_pad` filters with (1, 0)."""
+    if bias is not None:
+        bias = bias.detach().float().contiguous()
+    if bn is None:
+        s, t = torch.ones_like(bias), bias
+    else:
+        s, t = ops.bn_fold(*(p.detach().float().contiguous() for p in epilogue_tensors(bn)), eps=bn.eps)
+        if bias is not None:
+            t = t + s * bias
+    n = 0 if cout_pad is None else cout_pad - s.numel()
+    if n:
+        s = torch.cat([s, torch.ones(n, dtype=torch.float32, device=s.device)])
+        t = torch.cat([t, torch.zeros(n, dtype=torch.float32, device=t.device)])
+    return s, t
+
+
 class ConvUnit(object):
     """Operands of one `model.yolo2.Conv2d` unit (conv [+BN] [+leaky]); cached per parameter version."""
 

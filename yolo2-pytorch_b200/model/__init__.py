@@ -14,7 +14,66 @@ import torch.nn as nn
 import torch.distributed as _dist
 
 from b200 import ddp as _ddp
+from b200 import engine as _engine
 from b200 import ops as _ops
+
+
+class _TrainFunction(torch.autograd.Function):
+    """Training-mode forward/backward of a whole backbone as one autograd node: forward runs the plugin's train-mode kernel chain
+    (batch-statistics BatchNorm, running-stat update), backward its explicit backward chain (b200.train_engine) and hands every parameter
+    its fp32 gradient."""
+
+    @staticmethod
+    def forward(ctx, dnn, x, *params):
+        feature, saved = dnn.trainer.forward(x)
+        ctx.dnn, ctx.saved = dnn, saved
+        return feature
+
+    @staticmethod
+    def backward(ctx, dfeature):
+        dnn = ctx.dnn
+        grads = dnn.trainer.backward(ctx.saved, dfeature)
+        ctx.saved = None
+        # The gradients live in the trainer's persistent arena (b200.ddp.GradArena; in data-parallel runs its buckets are being
+        # all-reduced in place right now).  `.grad` is bound to those views directly -- handing them to autograd instead would let
+        # AccumulateGrad clone them whenever it cannot steal the tensor, silently detaching `.grad` from the reduced buffer.
+        # Like the reference (zero_grad before every backward, train.py:350), gradients are not accumulated across calls.
+        params = list(dnn.named_parameters())
+        for name, p in params:
+            p.grad = grads[name]
+        return (None, None) + (None,) * len(params)
+
+
+class Backbone(nn.Module):
+    """Base of the backbone plugins.  Holds the kernel operands cached per parameter version (`_cache`), the lazily built trainer (an
+    instance of the b200.train_engine class `TRAINER`) and the train-mode entry through it."""
+    TRAINER = None
+
+    def __init__(self):
+        nn.Module.__init__(self)
+        self._cache = _engine.OperandCache()
+        self._trainer = None
+
+    @property
+    def trainer(self):
+        if self._trainer is None:
+            self._trainer = self.TRAINER(self)
+        return self._trainer
+
+    def drop_operands(self):
+        """Forget every cached kernel operand."""
+        self._cache.clear()
+
+    def train(self, mode=True):
+        """nn.Module.train + drop cached kernel operands on a mode switch: fused optimizers and CUDA-graph replays update parameters without
+        advancing torch's version counters, so inference after training re-packs from the trained state."""
+        if bool(mode) != self.training:
+            self.drop_operands()
+        return nn.Module.train(self, mode)
+
+    def train_forward(self, x):
+        """Batch-statistics BatchNorm + autograd through the explicit backward chain of `TRAINER`."""
+        return _TrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
 
 
 class ConfigChannels(object):

@@ -29,7 +29,9 @@ import torch
 import torch.nn as nn
 
 import model
+from b200 import engine as _engine
 from b200 import ops as _ops
+from b200 import train_engine as _train
 
 # torchvision 0.2 (the reference's) named a dense layer's parameters `norm.1`, `conv.2`, ...; torchvision's own loader renames them
 _OLD_KEY = re.compile(r'^(.*denselayer\d+\.(?:norm|relu|conv))\.((?:[12])\.(?:weight|bias|running_mean|running_var|num_batches_tracked))$')
@@ -73,9 +75,11 @@ class _Transition(nn.Sequential):
         self.add_module('pool', nn.AvgPool2d(kernel_size=2, stride=2))
 
 
-class DenseNet(nn.Module):
+class DenseNet(model.Backbone):
+    TRAINER = _train.DenseNetTrainer
+
     def __init__(self, config_channels, anchors, num_cls, growth_rate=32, block_config=(6, 12, 24, 16), num_init_features=64, bn_size=4, drop_rate=0):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         # drop_rate (model/densenet.py:30): torchvision's dense-layer dropout acts in training only, so the eval-mode forward is the same for any rate
         self.drop_rate = float(drop_rate)
         self.growth_rate, self.block_config, self.num_init_features, self.bn_size = growth_rate, tuple(block_config), num_init_features, bn_size
@@ -103,18 +107,10 @@ class DenseNet(nn.Module):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
         self._register_load_state_dict_pre_hook(self._remap_hook)
-        self._cache = {}
-        self._trainer = None
 
     @staticmethod
     def _remap_hook(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
         remap_legacy_keys(state_dict, prefix)
-
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands."""
-        if bool(mode) != self.training:
-            self._cache = {}
-        return nn.Module.train(self, mode)
 
     def unsupported(self):
         """Why this configuration has no kernel path (None when it has one)."""
@@ -127,28 +123,13 @@ class DenseNet(nn.Module):
 
     # ---- operand preparation (cached per parameter version) ------------------------------------------
     def _fold(self, key, bn):
-        ts = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
-        ver = tuple((t.data_ptr(), t._version) for t in ts)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.bn_fold(*(t.detach().float().contiguous() for t in ts), eps=bn.eps))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, _engine.epilogue_tensors(bn), lambda: _engine.fold_epilogue(bn, None))
 
     def _packed(self, key, w):
-        ver = (w.data_ptr(), w._version)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.pack_weight_f16(w.detach().float().contiguous(), 0))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, (w,), lambda: _ops.pack_weight_f16(w.detach().float().contiguous(), 0))
 
     def _const(self, value, n, device):
-        key = ('const', value, n, str(device))
-        t = self._cache.get(key)
-        if t is None:
-            t = self._cache[key] = torch.full((n,), float(value), dtype=torch.float32, device=device)
-        return t
+        return self._cache.fetch(('const', value, n, str(device)), (), lambda: torch.full((n,), float(value), dtype=torch.float32, device=device))
 
     # ---- units -----------------------------------------------------------------------------------------
     def dense_layer(self, key, layer, buf, cin, tmp):
@@ -216,13 +197,6 @@ class DenseNet(nn.Module):
         return _ops.conv1x1_preact(buf, self._packed('head', f.conv.weight), s5, t5, False, self._const(1, cout, x.device),
                                    f.conv.bias.detach().float().contiguous(), 1.0, out_mode=_ops.OUT_F32_NCHW)
 
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            from b200 import train_engine as _train
-            self._trainer = _train.DenseNetTrainer(self)
-        return self._trainer
-
     def forward(self, x):
         if self.training:
             if not x.is_cuda:
@@ -232,9 +206,7 @@ class DenseNet(nn.Module):
                 raise NotImplementedError('DenseNet: no kernel path for %s' % why)
             if self.drop_rate > 0:
                 raise NotImplementedError('DenseNet: drop_rate=%g: dense-layer dropout is not implemented in training' % self.drop_rate)
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.DenseNetTrainer)
-            from model.yolo2 import _DarknetTrainFunction
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         return self.run(x)
 
 

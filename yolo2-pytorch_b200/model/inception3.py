@@ -15,7 +15,7 @@ head `conv` (:52).  Forward x[B,3,H,W] fp32 -> [B, A*(5+C), OH, OW] fp32, where 
 The tensor-core conv needs Cin % 32 == 0: Conv2d_3b_1x1 (80 filters) and branch5x5_1 (48) run with 96 / 64 filters whose extra rows are zero
 (scale 1, shift 0: ReLU stores exact zeros) and their consumers read those channels with zero weights -- exact, no kernel change.
 The folded BatchNorms and packed weights are cached per parameter version; switching train() / eval() drops the cache.
-In train() mode on a CUDA tensor the forward is one autograd node (model.yolo2._DarknetTrainFunction) over
+In train() mode on a CUDA tensor the forward is one autograd node (model._TrainFunction) over
 b200.train_engine.InceptionTrainer: batch-statistics BatchNorm (eps 1e-3, momentum from the module), the running-statistics update, and an
 explicit backward chain that gives every parameter its fp32 gradient.  There is no CPU path: a train-mode forward on a CPU tensor raises
 NotImplementedError, an eval-mode one RuntimeError.
@@ -24,6 +24,7 @@ import torch
 import torch.nn as nn
 
 import model
+from b200 import engine as _engine
 from b200 import ops as _ops
 from b200 import train_engine as _train
 
@@ -108,9 +109,11 @@ class InceptionE(nn.Module):
 BLOCKS = ('Mixed_5b', 'Mixed_5c', 'Mixed_5d', 'Mixed_6a', 'Mixed_6b', 'Mixed_6c', 'Mixed_6d', 'Mixed_6e', 'Mixed_7a', 'Mixed_7b', 'Mixed_7c')
 
 
-class Inception3(nn.Module):
+class Inception3(model.Backbone):
+    TRAINER = _train.InceptionTrainer
+
     def __init__(self, config_channels, anchors, num_cls, transform_input=False):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         self.transform_input = transform_input
         self.Conv2d_1a_3x3 = BasicConv2d(3, 32, kernel_size=3, stride=2)
         self.Conv2d_2a_3x3 = BasicConv2d(32, 32, kernel_size=3)
@@ -137,49 +140,24 @@ class Inception3(nn.Module):
             elif isinstance(m, nn.BatchNorm2d):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
-        self._cache = {}
-        self._trainer = None
         _pretrained(self, config_channels)
-
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.InceptionTrainer(self)
-        return self._trainer
-
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands."""
-        if bool(mode) != self.training:
-            self._cache = {}
-        return nn.Module.train(self, mode)
 
     # ---- operand preparation (cached per parameter version) ------------------------------------------
     def _operands(self, unit, cin_pad):
         """Folded BatchNorm (scale, shift) padded to the 32-rounded filter count with (1, 0), and the packed fp16 weight with zero filters and
         zero input channels up to (cout_pad, cin_pad)."""
         w, bn = unit.conv.weight, unit.bn
-        ts = (w, bn.weight, bn.bias, bn.running_mean, bn.running_var)
-        ver = tuple((t.data_ptr(), t._version) for t in ts) + (cin_pad,)
-        hit = self._cache.get(unit)
-        if hit is None or hit[0] != ver:
-            cout = w.shape[0]
-            cout_pad = _round32(cout)
-            s, t = _ops.bn_fold(*(p.detach().float().contiguous() for p in ts[1:]), eps=bn.eps)
-            if cout_pad != cout:
-                s = torch.cat([s, torch.ones(cout_pad - cout, dtype=torch.float32, device=s.device)])
-                t = torch.cat([t, torch.zeros(cout_pad - cout, dtype=torch.float32, device=t.device)])
-            w16 = _ops.pack_weight_khw_f16(w.detach().float().contiguous(), cout_pad, cin_pad)
-            hit = self._cache[unit] = (ver, w16, s, t)
-        return hit[1:]
+        cout_pad = _round32(w.shape[0])
+
+        def build():
+            s, t = _engine.fold_epilogue(bn, None, cout_pad)
+            return _ops.pack_weight_khw_f16(w.detach().float().contiguous(), cout_pad, cin_pad), s, t
+        return self._cache.fetch(unit, (w,) + _engine.epilogue_tensors(bn), build, extra=(cin_pad,))
 
     def _head(self):
         w, b = self.conv.weight, self.conv.bias
-        ver = tuple((t.data_ptr(), t._version) for t in (w, b))
-        hit = self._cache.get('head')
-        if hit is None or hit[0] != ver:
-            hit = self._cache['head'] = (ver, _ops.pack_weight_khw_f16(w.detach().float().contiguous()),
-                                         torch.ones(w.shape[0], dtype=torch.float32, device=w.device), b.detach().float().contiguous())
-        return hit[1:]
+        return self._cache.fetch('head', (w, b), lambda: (_ops.pack_weight_khw_f16(w.detach().float().contiguous()),
+                                                          torch.ones(w.shape[0], dtype=torch.float32, device=w.device), b.detach().float().contiguous()))
 
     # ---- units -----------------------------------------------------------------------------------------
     def unit(self, unit, x, out=None, y_ch_off=0):
@@ -268,12 +246,7 @@ class Inception3(nn.Module):
 
     def _operands_stem(self):
         bn = self.Conv2d_1a_3x3.bn
-        ts = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
-        ver = tuple((t.data_ptr(), t._version) for t in ts)
-        hit = self._cache.get('stem')
-        if hit is None or hit[0] != ver:
-            hit = self._cache['stem'] = (ver, _ops.bn_fold(*(p.detach().float().contiguous() for p in ts), eps=bn.eps))
-        return hit[1]
+        return self._cache.fetch('stem', _engine.epilogue_tensors(bn), lambda: _engine.fold_epilogue(bn, None))
 
     def run(self, x, collect=None):
         """Forward on the kernels; `collect` (a dict) receives both stem pools and every Mixed_* output (fp16 NHWC)."""
@@ -298,9 +271,7 @@ class Inception3(nn.Module):
         if self.training:
             if not x.is_cuda:
                 raise NotImplementedError('Inception3: training runs on the CUDA kernels only; the input is a CPU tensor')
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.InceptionTrainer)
-            from model.yolo2 import _DarknetTrainFunction
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         return self.run(x)
 
 

@@ -21,7 +21,7 @@ order, and a max-pool branch carries its input's layout through.  Each tensor ha
 a consumer's weight is scattered onto its input's layout, zero elsewhere, before the pack.  With ratio 1 and an unpruned model every width is a
 multiple of 32 and every layout is the identity.  The scattered weights, folded BatchNorms and packs are cached per parameter version;
 switching train() / eval() drops the cache.
-In train() mode on a CUDA tensor the forward is one autograd node (model.yolo2._DarknetTrainFunction) over
+In train() mode on a CUDA tensor the forward is one autograd node (model._TrainFunction) over
 b200.train_engine.Inception4Trainer: batch-statistics BatchNorm (eps 1e-3, momentum 0.1) with the running-statistics update, or conv + bias
 + ReLU with BatchNorm disabled, and an explicit backward chain that gives every parameter its fp32 gradient.  Training needs the full-width
 model: a channel-pruned or ratio != 1 model raises ValueError on a train-mode forward (its eval mode is unchanged).  There is no CPU path:
@@ -33,6 +33,7 @@ import torch
 import torch.nn as nn
 
 import model
+from b200 import engine as _engine
 from b200 import ops as _ops
 from b200 import train_engine as _train
 
@@ -209,9 +210,11 @@ BLOCKS = (Mixed_3a, Mixed_4a, Mixed_5a) + (Inception_A,) * 4 + (Reduction_A,) + 
 STEM = ((32, 3, 2, 0), (32, 3, 1, 0), (64, 3, 1, 1))      # (filters, kernel, stride, padding) of features.0 .. features.2
 
 
-class Inception4(nn.Module):
+class Inception4(model.Backbone):
+    TRAINER = _train.Inception4Trainer
+
     def __init__(self, config_channels, anchors, num_cls, ratio=1):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         config = config_channels.config
         bn = config.getboolean('batch_norm', 'enable')
         features = []
@@ -227,8 +230,6 @@ class Inception4(nn.Module):
         self.features = nn.Sequential(*features)
         self._init(config)
         self._plan()
-        self._cache = {}
-        self._trainer = None
         _pretrained(self, config)
 
     def _init(self, config):
@@ -270,63 +271,27 @@ class Inception4(nn.Module):
             self.blocks.append((m, tuple(segs), lay))
         self.layouts[f[-1]] = lay
 
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.Inception4Trainer(self)
-        return self._trainer
-
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands."""
-        if bool(mode) != self.training:
-            self._cache = {}
-        return nn.Module.train(self, mode)
-
     def scope(self, name):
         return '.'.join(name.split('.')[:-2])
 
     # ---- operand preparation (cached per parameter version) ------------------------------------------
-    @staticmethod
-    def _tensors(unit):
-        if unit.bn is None:
-            return (unit.conv.weight, unit.conv.bias)
-        bn = unit.bn
-        return (unit.conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var)
-
     def scattered(self, unit):
         """The fp32 weight handed to the pack: [round32(Cout), input width, kh, kw], the module's weight scattered onto its input's layout."""
         w = unit.conv.weight
         return scatter_weight(w, self.layouts[unit], _round32(w.shape[0]))
 
-    def _fold(self, unit, cout_pad):
-        """(scale, shift) of the epilogue: the folded BatchNorm, or (1, bias); padded to cout_pad with (1, 0)."""
-        if unit.bn is None:
-            t = unit.conv.bias.detach().float().contiguous()
-            s = torch.ones_like(t)
-        else:
-            bn = unit.bn
-            s, t = _ops.bn_fold(*(p.detach().float().contiguous() for p in (bn.weight, bn.bias, bn.running_mean, bn.running_var)), eps=bn.eps)
-        n = cout_pad - s.numel()
-        if n:
-            s = torch.cat([s, torch.ones(n, dtype=torch.float32, device=s.device)])
-            t = torch.cat([t, torch.zeros(n, dtype=torch.float32, device=t.device)])
-        return s, t
-
     def _operands(self, unit):
-        ts = self._tensors(unit)
-        ver = tuple((t.data_ptr(), t._version) for t in ts)
-        hit = self._cache.get(unit)
-        if hit is None or hit[0] != ver:
+        """(weight, scale, shift) of one Conv2d: features.0's fp32 weight with zero filters up to 32, else the packed scattered weight; the
+        epilogue padded to the weight's filter count."""
+        def build():
             if unit is self.features[0]:
                 w = unit.conv.weight.detach().float()
                 w32 = torch.zeros(STEM_FILTERS, 3, 3, 3, dtype=torch.float32, device=w.device)
                 w32[:w.shape[0]] = w
-                hit = (ver, w32) + self._fold(unit, STEM_FILTERS)
-            else:
-                full = self.scattered(unit)
-                hit = (ver, _ops.pack_weight_khw_f16(full.contiguous())) + self._fold(unit, full.shape[0])
-            self._cache[unit] = hit
-        return hit[1:]
+                return (w32,) + _engine.fold_epilogue(unit.bn, unit.conv.bias, STEM_FILTERS)
+            full = self.scattered(unit)
+            return (_ops.pack_weight_khw_f16(full.contiguous()),) + _engine.fold_epilogue(unit.bn, unit.conv.bias, full.shape[0])
+        return self._cache.fetch(unit, (unit.conv.weight,) + _engine.epilogue_tensors(unit.bn, unit.conv.bias), build)
 
     def scattered_head(self):
         """The head's fp32 weight handed to the pack: [Cout, input width, 1, 1], scattered onto the last block's layout."""
@@ -335,13 +300,8 @@ class Inception4(nn.Module):
 
     def _head(self):
         w, b = self.features[-1].weight, self.features[-1].bias
-        ver = tuple((t.data_ptr(), t._version) for t in (w, b))
-        hit = self._cache.get('head')
-        if hit is None or hit[0] != ver:
-            full = self.scattered_head()
-            hit = self._cache['head'] = (ver, _ops.pack_weight_khw_f16(full.contiguous()), torch.ones(w.shape[0], dtype=torch.float32, device=w.device),
-                                         b.detach().float().contiguous())
-        return hit[1:]
+        return self._cache.fetch('head', (w, b), lambda: (_ops.pack_weight_khw_f16(self.scattered_head().contiguous()),
+                                                          torch.ones(w.shape[0], dtype=torch.float32, device=w.device), b.detach().float().contiguous()))
 
     # ---- units -----------------------------------------------------------------------------------------
     def unit(self, unit, x, out=None, y_ch_off=0):
@@ -406,9 +366,7 @@ class Inception4(nn.Module):
         if self.training:
             if not x.is_cuda:
                 raise NotImplementedError('Inception4: training runs on the CUDA kernels only; the input is a CPU tensor')
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.Inception4Trainer)
-            from model.yolo2 import _DarknetTrainFunction
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         return self.run(x)
 
 

@@ -21,6 +21,7 @@ import torch
 import torch.nn as nn
 
 import model
+from b200 import engine as _engine
 from b200 import ops as _ops
 from b200 import train_engine as _train
 
@@ -59,9 +60,11 @@ def conv_unit(in_channels, out_channels, stride):
 UNITS = [(64, 1), (128, 2), (128, 1), (256, 2), (256, 1), (512, 2), (512, 1), (512, 1), (512, 1), (512, 1), (512, 1), (1024, 2), (1024, 1)]
 
 
-class MobileNet(nn.Module):
+class MobileNet(model.Backbone):
+    TRAINER = _train.MobileNetTrainer
+
     def __init__(self, config_channels, anchors, num_cls):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         cc = config_channels
         layers = [conv_bn(cc.channels, cc(32, 'layers.0.conv.weight'), 2)]
         for width, stride in UNITS:
@@ -74,8 +77,6 @@ class MobileNet(nn.Module):
             elif isinstance(m, nn.BatchNorm2d):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
-        self._cache = {}
-        self._trainer = None
         config = getattr(config_channels, 'config', None)
         precision = os.environ.get('YB_PRECISION')
         if precision is None and config is not None and config.has_option('b200', 'precision'):
@@ -87,47 +88,19 @@ class MobileNet(nn.Module):
         if precision not in ('fast', 'strict'):
             raise ValueError("precision must be 'fast' or 'strict', got %r" % (precision,))
         if precision != self.precision:
-            self._cache = {}
+            self.drop_operands()
         self.precision = precision
         return self
 
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.MobileNetTrainer(self)
-        return self._trainer
-
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands (fused optimizers update parameters behind torch's version counters)."""
-        if bool(mode) != self.training:
-            self._cache = {}
-        return nn.Module.train(self, mode)
-
     # ---- operand preparation (cached per parameter version) ------------------------------------------
     def _fold(self, key, bn):
-        ts = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
-        ver = tuple((t.data_ptr(), t._version) for t in ts)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.bn_fold(*(t.detach().contiguous() for t in ts), eps=bn.eps))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, _engine.epilogue_tensors(bn), lambda: _engine.fold_epilogue(bn, None))
 
     def _packed(self, key, w):
-        ver = (w.data_ptr(), w._version)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.pack_weight_f16(w.detach().contiguous(), 0))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, (w,), lambda: _ops.pack_weight_f16(w.detach().contiguous(), 0))
 
     def _packed_split(self, key, w):
-        ver = (w.data_ptr(), w._version)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.pack_weight_split_f16(w.detach().contiguous(), True, True))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, (w,), lambda: _ops.pack_weight_split_f16(w.detach().contiguous(), True, True))
 
     def _forward_strict(self, x):
         b, c, h, w = x.shape
@@ -160,9 +133,7 @@ class MobileNet(nn.Module):
 
     def forward(self, x):
         if self.training:
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.MobileNetTrainer)
-            from model.yolo2 import _DarknetTrainFunction
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         if not x.is_cuda:
             raise RuntimeError('MobileNet: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape
@@ -190,9 +161,6 @@ class MobileNet(nn.Module):
             cur = _ops.conv_bn_act(out, self._packed('pww%d' % i, pw.conv.weight), scale, shift, 0.0)      # slope 0 == ReLU
         head = self.layers[-1]
         cout = head.weight.shape[0]
-        ones = self._cache.get('ones')
-        if ones is None or ones.numel() != cout or ones.device != x.device:
-            ones = torch.ones(cout, dtype=torch.float32, device=x.device)
-            self._cache['ones'] = ones
+        ones = self._cache.fetch('ones', (), lambda: torch.ones(cout, dtype=torch.float32, device=x.device), extra=(cout, x.device))
         return _ops.conv_bn_act(cur, self._packed('head', head.weight), ones, head.bias.detach().float().contiguous(), 1.0,
                                 out_mode=_ops.OUT_F32_NCHW)

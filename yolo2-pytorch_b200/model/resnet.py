@@ -12,7 +12,7 @@ parameters; the forward pass is:
                                     form at the even pixels); stride-2 1x1 downsample -> yb_subsample2_f16, then the 1x1 conv
   out += residual; relu          -> yb_add_relu_f16
   nn.Conv2d(C, A*(5+C), 1) + bias-> wgmma 1x1 conv writing fp32 NCHW.
-In train() mode the forward is one autograd node (model.yolo2._DarknetTrainFunction) over b200.train_engine.ResNetTrainer: batch-statistics
+In train() mode the forward is one autograd node (model._TrainFunction) over b200.train_engine.ResNetTrainer: batch-statistics
 BatchNorm (momentum 0.1, read from the modules) on the raw conv outputs, the explicit backward chain (stride-2 convs as the stride-1 gradients of the
 zero-inserted dz, max-pool backward to the first maximum of each window, the stem's weight gradient on the fp32 image).  There is no CPU path.
 Switching back to eval() drops the cached folded BatchNorm and packed weights, so inference uses the trained state.
@@ -23,6 +23,7 @@ import torch
 import torch.nn as nn
 
 import model
+from b200 import engine as _engine
 from b200 import ops as _ops
 from b200 import train_engine as _train
 
@@ -71,9 +72,11 @@ class Bottleneck(nn.Module):
         return [('conv1', self.conv1, self.bn1, True), ('conv2', self.conv2, self.bn2, True), ('conv3', self.conv3, self.bn3, False)]
 
 
-class ResNet(nn.Module):
+class ResNet(model.Backbone):
+    TRAINER = _train.ResNetTrainer
+
     def __init__(self, config_channels, anchors, num_cls, block, layers):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         cc = config_channels
         self.conv1 = nn.Conv2d(cc.channels, cc(64, 'conv1.weight'), kernel_size=7, stride=2, padding=3, bias=False)
         self.bn1 = nn.BatchNorm2d(cc.channels)
@@ -90,8 +93,6 @@ class ResNet(nn.Module):
             elif isinstance(m, nn.BatchNorm2d):
                 nn.init.ones_(m.weight)
                 nn.init.zeros_(m.bias)
-        self._cache = {}
-        self._trainer = None
 
     def _make_layer(self, config_channels, prefix, block, channels, blocks, stride=1):
         seq = [block(config_channels, '%s.0' % prefix, channels, stride)]
@@ -112,36 +113,12 @@ class ResNet(nn.Module):
             assert comp[-1] == 'conv', name
         return '.'.join(comp)
 
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.ResNetTrainer(self)
-        return self._trainer
-
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands (training updates running statistics and, with fused optimizers, parameters behind
-        torch's version counters)."""
-        if bool(mode) != self.training:
-            self._cache = {}
-        return nn.Module.train(self, mode)
-
     # ---- operand preparation (cached per parameter version) ------------------------------------------
     def _fold(self, key, bn):
-        ts = (bn.weight, bn.bias, bn.running_mean, bn.running_var)
-        ver = tuple((t.data_ptr(), t._version) for t in ts)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.bn_fold(*(t.detach().contiguous() for t in ts), eps=bn.eps))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, _engine.epilogue_tensors(bn), lambda: _engine.fold_epilogue(bn, None))
 
     def _packed(self, key, w):
-        ver = (w.data_ptr(), w._version)
-        hit = self._cache.get(key)
-        if hit is None or hit[0] != ver:
-            hit = (ver, _ops.pack_weight_f16(w.detach().contiguous(), 0))
-            self._cache[key] = hit
-        return hit[1]
+        return self._cache.fetch(key, (w,), lambda: _ops.pack_weight_f16(w.detach().contiguous(), 0))
 
     @staticmethod
     def _subsample(x):
@@ -173,9 +150,7 @@ class ResNet(nn.Module):
         if self.training:
             if not x.is_cuda:
                 raise NotImplementedError('ResNet training: no CPU path, input must be a CUDA tensor')
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.ResNetTrainer)
-            from model.yolo2 import _DarknetTrainFunction
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         if not x.is_cuda:
             raise RuntimeError('ResNet: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape
@@ -193,10 +168,7 @@ class ResNet(nn.Module):
             for bname, blk in getattr(self, lname).named_children():
                 cur = self._block('%s.%s' % (lname, bname), blk, cur)
         cout = self.conv.weight.shape[0]
-        ones = self._cache.get('ones')
-        if ones is None or ones.numel() != cout or ones.device != x.device:
-            ones = torch.ones(cout, dtype=torch.float32, device=x.device)
-            self._cache['ones'] = ones
+        ones = self._cache.fetch('ones', (), lambda: torch.ones(cout, dtype=torch.float32, device=x.device), extra=(cout, x.device))
         return _ops.conv_bn_act(cur, self._packed('head', self.conv.weight), ones, self.conv.bias.detach().float().contiguous(), 1.0,
                                 out_mode=_ops.OUT_F32_NCHW)
 

@@ -18,7 +18,7 @@ Padded channel layout: the tensor-core conv needs Cin % 32 == 0, so a conv with 
 extra filters zero with scale 1, shift 0 (exact zeros after the ReLU), and the consumer's packed weight is zero on those input channels
 (pack_weight_khw_f16 with cout_pad / cin_pad).  Folded BatchNorms and packed weights are cached per parameter version; switching train() /
 eval() drops the cache, so inference after training uses the trained state.
-In train() mode the forward is one autograd node (model.yolo2._DarknetTrainFunction) over b200.train_engine.VGGTrainer: batch-statistics
+In train() mode the forward is one autograd node (model._TrainFunction) over b200.train_engine.VGGTrainer: batch-statistics
 BatchNorm (momentum and eps read from the modules), the explicit backward chain, the first layer's weight gradient from the fp32 image
 (yb_conv0_c64_wgrad).  Training needs features.0 with 64 filters and every other width a multiple of 32.  There is no CPU path.
 """
@@ -28,6 +28,7 @@ import torch
 import torch.nn as nn
 
 import model
+from b200 import engine as _engine
 from b200 import ops as _ops
 from b200 import train_engine as _train
 
@@ -74,9 +75,11 @@ class _Unit(object):
         return self.pool_index is not None
 
 
-class VGG(nn.Module):
+class VGG(model.Backbone):
+    TRAINER = _train.VGGTrainer
+
     def __init__(self, config_channels, anchors, num_cls, features):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         self.features = features
         self.conv = nn.Conv2d(config_channels.channels, model.output_channels(len(anchors), num_cls), 1)
         self._initialize_weights()
@@ -84,14 +87,6 @@ class VGG(nn.Module):
         if self.units[0].conv.out_channels > FIRST_FILTERS:
             raise ValueError('VGG: features.0 has %d filters; the first-layer kernel computes at most %d'
                              % (self.units[0].conv.out_channels, FIRST_FILTERS))
-        self._cache = {}
-        self._trainer = None
-
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.VGGTrainer(self)
-        return self._trainer
 
     def _initialize_weights(self):
         """torchvision 0.2's VGG._initialize_weights, which the reference calls (model/vgg.py:33)."""
@@ -120,37 +115,7 @@ class VGG(nn.Module):
             units.append(_Unit(m, bn, j if j < len(f) and isinstance(f[j], nn.MaxPool2d) else None))
         return units
 
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands."""
-        if bool(mode) != self.training:
-            self._cache = {}
-        return nn.Module.train(self, mode)
-
     # ---- operand preparation (cached per parameter version) ------------------------------------------
-    @staticmethod
-    def _tensors(u):
-        ts = (u.conv.weight, u.conv.bias)
-        if u.bn is not None:
-            ts += (u.bn.weight, u.bn.bias, u.bn.running_mean, u.bn.running_var)
-        return ts
-
-    @staticmethod
-    def _fold(u, cout_pad):
-        """(scale, shift) of the epilogue: the folded BatchNorm (with the conv bias folded into the shift), or (1, bias); padded to cout_pad
-        with (1, 0)."""
-        bias = u.conv.bias.detach().float().contiguous()
-        if u.bn is None:
-            s, t = torch.ones_like(bias), bias
-        else:
-            bn = u.bn
-            s, t = _ops.bn_fold(*(p.detach().float().contiguous() for p in (bn.weight, bn.bias, bn.running_mean, bn.running_var)), eps=bn.eps)
-            t = t + s * bias
-        n = cout_pad - s.numel()
-        if n:
-            s = torch.cat([s, torch.ones(n, dtype=torch.float32, device=s.device)])
-            t = torch.cat([t, torch.zeros(n, dtype=torch.float32, device=t.device)])
-        return s.contiguous(), t.contiguous()
-
     def in_width(self, index):
         """Channels of the fp16 buffer unit `index` reads: 64 after features.0, else round32 of the producer's filters."""
         if index == 0:
@@ -161,30 +126,25 @@ class VGG(nn.Module):
         return FIRST_FILTERS if index == 0 else _round32(self.units[index].conv.out_channels)
 
     def _operands(self, index):
+        """(weight, scale, shift) of unit `index`: features.0's fp32 weight with zero filters up to 64, else the packed fp16 weight on the
+        padded layout; the epilogue padded to the unit's output width."""
         u = self.units[index]
-        ts = self._tensors(u)
-        ver = tuple((t.data_ptr(), t._version) for t in ts)
-        hit = self._cache.get(index)
-        if hit is None or hit[0] != ver:
+
+        def build():
             w = u.conv.weight.detach().float().contiguous()
             if index == 0:
                 wp = torch.zeros(FIRST_FILTERS, 3, 3, 3, dtype=torch.float32, device=w.device)
                 wp[:w.shape[0]] = w
             else:
                 wp = _ops.pack_weight_khw_f16(w, self.out_width(index), self.in_width(index))
-            hit = (ver, wp) + self._fold(u, self.out_width(index))
-            self._cache[index] = hit
-        return hit[1:]
+            return (wp,) + _engine.fold_epilogue(u.bn, u.conv.bias, self.out_width(index))
+        return self._cache.fetch(index, (u.conv.weight,) + _engine.epilogue_tensors(u.bn, u.conv.bias), build)
 
     def _head(self):
         w, b = self.conv.weight, self.conv.bias
-        ver = tuple((t.data_ptr(), t._version) for t in (w, b))
-        hit = self._cache.get('head')
-        if hit is None or hit[0] != ver:
-            cin_pad = self.out_width(len(self.units) - 1)
-            hit = self._cache['head'] = (ver, _ops.pack_weight_khw_f16(w.detach().float().contiguous(), None, cin_pad),
-                                         torch.ones(w.shape[0], dtype=torch.float32, device=w.device), b.detach().float().contiguous())
-        return hit[1:]
+        cin_pad = self.out_width(len(self.units) - 1)
+        return self._cache.fetch('head', (w, b), lambda: (_ops.pack_weight_khw_f16(w.detach().float().contiguous(), None, cin_pad),
+                                                          torch.ones(w.shape[0], dtype=torch.float32, device=w.device), b.detach().float().contiguous()))
 
     # ---- forward ---------------------------------------------------------------------------------------
     def run(self, x, collect=None):
@@ -217,9 +177,7 @@ class VGG(nn.Module):
         if self.training:
             if not x.is_cuda:
                 raise RuntimeError('VGG training: input must be a CUDA tensor; there is no CPU fallback')
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.VGGTrainer)
-            from model.yolo2 import _DarknetTrainFunction
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         return self.run(x)
 
 

@@ -80,35 +80,11 @@ class Conv2d(nn.Module):
         return y
 
 
-class _DarknetTrainFunction(torch.autograd.Function):
-    """Training-mode forward/backward of the whole backbone as one autograd node: forward runs the
-    train-mode kernel chain (batch-statistics BatchNorm, running-stat update), backward the explicit
-    backward chain (b200.train_engine) and hands every parameter its fp32 gradient."""
+class Darknet(model.Backbone):
+    TRAINER = _train.DarknetTrainer
 
-    @staticmethod
-    def forward(ctx, dnn, x, *params):
-        feature, saved = dnn.trainer.forward(x)
-        ctx.dnn, ctx.saved = dnn, saved
-        return feature
-
-    @staticmethod
-    def backward(ctx, dfeature):
-        dnn = ctx.dnn
-        grads = dnn.trainer.backward(ctx.saved, dfeature)
-        ctx.saved = None
-        # The gradients live in the trainer's persistent arena (b200.ddp.GradArena; in data-parallel runs its buckets are being
-        # all-reduced in place right now).  `.grad` is bound to those views directly -- handing them to autograd instead would let
-        # AccumulateGrad clone them whenever it cannot steal the tensor, silently detaching `.grad` from the reduced buffer.
-        # Like the reference (zero_grad before every backward, train.py:350), gradients are not accumulated across calls.
-        params = list(dnn.named_parameters())
-        for name, p in params:
-            p.grad = grads[name]
-        return (None, None) + (None,) * len(params)
-
-
-class Darknet(nn.Module):
     def __init__(self, config_channels, anchors, num_cls, stride=2, ratio=1):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         if stride != 2:
             raise ValueError('Darknet: passthrough stride must be 2')
         self.stride = stride
@@ -158,7 +134,6 @@ class Darknet(nn.Module):
 
         self.init()
         self._engine = None
-        self._trainer = None
         # optional `[b200] precision = fast | strict` in the INI (not a reference key): see b200.engine.DarknetEngine.set_precision
         cfg = config_channels.config
         self._precision = cfg.get('b200', 'precision') if cfg.has_option('b200', 'precision') else None
@@ -180,23 +155,14 @@ class Darknet(nn.Module):
                 self._engine.set_precision(self._precision)
         return self._engine
 
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.DarknetTrainer(self)
-        return self._trainer
-
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands: parameters may have been updated by an optimizer that does not
-        advance torch's version counters (fused multi-tensor steps), so the eval engine re-packs after training."""
-        if getattr(self, '_engine', None) is not None and bool(mode) != self.training:
+    def drop_operands(self):
+        """The engine's per-unit operands (Darknet caches nothing on the module)."""
+        if self._engine is not None:
             self._engine.invalidate()
-        return nn.Module.train(self, mode)
 
     def forward(self, x):
         if self.training:
-            # batch-statistics BatchNorm + autograd through the explicit backward chain
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         return self.engine.forward(x).clone()     # the plan-owned buffer is overwritten by the next call; callers own what we return
 
     def scope(self, name):
@@ -231,7 +197,7 @@ class MaxPool2dStride1(nn.Module):
         self.kernel_size, self.stride = 2, 1
 
 
-class Tiny(nn.Module):
+class Tiny(model.Backbone):
     """Tiny YOLOv2 backbone plugin (reference model/yolo2.py:140-173; the repo's default `model/dnn`, config.ini:25),
     inference and training on the CUDA kernels.  Same constructor contract `Tiny(config_channels, anchors, num_cls, channels=16)`, same
     state_dict keys (`layers.{0,2,4,6,8,10,13,14,15}.conv.*`, `.bn.*`), `init()` (xavier-normal, :159-165), `scope()`
@@ -242,8 +208,10 @@ class Tiny(nn.Module):
     two Cin = 32 layers on the halo-tile wgmma kernel with the 2x2 max-pool fused, the rest on the implicit-GEMM
     kernel; `ConstantPad2d + MaxPool2d(2, stride=1)` is one HBM kernel."""
 
+    TRAINER = _train.TinyTrainer
+
     def __init__(self, config_channels, anchors, num_cls, channels=16):
-        nn.Module.__init__(self)
+        model.Backbone.__init__(self)
         cc = config_channels
         bn = cc.config.getboolean('batch_norm', 'enable')
         layers = []
@@ -261,27 +229,17 @@ class Tiny(nn.Module):
         self.layers = nn.Sequential(*layers)
         self.init()
         self._units = None
-        self._pad_cache = {}
-        self._trainer = None
-
-    @property
-    def trainer(self):
-        if self._trainer is None:
-            self._trainer = _train.TinyTrainer(self)
-        return self._trainer
 
     def unit_keys(self):
         """[(state_dict prefix 'layers.N', ConvUnit, followed_by)] in network order."""
         keys = ['layers.%d' % i for i, m in enumerate(self.layers) if not m.is_pool]
         return [(k, u, after) for k, (u, after) in zip(keys, self._plan())]
 
-    def train(self, mode=True):
-        """nn.Module.train + drop cached kernel operands (fused optimizers update parameters behind torch's version counters)."""
-        if getattr(self, '_units', None) is not None and bool(mode) != self.training:
-            self._pad_cache = {}
-            for u, _ in self._units:
-                u._wver = u._bver = None
-        return nn.Module.train(self, mode)
+    def drop_operands(self):
+        """The padded operands and the units' own (ConvUnit.refresh)."""
+        model.Backbone.drop_operands(self)
+        for u, _ in self._units or ():
+            u._wver = u._bver = None
 
     def init(self):
         for m in self.modules():
@@ -313,26 +271,22 @@ class Tiny(nn.Module):
         return self._units
 
     def _padded(self, key, u, cout_to, cin_to, first):
-        """Zero-padded copy of a unit's operands (weights, scale, shift), cached per parameter version."""
-        ver = (u._wver, u._bver)
-        hit = self._pad_cache.get(key)
-        if hit is not None and hit[0] == ver:
-            return hit[1]
-        w = u.conv.weight.detach()
-        cout, cin, k, _ = w.shape
-        wp = torch.zeros(cout_to, cin_to, k, k, dtype=torch.float32, device=w.device)
-        wp[:cout, :cin] = w
-        w_op = wp.contiguous() if first else _ops.pack_weight_f16(wp.contiguous(), 0)
-        scale = torch.zeros(cout_to, dtype=torch.float32, device=w.device)
-        shift = torch.zeros(cout_to, dtype=torch.float32, device=w.device)
-        scale[:cout], shift[:cout] = u.scale, u.shift
-        self._pad_cache[key] = (ver, (w_op, scale, shift))
-        return self._pad_cache[key][1]
+        """Zero-padded copy of a unit's operands (weights, scale, shift), cached per version of the unit's own operands."""
+        def build():
+            w = u.conv.weight.detach()
+            cout, cin, k, _ = w.shape
+            wp = torch.zeros(cout_to, cin_to, k, k, dtype=torch.float32, device=w.device)
+            wp[:cout, :cin] = w
+            w_op = wp.contiguous() if first else _ops.pack_weight_f16(wp.contiguous(), 0)
+            scale = torch.zeros(cout_to, dtype=torch.float32, device=w.device)
+            shift = torch.zeros(cout_to, dtype=torch.float32, device=w.device)
+            scale[:cout], shift[:cout] = u.scale, u.shift
+            return w_op, scale, shift
+        return self._cache.fetch(key, (), build, extra=(u._wver, u._bver))
 
     def forward(self, x):
         if self.training:
-            # batch-statistics BatchNorm + autograd through the explicit backward chain (b200.train_engine.TinyTrainer)
-            return _DarknetTrainFunction.apply(self, x, *[p for _, p in self.named_parameters()])
+            return self.train_forward(x)
         if not x.is_cuda:
             raise RuntimeError('Tiny: input must be a CUDA tensor; there is no CPU fallback')
         b, c, h, w = x.shape

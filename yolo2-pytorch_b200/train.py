@@ -196,12 +196,7 @@ class GraphedStep(object):
 
     def finish(self):
         """Drop operand caches that the graph kept current on its own buffers (see the class docstring)."""
-        dnn = self.inference.dnn
-        engine = getattr(dnn, 'engine', None)
-        if engine is not None:
-            engine.invalidate()
-        elif hasattr(dnn, '_cache'):
-            dnn._cache = {}          # plugins that cache their operands on the module (MobileNet, ResNet)
+        self.inference.dnn.drop_operands()
 
     def close(self):
         """Destroy the captured graphs (required before the NCCL communicator whose collectives they captured is destroyed)."""
