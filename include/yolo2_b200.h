@@ -38,7 +38,9 @@ typedef void* yb_stream_t; /* cudaStream_t */
 #define YB_CONV_A_TILED 1      /* 1x1 only: fetch A with a plain 2-D tiled TMA instead of im2col mode */
 #define YB_CONV_WIDE_N 2       /* allow the 128x256 tile when Cout % 256 == 0 */
 #define YB_CONV_FORCE_BN(bn) ((bn) << 8) /* testing: force BLOCK_N in {64,128,256} */
-#define YB_CONV_POOL2X2 16     /* also apply MaxPool2d(2): y is [B,H/2,W/2,Cout]; implemented for the 3x3 Cin=32 layer (layers1.2) */
+#define YB_CONV_POOL2X2 16     /* also apply MaxPool2d(2): y is [B,H/2,W/2,Cout]; implemented for the 3x3 Cin=32 layer (layers1.2) and for
+                                  3x3 same-padded layers with even H, W, fp16 NHWC output and plain operands whose selection is the
+                                  256 x 128 two-consumer tile (no stream-K); anything else is refused with YB_ERR_UNSUPPORTED */
 #define YB_CONV_C32_IM2COL 32  /* testing: Cin=32 3x3 through the im2col small-K kernel instead of the halo-tile kernel */
 #define YB_CONV_NO_STREAMK 8   /* never split tiles along K even when a workspace is supplied */
 #define YB_CONV_FORCE_STREAMK (1 << 30) /* testing: split along K whenever the shape allows it */

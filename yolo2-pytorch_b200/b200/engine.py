@@ -207,6 +207,23 @@ class DarknetEngine(object):
             raise RuntimeError('Darknet: layers1.0 must be followed by MaxPool2d (fused first-layer kernel)')
         self.precision = 'fast'
         self.set_precision(os.environ.get('YB_PRECISION', 'fast'))
+        # the fast forward fuses a layers1 max-pool into the conv before it wherever the library has a pooled form for that launch;
+        # False keeps the 3x3 Cin = 32 halo kernel's fusion only (A/B runs and tests)
+        self.fuse_wide_pool = True
+        self._pool_ok = {}
+
+    def _pooled_form(self, u, x, conv_flags):
+        """Whether the library runs unit u on input x [B,H,W,C] with the 2x2 max-pool fused on the two-consumer tile (asked once per shape)."""
+        b, h, w, _ = x.shape
+        key = (u.cin, u.cout, u.ksize, b, h, w, conv_flags)
+        ok = self._pool_ok.get(key)
+        if ok is None:
+            try:
+                ok = ops.conv_choice(b, h, w, u.cin, u.cout, u.ksize, flags=conv_flags | ops.CONV_POOL2X2)['kernel'] == 'conv_wide_kernel'
+            except RuntimeError:
+                ok = False
+            self._pool_ok[key] = ok
+        return ok
 
     def unit_keys(self):
         return self._k1 + self._k2 + ['passthrough', 'layers3.0', 'layers3.1']
@@ -293,11 +310,14 @@ class DarknetEngine(object):
         last1 = self.units1[-1]
         for u, (out, pooled), key in zip(self.units1[1:], p.l1, self._k1[1:]):
             # layers1.2 (3x3, Cin = 32) has a kernel whose epilogue applies the MaxPool2d that follows it, so the
-            # 208x208x64 activation never goes to HBM; tests that inspect every layer (collect / ref) keep the two steps
-            fuse_pool = (pooled is not None and u is not last1 and collect is None and not ref and u.cin == 32 and u.ksize == 3
-                         and u.cout <= 64 and (conv_flags & (ops.CONV_NO_SMALLK | ops.CONV_C32_IM2COL)) == 0 and conv_flags < 256)
+            # 208x208x64 activation never goes to HBM, and so do the 3x3 layers on the two-consumer tile (layers1.6 and 1.10 at
+            # 416x416); tests that inspect every layer (collect / ref) keep the two steps.  last1's full-resolution output feeds the
+            # passthrough, so its pool stays a kernel of its own.
+            fuse_pool = pooled is not None and u is not last1 and collect is None and not ref and (
+                (u.cin == 32 and u.ksize == 3 and u.cout <= 64 and (conv_flags & (ops.CONV_NO_SMALLK | ops.CONV_C32_IM2COL)) == 0
+                 and conv_flags < 256) or (self.fuse_wide_pool and self._pooled_form(u, cur, conv_flags)))
             if fuse_pool:
-                ops.conv_bn_act(cur, u.w16, u.scale, u.shift, u.slope, out=pooled, flags=conv_flags | ops.CONV_POOL2X2)
+                ops.conv_bn_act(cur, u.w16, u.scale, u.shift, u.slope, out=pooled, flags=conv_flags | ops.CONV_POOL2X2, workspace=p.workspace)
                 cur = pooled
                 continue
             conv(u, cur, out)

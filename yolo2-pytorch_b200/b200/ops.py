@@ -163,16 +163,19 @@ CONV_KERNELS = ('conv_igemm_kernel', 'conv_wide_kernel', 'conv_c32_kernel')
 
 
 def conv_choice(batch, height, width, cin, cout, k, out_mode=OUT_F16_NHWC, flags=0, workspace=True):
-    """The kernel and tile shape conv_bn_act picks for this shape (the library's own selection, yb_conv_choice)."""
+    """The kernel and tile shape conv_bn_act picks for this shape (the library's own selection, yb_conv_choice).  `pooled`: the launch
+    applies the fused 2x2 max-pool (CONV_POOL2X2; the library refuses the flag where it has no pooled form)."""
     out = (ctypes.c_int * 6)()
     _l.check(_l.load().yb_conv_choice(batch, height, width, cin, cout, k, out_mode, flags, int(bool(workspace)), ctypes.byref(out)),
              'yb_conv_choice')
-    return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5])
+    return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5],
+                pooled=bool(flags & CONV_POOL2X2))
 
 
 def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, ref=False, workspace=None):
     """x: fp16 [B,H,W,x_ld] (uses the first `cin` channels, default all); w: fp16 [Cout,k,k,Cin].
-    out (fp16): [B,H,W,y_ld] written at channels [y_ch_off, y_ch_off+Cout); out (fp32): [B,Cout,H,W]."""
+    out (fp16): [B,H,W,y_ld] written at channels [y_ch_off, y_ch_off+Cout); out (fp32): [B,Cout,H,W].
+    flags & CONV_POOL2X2: the 2x2 max-pool is fused, out is [B,H/2,W/2,y_ld]."""
     _req(x, torch.float16, 'x'); _req(w, torch.float16, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
     b, h, wd, x_ld = x.shape
     cout, k, _, wcin = w.shape
@@ -189,6 +192,12 @@ def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch
     else:
         _req(out, torch.float32, 'out')
         y_ld = 0
+    if flags & CONV_POOL2X2:
+        if ref:
+            raise ValueError('conv_bn_act: the CUDA-core reference has no fused max-pool')
+        if out.dim() != 4 or tuple(out.shape[:3]) != (b, h // 2, wd // 2) or y_ch_off < 0 or y_ch_off + cout > y_ld:
+            raise ValueError('conv_bn_act: pooled out must be [%d,%d,%d,y_ld] with y_ch_off + Cout <= y_ld, got %s at y_ch_off %d'
+                             % (b, h // 2, wd // 2, tuple(out.shape), y_ch_off))
     _conv_common('yb_conv_ref_fwd' if ref else 'yb_conv_bn_act_fwd', x, w, scale, shift, slope, out, b, h, wd, cin, cout, k, x_ld, y_ld,
                  y_ch_off, out_mode, flags, workspace=None if ref else workspace)
     return out
@@ -203,7 +212,8 @@ def conv2d_choice(batch, height, width, cin, cout, kh, kw, stride=1, pad=(0, 0),
     out = (ctypes.c_int * 6)()
     _l.check(_l.load().yb_conv2d_choice(batch, height, width, cin, cout, kh, kw, stride, pad[0], pad[1], out_mode, flags, int(bool(workspace)),
                                         ctypes.byref(out)), 'yb_conv2d_choice')
-    return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5])
+    return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5],
+                pooled=bool(flags & CONV_POOL2X2))
 
 
 def conv2d_bn_act(x, w, scale, shift, slope, stride=1, pad=(0, 0), out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, workspace=None):

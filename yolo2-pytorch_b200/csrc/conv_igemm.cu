@@ -694,6 +694,12 @@ conv_preact_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 constexpr int kWideThreads = 384;
 constexpr int kWideRows = 256;
 constexpr int kWideBN = 128;
+constexpr int kWidePoolRows = kWideRows / 4;   // pooled form: output rows (pool windows) per tile
+
+__device__ __forceinline__ uint32_t hmax2_u32(uint32_t a, uint32_t b) {
+  const __half2 m = __hmax2(*reinterpret_cast<const __half2*>(&a), *reinterpret_cast<const __half2*>(&b));
+  return *reinterpret_cast<const uint32_t*>(&m);
+}
 
 template <int BK>
 struct WideCfg {
@@ -710,10 +716,11 @@ struct WideCfg {
   static_assert(kStages >= (BK == 64 ? 4 : 8), "shared memory budget: the epilogue's slices and table must not cost a pipeline stage");
 };
 
-template <int BK>
-__global__ void __launch_bounds__(kWideThreads, 1)
-conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
+// kPool: the pooled form (conv_wide_pool_kernel), see below.  tmap_a[0] is the A map of the plain form; the pooled form reads one map
+// per pool-window position.
+template <int BK, bool kPool>
+__device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a)[4], const CUtensorMap& tmap_b, const CUtensorMap& tmap_y,
+                                               const ConvParams p) {
   using Cfg = WideCfg<BK>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -737,11 +744,15 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     }
     for (int c = 0; c < 2; ++c) {
       mbar_init(bar_slice_full + 8 * c, 4);                // one arrival per warp of consumer c
-      mbar_init(bar_slice_empty + 8 * c, 1);               // its store thread
+      if constexpr (kPool) mbar_init(bar_slice_empty + 8 * c, c == 1 ? 4 : 1);   // pooled: consumer 1's slice is read by consumer 0's warps
+      else mbar_init(bar_slice_empty + 8 * c, 1);          // its store thread
     }
     fence_mbar_init();
     fence_proxy_async_smem();
-    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(tmap_a[0]);
+    if constexpr (kPool) {
+      for (int b = 1; b < 4; ++b) tma_prefetch_desc(tmap_a[b]);
+    }
     tma_prefetch_desc(&tmap_b);
     tma_prefetch_desc(&tmap_y);
   }
@@ -758,7 +769,7 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       int tr_p = 0;
       for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
         const int n_tile = it.tile % p.n_tiles;
-        const int m_cta = (it.tile / p.n_tiles) * kWideRows;
+        const int m_cta = (it.tile / p.n_tiles) * (kPool ? kWidePoolRows : kWideRows);
         const int img = m_cta / p.hw;
         const int rem = m_cta - img * p.hw;
         const int oh = rem / p.width;
@@ -775,22 +786,31 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           const uint32_t full = bar_full + 8 * stage;
           mbar_arrive_expect_tx(full, Cfg::kStageBytes);      // the A box always transfers (and zero-fills) all 256 rows
           const uint32_t dst = smem_a + stage * Cfg::kABytes;
-          if (p.a_im2col) tma_load_im2col_4d(dst, &tmap_a, full, ca, w0, h0, img, static_cast<uint16_t>(s), static_cast<uint16_t>(r));
-          else tma_load_2d(dst, &tmap_a, full, ca, m_cta);
+          if constexpr (kPool) {
+            // box b = 2 dy + dx: window position (dy, dx) of the tile's 64 pool windows, stage rows 64 b .. 64 b + 63
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+              tma_load_im2col_4d(dst + b * kWidePoolRows * BK * 2, tmap_a[b], full, ca, w0 + (b & 1), h0 + (b >> 1), img, static_cast<uint16_t>(s),
+                                 static_cast<uint16_t>(r));
+          } else {
+            if (p.a_im2col) tma_load_im2col_4d(dst, tmap_a[0], full, ca, w0, h0, img, static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+            else tma_load_2d(dst, tmap_a[0], full, ca, m_cta);
+          }
           tma_load_2d(smem_b + stage * Cfg::kBBytes, &tmap_b, full, tap * p.cin + c0, n_tile * kWideBN);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
-    } else if (threadIdx.x == 32 || threadIdx.x == 64) {
-      // store thread of consumer c: ships each staged 64-row half (rows >= M and channels >= Cout are clipped by the tensor map)
+    } else if (threadIdx.x == 32 || (!kPool && threadIdx.x == 64)) {
+      // store thread of consumer c: ships each staged 64-row half (rows >= M and channels >= Cout are clipped by the tensor map); the
+      // pooled form stores once per tile, the 64 pooled rows consumer 0 staged
       const int c = (threadIdx.x >> 5) - 1;
       const uint32_t slice = smem_o + c * Cfg::kOutBytes;
       uint32_t sph = 0;
       for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
         if (it.kb1 < p.num_kb) continue;                      // stream-K dump: nothing to store
         const int n0 = (it.tile % p.n_tiles) * kWideBN;
-        const int m_base = (it.tile / p.n_tiles) * kWideRows + c * 128;
-        for (int h = 0; h < 2; ++h) {
+        const int m_base = kPool ? (it.tile / p.n_tiles) * kWidePoolRows : (it.tile / p.n_tiles) * kWideRows + c * 128;
+        for (int h = 0; h < (kPool ? 1 : 2); ++h) {
           mbar_wait(bar_slice_full + 8 * c, sph, p.dbg, 0x900 | c);
 #pragma unroll
           for (int c2 = 0; c2 < 2; ++c2) {
@@ -918,6 +938,7 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     }
     // per-thread partial layout: float4 g of thread t of consumer cw at ((cw * 32 + g) * 128 + t) * 4 -- coalesced both ways;
     // g / 16 is the accumulator row half h
+    uint32_t pk_dx0[kPool ? 32 : 1];           // pooled form: the converted h = 0 half (window column dx = 0), kept for the dx max
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (h == 1) {
@@ -960,7 +981,35 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           }
         }
       }
-      // the slice is free once the store thread has seen the previous half's stores read it
+      if constexpr (kPool) {
+        if (h == 0) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) pk_dx0[i] = pk[i];
+          continue;
+        }
+        // fp16 max in maxpool2x2_kernel's order: max(max(dx 0, dx 1) of row dy 0, the same of row dy 1), pair by pair
+#pragma unroll
+        for (int i = 0; i < 32; ++i) pk[i] = hmax2_u32(pk_dx0[i], pk[i]);
+        if (cw == 0) {
+          // consumer 1 staged row dy = 1 at the same slice positions this thread stages: take the dy max, then hand its slice back
+          mbar_wait(bar_slice_full + 8, sph, p.dbg, 0xB00);
+#pragma unroll
+          for (int c2 = 0; c2 < 2; ++c2)
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+              for (int hh = 0; hh < 2; ++hh) {
+                const int r = warp * 16 + (lane >> 2) + hh * 8;
+                const uint32_t addr = smem_o + Cfg::kOutBytes + c2 * 8192 + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
+                uint32_t v;
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+                pk[16 * c2 + 2 * jj + hh] = hmax2_u32(pk[16 * c2 + 2 * jj + hh], v);
+              }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_slice_empty + 8);
+        }
+      }
+      // the slice is free once the store thread (pooled, consumer 1: consumer 0) has seen the previous half's stores read it
       mbar_wait(bar_slice_empty + 8 * cw, sph ^ 1, p.dbg, 0xA00 | cw);
 #pragma unroll
       for (int c2 = 0; c2 < 2; ++c2)
@@ -990,6 +1039,30 @@ conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       for (int j = sk_lo + t + 128 * cw; j < static_cast<int>(blockIdx.x); j += 256) p.flags[j] = 0u;
     }
   }
+}
+
+template <int BK>
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
+  const CUtensorMap* const ta[4] = {&tmap_a, &tmap_a, &tmap_a, &tmap_a};
+  conv_wide_body<BK, false>(ta, tmap_b, tmap_y, p);
+}
+
+// The same tile with the 2x2 max-pool that follows a 3x3 same-padded layer fused into its epilogue (YB_CONV_POOL2X2): a tile is 64 pool
+// windows x their 4 positions, and only the 64 x 128 pooled outputs are stored.  Position (dy, dx) of window (i, j) is output pixel
+// (2 i + dy, 2 j + dx), so each position is a stride-2 conv whose window corners start at (dy - 1, dx - 1): tmap_a<2 dy + dx> is that
+// im2col map and fills stage rows 64 (2 dy + dx) .. + 63.  Consumer dy thus holds positions (dy, 0) and (dy, 1) of the same window in
+// its two accumulator halves, on the same thread: it takes the dx max in registers after the fp16 rounding, consumer 1 stages its
+// result, consumer 0 takes the dy max against it and stages the pooled slice for one TMA store.  Every output is the fp32 sum of the
+// plain tile (same K-blocks, same k16 steps), so the result equals conv_wide_kernel + maxpool2x2_kernel bit for bit.  No stream-K.
+template <int BK>
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_wide_pool_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ CUtensorMap tmap_a1,
+                      const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_a3,
+                      const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
+  const CUtensorMap* const ta[4] = {&tmap_a0, &tmap_a1, &tmap_a2, &tmap_a3};
+  conv_wide_body<BK, true>(ta, tmap_b, tmap_y, p);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1267,6 +1340,7 @@ constexpr int kKernelWide = 1;       // conv_wide_kernel (256 x 128, two consume
 constexpr int kKernelC32 = 2;        // conv_c32_kernel (3x3, Cin = 32 halo tiles)
 struct ConvChoice {
   int kernel, bk, bn, mt, streamk, grid;
+  int pool;        // the 2x2 max-pool is fused (conv_c32_kernel, conv_wide_pool_kernel)
 };
 
 static unsigned long long* g_conv_trace = nullptr;
@@ -1367,6 +1441,20 @@ static int launch_wide(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   cfg.attrs = attr; cfg.numAttrs = nattr;
   YB_CUDA(cudaLaunchKernelEx(&cfg, conv_wide_kernel<BK>, ta, tb, ty, p));
   return check_launch("conv_wide_kernel");
+}
+
+// the pooled form: ta[2 dy + dx] is the A map of window position (dy, dx)
+template <int BK>
+static int launch_wide_pool(const CUtensorMap (&ta)[4], const CUtensorMap& tb, const CUtensorMap& ty, const ConvParams& p, int grid,
+                            cudaStream_t stream) {
+  using Cfg = WideCfg<BK>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    YB_CUDA(cudaFuncSetAttribute(conv_wide_pool_kernel<BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    attr_set = true;
+  }
+  conv_wide_pool_kernel<BK><<<grid, kWideThreads, Cfg::kSmemBytes, stream>>>(ta[0], ta[1], ta[2], ta[3], tb, ty, p);
+  return check_launch("conv_wide_pool_kernel");
 }
 
 // CTA tile shapes (BLOCK_N, M-subtiles): the one-warpgroup kernel keeps MT * BLOCK_N <= 128 accumulators per thread; 128 x 2 is
@@ -1473,14 +1561,21 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int kh, int
   // 3x3 same-padded stride 1, Cin = 32, Cout <= 64 (layers1.2): halo-tile kernel unless a test asks for one of the im2col kernels
   if (!split && cin == 32 && same3x3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 8) & 0xFFFF) == 0) {
     const long long tiles = static_cast<long long>(batch) * ((width + C32Cfg::TW - 1) / C32Cfg::TW) * ((height + C32Cfg::TH - 1) / C32Cfg::TH);
-    c.kernel = kKernelC32; c.bk = 32; c.bn = C32Cfg::BN; c.mt = 1;
+    c.kernel = kKernelC32; c.bk = 32; c.bn = C32Cfg::BN; c.mt = 1; c.pool = (flags >> 4) & 1;
     c.grid = static_cast<int>(tiles < sms ? tiles : sms);
     *out = c;
     return 0;
   }
-  if ((flags >> 4) & 1) return fail(YB_ERR_UNSUPPORTED, "conv: YB_CONV_POOL2X2 is only implemented for the Cin = 32 3x3 layer");
+  // the fused 2x2 max-pool outside the Cin = 32 kernel: the two-consumer tile's pooled form, on the layers whose selection is that tile
+  const bool pool = (flags >> 4) & 1;
+  if (pool) {
+    if (!(same3x3 && height % 2 == 0 && width % 2 == 0 && out_mode == 0 && !split && !stats && !pre))
+      return fail(YB_ERR_UNSUPPORTED, "conv: YB_CONV_POOL2X2 needs a 3x3 same-padded stride-1 layer with even H and W, fp16 NHWC output and "
+                                      "plain operands");
+    if ((flags >> 30) & 1) return fail(YB_ERR_UNSUPPORTED, "conv: the fused 2x2 max-pool has no stream-K form");
+  }
   const int bk = (cin % 64 == 0 && a_channels % 64 == 0) ? 64 : 32;     // K-blocks never straddle the wrap point
-  const bool sk_possible = !stats && workspace_ok && (flags & 8) == 0;
+  const bool sk_possible = !stats && !pool && workspace_ok && (flags & 8) == 0;
   const bool sk_force = sk_possible && ((flags >> 30) & 1);
   // the two-consumer kernel: fp16 NHWC through the TMA store, no residual output, statistics or profiling ablation
   // (the pre-activation form exists only for the one-warpgroup kernel)
@@ -1532,6 +1627,10 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int kh, int
   YB_REQUIRE((c.bn == 64 || c.bn == 128) && (c.mt == 1 || c.mt == 2) && (c.mt * c.bn <= 128 || wide_ok), "conv: tile %d x %d", c.bn, c.mt);
   c.kernel = c.mt * c.bn > 128 ? kKernelWide : kKernelIgemm;
   c.bk = bk;
+  if (pool && c.kernel != kKernelWide)
+    return fail(YB_ERR_UNSUPPORTED, "conv: the fused 2x2 max-pool runs on the 256 x 128 two-consumer tile only; this launch takes %d x %d tiles",
+                BM * c.mt, c.bn);
+  c.pool = pool;
   const long long tiles = ((m_total + BM * c.mt - 1) / (BM * c.mt)) * ((cout + c.bn - 1) / c.bn);
   c.grid = c.streamk ? sms : static_cast<int>(tiles < sms ? tiles : sms);      // sk_base / sk_rem are computed for exactly sms CTAs
   *out = c;
@@ -1628,13 +1727,17 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
   rc = get_encoders(&enc_tiled, &enc_im2col);
   if (rc) return rc;
 
+  // the pooled form enumerates pool windows: M, H and W are the pooled output's, and each window position is a stride-2 conv
+  // (conv_wide_pool_kernel), so the producer's window corners are 2 i - 1, 2 j - 1 plus the position
+  const bool pooled = ch.pool != 0;
+  if (pooled) { height /= 2; width /= 2; }
   ConvParams p;
-  p.m_total = static_cast<int>(m_total_ll);
+  p.m_total = static_cast<int>(static_cast<long long>(batch) * height * width);
   p.height = height; p.width = width; p.cin = cin; p.cout = cout;
-  p.kh = kh; p.kw = kw; p.pad_h = pad_h; p.pad_w = pad_w; p.stride = stride; p.in_h = in_h; p.in_w = in_w;
+  p.kh = kh; p.kw = kw; p.pad_h = pad_h; p.pad_w = pad_w; p.stride = pooled ? 2 : stride; p.in_h = in_h; p.in_w = in_w;
   p.kb_per_tap = cin / bk;
   p.num_kb = kh * kw * p.kb_per_tap;
-  const int rows_tile = BM * mt;
+  const int rows_tile = pooled ? kWidePoolRows : BM * mt;
   p.m_tiles = (p.m_total + rows_tile - 1) / rows_tile;
   p.n_tiles = (cout + bn - 1) / bn;
   p.a_im2col = a_im2col;
@@ -1660,29 +1763,35 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
   }
 
   const CUtensorMapSwizzle swz = (bk == 64) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  alignas(64) CUtensorMap ta, tb;
+  alignas(64) CUtensorMap ta_pos[4];   // ta_pos[0] is the A map; the pooled form has one per window position
+  alignas(64) CUtensorMap tb;
+  CUtensorMap& ta = ta_pos[0];
   CUresult cr;
-  const int a_rows = BM * mt;     // pixels per A box (ConvCfg::kMergedA)
+  const int a_rows = pooled ? kWidePoolRows : BM * mt;     // pixels per A box (ConvCfg::kMergedA)
   if (a_im2col) {
     // the input tensor; the bounding box of window corners is [-pad, in + pad - k] on each axis, walked with the conv's stride, so
-    // consecutive box pixels are consecutive output pixels (row-major, then the next image)
+    // consecutive box pixels are consecutive output pixels (row-major, then the next image).  Pooled, position (dy, dx): corners
+    // [d - 1, in + d - 3] walked with stride 2, one per pool window
     const cuuint64_t dims[4] = {static_cast<cuuint64_t>(a_channels), static_cast<cuuint64_t>(in_w), static_cast<cuuint64_t>(in_h),
                                 static_cast<cuuint64_t>(batch)};
     const cuuint64_t strides[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * in_w,
                                    static_cast<cuuint64_t>(x_ld) * 2 * in_w * in_h};
-    const int lower[2] = {-pad_w, -pad_h};                    // {W, H}
-    const int upper[2] = {pad_w - (kw - 1), pad_h - (kh - 1)};
-    const cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
-    cr = enc_im2col(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x), dims, strides, lower, upper,
-                    static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(a_rows), estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeIm2col failed (%d)", static_cast<int>(cr));
-    // Driver workaround (same one CUTLASS carries, cute/atom/copy_traits_sm90_im2col.hpp): for
-    // tensors smaller than 128 KiB drivers <= 13.1 set a descriptor bit that breaks im2col loads.
+    const cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(p.stride), static_cast<cuuint32_t>(p.stride), 1};
     int drv = 0;
     cudaDriverGetVersion(&drv);
-    const unsigned long long span_bytes = static_cast<unsigned long long>(x_ld) * 2ull * in_w * in_h * batch;
-    if (drv <= 13010 && span_bytes < 131072ull) reinterpret_cast<uint64_t*>(&ta)[1] &= ~(1ull << 21);
+    for (int b = 0; b < (pooled ? 4 : 1); ++b) {
+      const int dx = pooled ? (b & 1) : 0, dy = pooled ? (b >> 1) : 0;
+      const int lower[2] = {dx - pad_w, dy - pad_h};                    // {W, H}
+      const int upper[2] = {dx + pad_w - (kw - 1) - (pooled ? 1 : 0), dy + pad_h - (kh - 1) - (pooled ? 1 : 0)};
+      cr = enc_im2col(&ta_pos[b], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x), dims, strides, lower, upper,
+                      static_cast<cuuint32_t>(bk), static_cast<cuuint32_t>(a_rows), estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeIm2col failed (%d)", static_cast<int>(cr));
+      // Driver workaround (same one CUTLASS carries, cute/atom/copy_traits_sm90_im2col.hpp): for
+      // tensors smaller than 128 KiB drivers <= 13.1 set a descriptor bit that breaks im2col loads.
+      const unsigned long long span_bytes = static_cast<unsigned long long>(x_ld) * 2ull * in_w * in_h * batch;
+      if (drv <= 13010 && span_bytes < 131072ull) reinterpret_cast<uint64_t*>(&ta_pos[b])[1] &= ~(1ull << 21);
+    }
   } else {
     const cuuint64_t dims[2] = {static_cast<cuuint64_t>(a_channels), static_cast<cuuint64_t>(p.m_total)};
     const cuuint64_t strides[1] = {static_cast<cuuint64_t>(x_ld) * 2};
@@ -1717,6 +1826,7 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
   }
+  if (pooled) return bk == 64 ? launch_wide_pool<64>(ta_pos, tb, ty, p, ch.grid, stream) : launch_wide_pool<32>(ta_pos, tb, ty, p, ch.grid, stream);
   if (bk == 64) return dispatch_conv<64>(bn, mt, ch.grid, ta, tb, ty, p, pre ? &pre_act : nullptr, stream);
   return dispatch_conv<32>(bn, mt, ch.grid, ta, tb, ty, p, pre ? &pre_act : nullptr, stream);
 }
