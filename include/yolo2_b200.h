@@ -41,6 +41,9 @@ typedef void* yb_stream_t; /* cudaStream_t */
 #define YB_CONV_POOL2X2 16     /* also apply MaxPool2d(2): y is [B,H/2,W/2,Cout]; implemented for the 3x3 Cin=32 layer (layers1.2) and for
                                   3x3 same-padded layers with even H, W, fp16 NHWC output and plain operands whose selection is the
                                   256 x 128 two-consumer tile (no stream-K); anything else is refused with YB_ERR_UNSUPPORTED */
+#define YB_CONV_CHAIN1X1 128   /* yb_conv_choice: whether yb_conv_bn_act_chain_fwd accepts this layer as the producer of a fused 1x1 unit
+                                  (Cout = 128, Cin % 64 == 0, fp16 NHWC output and plain operands whose selection is the 256 x 128
+                                  two-consumer tile, no stream-K); anything else is refused with YB_ERR_UNSUPPORTED */
 #define YB_CONV_C32_IM2COL 32  /* testing: Cin=32 3x3 through the im2col small-K kernel instead of the halo-tile kernel */
 #define YB_CONV_NO_STREAMK 8   /* never split tiles along K even when a workspace is supplied */
 #define YB_CONV_FORCE_STREAMK (1 << 30) /* testing: split along K whenever the shape allows it */
@@ -113,6 +116,15 @@ int yb_conv_choice(int batch, int height, int width, int cin, int cout, int ksiz
 int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                           int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);
+/* Two units in one launch: the conv above (x, w, scale, shift, slope; Cin, Cout, ksize) followed by a 1x1 stride-1 unit whose input
+ * is that conv's whole output -- w2 fp16 [Cout2][1][1][Cout], scale2 / shift2 [Cout2], slope2.  Only the second unit's output is
+ * written: y fp16 NHWC [B,H,W,y_ld] at channels [y_ch_off, y_ch_off + Cout2).  The first output stays on the SM and goes into the
+ * second GEMM from registers; the result equals the two yb_conv_bn_act_fwd_ws launches bit for bit.  Needs the YB_CONV_CHAIN1X1
+ * conditions on the first conv and 8 <= Cout2 <= 64 (multiple of 8); anything else is refused with YB_ERR_UNSUPPORTED or
+ * YB_ERR_BAD_ARG.  Flags and workspace as yb_conv_bn_act_fwd_ws (the chained form never splits along K). */
+int yb_conv_bn_act_chain_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, const void* w2, const float* scale2,
+                             const float* shift2, float slope2, void* y, int batch, int height, int width, int cin, int cout, int cout2, int ksize,
+                             int x_ld, long long y_ld, int y_ch_off, int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);
 /* Split-precision ("strict") form of the same unit, for callers that need the reference's fp32 results to 1e-3 end to end
  * (model/yolo2.py:125-130 runs in fp32; 23 fp16-operand layers drift 1.6e-3).  The GEMM's reduction dimension is a concatenation
  * of fp16 terms accumulated in one fp32 accumulator:  A = [a_hi | a_lo | a_hi],  W = [w_hi | w_hi | w_lo]  (or the two-term

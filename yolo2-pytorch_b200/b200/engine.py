@@ -211,6 +211,27 @@ class DarknetEngine(object):
         # False keeps the 3x3 Cin = 32 halo kernel's fusion only (A/B runs and tests)
         self.fuse_wide_pool = True
         self._pool_ok = {}
+        # the fast forward also runs a layers1 1x1 unit in the epilogue of the conv before it wherever the library accepts that pair
+        # (layers1.4 -> 1.5 at 416x416), so the producer's output never goes to HBM; False keeps the separate launches
+        self.fuse_chain = True
+        self._chain_ok = {}
+
+    def _chained_form(self, u, v, x, conv_flags):
+        """Whether the library runs unit u on input x [B,H,W,C] with the 1x1 unit v fused into its epilogue, with the same bits as v's
+        own launch (which must not split along K), asked once per shape."""
+        b, h, w, _ = x.shape
+        key = (u.cin, u.cout, u.ksize, v.cout, b, h, w, conv_flags)
+        ok = self._chain_ok.get(key)
+        if ok is None:
+            ok = v.ksize == 1 and v.cin == u.cout and v.cout <= 64 and v.cout % 8 == 0
+            if ok:
+                try:
+                    ok = (ops.conv_choice(b, h, w, u.cin, u.cout, u.ksize, flags=conv_flags | ops.CONV_CHAIN1X1)['kernel'] == 'conv_wide_kernel'
+                          and not ops.conv_choice(b, h, w, v.cin, v.cout, 1, flags=conv_flags)['streamk'])
+                except RuntimeError:
+                    ok = False
+            self._chain_ok[key] = ok
+        return ok
 
     def _pooled_form(self, u, x, conv_flags):
         """Whether the library runs unit u on input x [B,H,W,C] with the 2x2 max-pool fused on the two-consumer tile (asked once per shape)."""
@@ -308,7 +329,22 @@ class DarknetEngine(object):
             collect['layers1.0(pooled)'] = cur
         x1 = None
         last1 = self.units1[-1]
-        for u, (out, pooled), key in zip(self.units1[1:], p.l1, self._k1[1:]):
+        l1 = list(zip(self.units1[1:], p.l1, self._k1[1:]))
+        chained = False         # this unit already ran in the previous launch's epilogue
+        for i, (u, (out, pooled), key) in enumerate(l1):
+            if chained:
+                x1 = out
+                cur = ops.maxpool2x2(out, out=pooled) if pooled is not None else out
+                chained = False
+                continue
+            # a 1x1 unit that reads only this unit's output (layers1.5 after 1.4 at 416x416) runs in this launch's epilogue
+            if (self.fuse_chain and pooled is None and collect is None and not ref and i + 1 < len(l1)
+                    and self._chained_form(u, l1[i + 1][0], cur, conv_flags)):
+                v, (v_out, _), _ = l1[i + 1]
+                ops.conv_bn_act(cur, u.w16, u.scale, u.shift, u.slope, out=v_out, flags=conv_flags, workspace=p.workspace,
+                                chain=(v.w16, v.scale, v.shift, v.slope))
+                chained = True
+                continue
             # layers1.2 (3x3, Cin = 32) has a kernel whose epilogue applies the MaxPool2d that follows it, so the
             # 208x208x64 activation never goes to HBM, and so do the 3x3 layers on the two-consumer tile (layers1.6 and 1.10 at
             # 416x416); tests that inspect every layer (collect / ref) keep the two steps.  last1's full-resolution output feeds the

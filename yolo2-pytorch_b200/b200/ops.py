@@ -10,7 +10,7 @@ from . import lib as _l
 OUT_F16_NHWC, OUT_F32_NCHW = 0, 1
 CONV_A_TILED, CONV_WIDE_N = 1, 2
 CONV_NO_STREAMK, CONV_FORCE_STREAMK, CONV_NO_SMALLK, CONV_PLAIN_STORE = 8, 1 << 30, 1 << 28, 1 << 29
-CONV_POOL2X2, CONV_C32_IM2COL, CONV_C32_SWAP = 16, 32, 64
+CONV_POOL2X2, CONV_C32_IM2COL, CONV_C32_SWAP, CONV_CHAIN1X1 = 16, 32, 64, 128
 FILTER_THRESHOLD, FILTER_FIX, FILTER_NONE = 0, 1, 2
 
 
@@ -164,24 +164,30 @@ CONV_KERNELS = ('conv_igemm_kernel', 'conv_wide_kernel', 'conv_c32_kernel')
 
 def conv_choice(batch, height, width, cin, cout, k, out_mode=OUT_F16_NHWC, flags=0, workspace=True):
     """The kernel and tile shape conv_bn_act picks for this shape (the library's own selection, yb_conv_choice).  `pooled`: the launch
-    applies the fused 2x2 max-pool (CONV_POOL2X2; the library refuses the flag where it has no pooled form)."""
+    applies the fused 2x2 max-pool (CONV_POOL2X2; the library refuses the flag where it has no pooled form).  `chained`: the launch runs
+    the following 1x1 unit in its epilogue (CONV_CHAIN1X1, conv_bn_act's `chain`; refused where this conv cannot be its producer)."""
     out = (ctypes.c_int * 6)()
     _l.check(_l.load().yb_conv_choice(batch, height, width, cin, cout, k, out_mode, flags, int(bool(workspace)), ctypes.byref(out)),
              'yb_conv_choice')
     return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5],
-                pooled=bool(flags & CONV_POOL2X2))
+                pooled=bool(flags & CONV_POOL2X2), chained=bool(flags & CONV_CHAIN1X1))
 
 
-def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, ref=False, workspace=None):
+def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, ref=False, workspace=None,
+                chain=None):
     """x: fp16 [B,H,W,x_ld] (uses the first `cin` channels, default all); w: fp16 [Cout,k,k,Cin].
     out (fp16): [B,H,W,y_ld] written at channels [y_ch_off, y_ch_off+Cout); out (fp32): [B,Cout,H,W].
-    flags & CONV_POOL2X2: the 2x2 max-pool is fused, out is [B,H/2,W/2,y_ld]."""
+    flags & CONV_POOL2X2: the 2x2 max-pool is fused, out is [B,H/2,W/2,y_ld].
+    chain = (w2, scale2, shift2, slope2): the 1x1 unit that reads this conv's output runs in the same launch (yb_conv_bn_act_chain_fwd),
+    w2 fp16 [Cout2,1,1,Cout]; out is that unit's fp16 output [B,H,W,y_ld] at channels [y_ch_off, y_ch_off+Cout2)."""
     _req(x, torch.float16, 'x'); _req(w, torch.float16, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
     b, h, wd, x_ld = x.shape
     cout, k, _, wcin = w.shape
     cin = wcin if cin is None else cin
     if cin != wcin:
         raise ValueError('weight Cin %d != %d' % (wcin, cin))
+    if chain is not None:
+        return _conv_chain(x, w, scale, shift, slope, chain, out, out_mode, y_ch_off, cin, flags, ref, workspace)
     if out is None:
         oh, ow = (h // 2, wd // 2) if (flags & CONV_POOL2X2) else (h, wd)
         out = (torch.empty(b, oh, ow, cout, dtype=torch.float16, device=x.device) if out_mode == OUT_F16_NHWC
@@ -203,6 +209,30 @@ def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch
     return out
 
 
+def _conv_chain(x, w, scale, shift, slope, chain, out, out_mode, y_ch_off, cin, flags, ref, workspace):
+    w2, scale2, shift2, slope2 = chain
+    _req(w2, torch.float16, 'w2'); _req(scale2, torch.float32, 'scale2'); _req(shift2, torch.float32, 'shift2')
+    b, h, wd, x_ld = x.shape
+    cout, k = w.shape[0], w.shape[1]
+    cout2 = w2.shape[0]
+    if tuple(w2.shape) != (cout2, 1, 1, cout) or scale2.numel() != cout2 or shift2.numel() != cout2:
+        raise ValueError('conv_bn_act chain: w2 must be [Cout2,1,1,%d] with Cout2 scales / shifts, got %s' % (cout, tuple(w2.shape)))
+    if ref or out_mode != OUT_F16_NHWC:
+        raise ValueError('conv_bn_act chain: the fused form has fp16 NHWC output and no CUDA-core reference')
+    if out is None:
+        out = torch.empty(b, h, wd, cout2, dtype=torch.float16, device=x.device)
+    _req(out, torch.float16, 'out')
+    if out.dim() != 4 or tuple(out.shape[:3]) != (b, h, wd) or y_ch_off < 0 or y_ch_off + cout2 > out.shape[-1]:
+        raise ValueError('conv_bn_act chain: out must be [%d,%d,%d,y_ld] with y_ch_off + Cout2 <= y_ld, got %s at y_ch_off %d'
+                         % (b, h, wd, tuple(out.shape), y_ch_off))
+    if workspace is not None:
+        _req(workspace, torch.uint8, 'workspace')
+    _ck(_l.load().yb_conv_bn_act_chain_fwd(_p(x), _p(w), _p(scale), _p(shift), float(slope), _p(w2), _p(scale2), _p(shift2), float(slope2),
+                                           _p(out), b, h, wd, cin, cout, cout2, k, x_ld, out.shape[-1], y_ch_off, flags, _p(workspace),
+                                           0 if workspace is None else workspace.numel(), _s()), 'yb_conv_bn_act_chain_fwd')
+    return out
+
+
 def conv2d_out_size(size, k, stride, pad):
     return (size + 2 * pad - k) // stride + 1
 
@@ -213,7 +243,7 @@ def conv2d_choice(batch, height, width, cin, cout, kh, kw, stride=1, pad=(0, 0),
     _l.check(_l.load().yb_conv2d_choice(batch, height, width, cin, cout, kh, kw, stride, pad[0], pad[1], out_mode, flags, int(bool(workspace)),
                                         ctypes.byref(out)), 'yb_conv2d_choice')
     return dict(kernel=CONV_KERNELS[out[0]], bk=out[1], bn=out[2], rows=out[3], streamk=bool(out[4]), grid=out[5],
-                pooled=bool(flags & CONV_POOL2X2))
+                pooled=bool(flags & CONV_POOL2X2), chained=bool(flags & CONV_CHAIN1X1))
 
 
 def conv2d_bn_act(x, w, scale, shift, slope, stride=1, pad=(0, 0), out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, cin=None, flags=0, workspace=None):

@@ -135,7 +135,7 @@ int dw_wgrad(const void*, const void*, float*, int, int, int, int, int, cudaStre
 int mb_conv0_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
 int conv2d_choice(int, int, int, int, int, int, int, int, int, int, int, int, int, int*);
 int conv2d_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, int, int, int, int,
-                   long long, int, int, int, void*, long long, double*, int, int, const float*, const float*, int, cudaStream_t);
+                   long long, int, int, int, void*, long long, double*, int, int, const float*, const float*, int, const ConvChain*, cudaStream_t);
 int pack_weight_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
 int stem3x3_s2(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
 int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
@@ -224,6 +224,15 @@ int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, cons
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
   return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, x_ld, y_ld, y_ch_off, out_mode,
                                 flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, S(stream));
+}
+
+int yb_conv_bn_act_chain_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, const void* w2, const float* scale2,
+                             const float* shift2, float slope2, void* y, int batch, int height, int width, int cin, int cout, int cout2, int ksize,
+                             int x_ld, long long y_ld, int y_ch_off, int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
+  if (ksize != 1 && ksize != 3) return yb::fail(YB_ERR_BAD_ARG, "conv chain: ksize %d unsupported (1 or 3)", ksize);
+  const yb::ConvChain chain{w2, scale2, shift2, slope2, cout2};
+  return yb::conv2d_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, ksize, 1, (ksize - 1) / 2, (ksize - 1) / 2, x_ld,
+                            y_ld, y_ch_off, YB_OUT_F16_NHWC, flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, &chain, S(stream));
 }
 
 int yb_conv_bn_act_split_fwd(const void* x, const void* w_split, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -546,7 +555,7 @@ int yb_conv2d_bn_act_fwd(const void* x, const void* w, const float* scale, const
                          int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                          int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
   return yb::conv2d_forward(x, w, scale, shift, slope, y, batch, in_h, in_w, cin, cout, kh, kw, stride, pad_h, pad_w, x_ld, y_ld, y_ch_off, out_mode,
-                            flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, S(stream));
+                            flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, nullptr, S(stream));
 }
 
 int yb_conv2d_choice(int batch, int in_h, int in_w, int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int out_mode, int flags,

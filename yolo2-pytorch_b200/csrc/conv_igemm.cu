@@ -69,6 +69,12 @@ struct ConvParams {
   // one lane ships them with a single bulk store, instead of per-thread 16 B stores that write 32 half-used sectors per instruction
   // (lanes = pixels, 2*y_ld bytes apart).
   int tma_store;
+  // chained form (conv_wide_chain_kernel): the 1x1 unit that consumes this conv's output inside the tile -- its scale / shift /
+  // slope and Cout; y / tmap_y are that unit's output
+  const float* scale2;
+  const float* shift2;
+  float slope2;
+  int cout2;
 };
 
 // role 0 = TMA producer, 1 = MMA issuer, 2 = epilogue thread 0; slot = running event index of that role
@@ -714,13 +720,19 @@ struct WideCfg {
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static constexpr int kWsFloats = kWideRows * kWideBN;         // one CTA's stream-K partial tile
   static_assert(kStages >= (BK == 64 ? 4 : 8), "shared memory budget: the epilogue's slices and table must not cost a pipeline stage");
+  // chained form: the second unit's scale / shift table (float4 per column pair of its 64 channels) after the barriers
+  static constexpr int kChainTableBytes = 64 * 2 * 4;
+  static constexpr int kChainSmemBytes = kSmemBytes + kChainTableBytes;
+  static_assert(kChainSmemBytes <= kSmemLimit, "shared memory budget: the chained form must not cost a pipeline stage");
 };
+constexpr int kChainN = 64;       // chained form: output channels of the second (1x1) unit per tile
 
-// kPool: the pooled form (conv_wide_pool_kernel), see below.  tmap_a[0] is the A map of the plain form; the pooled form reads one map
-// per pool-window position.
-template <int BK, bool kPool>
+// kPool: the pooled form (conv_wide_pool_kernel), kChain: the chained form (conv_wide_chain_kernel), see below.  tmap_a[0] is the A map
+// of the plain form; the pooled form reads one map per pool-window position.  tmap_w2: the chained form's second weight.
+template <int BK, bool kPool, bool kChain>
 __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a)[4], const CUtensorMap& tmap_b, const CUtensorMap& tmap_y,
-                                               const ConvParams p) {
+                                               const CUtensorMap* tmap_w2, const ConvParams p) {
+  static_assert(!(kPool && kChain), "one fused epilogue at a time");
   using Cfg = WideCfg<BK>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -733,6 +745,10 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
   const uint32_t bar_empty = bar_full + 8 * kStages;                      // [kStages]
   const uint32_t bar_slice_full = bar_empty + 8 * kStages;                // [2 consumers]: a 64-row half is staged
   const uint32_t bar_slice_empty = bar_slice_full + 16;                   // [2 consumers]: its stores have read the slice
+  // chained form: the second unit's [64][128] fp16 weight is resident as two K-blocks of [64 rows][128 B] (128B-swizzled), in the
+  // upper 8 KB of consumer kb2's staging slice -- its 64-channel output only uses the lower half.  One load per CTA on bar_w.
+  const uint32_t bar_w = bar_slice_empty + 16;
+  const uint32_t table2 = table + Cfg::kTableBytes + 256;                 // [kChainN / 2] float4
   const int num_tiles = p.m_tiles * p.n_tiles;
   const int unit_id = static_cast<int>(blockIdx.x);
   const int num_units = static_cast<int>(gridDim.x);
@@ -747,6 +763,7 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
       if constexpr (kPool) mbar_init(bar_slice_empty + 8 * c, c == 1 ? 4 : 1);   // pooled: consumer 1's slice is read by consumer 0's warps
       else mbar_init(bar_slice_empty + 8 * c, 1);          // its store thread
     }
+    if constexpr (kChain) mbar_init(bar_w, 1);
     fence_mbar_init();
     fence_proxy_async_smem();
     tma_prefetch_desc(tmap_a[0]);
@@ -755,6 +772,7 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
     }
     tma_prefetch_desc(&tmap_b);
     tma_prefetch_desc(&tmap_y);
+    if constexpr (kChain) tma_prefetch_desc(tmap_w2);
   }
   __syncthreads();
   pdl_trigger();
@@ -767,6 +785,10 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
       int stage = 0;
       uint32_t phase = 0;
       int tr_p = 0;
+      if constexpr (kChain) {
+        mbar_arrive_expect_tx(bar_w, 2 * kChainN * 128);    // rows >= Cout2 are zero-filled and still counted
+        for (int kb2 = 0; kb2 < 2; ++kb2) tma_load_2d(smem_o + kb2 * Cfg::kOutBytes + 8192, tmap_w2, bar_w, kb2 * 64, 0);
+      }
       for (WorkIter it(p, unit_id, num_units, num_tiles); it.valid(); it.next()) {
         const int n_tile = it.tile % p.n_tiles;
         const int m_cta = (it.tile / p.n_tiles) * (kPool ? kWidePoolRows : kWideRows);
@@ -813,8 +835,8 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
         for (int h = 0; h < (kPool ? 1 : 2); ++h) {
           mbar_wait(bar_slice_full + 8 * c, sph, p.dbg, 0x900 | c);
 #pragma unroll
-          for (int c2 = 0; c2 < 2; ++c2) {
-            if (n0 + c2 * 64 < p.cout) {
+          for (int c2 = 0; c2 < (kChain ? 1 : 2); ++c2) {       // chained: the 64 channels of the second unit
+            if (kChain || n0 + c2 * 64 < p.cout) {
 #pragma unroll
               for (int g = 0; g < 2; ++g) {
                 const int row = m_base + h * 64 + g * 32;
@@ -846,6 +868,15 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
   int stage = 0;
   uint32_t phase = 0;
   uint32_t sph = 0;                            // staging slice phase
+  if constexpr (kChain) {
+    // the second unit's table, once per CTA (read after the first tile's table barriers): entry te < 128 is column pair te / 4,
+    // {scale, scale, shift, shift}[te % 4]
+    if (te < 2 * kChainN) {
+      const int col = 2 * (te >> 2) + (te & 1);
+      const float v = col < p.cout2 ? __ldg(((te & 2) ? p.shift2 : p.scale2) + col) : 0.f;
+      asm volatile("st.shared.f32 [%0], %1;" :: "r"(table2 + 4 * te), "f"(v) : "memory");
+    }
+  }
   // trace (yb_conv_set_trace; block 0, consumer 0's first thread), tile i of the CTA: role 1 slot 2i = its last full-barrier wait,
   // 2i + 1 = its first wgmma issue; role 2 slot 2i = its K-loop end (every MMA retired), 2i + 1 = its epilogue end.  tr_t = 2i
   int tr_t = 0;
@@ -855,8 +886,8 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
     const int n0 = (tile % p.n_tiles) * kWideBN;
     // stream-K roles of this segment: it stops short of the tile's last K-block (dump the partial sums), or finishes a tile whose
     // first K-blocks were summed by lower-numbered CTAs (collect their partials first)
-    const bool sk_dump = it.kb1 < p.num_kb;
-    const bool sk_collect = !sk_dump && it.kb0 > 0;
+    const bool sk_dump = !kChain && it.kb1 < p.num_kb;      // the chained form has no stream-K
+    const bool sk_collect = !kChain && !sk_dump && it.kb0 > 0;
     float tab = 0.f;                           // table entry te: column pair te / 4, {scale, scale, shift, shift}[te % 4]
     {
       const int col = n0 + 2 * (te >> 2) + (te & 1);
@@ -939,13 +970,56 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
     // per-thread partial layout: float4 g of thread t of consumer cw at ((cw * 32 + g) * 128 + t) * 4 -- coalesced both ways;
     // g / 16 is the accumulator row half h
     uint32_t pk_dx0[kPool ? 32 : 1];           // pooled form: the converted h = 0 half (window column dx = 0), kept for the dx max
+    // chained form: converted half h is the register A operand of the second GEMM into acc2[h]; it stays live until that GEMM retires
+    uint32_t pk_a[kChain ? 2 : 1][kChain ? 32 : 1];
+    float acc2[kChain ? 2 : 1][kChain ? 32 : 1];
+    // chained form: scale / shift, leaky, fp16 of the second unit for one 64-row half, staged for its 64-channel store
+    auto chain_store = [&](const float (&d)[kChain ? 32 : 1]) {
+      if constexpr (kChain) {
+        const float4* tab2 = reinterpret_cast<const float4*>(smem_raw + (table2 - smem_u32(smem_raw)));
+        uint32_t pk2[16];
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const float4 ss = tab2[4 * jj + (lane & 3)];
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            float x0 = d[4 * jj + 2 * hh] * ss.x + ss.z;
+            float x1 = d[4 * jj + 2 * hh + 1] * ss.y + ss.w;
+            x0 = x0 > 0.f ? x0 : x0 * p.slope2;
+            x1 = x1 > 0.f ? x1 : x1 * p.slope2;
+            __half2 v = __floats2half2_rn(x0, x1);
+            pk2[2 * jj + hh] = *reinterpret_cast<uint32_t*>(&v);
+          }
+        }
+        mbar_wait(bar_slice_empty + 8 * cw, sph ^ 1, p.dbg, 0xA00 | cw);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = warp * 16 + (lane >> 2) + hh * 8;
+            const uint32_t addr = slice + r * 128 + ((jj ^ (r & 7)) << 4) + 4 * (lane & 3);
+            asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(pk2[2 * jj + hh]) : "memory");
+          }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_slice_full + 8 * cw);
+        sph ^= 1;
+      }
+    };
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (h == 1) {
-        wgmma_wait<0>();
+        wgmma_wait<0>();                       // chained: also the second GEMM of rows 0..63, committed after these MMAs
         fence_regs(acc[1]);
         if (leader) YB_TRACE(2, tr_t);
         release_prev();
+        if constexpr (kChain) {
+          // rows 0..63 of the second unit go out before rows 64..127 are converted (keeping both halves' second-GEMM operands live
+          // at once would spill); the last stage is already back with the producer
+          fence_regs(acc2[0]);
+          fence_regs_u32(pk_a[0]);
+          chain_store(acc2[0]);
+        }
       }
       if (sk_dump) {
         float4* dst = reinterpret_cast<float4*>(p.ws + static_cast<size_t>(blockIdx.x) * Cfg::kWsFloats) + (cw * 32 + 16 * h) * 128 + t;
@@ -1009,6 +1083,28 @@ __device__ __forceinline__ void conv_wide_body(const CUtensorMap* const (&tmap_a
           if (lane == 0) mbar_arrive(bar_slice_empty + 8);
         }
       }
+      if constexpr (kChain) {
+        // the 1x1 unit that follows: its 128 input channels of these 64 rows are pk, which is exactly the A fragment of an
+        // m64 x 16 step -- k-step kk (channels 16 kk .. 16 kk + 15) is pk[4 kk .. 4 kk + 3].  The k16 steps run in channel order
+        // from scale-d = 0, as in the plain launch of that unit.
+#pragma unroll
+        for (int i = 0; i < 32; ++i) pk_a[h][i] = pk[i];
+        mbar_wait(bar_w, 0, p.dbg, 0xC00);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const uint32_t a[4] = {pk_a[h][4 * kk], pk_a[h][4 * kk + 1], pk_a[h][4 * kk + 2], pk_a[h][4 * kk + 3]};
+          const uint64_t bdesc = make_kmajor_desc<128>(smem_o + (kk >> 2) * Cfg::kOutBytes + 8192) + 2 * (kk & 3);
+          wgmma_f16_rs_n64(acc2[h], a, bdesc, kk != 0);
+        }
+        wgmma_commit();
+        if (h == 0) continue;                  // rows 0..63's second GEMM queues behind the MMAs of rows 64..127
+        wgmma_wait<0>();
+        fence_regs(acc2[1]);
+        fence_regs_u32(pk_a[1]);
+        chain_store(acc2[1]);
+        continue;
+      }
       // the slice is free once the store thread (pooled, consumer 1: consumer 0) has seen the previous half's stores read it
       mbar_wait(bar_slice_empty + 8 * cw, sph ^ 1, p.dbg, 0xA00 | cw);
 #pragma unroll
@@ -1046,7 +1142,7 @@ __global__ void __launch_bounds__(kWideThreads, 1)
 conv_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
   const CUtensorMap* const ta[4] = {&tmap_a, &tmap_a, &tmap_a, &tmap_a};
-  conv_wide_body<BK, false>(ta, tmap_b, tmap_y, p);
+  conv_wide_body<BK, false, false>(ta, tmap_b, tmap_y, nullptr, p);
 }
 
 // The same tile with the 2x2 max-pool that follows a 3x3 same-padded layer fused into its epilogue (YB_CONV_POOL2X2): a tile is 64 pool
@@ -1062,7 +1158,22 @@ conv_wide_pool_kernel(const __grid_constant__ CUtensorMap tmap_a0, const __grid_
                       const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_a3,
                       const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_y, const ConvParams p) {
   const CUtensorMap* const ta[4] = {&tmap_a0, &tmap_a1, &tmap_a2, &tmap_a3};
-  conv_wide_body<BK, true>(ta, tmap_b, tmap_y, p);
+  conv_wide_body<BK, true, false>(ta, tmap_b, tmap_y, nullptr, p);
+}
+
+// The same tile with the 1x1 unit that follows the layer run in its epilogue (YB_CONV_CHAIN1X1): after a 64-row half of the tile is
+// converted to fp16, its 128 channels (the layer's whole Cout, one N tile) are the A operand of a second GEMM against the unit's
+// [Cout2 <= 64][128] weight, straight from the registers.  Only that unit's scale / shift / leaky output is stored; the layer's own
+// output never leaves the SM.  The second GEMM runs the same k16 steps in the same channel order from scale-d = 0 on the same fp16
+// operands as the unit's plain launch, and the epilogue arithmetic is the same, so the result equals conv_wide_kernel followed by
+// the unit's launch bit for bit.  BK = 64, no stream-K.
+template <int BK>
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_wide_chain_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                       const __grid_constant__ CUtensorMap tmap_y, const __grid_constant__ CUtensorMap tmap_w2, const ConvParams p) {
+  static_assert(BK == 64, "chained form: instantiated for producers with Cin % 64 == 0 only (conv_choose refuses the others)");
+  const CUtensorMap* const ta[4] = {&tmap_a, &tmap_a, &tmap_a, &tmap_a};
+  conv_wide_body<BK, false, true>(ta, tmap_b, tmap_y, &tmap_w2, p);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1341,7 +1452,9 @@ constexpr int kKernelC32 = 2;        // conv_c32_kernel (3x3, Cin = 32 halo tile
 struct ConvChoice {
   int kernel, bk, bn, mt, streamk, grid;
   int pool;        // the 2x2 max-pool is fused (conv_c32_kernel, conv_wide_pool_kernel)
+  int chain;       // the following 1x1 unit is fused (conv_wide_chain_kernel)
 };
+constexpr int kFlagChain = 1 << 7;   // YB_CONV_CHAIN1X1
 
 static unsigned long long* g_conv_trace = nullptr;
 void conv_set_trace(void* dev_ptr) { g_conv_trace = static_cast<unsigned long long*>(dev_ptr); }
@@ -1457,6 +1570,19 @@ static int launch_wide_pool(const CUtensorMap (&ta)[4], const CUtensorMap& tb, c
   return check_launch("conv_wide_pool_kernel");
 }
 
+// the chained form: ty is the second unit's output, tw2 its weight
+static int launch_wide_chain(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, const CUtensorMap& tw2, const ConvParams& p,
+                             int grid, cudaStream_t stream) {
+  using Cfg = WideCfg<64>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    YB_CUDA(cudaFuncSetAttribute(conv_wide_chain_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kChainSmemBytes));
+    attr_set = true;
+  }
+  conv_wide_chain_kernel<64><<<grid, kWideThreads, Cfg::kChainSmemBytes, stream>>>(ta, tb, ty, tw2, p);
+  return check_launch("conv_wide_chain_kernel");
+}
+
 // CTA tile shapes (BLOCK_N, M-subtiles): the one-warpgroup kernel keeps MT * BLOCK_N <= 128 accumulators per thread; 128 x 2 is
 // the two-consumer kernel
 // the two-consumer shape has no pre-activation form (conv_choose never picks it when `pre` is set)
@@ -1559,7 +1685,8 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int kh, int
   const bool same3x3 = kh == 3 && kw == 3 && stride == 1 && pad_h == 1 && pad_w == 1;
   const bool im2col_cost = !(kh == 1 && kw == 1 && stride == 1);
   // 3x3 same-padded stride 1, Cin = 32, Cout <= 64 (layers1.2): halo-tile kernel unless a test asks for one of the im2col kernels
-  if (!split && cin == 32 && same3x3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 8) & 0xFFFF) == 0) {
+  if (!split && cin == 32 && same3x3 && cout <= 64 && out_mode == 0 && ((flags >> 28) & 1) == 0 && ((flags >> 5) & 1) == 0 && ((flags >> 7) & 1) == 0 &&
+      ((flags >> 8) & 0xFFFF) == 0) {
     const long long tiles = static_cast<long long>(batch) * ((width + C32Cfg::TW - 1) / C32Cfg::TW) * ((height + C32Cfg::TH - 1) / C32Cfg::TH);
     c.kernel = kKernelC32; c.bk = 32; c.bn = C32Cfg::BN; c.mt = 1; c.pool = (flags >> 4) & 1;
     c.grid = static_cast<int>(tiles < sms ? tiles : sms);
@@ -1575,7 +1702,15 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int kh, int
     if ((flags >> 30) & 1) return fail(YB_ERR_UNSUPPORTED, "conv: the fused 2x2 max-pool has no stream-K form");
   }
   const int bk = (cin % 64 == 0 && a_channels % 64 == 0) ? 64 : 32;     // K-blocks never straddle the wrap point
-  const bool sk_possible = !stats && !pool && workspace_ok && (flags & 8) == 0;
+  // the following 1x1 unit fused into the epilogue: the two-consumer tile whose one N tile is the layer's whole Cout = 128
+  const bool chain = (flags >> 7) & 1;
+  if (chain) {
+    if (!(out_mode == 0 && !split && !stats && !pre && !pool && bk == 64 && cout == kWideBN))
+      return fail(YB_ERR_UNSUPPORTED, "conv: YB_CONV_CHAIN1X1 needs Cout = %d, Cin %% 64 == 0, fp16 NHWC output, plain operands and no fused "
+                                      "pool (Cout %d, Cin %d)", kWideBN, cout, cin);
+    if ((flags >> 30) & 1) return fail(YB_ERR_UNSUPPORTED, "conv: the chained form has no stream-K form");
+  }
+  const bool sk_possible = !stats && !pool && !chain && workspace_ok && (flags & 8) == 0;
   const bool sk_force = sk_possible && ((flags >> 30) & 1);
   // the two-consumer kernel: fp16 NHWC through the TMA store, no residual output, statistics or profiling ablation
   // (the pre-activation form exists only for the one-warpgroup kernel)
@@ -1631,6 +1766,10 @@ int conv_choose(int batch, int height, int width, int cin, int cout, int kh, int
     return fail(YB_ERR_UNSUPPORTED, "conv: the fused 2x2 max-pool runs on the 256 x 128 two-consumer tile only; this launch takes %d x %d tiles",
                 BM * c.mt, c.bn);
   c.pool = pool;
+  if (chain && c.kernel != kKernelWide)
+    return fail(YB_ERR_UNSUPPORTED, "conv: the chained form runs on the 256 x 128 two-consumer tile only; this launch takes %d x %d tiles",
+                BM * c.mt, c.bn);
+  c.chain = chain;
   const long long tiles = ((m_total + BM * c.mt - 1) / (BM * c.mt)) * ((cout + c.bn - 1) / c.bn);
   c.grid = c.streamk ? sms : static_cast<int>(tiles < sms ? tiles : sms);      // sk_base / sk_rem are computed for exactly sms CTAs
   *out = c;
@@ -1674,8 +1813,18 @@ int conv_choice(int batch, int height, int width, int cin, int cout, int ksize, 
 int conv2d_forward(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch, int in_h, int in_w,
                    int cin, int cout, int kh, int kw, int stride, int pad_h, int pad_w, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                    int flags, void* workspace, long long workspace_bytes, double* stats, int a_channels, int lo_ch_off,
-                   const float* pre_scale, const float* pre_shift, int pre_relu, cudaStream_t stream) {
+                   const float* pre_scale, const float* pre_shift, int pre_relu, const ConvChain* chain, cudaStream_t stream) {
   YB_REQUIRE(x && w && scale && shift && y, "conv: null pointer");
+  // the chained form: y is the second unit's output, Cout2 channels at y_ch_off
+  if (chain != nullptr) flags |= kFlagChain;
+  YB_REQUIRE(chain != nullptr || !(flags & kFlagChain), "conv: YB_CONV_CHAIN1X1 needs the second unit (yb_conv_bn_act_chain_fwd)");
+  if (chain != nullptr) {
+    YB_REQUIRE(chain->w && chain->scale && chain->shift && (reinterpret_cast<uintptr_t>(chain->w) & 15) == 0,
+               "conv chain: null or misaligned second-unit operand");
+    YB_REQUIRE(chain->cout > 0 && chain->cout <= kChainN && chain->cout % 8 == 0, "conv chain: the second unit's Cout=%d (8 .. %d, multiple of 8)",
+               chain->cout, kChainN);
+  }
+  const int y_cout = chain != nullptr ? chain->cout : cout;
   YB_REQUIRE(batch > 0, "conv: bad shape");
   int height = 0, width = 0;      // output dims
   int rc = conv_geometry(in_h, in_w, kh, kw, stride, pad_h, pad_w, &height, &width);
@@ -1702,7 +1851,7 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
   YB_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0, "conv: x/w must be 16B aligned");
   YB_REQUIRE(out_mode == 0 || out_mode == 1, "conv: out_mode");
   if (out_mode == 0) {
-    YB_REQUIRE(cout % 8 == 0 && y_ld % 8 == 0 && y_ch_off % 8 == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0,
+    YB_REQUIRE(y_cout % 8 == 0 && y_ld % 8 == 0 && y_ch_off % 8 == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0,
                "conv: fp16 NHWC output needs Cout, y_ld, y_ch_off multiples of 8 and a 16B aligned pointer");
   }
   const long long m_total_ll = static_cast<long long>(batch) * height * width;
@@ -1753,6 +1902,8 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
   p.a_wrap = a_channels;
   p.lo_off = lo_ch_off >= 0 ? static_cast<long long>(lo_ch_off - y_ch_off) : 0;
   p.sk_base = 0; p.sk_rem = 0; p.ws = nullptr; p.flags = nullptr;
+  p.scale2 = chain ? chain->scale : nullptr; p.shift2 = chain ? chain->shift : nullptr;
+  p.slope2 = chain ? chain->slope : 0.f; p.cout2 = chain ? chain->cout : 0;
   if (streamk) {
     const long long units = static_cast<long long>(p.m_tiles) * p.n_tiles * p.num_kb;
     YB_REQUIRE(units < (1ll << 31), "conv: stream-K unit count overflows");
@@ -1818,13 +1969,25 @@ int conv2d_forward(const void* x, const void* w, const float* scale, const float
   memset(&ty, 0, sizeof(ty));
   p.tma_store = (out_mode == 0 && lo_ch_off < 0 && ((flags >> 29) & 1) == 0) ? 1 : 0;
   if (p.tma_store) {
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cout), static_cast<cuuint64_t>(p.m_total)};
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(y_cout), static_cast<cuuint64_t>(p.m_total)};
     const cuuint64_t strides[1] = {static_cast<cuuint64_t>(y_ld) * 2};
     const cuuint32_t box[2] = {64, 32};                 // one epilogue warp's rows
     const cuuint32_t estr[2] = {1, 1};
     cr = enc_tiled(&ty, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, static_cast<__half*>(y) + y_ch_off, dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
+  }
+  if (ch.chain) {
+    // the second unit's weight [Cout2][Cin2 = 128] as two 64-channel K-blocks of 64 rows (rows >= Cout2 zero-filled)
+    alignas(64) CUtensorMap tw2;
+    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cout), static_cast<cuuint64_t>(chain->cout)};
+    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cout) * 2};
+    const cuuint32_t box[2] = {64, static_cast<cuuint32_t>(kChainN)};
+    const cuuint32_t estr[2] = {1, 1};
+    cr = enc_tiled(&tw2, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(chain->w), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(W2) failed (%d)", static_cast<int>(cr));
+    return launch_wide_chain(ta, tb, ty, tw2, p, ch.grid, stream);
   }
   if (pooled) return bk == 64 ? launch_wide_pool<64>(ta_pos, tb, ty, p, ch.grid, stream) : launch_wide_pool<32>(ta_pos, tb, ty, p, ch.grid, stream);
   if (bk == 64) return dispatch_conv<64>(bn, mt, ch.grid, ta, tb, ty, p, pre ? &pre_act : nullptr, stream);
@@ -1838,7 +2001,8 @@ int conv_igemm_forward(const void* x, const void* w, const float* scale, const f
                        const float* pre_scale, const float* pre_shift, int pre_relu, cudaStream_t stream) {
   YB_REQUIRE(ksize == 1 || ksize == 3, "conv: ksize %d unsupported (1 or 3)", ksize);
   return conv2d_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, ksize, 1, (ksize - 1) / 2, (ksize - 1) / 2, x_ld, y_ld,
-                        y_ch_off, out_mode, flags, workspace, workspace_bytes, stats, a_channels, lo_ch_off, pre_scale, pre_shift, pre_relu, stream);
+                        y_ch_off, out_mode, flags, workspace, workspace_bytes, stats, a_channels, lo_ch_off, pre_scale, pre_shift, pre_relu, nullptr,
+                        stream);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -16,6 +16,15 @@ int fail(int code, const char* fmt, ...);
 int check_launch(const char* what);   // cudaGetLastError() -> code + message
 int sm_count();                // cached multiProcessorCount of the current device
 int* debug_word_device();      // host-mapped int[4] (device pointer), nullptr if unavailable
+// the 1x1 unit a conv launch runs in its epilogue (yb_conv_bn_act_chain_fwd): fp16 weight [cout][Cin2 = the conv's Cout], its
+// scale / shift / leaky slope
+struct ConvChain {
+  const void* w;
+  const float* scale;
+  const float* shift;
+  float slope;
+  int cout;
+};
 }  // namespace yb
 
 #define YB_REQUIRE(cond, ...)                                   \

@@ -214,6 +214,24 @@ __device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t adesc, 
       : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(kTransA), "n"(kTransB));
 }
 
+// The same m64n64k16 step with A from registers: a[0..3] is thread t's fragment of the 64 x 16 A tile, laid out like the
+// accumulator of an m64 x 16 MMA converted to fp16 pairs -- a[0] / a[1] rows l / 4 and l / 4 + 8 (of warp w's 16 rows), columns
+// 2 (l % 4) + {0, 1}; a[2] / a[3] the same rows, columns 8 + 2 (l % 4) + {0, 1}.  B is K-major from shared memory.  The registers
+// are read asynchronously: they must not change before the wgmma_wait that retires this MMA.
+__device__ __forceinline__ void wgmma_f16_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+// keeps register operands of in-flight MMAs live (and unmoved) up to the wgmma_wait that retires them
+template <int R>
+__device__ __forceinline__ void fence_regs_u32(uint32_t (&r)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(r[i]) :: "memory");
+}
+
 // D(64 x N) dispatch on the compile-time N
 template <int N, int kTransA = 0, int kTransB = 0>
 __device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
