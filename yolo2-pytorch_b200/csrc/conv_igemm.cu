@@ -1183,9 +1183,10 @@ conv_wide_chain_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 // [pixel][16 B].  In that layout a 3x3 tap is just a shifted window: 8 consecutive pixels of a halo row form one 8 x 16 B
 // core matrix of the un-swizzled K-major operand format, the next output row is +10 pixels (SBO = 160 B) and the second
 // K chunk is the next plane (LBO), so wgmma reads all nine taps straight out of the halo tile by moving the
-// descriptor's start address by (r * 10 + s) * 16 B.  Weights stay resident in shared memory; the epilogue can
-// apply the 2x2 max-pool that follows this layer (lane ^ 1 and lane ^ 8 hold the horizontal / vertical neighbours) and
-// ships the tile with one TMA store, so the un-pooled activation never reaches HBM in inference.
+// descriptor's start address by (r * 10 + s) * 16 B.  The epilogue can apply the 2x2 max-pool that follows this layer
+// and ships the tile with one TMA store, so the un-pooled activation never reaches HBM in inference.  The first form
+// (conv_c32_kernel_v1) keeps the weights resident in shared memory and pools across lanes (lane ^ 1 and lane ^ 8 hold the
+// horizontal / vertical neighbours); conv_c32_kernel below holds them in registers and pools within a thread.
 // ---------------------------------------------------------------------------------------------
 struct C32Params {
   int batch, height, width, cout;
@@ -1219,9 +1220,11 @@ struct C32Cfg {
   static_assert(kSmemBytes <= kSmemLimit, "c32: shared memory budget");
 };
 
+// The first form (YB_CONV_C32_V1=1 for A/B runs, and the training forward with statistics): one MMA warpgroup with both operands in
+// shared memory, the accumulator handed through a shared-memory tile to two epilogue groups.
 __global__ void __launch_bounds__(C32Cfg::kThreads, 1)
-conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                const __grid_constant__ CUtensorMap tmap_y, const C32Params p) {
+conv_c32_kernel_v1(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                   const __grid_constant__ CUtensorMap tmap_y, const C32Params p) {
   using Cfg = C32Cfg;
   constexpr int BN = Cfg::BN;
   constexpr int kGroups = Cfg::kGroups;
@@ -1439,6 +1442,201 @@ conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constan
   }
 }
 
+// The halo tile computed transposed, D^T[64 channels x 128 pixels] = W . X^T, so shared memory is off the critical path:
+//   * A is the weight, held in registers for the whole kernel (18 k16 steps x 4 registers per thread, loaded once per CTA);
+//   * B is the halo window, read by one m64n128k16 per k16 step with the same descriptor form as the first form's A (K-major, no
+//     swizzle, LBO = plane, SBO = one halo row; tap (r, s) = start shifted by (r * 10 + s) * 16 B), so a tile reads 72 KB of shared
+//     memory for its MMAs instead of 144 KB;
+//   * warpgroup 0 is the TMA producer (one thread); warpgroups 1 and 2 each take alternate tiles of the CTA's list and run their own
+//     epilogue from the registers, so one consumer's epilogue runs under the other's MMAs.
+// The k16 steps run in the first form's order (per tap, channels 0-15 then 16-31; taps 0..8) on the same fp16 operands and the
+// epilogue arithmetic is the same (scale / shift and leaky in fp32, the 2x2 max on the fp32 values in the first form's operand
+// order, then RN to fp16), so the output equals conv_c32_kernel_v1's bit for bit.  Thread l of warp w holds channels
+// 16 w + l / 4 (+ 8) of tile pixels (row j, columns 2 (l % 4) + {0, 1}) for all 16 rows j: a 2x2 pool window is in one thread.
+struct C32RegCfg {
+  static constexpr int kStages = 8;
+  static constexpr int kOutBytes = 128 * 128;                     // one tile's staged output: 128 pixels x 64 channels fp16, 128B-swizzled
+  static constexpr int kSmemBytes = 1024 + 4 * kOutBytes + kStages * C32Cfg::kHalo + 256;    // 2 staging buffers per consumer, barriers
+  static_assert(kSmemBytes <= kSmemLimit, "c32: shared memory budget");
+};
+
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_c32_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_y, const __half* __restrict__ w,
+                const C32Params p) {
+  using Cfg = C32Cfg;
+  constexpr int kStages = C32RegCfg::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_o = smem_base;                                      // [2 consumers][2 buffers][kOutBytes]
+  const uint32_t smem_h = smem_o + 4 * C32RegCfg::kOutBytes;              // [kStages][kHalo]
+  const uint32_t bar_full = smem_h + kStages * Cfg::kHalo;
+  const uint32_t bar_empty = bar_full + 8 * kStages;
+  const uint32_t bar_turn = bar_empty + 8 * kStages;                      // [2 consumers]: the other consumer's MMAs have retired
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kStages; ++i) { mbar_init(bar_full + 8 * i, 1); mbar_init(bar_empty + 8 * i, 4); }   // one arrival per consumer warp
+    for (int c = 0; c < 2; ++c) mbar_init(bar_turn + 8 * c, 4);
+    fence_mbar_init();
+    fence_proxy_async_smem();
+    tma_prefetch_desc(&tmap_x);
+    tma_prefetch_desc(&tmap_y);
+  }
+  __syncthreads();
+  pdl_trigger();        // an ordinary launch itself; lets a PDL successor set up while this grid drains
+
+  // trace (yb_conv_set_trace; block 0), tile i of the CTA: role 0 slot i = its halo load issue, role 1 slot i = its first wgmma issue;
+  // role 2 slot 2i = its MMAs retired, 2i + 1 = its epilogue end (store issued)
+  if (threadIdx.x < 128) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0; uint32_t phase = 0; int tr = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int tw = tile % p.tiles_w;
+        const int rest = tile / p.tiles_w;
+        const int th = rest % p.tiles_h;
+        const int n = rest / p.tiles_h;
+        mbar_wait(bar_empty + 8 * stage, phase ^ 1, p.dbg, 0xB50 | stage);
+        YB_TRACE(0, tr); ++tr;
+        if (p.skip & 1) {
+          mbar_arrive(bar_full + 8 * stage);
+        } else {
+          mbar_arrive_expect_tx(bar_full + 8 * stage, 4 * Cfg::kPlaneData);
+          for (int c = 0; c < 4; ++c)
+            tma_load_4d(smem_h + stage * Cfg::kHalo + c * Cfg::kPlane, &tmap_x, bar_full + 8 * stage, c * 8, tw * Cfg::TW - 1, th * Cfg::TH - 1, n);
+        }
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<232>();
+  const int cw = (threadIdx.x >> 7) - 1;        // consumer cw takes the CTA's tiles cw, cw + 2, ...
+  const int t = threadIdx.x & 127;
+  const int warp = t >> 5, lane = t & 31;
+  const int ch0 = 16 * warp + (lane >> 2);      // this thread's channels: ch0 (h = 0) and ch0 + 8 (h = 1)
+  // the weight as the A fragment of every k16 step ks (tap ks / 2, channels 16 (ks % 2) ..): rows ch0 / ch0 + 8, K columns
+  // 2 (l % 4) + {0, 1} and 8 + the same.  Rows >= Cout are zero.
+  uint32_t wa[18][4];
+  {
+    const unsigned int* wrow[2];
+    bool live[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      live[h] = ch0 + 8 * h < p.cout;
+      wrow[h] = reinterpret_cast<const unsigned int*>(w + (live[h] ? ch0 + 8 * h : 0) * 288 + 2 * (lane & 3));
+    }
+#pragma unroll
+    for (int ks = 0; ks < 18; ++ks)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) wa[ks][i] = live[i & 1] ? __ldg(wrow[i & 1] + ks * 8 + 4 * (i >> 1)) : 0u;
+  }
+  float sc[2], sh[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    sc[h] = ch0 + 8 * h < p.cout ? __ldg(p.scale + ch0 + 8 * h) : 0.f;
+    sh[h] = ch0 + 8 * h < p.cout ? __ldg(p.shift + ch0 + 8 * h) : 0.f;
+  }
+  const uint32_t lbo = p.swap_lbo ? Cfg::HW * 16 : Cfg::kPlane;
+  const uint32_t sbo = p.swap_lbo ? Cfg::kPlane : Cfg::HW * 16;
+  const int mi = lane >> 3, mr = lane & 7;       // stmatrix: this thread addresses row mr of matrix mi
+  float acc[64];
+  int use = 0;                                   // tiles this consumer has staged
+  for (int local = cw, tile = blockIdx.x + cw * gridDim.x; tile < p.num_tiles; local += 2, tile += 2 * gridDim.x, ++use) {
+    const int stage = local % kStages;
+    // the consumers take turns on the tensor cores (tile local - 1's MMAs have retired), so one's epilogue runs under the other's
+    // MMAs instead of both issuing together and then both converting
+    if (local > 0) mbar_wait(bar_turn + 8 * cw, ((local - 1) >> 1) & 1, p.dbg, 0xB70 | cw);
+    mbar_wait(bar_full + 8 * stage, (local / kStages) & 1, p.dbg, 0xB60 | stage);
+    if (t == 0) YB_TRACE(1, local);
+    const uint32_t halo = smem_h + stage * Cfg::kHalo;
+    if (!(p.skip & 4)) {
+      wgmma_fence();
+#pragma unroll
+      for (int tap = 0; tap < 9; ++tap) {
+        const uint32_t win = halo + ((tap / 3) * Cfg::HW + (tap % 3)) * 16;      // tap (r, s): window shifted by r rows, s pixels
+        wgmma_f16_rs_n128(acc, wa[2 * tap], make_kmajor_desc_noswz(win, lbo, sbo), tap != 0);
+        wgmma_f16_rs_n128(acc, wa[2 * tap + 1], make_kmajor_desc_noswz(win + 2 * Cfg::kPlane, lbo, sbo), 1);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+    }
+    fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) {
+      mbar_arrive(bar_empty + 8 * stage);
+      mbar_arrive(bar_turn + 8 * (cw ^ 1));
+    }
+    if (t == 0) YB_TRACE(2, 2 * local);
+    const int tw = tile % p.tiles_w;
+    const int rest = tile / p.tiles_w;
+    const int th = rest % p.tiles_h;
+    const int n = rest / p.tiles_h;
+    // scale / shift, leaky: acc[4 j + 2 h + e] is channel ch0 + 8 h, pixel (row j, column 2 (l % 4) + e)
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float x = acc[4 * j + 2 * h + e] * sc[h] + sh[h];
+          acc[4 * j + 2 * h + e] = x > 0.f ? x : x * p.slope;
+        }
+    const uint32_t obuf = smem_o + (cw * 2 + (use & 1)) * C32RegCfg::kOutBytes;
+    if (t == 0) tma_store_wait_read<1>();        // this consumer's store from two of its tiles ago has drained the buffer
+    asm volatile("bar.sync %0, 128;" :: "r"(1 + cw) : "memory");
+    // staged as [pixel][64 channels], 16-byte chunk c of pixel row px at (c ^ (px & 7)): the TMA store's 128B swizzle.  The matrices of
+    // one stmatrix are (rows = channels ch0 - lane / 4 + 8 h, columns = 8 pixels); chunk 2 warp + h of the pixels they cover.
+    if (p.pool) {
+      // window (i, l % 4) is rows 2 i, 2 i + 1, columns 2 (l % 4) + {0, 1}: max(max(row 2 i), max(row 2 i + 1)) in the first form's order.
+      // Matrix (i2, h): fragment column 2 (l % 4) + e is pooled pixel (2 i2 + e, l % 4), stored at pooled row (2 i2 + e) * 4 + l % 4.
+      float pm[8][2];
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          pm[i][h] = fmaxf(fmaxf(acc[4 * (2 * i) + 2 * h], acc[4 * (2 * i) + 2 * h + 1]),
+                           fmaxf(acc[4 * (2 * i + 1) + 2 * h], acc[4 * (2 * i + 1) + 2 * h + 1]));
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        uint32_t r[4];
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          const int i2 = 2 * k + (m >> 1), h = m & 1;
+          __half2 v = __floats2half2_rn(pm[2 * i2][h], pm[2 * i2 + 1][h]);
+          r[m] = *reinterpret_cast<uint32_t*>(&v);
+        }
+        const int px = 8 * (2 * k + (mi >> 1)) + 4 * (mr & 1) + (mr >> 1);
+        stmatrix_x4_trans(obuf + px * 128 + (((2 * warp + (mi & 1)) ^ (px & 7)) << 4), r[0], r[1], r[2], r[3]);
+      }
+    } else {
+      // matrix (j, h): fragment column 2 (l % 4) + e is pixel 8 j + 2 (l % 4) + e
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        uint32_t r[4];
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+          const int j = 2 * k + (m >> 1), h = m & 1;
+          __half2 v = __floats2half2_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          r[m] = *reinterpret_cast<uint32_t*>(&v);
+        }
+        const int px = 8 * (2 * k + (mi >> 1)) + mr;
+        stmatrix_x4_trans(obuf + px * 128 + (((2 * warp + (mi & 1)) ^ (px & 7)) << 4), r[0], r[1], r[2], r[3]);
+      }
+    }
+    fence_proxy_async_smem();
+    asm volatile("bar.sync %0, 128;" :: "r"(1 + cw) : "memory");
+    if (t == 0) {
+      if (!(p.skip & 8)) {
+        if (p.pool) tma_store_4d(&tmap_y, obuf, 0, tw * (Cfg::TW / 2), th * (Cfg::TH / 2), n);
+        else tma_store_4d(&tmap_y, obuf, 0, tw * Cfg::TW, th * Cfg::TH, n);
+      }
+      tma_store_commit();
+      YB_TRACE(2, 2 * local + 1);
+    }
+  }
+  if (t == 0) tma_store_wait<0>();
+}
+
 // ---------------------------------------------------------------------------------------------
 // Host side: tensor-map encoding through the driver entry points (no link-time libcuda dependency)
 // ---------------------------------------------------------------------------------------------
@@ -1632,7 +1830,10 @@ static int conv_c32_forward(const void* x, const void* w, const float* scale, co
                    CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(halo) failed (%d)", static_cast<int>(cr));
   }
-  {
+  // the first form (conv_c32_kernel_v1) for the training forward's statistics, and for every launch with YB_CONV_C32_V1=1 (A/B runs)
+  static const int force_v1 = getenv("YB_CONV_C32_V1") ? atoi(getenv("YB_CONV_C32_V1")) : 0;
+  const bool v1 = force_v1 != 0 || stats != nullptr;
+  if (v1) {
     const cuuint64_t dims[2] = {9 * 32, static_cast<cuuint64_t>(cout)};
     const cuuint64_t strides[1] = {9 * 32 * 2};
     const cuuint32_t box[2] = {32, 64};
@@ -1651,13 +1852,22 @@ static int conv_c32_forward(const void* x, const void* w, const float* scale, co
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (cr != CUDA_SUCCESS) return fail(YB_ERR_DRIVER, "cuTensorMapEncodeTiled(Y) failed (%d)", static_cast<int>(cr));
   }
+  const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
+  if (v1) {
+    static bool attr_set = false;
+    if (!attr_set) {
+      YB_CUDA(cudaFuncSetAttribute(conv_c32_kernel_v1, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+      attr_set = true;
+    }
+    conv_c32_kernel_v1<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(tx, tw, ty, p);
+    return check_launch("conv_c32_kernel_v1");
+  }
   static bool attr_set = false;
   if (!attr_set) {
-    YB_CUDA(cudaFuncSetAttribute(conv_c32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    YB_CUDA(cudaFuncSetAttribute(conv_c32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C32RegCfg::kSmemBytes));
     attr_set = true;
   }
-  const int grid = p.num_tiles < sm_count() ? p.num_tiles : sm_count();
-  conv_c32_kernel<<<grid, Cfg::kThreads, Cfg::kSmemBytes, stream>>>(tx, tw, ty, p);
+  conv_c32_kernel<<<grid, kWideThreads, C32RegCfg::kSmemBytes, stream>>>(tx, ty, static_cast<const __half*>(w), p);
   return check_launch("conv_c32_kernel");
 }
 
