@@ -249,13 +249,15 @@ constexpr int kV2Iters = (kV2Pixels + 127) / 128;               // 5 pixels per 
 // store instruction would touch many different 128-byte lines (bound by L2 write transactions); instead the tile is staged in shared memory
 // (swizzled) and leaves as 512 contiguous bytes per warp instruction.  The copy-out loop hands every thread
 // the same 8 channels on every trip, so the BatchNorm batch statistics (sum z, sum z^2 of the fp16 values that are stored) accumulate in 16
-// registers over all of the CTA's tiles and are reduced once at the end (p.stats: double [2][32], as yb_bn_stats).
+// fp32 registers over one tile (16 rows per thread), are reduced across the warp and added into a double shared accumulator per tile, and
+// leave once at the end (p.stats: double [2][32], as yb_bn_stats).  Keeping the fp32 part to one tile bounds its rounding error by 19 fp32
+// roundings of sum |z| however many tiles a CTA runs: the variance var = sum z^2 / n - mean^2 amplifies that error by 1 + (mean / std)^2.
 constexpr int kV2StageBytes = kV2Rows * kV2Cols * kC0Out * 2;   // 32 KB
 
 template <bool kU8, bool kRaw>
 __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv0Params p) {
   __shared__ __align__(128) uint8_t stage[kRaw ? kV2StageBytes : 16];
-  __shared__ float s_stats[2 * kC0Out];
+  __shared__ double s_stats[2 * kC0Out];
   __shared__ __align__(128) uint8_t patch_e[kV2Copy + 48];      // pixel (r, c) at (r * 18 + c) * 8: even columns 16 B aligned
   __shared__ __align__(128) uint8_t patch_o[kV2Copy + 48];      // the same pixels at + 8 B: odd columns 16 B aligned
   __shared__ __align__(128) uint8_t b_smem[3 * 1024];           // per filter row: [n / 8][k / 8][n % 8][k % 8] fp16 (32 x 16)
@@ -316,7 +318,7 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv
   float st1[8], st2[8];                           // kRaw: statistics of channels (tid & 3) * 8 .. + 7
 #pragma unroll
   for (int e = 0; e < 8; ++e) { st1[e] = 0.f; st2[e] = 0.f; }
-  if (kRaw && tid < 2 * kC0Out) s_stats[tid] = 0.f;
+  if (kRaw && tid < 2 * kC0Out) s_stats[tid] = 0.0;
 
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     const int tx = tile % p.tiles_x;
@@ -423,28 +425,32 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv
           }
         }
       }
+      if (p.stats != nullptr) {
+        // this tile's partials: lanes with equal (lane & 3) hold the same 8 channels; their warp sum goes into the double accumulator
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+#pragma unroll
+          for (int sft = 4; sft <= 16; sft <<= 1) {
+            st1[e] += __shfl_xor_sync(0xffffffffu, st1[e], sft);
+            st2[e] += __shfl_xor_sync(0xffffffffu, st2[e], sft);
+          }
+        }
+        if ((tid & 31) < 4) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            atomicAdd(&s_stats[(tid & 3) * 8 + e], static_cast<double>(st1[e]));
+            atomicAdd(&s_stats[kC0Out + (tid & 3) * 8 + e], static_cast<double>(st2[e]));
+          }
+        }
+#pragma unroll
+        for (int e = 0; e < 8; ++e) { st1[e] = 0.f; st2[e] = 0.f; }
+      }
       // the next iteration's __syncthreads (after the patch is written) orders this copy-out before the next tile's staging stores
     }
   }
   if (kRaw && p.stats != nullptr) {
-    // lanes with equal (lane & 3) hold the same 8 channels
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-#pragma unroll
-      for (int sft = 4; sft <= 16; sft <<= 1) {
-        st1[e] += __shfl_xor_sync(0xffffffffu, st1[e], sft);
-        st2[e] += __shfl_xor_sync(0xffffffffu, st2[e], sft);
-      }
-    }
-    if ((tid & 31) < 4) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        atomicAdd(&s_stats[(tid & 3) * 8 + e], st1[e]);
-        atomicAdd(&s_stats[kC0Out + (tid & 3) * 8 + e], st2[e]);
-      }
-    }
     __syncthreads();
-    if (tid < 2 * kC0Out) atomicAdd(p.stats + tid, static_cast<double>(s_stats[tid]));
+    if (tid < 2 * kC0Out) atomicAdd(p.stats + tid, s_stats[tid]);
   }
 }
 
@@ -452,11 +458,12 @@ int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* sc
                      int height, int width, int cout, int raw, double* stats, cudaStream_t stream) {
   YB_REQUIRE(x && w && y && (raw || (scale && shift)), "conv0: null pointer");
   YB_REQUIRE(cout == kC0Out, "conv0: Cout=%d unsupported (32)", cout);
-  YB_REQUIRE(batch > 0 && height > 0 && width > 0 && height % kT0Rows == 0 && width % kT0Cols == 0,
-             "conv0: H must be a multiple of %d and W of %d (got %dx%d)", kT0Rows, kT0Cols, height, width);
   // operands-in-place form when the shape tiles 32 x 16 (every multiple of 32, i.e. every Darknet input); YB_CONV0_V1=1 forces the first form
   static const int force_v1 = getenv("YB_CONV0_V1") ? atoi(getenv("YB_CONV0_V1")) : 0;
-  const bool v2 = !force_v1 && height % kV2Rows == 0 && width % kV2Cols == 0;
+  const bool v2 = !force_v1 && batch > 0 && height > 0 && width > 0 && height % kV2Rows == 0 && width % kV2Cols == 0;
+  YB_REQUIRE(v2 || (batch > 0 && height > 0 && width > 0 && height % kT0Rows == 0 && width % kT0Cols == 0),
+             "conv0: H must be a multiple of %d and W of %d, or H of %d and W of %d (got %dx%d)", kV2Rows, kV2Cols, kT0Rows, kT0Cols, height,
+             width);
   Conv0Params p;
   p.x = x; p.w = w; p.scale = scale; p.shift = shift; p.slope = slope; p.y = reinterpret_cast<__half*>(y);
   p.batch = batch; p.height = height; p.width = width;

@@ -1216,7 +1216,7 @@ struct C32Cfg {
   static constexpr int kAccBytes = BN * kAccPitch * 4;
   static constexpr int kEpiThreads = kGroups * 128;
   static constexpr int kThreads = 128 + 32 + kEpiThreads;         // MMA warpgroup, TMA warp, epilogue groups
-  static constexpr int kSmemBytes = 1024 + kBBytes + 2 * kGroups * kOutBytes + kStages * kHalo + kGroups * kAccBytes + 2 * BN * 4 + 256 + 2 * BN * 4 /*stats*/;
+  static constexpr int kSmemBytes = 1024 + kBBytes + 2 * kGroups * kOutBytes + kStages * kHalo + kGroups * kAccBytes + 2 * BN * 4 + 256 + 2 * BN * 8 /*stats*/;
   static_assert(kSmemBytes <= kSmemLimit, "c32: shared memory budget");
 };
 
@@ -1243,7 +1243,9 @@ conv_c32_kernel_v1(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
   const uint32_t bar_tfull = bar_empty + 8 * Cfg::kStages;
   const uint32_t bar_tempty = bar_tfull + 8 * kGroups;
   const uint32_t bar_w = bar_tempty + 8 * kGroups;
-  float* ep_stats = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);      // [2][BN], accumulated over all of this CTA's tiles
+  // [2][BN] double, accumulated over all of this CTA's tiles: each warp's 32-pixel fp32 column sum is added in double, so the fp32 part of the
+  // statistics is five roundings deep however many tiles the CTA runs (the variance amplifies it by 1 + (mean / std)^2)
+  double* ep_stats = reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(bars) + 256);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
@@ -1338,7 +1340,7 @@ conv_c32_kernel_v1(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
     for (int i = et; i < BN; i += Cfg::kEpiThreads) {
       ep_scale[i] = (i < p.cout) ? __ldg(p.scale + i) : 0.f;
       ep_shift[i] = (i < p.cout) ? __ldg(p.shift + i) : 0.f;
-      ep_stats[i] = 0.f; ep_stats[BN + i] = 0.f;
+      ep_stats[i] = 0.0; ep_stats[BN + i] = 0.0;
     }
     asm volatile("bar.sync 8, %0;" :: "n"(Cfg::kEpiThreads) : "memory");
     const int m = q * 32 + lane;            // tile-local pixel: row m >> 3, column m & 7
@@ -1396,8 +1398,8 @@ conv_c32_kernel_v1(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
               a2[j] = k2 + __shfl_xor_sync(0xffffffffu, g2, sft);
             }
           }
-          atomicAdd(&ep_stats[half * 32 + lane], a1[0]);
-          atomicAdd(&ep_stats[BN + half * 32 + lane], a2[0]);
+          atomicAdd(&ep_stats[half * 32 + lane], static_cast<double>(a1[0]));
+          atomicAdd(&ep_stats[BN + half * 32 + lane], static_cast<double>(a2[0]));
         }
         if (p.pool) {
 #pragma unroll
@@ -1435,8 +1437,8 @@ conv_c32_kernel_v1(const __grid_constant__ CUtensorMap tmap_x, const __grid_cons
     if (p.stats != nullptr) {
       asm volatile("bar.sync 8, %0;" :: "n"(Cfg::kEpiThreads) : "memory");       // every group has added its last tile
       for (int i = et; i < p.cout; i += Cfg::kEpiThreads) {
-        atomicAdd(p.stats + i, static_cast<double>(ep_stats[i]));
-        atomicAdd(p.stats + p.cout + i, static_cast<double>(ep_stats[BN + i]));
+        atomicAdd(p.stats + i, ep_stats[i]);
+        atomicAdd(p.stats + p.cout + i, ep_stats[BN + i]);
       }
     }
   }

@@ -32,19 +32,21 @@ __device__ __forceinline__ uint4 f_to_h8(const float (&f)[8]) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// sums[0..C) += sum_rows z, sums[C..2C) += sum_rows z^2   (double accumulators, zero on entry)
+// sums[0..C) += sum_rows z, sums[C..2C) += sum_rows z^2   (double accumulators, zero on entry).  Each trip's four rows are added in fp32,
+// everything after that in double: the fp32 part stays three roundings deep at any row count, which matters because bn_finalize's
+// var = sum z^2 / n - mean^2 amplifies the error of the sums by 1 + (mean / std)^2.
 __global__ void __launch_bounds__(kTrainThreads) bn_stats_kernel(const __half* __restrict__ z, long long ld, long long rows, int channels,
                                                                  double* __restrict__ sums) {
-  extern __shared__ float s_acc[];  // [2][channels]
-  for (int i = threadIdx.x; i < 2 * channels; i += blockDim.x) s_acc[i] = 0.f;
+  extern __shared__ double s_sum[];  // [2][channels]
+  for (int i = threadIdx.x; i < 2 * channels; i += blockDim.x) s_sum[i] = 0.0;
   __syncthreads();
   const int c8 = channels >> 3;
   const int cg = threadIdx.x % c8;
   const int rpi = blockDim.x / c8;                 // rows per iteration
   const int rib = threadIdx.x / c8;
-  float s[8], q[8];
+  double s[8], q[8];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { s[i] = 0.f; q[i] = 0.f; }
+  for (int i = 0; i < 8; ++i) { s[i] = 0.0; q[i] = 0.0; }
   if (rib < rpi) {
     const long long rstride = static_cast<long long>(gridDim.x) * rpi;
     for (long long r0 = static_cast<long long>(blockIdx.x) * rpi + rib; r0 < rows; r0 += 4 * rstride) {
@@ -54,22 +56,27 @@ __global__ void __launch_bounds__(kTrainThreads) bn_stats_kernel(const __half* _
         const long long r = r0 + u * rstride;
         raw[u] = r < rows ? __ldg(reinterpret_cast<const uint4*>(z + r * ld + cg * 8)) : make_uint4(0u, 0u, 0u, 0u);   // fp16 zeros add nothing
       }
+      float ts[8], tq[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { ts[i] = 0.f; tq[i] = 0.f; }
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         float f[8];
         h8_to_f(raw[u], f);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) { s[i] += f[i]; q[i] += f[i] * f[i]; }
+        for (int i = 0; i < 8; ++i) { ts[i] += f[i]; tq[i] = fmaf(f[i], f[i], tq[i]); }
       }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { s[i] += static_cast<double>(ts[i]); q[i] += static_cast<double>(tq[i]); }
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      atomicAdd(&s_acc[cg * 8 + i], s[i]);
-      atomicAdd(&s_acc[channels + cg * 8 + i], q[i]);
+      atomicAdd(&s_sum[cg * 8 + i], s[i]);
+      atomicAdd(&s_sum[channels + cg * 8 + i], q[i]);
     }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < 2 * channels; i += blockDim.x) atomicAdd(&sums[i], static_cast<double>(s_acc[i]));
+  for (int i = threadIdx.x; i < 2 * channels; i += blockDim.x) atomicAdd(&sums[i], s_sum[i]);
 }
 
 // mean/invstd for this batch, running-stat update (unbiased variance, like torch), sums reset to 0
@@ -411,7 +418,7 @@ int bn_stats(const void* z, long long ld, long long rows, int channels, double* 
   long long blocks = (rows + static_cast<long long>(rpi) * 16 - 1) / (static_cast<long long>(rpi) * 16);   // >= 16 rows per thread: 2C double atomics per block
   const long long cap = static_cast<long long>(sm_count()) * 8;
   if (blocks > cap) blocks = cap;
-  bn_stats_kernel<<<static_cast<int>(blocks), kTrainThreads, 2 * channels * sizeof(float), stream>>>(reinterpret_cast<const __half*>(z), ld, rows,
+  bn_stats_kernel<<<static_cast<int>(blocks), kTrainThreads, 2 * channels * sizeof(double), stream>>>(reinterpret_cast<const __half*>(z), ld, rows,
                                                                                                   channels, sums);
   return check_launch("bn_stats_kernel");
 }
