@@ -1,12 +1,13 @@
 """Error budget of one ResNet TRAINING step under fp16 storage, in pure CPU fp32 arithmetic with only the roundings of the GPU path added:
 conv weights -> fp16 (not the stem's, which is read as fp32), raw conv output z -> fp16, every stored activation -> fp16, and in the backward
-every stored gradient -> fp16 at the static loss scale (16384) -- through a rounding op whose backward rounds the scaled gradient.  The step
+every stored gradient -> fp16 at the trainer's static loss scale (b200.train_engine.ResNetTrainer.default_grad_scale: 16384 for resnet18 / 34
+/ 50, 4096 for resnet101, 1024 for resnet152) -- through a rounding op whose backward rounds the scaled gradient.  The step
 (train-mode forward, region loss, autograd backward) is compared with the exact fp32 step on the same batch as
 tests/test_resnet_train.py::test_resnet_training_step_vs_oracle_and_descent: head feature, gradient cosine per parameter (worst overall and
 worst of the head + last block).  If these figures match what the GPU run measures, the discrepancy is the roundings amplified by the
 train-mode BatchNorm chain (DESIGN §2), not a kernel.
 
-    python tools/resnet_train_error_budget.py resnet50 8 160     # net, batch, size
+    python tools/resnet_train_error_budget.py resnet50 8 160     # net (resnet18 / 34 / 50 / 101 / 152), batch, size
 """
 import os
 import sys
@@ -15,24 +16,32 @@ import torch
 import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path[:0] = [ROOT, os.path.join(ROOT, 'tests')]
+sys.path[:0] = [ROOT, os.path.join(ROOT, 'tests'), os.path.join(ROOT, 'yolo2-pytorch_b200')]
 from oracle import yolo2_oracle as O  # noqa: E402
+import resnet_deep_oracle  # noqa: E402,F401  (resnet101 / 152 in the oracle's ResNet table)
 
 SCALE = 16384.0
 
 
 class _R16(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x):
+    def forward(ctx, x, scale=SCALE):
+        ctx.scale = scale
         return x.half().float()
 
     @staticmethod
     def backward(ctx, g):
-        return (g * SCALE).half().float() / SCALE
+        return (g * ctx.scale).half().float() / ctx.scale, None
 
 
-def step(sd0, x, data, name, rounded):
-    r = _R16.apply if rounded else (lambda t: t)
+def grad_scale(name):
+    """The static loss scale the trainer uses for this net."""
+    from b200 import train_engine
+    return train_engine.ResNetTrainer.default_grad_scale(len(O.resnet_blocks(name)))
+
+
+def step(sd0, x, data, name, rounded, scale=SCALE):
+    r = (lambda t: _R16.apply(t, scale)) if rounded else (lambda t: t)
     sd = {k: (v.clone().requires_grad_(True) if v.is_floating_point() and 'running' not in k else v.clone()) for k, v in sd0.items()}
 
     def w(key):
@@ -75,7 +84,7 @@ def main():
     x = O.synth_images(b, size, size, seed=90)
     data = O.norm_data(O.synth_targets(b, size, size, slots=5, seed=91), size, size, s, s)
     f_ref, g_ref = step(sd0, x, data, name, False)
-    f_16, g_16 = step(sd0, x, data, name, True)
+    f_16, g_16 = step(sd0, x, data, name, True, grad_scale(name))
     last = [blk['prefix'] for blk in O.resnet_blocks(name)][-1]
     worst, late = (1.0, None), (1.0, None)
     for k, g in g_ref.items():

@@ -919,12 +919,26 @@ class ResNetTrainer(TrainerBase):
     subsampled input.  Backward of a stride-2 3x3 conv is the transpose: dz zero-inserted to full resolution (yb_upsample2_zero_f16), then the
     stride-1 weight and data gradients.  At each block boundary yb_residual_bwd_f16 sums the main path's data gradient and the skip path's and
     applies the previous block's ReLU mask in one pass.  The stem's gradient runs through the max-pool backward (first maximum of each window),
-    the BN + ReLU backward and a CUDA-core weight-gradient kernel on the fp32 image."""
-    NAME = 'ResNet'
+    the BN + ReLU backward and a CUDA-core weight-gradient kernel on the fp32 image.
 
-    def __init__(self, dnn, grad_scale=16384.0):
+    The static loss scale depends on the depth (`default_grad_scale`, from the number of blocks).  The largest stored |gradient| is the stem
+    conv's dz, and it grows with the number of train-mode BatchNorms between it and the head: on the synthetic step of the tests (8 x 160^2)
+    the fp32 restatement's largest |dL/dz| is 0.11 (resnet50), 0.43 (resnet101) and 3.3 (resnet152), so at 16384 resnet152's would come
+    within 1.2x of 65504.  resnet18 / 34 / 50 keep 16384; resnet101 takes 4096 and resnet152 1024.  The GPU's own steps then store at most
+    2015 (resnet101, 8 x 160^2), 575 (resnet101, 2 x 416^2) and 3594 (resnet152, 8 x 160^2): 18- to 114-fold below 65504 (DESIGN §6)."""
+    NAME = 'ResNet'
+    GRAD_SCALES = ((16, 16384.0), (33, 4096.0), (None, 1024.0))     # (up to this many blocks, static loss scale)
+
+    def __init__(self, dnn, grad_scale=None):
+        if grad_scale is None:
+            grad_scale = self.default_grad_scale(sum(len(getattr(dnn, name)) for name in ('layer1', 'layer2', 'layer3', 'layer4')))
         TrainerBase.__init__(self, dnn, grad_scale, slope=0.0)
         self._blocks = None
+
+    @classmethod
+    def default_grad_scale(cls, blocks):
+        """Static loss scale of a ResNet with `blocks` residual blocks: 16384 up to resnet50's 16, 4096 up to resnet101's 33, else 1024."""
+        return next(scale for limit, scale in cls.GRAD_SCALES if limit is None or blocks <= limit)
 
     def _plan(self):
         if self._blocks is None:

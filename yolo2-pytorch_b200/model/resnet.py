@@ -1,7 +1,7 @@
 """model.resnet -- ResNet backbone plugin on the CUDA kernels (inference and training).
 
-Drop-in for the reference's `model/resnet.py` (file:line cited per item): same constructors `resnet18 / resnet34 / resnet50
-(config_channels, anchors, num_cls)` (:161-197), same state_dict keys as torchvision's ResNet (`conv1.weight`, `bn1.*`,
+Drop-in for the reference's `model/resnet.py` (file:line cited per item): same constructors `resnet18 / resnet34 / resnet50 /
+resnet101 / resnet152(config_channels, anchors, num_cls)` (:161-224), same state_dict keys as torchvision's ResNet (`conv1.weight`, `bn1.*`,
 `layerL.B.conv1.weight`, `layerL.B.downsample.0.weight`, ...) plus the 1x1 detection head `conv.weight / conv.bias` (:115), same
 `scope(name)` (:144-158), same forward contract x[B,3,H,W] fp32 -> [B, A*(5+C), H/32, W/32] fp32 (:131-142).  Modules only hold
 parameters; the forward pass is:
@@ -15,7 +15,9 @@ parameters; the forward pass is:
 In train() mode the forward is one autograd node (model._TrainFunction) over b200.train_engine.ResNetTrainer: batch-statistics
 BatchNorm (momentum 0.1, read from the modules) on the raw conv outputs, the explicit backward chain (stride-2 convs as the stride-1 gradients of the
 zero-inserted dz, max-pool backward to the first maximum of each window, the stem's weight gradient on the fp32 image).  There is no CPU path.
-Switching back to eval() drops the cached folded BatchNorm and packed weights, so inference uses the trained state.
+Switching back to eval() drops the cached folded BatchNorm and packed weights, so inference uses the trained state.  The forward and the
+trainer walk layer1-layer4 whatever their block counts, so resnet101 ([3, 4, 23, 3]) and resnet152 ([3, 8, 36, 3]) run the Bottleneck path of
+resnet50; only the trainer's loss scale depends on the depth (ResNetTrainer.default_grad_scale).
 """
 import re
 
@@ -198,3 +200,11 @@ def resnet34(config_channels, anchors, num_cls, **kwargs):
 
 def resnet50(config_channels, anchors, num_cls, **kwargs):
     return _pretrained(ResNet(config_channels, anchors, num_cls, Bottleneck, [3, 4, 6, 3], **kwargs), config_channels, 'resnet50')
+
+
+def resnet101(config_channels, anchors, num_cls, **kwargs):
+    return _pretrained(ResNet(config_channels, anchors, num_cls, Bottleneck, [3, 4, 23, 3], **kwargs), config_channels, 'resnet101')
+
+
+def resnet152(config_channels, anchors, num_cls, **kwargs):
+    return _pretrained(ResNet(config_channels, anchors, num_cls, Bottleneck, [3, 8, 36, 3], **kwargs), config_channels, 'resnet152')
