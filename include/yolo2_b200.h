@@ -286,6 +286,14 @@ int yb_unpack_wgrad(const float* dw_krsc, float* dw_oihw, int cout, int cin, int
  * so the optimizer takes a null step instead of absorbing the overflow into its state.  Asynchronous, no host sync, capturable. */
 int yb_grad_guard(float* grads, long long count, float* found_inf, int zero_if_found, yb_stream_t stream);
 
+/* The guard of dynamic loss scaling, in place of yb_grad_guard: the backward ran at the static scale times `factor` (device float, a
+ * power of two) and was un-scaled by the static scale only.  found_inf[0] = 1 if any of the `count` fp32 gradient values is inf / NaN
+ * (then the buffer is zeroed), else 0 and the buffer is multiplied by 1 / factor (not written when factor is 1).  Then factor and
+ * growth_tracker (device int) move by torch.amp.GradScaler's rule: overflow -> factor * 0.5, tracker 0; else tracker + 1, and at
+ * `growth_interval` factor * 2, tracker 0; factor is clamped to [2^-24, 2^24].  Asynchronous, no host sync, capturable. */
+int yb_grad_unscale_guard(float* grads, long long count, float* found_inf, float* factor, int* growth_tracker, int growth_interval,
+                          yb_stream_t stream);
+
 /* ---- GPU input pipeline (SURVEY 8f rank 2; transform/resize/image.py:23-24, transform/resize/label.py:25-31, transform/image.py:27-29) ----
  * A batch of decoded uint8 HWC frames of DIFFERENT sizes -> [B,height,width,3] uint8 in one launch: cv2.resize(image, (width, height))
  * (8-bit INTER_LINEAR, bit-exact) + optional BGR->RGB swap.  src = packed frames, image i starts at byte src_off[i] and is

@@ -61,6 +61,7 @@ SIGNATURES = {
     'yb_conv_wgrad': [P, P, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P],
     'yb_unpack_wgrad': [P, P, c_int, c_int, c_int, c_float, P],
     'yb_grad_guard': [P, c_longlong, P, c_int, P],
+    'yb_grad_unscale_guard': [P, c_longlong, P, P, P, c_int, P],
     'yb_resize_batch_u8': [P, P, P, P, c_int, c_int, c_int, c_int, P, P, c_int, P],
     'yb_resize_aug_batch_u8': [P, P, P, P, P, P, P, c_int, c_int, c_int, c_int, P, P, c_int, P],
     'yb_warp_affine_u8': [P, c_int, c_int, P, c_int, c_int, ctypes.POINTER(ctypes.c_double * 6), ctypes.POINTER(c_int * 3), P],

@@ -9,7 +9,8 @@ reorg / cat (model/yolo2.py:49-65,125-130; train.py:344-351) is issued here as a
                       -> wgmma weight gradient (pixels are the reduction dim) + wgmma data gradient
                       (the forward kernel on dz with rotated, transposed weights)
 
-Gradients travel in fp16 multiplied by `grad_scale` (static loss scaling; parameter gradients are un-scaled in fp32).
+Gradients travel in fp16 multiplied by `grad_scale` (static loss scaling; parameter gradients are un-scaled in fp32), or, with
+`set_loss_scale('dynamic')`, by `grad_scale` times a device power-of-two factor that backs off on overflow and grows back.
 BatchNorm statistics are per process (per GPU), exactly like the per-replica statistics of the reference's
 nn.DataParallel.
 
@@ -94,6 +95,11 @@ class TrainerBase(object):
         self.reducer = None
         self.arena = None
         self.found_inf = None  # device float[1]: 1 when the last backward produced a non-finite gradient (then zeroed), see _finish_backward()
+        # loss scaling: 'static' runs at grad_scale; 'dynamic' at grad_scale * loss_factor (set_loss_scale)
+        self.loss_scale = 'static'
+        self.growth_interval = 2000
+        self.loss_factor = None      # device fp32 0-dim, a power of two in [2^-24, 2^24], starts at 1
+        self.growth_tracker = None   # device int32 0-dim: clean steps in a row since the factor last moved
         self._arenas = {}      # one per (device, parameter set, reducer): CUDA graphs keep writing the arena they were captured with
         self._main = None
         # BN batch statistics in the conv epilogue (yb_conv_bn_act_stats_fwd) instead of yb_bn_stats; YB_FUSE_STATS=0 for A/B runs
@@ -127,13 +133,38 @@ class TrainerBase(object):
     def _finish_backward(self, dev):
         """End of the backward chain: the main stream waits for the weight-gradient stream and for every bucket's all-reduce (no host
         wait), then the fp16 gradient overflow guard runs (after the exchange, so every rank takes the same decision): `found_inf` is raised
-        and the gradients are zeroed instead of poisoning the optimizer state; train.iterate hands the flag to optimizers that can skip."""
+        and the gradients are zeroed instead of poisoning the optimizer state; train.iterate hands the flag to optimizers that can skip.
+        In dynamic mode the guard also divides the gradients by the loss factor and moves the factor (yb_grad_unscale_guard)."""
         self._join(dev)
         if self.reducer is not None:
             self.reducer.finish()
         if self.found_inf is None or self.found_inf.device != dev:
             self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)      # 0-dim like GradScaler's (fused optimizers subtract it from their step counters)
-        ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+        if self.loss_scale == 'dynamic':
+            factor, tracker = self.loss_scale_state(dev)
+            ops.call('yb_grad_unscale_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, factor, tracker, self.growth_interval)
+        else:
+            ops.call('yb_grad_guard', self.arena.flat, self.arena.flat.numel(), self.found_inf, 1)
+
+    def set_loss_scale(self, mode, growth_interval=2000):
+        """'static': the backward runs at `grad_scale` (the default).  'dynamic': at `grad_scale` times a device power-of-two factor that
+        starts at 1, halves on every step whose gradients overflow (the step is skipped or null, see `found_inf`) and doubles after
+        `growth_interval` clean steps in a row, like torch.amp.GradScaler.  Powers of two make a dynamic step at factor 2^k compute the
+        same gradients as a static one at grad_scale * 2^k."""
+        if mode not in ('static', 'dynamic'):
+            raise ValueError('loss_scale must be static or dynamic, got %r' % (mode,))
+        if int(growth_interval) != growth_interval or growth_interval <= 0:
+            raise ValueError('loss_scale_growth_interval must be a positive integer, got %r' % (growth_interval,))
+        self.loss_scale, self.growth_interval = mode, int(growth_interval)
+
+    def loss_scale_state(self, dev):
+        """The dynamic factor and growth tracker on `dev` (created at 1 and 0 on first use), or [] in static mode."""
+        if self.loss_scale != 'dynamic':
+            return []
+        if self.loss_factor is None or self.loss_factor.device != dev:
+            self.loss_factor = torch.ones((), dtype=torch.float32, device=dev)
+            self.growth_tracker = torch.zeros((), dtype=torch.int32, device=dev)
+        return [self.loss_factor, self.growth_tracker]
 
     def _ensure_arena(self, dnn, device):
         """Persistent flat fp32 gradient buffer (b200.ddp.GradArena) for the parameters of `dnn` (the trainer's module): gradient
@@ -390,7 +421,10 @@ class TrainerBase(object):
         cpad = (chead + 31) // 32 * 32
         dzh = torch.empty(b, hh, ww, cpad, dtype=torch.float16, device=dev)
         dbias = self.arena.views[bias]
-        ops.call('yb_head_grad_prepare', dfeature.contiguous().float() * self.grad_scale, dzh, dbias, b, chead, cpad, hh * ww)
+        dscaled = dfeature.contiguous().float() * self.grad_scale
+        if self.loss_scale == 'dynamic':
+            dscaled.mul_(self.loss_scale_state(dev)[0])      # exact: the factor is a power of two
+        ops.call('yb_head_grad_prepare', dscaled, dzh, dbias, b, chead, cpad, hh * ww)
         grads[bias] = dbias.mul_(self._unscale)
         self._emit(bias, grads)
         return dzh

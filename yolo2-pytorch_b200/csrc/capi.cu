@@ -112,6 +112,7 @@ int eval_match(const float*, const float*, const int*, const int*, const float*,
                unsigned char*, cudaStream_t);
 int unpack_wgrad(const float*, float*, int, int, int, float, cudaStream_t);
 int grad_guard(float*, long long, float*, int, cudaStream_t);
+int grad_unscale_guard(float*, long long, float*, float*, int*, int, cudaStream_t);
 int conv_wgrad_forward(const void*, const void*, float*, int, int, int, int, int, int, int, int, cudaStream_t);
 int stem7x7(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
 int stem7x7_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
@@ -442,6 +443,11 @@ int yb_unpack_wgrad(const float* dw_krsc, float* dw_oihw, int cout, int cin, int
 
 int yb_grad_guard(float* grads, long long count, float* found_inf, int zero_if_found, yb_stream_t stream) {
   return yb::grad_guard(grads, count, found_inf, zero_if_found, S(stream));
+}
+
+int yb_grad_unscale_guard(float* grads, long long count, float* found_inf, float* factor, int* growth_tracker, int growth_interval,
+                          yb_stream_t stream) {
+  return yb::grad_unscale_guard(grads, count, found_inf, factor, growth_tracker, growth_interval, S(stream));
 }
 
 int yb_resize_batch_u8(const void* src, const long long* src_off, const int* src_hw, void* dst, int batch, int height, int width, int swap_rb,

@@ -866,6 +866,58 @@ int grad_guard(float* buf, long long count, float* found, int zero_if_found, cud
   return check_launch("grad_guard_zero_kernel");
 }
 
+// ------------------------------------------------------------------------------------------------
+// Gradient guard of dynamic loss scaling.  The backward ran at grad_scale * f, where f (device float, a power of two) is the
+// dynamic factor, and un-scaled by 1 / grad_scale only; this pass finishes the un-scaling and moves f.  Detection is the guard's
+// pass 1 (grad_guard_detect_kernel); then, if found, the buffer is zeroed, else multiplied by 1 / f -- exact, a power of two -- and
+// left unwritten when f == 1.  Last, one thread applies GradScaler's rule to f and the growth tracker: backoff 0.5 on overflow,
+// growth 2 after `growth_interval` clean steps in a row, clamped to [2^-24, 2^24] so that a gradient no factor can bring into
+// fp16 range cannot drive f to 0.  It runs after every block has read f, hence a launch of its own.  No host sync; capturable.
+__global__ void grad_unscale_apply_kernel(float4* __restrict__ buf, long long count4, float* __restrict__ tail, int ntail,
+                                          const float* __restrict__ found, const float* __restrict__ factor) {
+  const bool bad = *found != 0.f;
+  const float f = *factor;
+  if (!bad && f == 1.f) return;
+  const float s = bad ? 0.f : 1.f / f;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < count4; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float4 v = bad ? make_float4(0.f, 0.f, 0.f, 0.f) : buf[i];
+    v.x *= s; v.y *= s; v.z *= s; v.w *= s;
+    buf[i] = v;
+  }
+  if (blockIdx.x == 0 && static_cast<int>(threadIdx.x) < ntail) tail[threadIdx.x] = bad ? 0.f : tail[threadIdx.x] * s;
+}
+
+__global__ void loss_scale_update_kernel(const float* __restrict__ found, float* __restrict__ factor, int* __restrict__ tracker, int growth_interval) {
+  float f = *factor;
+  int t = *tracker;
+  if (*found != 0.f) {
+    f *= 0.5f;
+    t = 0;
+  } else if (++t >= growth_interval) {
+    f *= 2.f;
+    t = 0;
+  }
+  *factor = fminf(fmaxf(f, 0x1p-24f), 0x1p24f);
+  *tracker = t;
+}
+
+int grad_unscale_guard(float* buf, long long count, float* found, float* factor, int* tracker, int growth_interval, cudaStream_t stream) {
+  YB_REQUIRE(buf && found && factor && tracker && count > 0 && growth_interval > 0 && (reinterpret_cast<uintptr_t>(buf) & 15) == 0,
+             "grad_unscale_guard: bad argument (16 B aligned buffer, growth_interval > 0)");
+  YB_CUDA(cudaMemsetAsync(found, 0, sizeof(float), stream));
+  const long long count4 = count / 4;
+  const int ntail = static_cast<int>(count - count4 * 4);
+  const int grid = sm_count() * 8;
+  grad_guard_detect_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(buf), count4, buf + count4 * 4, ntail, found);
+  int rc = check_launch("grad_guard_detect_kernel");
+  if (rc) return rc;
+  grad_unscale_apply_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<float4*>(buf), count4, buf + count4 * 4, ntail, found, factor);
+  rc = check_launch("grad_unscale_apply_kernel");
+  if (rc) return rc;
+  loss_scale_update_kernel<<<1, 1, 0, stream>>>(found, factor, tracker, growth_interval);
+  return check_launch("loss_scale_update_kernel");
+}
+
 int unpack_wgrad(const float* g_krsc, float* out_oihw, int cout, int cin, int k, float scale, cudaStream_t stream) {
   YB_REQUIRE(g_krsc && out_oihw && cout > 0 && cin > 0 && (k == 1 || k == 3), "unpack_wgrad: bad argument");
   unpack_wgrad_kernel<<<dim3((cin + 127) / 128, cout), 128, 0, stream>>>(g_krsc, out_oihw, cout, cin, k, scale);

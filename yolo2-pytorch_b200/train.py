@@ -9,6 +9,7 @@ reference (train.py:270,368).  TensorBoard summaries, checkpoint timers and the 
 hot path.  Multi-GPU is one process per GPU (torch.distributed, NCCL) instead of the reference's nn.DataParallel.
 """
 import configparser
+import warnings
 
 import torch
 import torch.distributed as dist
@@ -55,9 +56,29 @@ def build_optimizer(config, params, lr):
     return eval(config.get('train', 'optimizer'))(params, lr)
 
 
+def loss_scale_config(config):
+    """(mode, growth_interval) from `[train] loss_scale` ('static' when absent, or 'dynamic') and `[train] loss_scale_growth_interval`
+    (default 2000, a positive integer).  A bad value raises ValueError naming its key."""
+    def get(key, default):
+        return config.get('train', key).strip() if config.has_option('train', key) else default
+
+    mode = get('loss_scale', 'static')
+    if mode not in ('static', 'dynamic'):
+        raise ValueError('[train] loss_scale must be static or dynamic, got %r' % mode)
+    interval = get('loss_scale_growth_interval', '2000')
+    try:
+        interval = int(interval)
+    except ValueError:
+        raise ValueError('[train] loss_scale_growth_interval must be a positive integer, got %r' % interval) from None
+    if interval <= 0:
+        raise ValueError('[train] loss_scale_growth_interval must be a positive integer, got %d' % interval)
+    return mode, interval
+
+
 def iterate(inference, optimizer, anchors, config, data, reducer=None):
     """One training step (reference Train.iterate, train.py:338-362).  `data`: dict with `tensor` [B,3,H,W] fp32,
-    `yx_min`/`yx_max` [B,G,2] in pixels, `cls` [B,G].  Returns the same kind of dict as the reference."""
+    `yx_min`/`yx_max` [B,G,2] in pixels, `cls` [B,G].  Returns the same kind of dict as the reference; with `[train] loss_scale =
+    dynamic` it also holds `loss_scale`, the device scale (the trainer's static scale times its dynamic factor) the next step runs at."""
     dev = torch.device('cuda', torch.cuda.current_device())
     data = {k: (v.to(dev, non_blocking=True) if torch.is_tensor(v) else v) for k, v in data.items()}
     tensor = data['tensor']
@@ -75,7 +96,9 @@ def iterate(inference, optimizer, anchors, config, data, reducer=None):
         _ddp.set_default_reducer(reducer)          # model.loss normalises the class term through the same communicator
     if reducer is not None:
         sync_replicas(inference, reducer)          # unseeded ranks would otherwise train different models on averaged gradients
-    dnn.trainer.reducer = reducer
+    trainer = dnn.trainer
+    trainer.reducer = reducer
+    trainer.set_loss_scale(*loss_scale_config(config))
     pred = model._inference(inference, tensor)
     rows, cols = pred['feature'].shape[-2:]
     cross_entropy = config.getboolean('train', 'cross_entropy') if config.has_option('train', 'cross_entropy') else True
@@ -92,8 +115,13 @@ def iterate(inference, optimizer, anchors, config, data, reducer=None):
     if getattr(optimizer, '_step_supports_amp_scaling', False):
         # fused torch.optim optimizers skip the update (state untouched) when found_inf is raised -- the overflow guard of the fp16
         # backward (b200.train_engine.backward); the others step on the zeroed gradients
-        optimizer.found_inf = dnn.trainer.found_inf
+        optimizer.found_inf = trainer.found_inf
         optimizer.grad_scale = None
+    elif trainer.loss_scale == 'dynamic' and not getattr(trainer, '_warned_found_inf', False):
+        trainer._warned_found_inf = True
+        warnings.warn('[train] loss_scale = dynamic: %s cannot skip a step on found_inf, so each overflowed step (routine while the scale '
+                      'backs off) is a step on zeroed gradients; a fused optimizer (e.g. torch.optim.Adam(..., fused=True)) skips it'
+                      % type(optimizer).__name__, RuntimeWarning)
     optimizer.step()
     # What is returned is for summaries / logging only (the reference reads .data / float() of it, train.py:353-362), so it is detached:
     # a caller that keeps the dict must not keep the autograd graph -- and with it the parameters' AccumulateGrad nodes, which remember
@@ -102,8 +130,11 @@ def iterate(inference, optimizer, anchors, config, data, reducer=None):
     def _d(v):
         return v.detach() if torch.is_tensor(v) else v
 
-    return dict(height=height, width=width, rows=rows, cols=cols, data=data, pred={k: _d(v) for k, v in pred.items()}, debug=debug,
-                loss_total=loss_total.detach(), loss={k: _d(v) for k, v in loss.items()}, loss_hparam={k: _d(v) for k, v in loss_hparam.items()})
+    out = dict(height=height, width=width, rows=rows, cols=cols, data=data, pred={k: _d(v) for k, v in pred.items()}, debug=debug,
+               loss_total=loss_total.detach(), loss={k: _d(v) for k, v in loss.items()}, loss_hparam={k: _d(v) for k, v in loss_hparam.items()})
+    if trainer.loss_scale == 'dynamic':
+        out['loss_scale'] = trainer.loss_scale_state(dev)[0] * trainer.grad_scale
+    return out
 
 
 class GraphedStep(object):
@@ -117,8 +148,9 @@ class GraphedStep(object):
     * Inputs (host-pinned or device tensors) are copied into static device buffers, then the graph is replayed; the
       returned tensors are static too (overwritten by the next call with the same shapes).
     * One graph per distinct set of input shapes (multi-scale training, `data/sizes`: one per size).
-    * Capture needs two eager warm-up iterations (lazy optimizer state, kernel attribute setup).  Parameters, buffers
-      and optimizer state are restored afterwards, so the first replay is the first real update.
+    * Capture needs two eager warm-up iterations (lazy optimizer state, kernel attribute setup).  Parameters, buffers,
+      optimizer state and the dynamic loss scale's factor and growth tracker are restored afterwards, so the first replay
+      is the first real update.
     * The optimizer must be capture-safe: torch.optim.SGD as is, Adam/AdamW with `capturable=True`.  The learning
       rate is baked into the graph unless it is a tensor (`lr=torch.tensor(...)`).
     * Operand caches keyed by parameter version (packed fp16 weights) are refreshed inside the graph; call
@@ -132,9 +164,14 @@ class GraphedStep(object):
         self.launches = 0          # library kernels replayed so far (bench.py's gpu_launches)
         self.keys = ('tensor', 'yx_min', 'yx_max', 'cls')
 
-    def _snapshot(self):
+    def _snapshot(self, dev):
         mod = self.inference
         tensors = [p.data for p in mod.parameters()] + [b for b in mod.buffers()]
+        mode, interval = loss_scale_config(self.config)
+        if mode == 'dynamic':
+            trainer = mod.dnn.trainer
+            trainer.set_loss_scale(mode, interval)
+            tensors += trainer.loss_scale_state(dev)          # the factor and tracker, created here at 1 and 0 if new
         saved = [(t, t.clone()) for t in tensors]
         state = {}
         for p, st in self.optimizer.state.items():
@@ -163,7 +200,7 @@ class GraphedStep(object):
         red = None if self.reducer is False else (self.reducer if self.reducer is not None else _ddp.default_reducer())
         if red is not None:
             sync_replicas(self.inference, red)      # before the snapshot: the restore below must not undo rank 0's broadcast
-        snap = self._snapshot()
+        snap = self._snapshot(dev)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
