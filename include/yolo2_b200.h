@@ -116,6 +116,18 @@ int yb_conv_choice(int batch, int height, int width, int cin, int cout, int ksiz
 int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
                           int height, int width, int cin, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off, int out_mode,
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream);
+/* The same conv on an input whose channel count is a multiple of 8 but not necessarily of 32 (channel-pruned Darknet-19 / Tiny units):
+ *   x     fp16 NHWC [B,H,W,x_ld], channels [0, cin) read; cin % 8 == 0, x_ld >= cin, x_ld % 8 == 0.  Channels [cin, x_ld) are never read.
+ *   w     fp16 [Cout][k][k][cin_pad] with cin_pad = round_up(cin, 32) and zeros in channels [cin, cin_pad)
+ *         (yb_pack_weight_khw_f16 with that cin_pad).
+ * The GEMM runs the K-blocks of the plain conv on a zero-padded operand (BK from the plain rule on cin_pad); the TMA fills channels
+ * [cin, cin_pad) of each tap's last K-block with zeros.  The result equals yb_conv_bn_act_fwd_ws bit for bit on x materialised with
+ * zeros up to cin_pad and the same tile (flags YB_CONV_FORCE_BN and the M-subtile field are honoured).  Output, epilogue and other
+ * flags as yb_conv_bn_act_fwd.  Never the Cin = 32 halo-tile kernel; YB_CONV_POOL2X2, YB_CONV_CHAIN1X1 and YB_CONV_FORCE_STREAMK are
+ * refused with YB_ERR_UNSUPPORTED, bad shapes, pitches or pointers with YB_ERR_BAD_ARG, in both cases before anything is written. */
+int yb_conv_bn_act_tail_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
+                            int height, int width, int cin, int cin_pad, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off,
+                            int out_mode, int flags, yb_stream_t stream);
 /* Two units in one launch: the conv above (x, w, scale, shift, slope; Cin, Cout, ksize) followed by a 1x1 stride-1 unit whose input
  * is that conv's whole output -- w2 fp16 [Cout2][1][1][Cout], scale2 / shift2 [Cout2], slope2.  Only the second unit's output is
  * written: y fp16 NHWC [B,H,W,y_ld] at channels [y_ch_off, y_ch_off + Cout2).  The first output stays on the SM and goes into the

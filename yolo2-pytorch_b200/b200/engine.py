@@ -74,6 +74,15 @@ class ConvUnit(object):
         # strict precision: which operand of this unit is split into fp16 hi + lo (set by DarknetEngine.set_precision)
         self.split_a = self.split_w = False
         self.out_lo = False      # the epilogue also writes the rounding residual (a consumer reads [hi | lo])
+        # channel layout of a channel-pruned network (DarknetEngine._set_layout): the unit reads in_ch channels per pixel and stores out_ch,
+        # its own input channel i sits at channel cin_index[i] of the input (None: at i), and its packed weight has k_ch input channels
+        # per tap (round_up(in_ch, 32); zero past the real ones)
+        self.in_ch, self.out_ch, self.k_ch, self.cin_index = self.cin, self.cout, self.cin, None
+
+    @property
+    def padded(self):
+        """Whether the operands are zero-padded to a channel layout other than the conv's own widths."""
+        return self.in_ch != self.cin or self.k_ch != self.cin or self.out_ch != self.cout or self.cin_index is not None
 
     @property
     def cout(self):
@@ -99,7 +108,9 @@ class ConvUnit(object):
         wver = (w.data_ptr(), w._version)
         wver = wver + (self.split_a, self.split_w)
         if force or wver != self._wver:
-            if first_layer:
+            if self.padded:
+                self.w16 = self._layout_weight(w.detach(), first_layer)
+            elif first_layer:
                 self.w16 = w.detach().contiguous()
             elif self.split_a or self.split_w:
                 self.w16 = ops.pack_weight_split_f16(w.detach().contiguous(), self.split_a, self.split_w)
@@ -111,6 +122,7 @@ class ConvUnit(object):
             bver = tuple((t.data_ptr(), t._version) for t in ts)
             if bver != self._bver:
                 self.scale, self.shift = ops.bn_fold(*(t.detach().contiguous() for t in ts), eps=self.bn.eps)
+                self._pad_epilogue()
                 self._bver = bver
         else:
             b = self.conv.bias
@@ -119,7 +131,24 @@ class ConvUnit(object):
                 self.scale = torch.ones(self.cout, dtype=torch.float32, device=w.device)
                 self.shift = (b.detach().float().contiguous().clone() if b is not None
                               else torch.zeros(self.cout, dtype=torch.float32, device=w.device))
+                self._pad_epilogue()
                 self._bver = bver
+
+    def _layout_weight(self, w, first_layer):
+        """The weight scattered onto the unit's channel layout: filters [cout, out_ch) and input channels outside cin_index are zero.
+        fp32 [out_ch,3,k,k] for the first-layer kernel, else fp16 [out_ch,k,k,k_ch]."""
+        cout, cin, k, _ = w.shape
+        wp = torch.zeros(self.out_ch, cin if first_layer else self.k_ch, k, k, dtype=torch.float32, device=w.device)
+        idx = torch.arange(cin) if self.cin_index is None else self.cin_index
+        wp[:cout, idx.to(w.device)] = w.float()
+        return wp.contiguous() if first_layer else ops.pack_weight_f16(wp.contiguous(), 0)
+
+    def _pad_epilogue(self):
+        """Scale 1 and shift 0 on the zero filters [cout, out_ch): they store exact zeros."""
+        n = self.out_ch - self.cout
+        if n:
+            self.scale = torch.cat([self.scale, torch.ones(n, dtype=torch.float32, device=self.scale.device)])
+            self.shift = torch.cat([self.shift, torch.zeros(n, dtype=torch.float32, device=self.shift.device)])
 
 
 class StrictPlan(object):
@@ -160,24 +189,24 @@ class DarknetPlan(object):
         f16 = dict(dtype=torch.float16, device=device)
         self.batch, self.height, self.width = batch, height, width
         h, w = height // 2, width // 2
-        self.a0 = torch.empty(batch, h, w, units1[0].cout, **f16)
+        self.a0 = torch.empty(batch, h, w, units1[0].out_ch, **f16)
         self.l1 = []   # (out, pooled or None) per layers1 unit after the first
         for u, pooled in zip(units1[1:], pools1[1:]):
-            out = torch.empty(batch, h, w, u.cout, **f16)
+            out = torch.empty(batch, h, w, u.out_ch, **f16)
             if pooled:
                 h, w = h // 2, w // 2
-                self.l1.append((out, torch.empty(batch, h, w, u.cout, **f16)))
+                self.l1.append((out, torch.empty(batch, h, w, u.out_ch, **f16)))
             else:
                 self.l1.append((out, None))
         self.h16, self.w16 = h, w
-        self.pt = torch.empty(batch, h, w, unit_pt.cout, **f16)
-        self.x1_pool = torch.empty(batch, h // 2, w // 2, units1[-1].cout, **f16)
+        self.pt = torch.empty(batch, h, w, unit_pt.out_ch, **f16)
+        self.x1_pool = torch.empty(batch, h // 2, w // 2, units1[-1].out_ch, **f16)
         h, w = h // 2, w // 2
         self.h32, self.w32 = h, w
-        self.cat_ch = unit_pt.cout * 4 + units2[-1].cout
+        self.cat_ch = unit_pt.out_ch * 4 + units2[-1].out_ch
         self.cat = torch.empty(batch, h, w, self.cat_ch, **f16)
-        self.l2 = [torch.empty(batch, h, w, u.cout, **f16) for u in units2[:-1]]
-        self.l3 = torch.empty(batch, h, w, units3[0].cout, **f16)
+        self.l2 = [torch.empty(batch, h, w, u.out_ch, **f16) for u in units2[:-1]]
+        self.l3 = torch.empty(batch, h, w, units3[0].out_ch, **f16)
         self.feature = torch.empty(batch, units3[1].cout, h, w, dtype=torch.float32, device=device)
         # stream-K scratch (partial sums + flags): per plan, because plans are what run concurrently on different streams
         self.workspace = ops.conv_workspace(device)
@@ -185,8 +214,8 @@ class DarknetPlan(object):
 
 class DarknetEngine(object):
     def __init__(self, dnn):
-        """`dnn` is a model.yolo2.Darknet (parameter holder).  Units are discovered from its
-        nn.Sequential containers so channel-pruned checkpoints (model.ConfigChannels) just work."""
+        """`dnn` is a model.yolo2.Darknet (parameter holder).  Units are discovered from its nn.Sequential containers, so channel-pruned
+        checkpoints (model.ConfigChannels) and `ratio` models run at their own widths on the layout of `_set_layout`."""
         def unit(m):
             return ConvUnit(m.conv, m.bn if m.has_bn else None, m.has_act)
 
@@ -205,6 +234,7 @@ class DarknetEngine(object):
         self.plans = {}
         if not self.pools1[0]:
             raise RuntimeError('Darknet: layers1.0 must be followed by MaxPool2d (fused first-layer kernel)')
+        self._set_layout()
         self.precision = 'fast'
         self.set_precision(os.environ.get('YB_PRECISION', 'fast'))
         # the fast forward fuses a layers1 max-pool into the conv before it wherever the library has a pooled form for that launch;
@@ -216,18 +246,55 @@ class DarknetEngine(object):
         self.fuse_chain = True
         self._chain_ok = {}
 
+    def _set_layout(self):
+        """Channel layout of the activation buffers.  Every unit stores round_up(Cout, 8) channels (the extra filters are zero with scale 1
+        and shift 0, so they hold exact zeros); layers1.0 stores the first-layer kernel's 32.  The passthrough stores P = round_up(Cpt, 8),
+        the reorg writes its 4 offsets as 4 groups of P channels and layers2's last unit writes at channel 4P, so the reference's concat
+        channel s*Cpt + c (model/yolo2.py:129, the map of get_mapper(94)) sits at s*P + c and 4*Cpt + j at 4P + j.  Each unit reads its
+        producer's stored width; its weight is scattered onto that layout with zeros in the gaps.  At full width (every width a multiple
+        of 32) nothing is padded and every operand is the unit's own."""
+        u0 = self.units1[0]
+        if u0.cout > 32:
+            raise ValueError('Darknet: %s has %d filters; the first-layer kernel runs at most 32' % (self._k1[0], u0.cout))
+        u0.out_ch = 32
+        prev = 32
+        for u in self.units1[1:] + self.units2:         # layers2.1 reads the pooled output of layers1's last unit
+            u.in_ch, u.out_ch = prev, ops.round_up(u.cout, 8)
+            prev = u.out_ch
+        pt, u27 = self.unit_pt, self.units2[-1]
+        pt.in_ch, pt.out_ch = self.units1[-1].out_ch, ops.round_up(pt.cout, 8)
+        u30, u31 = self.units3
+        u30.in_ch, u30.out_ch = 4 * pt.out_ch + u27.out_ch, ops.round_up(u30.cout, 8)
+        if pt.out_ch != pt.cout:
+            u30.cin_index = self.concat_index(pt.cout, pt.out_ch, u27.cout)
+        u31.in_ch = u30.out_ch      # the head stores fp32 NCHW at its own width
+        for u in self.all_units()[1:]:
+            u.k_ch = ops.round_up(u.in_ch, 32)
+
+    @staticmethod
+    def concat_index(c_pt, p, c_trunk):
+        """Layout channel of each channel of the reference's concat [reorg(passthrough) | layers2]: s*c_pt + c -> s*p + c, 4*c_pt + j -> 4p + j."""
+        return torch.cat([torch.arange(c_pt) + s * p for s in range(4)] + [torch.arange(c_trunk) + 4 * p])
+
+    def padded_unit(self):
+        """The state_dict prefix of the first unit whose operands are padded to the channel layout, or None at full width."""
+        for key, u in zip(self.unit_keys(), self.all_units()):
+            if u.padded:
+                return key
+        return None
+
     def _chained_form(self, u, v, x, conv_flags):
         """Whether the library runs unit u on input x [B,H,W,C] with the 1x1 unit v fused into its epilogue, with the same bits as v's
         own launch (which must not split along K), asked once per shape."""
         b, h, w, _ = x.shape
-        key = (u.cin, u.cout, u.ksize, v.cout, b, h, w, conv_flags)
+        key = (u.in_ch, u.out_ch, u.ksize, v.out_ch, b, h, w, conv_flags)
         ok = self._chain_ok.get(key)
         if ok is None:
-            ok = v.ksize == 1 and v.cin == u.cout and v.cout <= 64 and v.cout % 8 == 0
+            ok = v.ksize == 1 and u.in_ch % 32 == 0 and v.in_ch == u.out_ch and v.out_ch <= 64 and v.out_ch % 8 == 0
             if ok:
                 try:
-                    ok = (ops.conv_choice(b, h, w, u.cin, u.cout, u.ksize, flags=conv_flags | ops.CONV_CHAIN1X1)['kernel'] == 'conv_wide_kernel'
-                          and not ops.conv_choice(b, h, w, v.cin, v.cout, 1, flags=conv_flags)['streamk'])
+                    ok = (ops.conv_choice(b, h, w, u.in_ch, u.out_ch, u.ksize, flags=conv_flags | ops.CONV_CHAIN1X1)['kernel'] == 'conv_wide_kernel'
+                          and not ops.conv_choice(b, h, w, v.in_ch, v.out_ch, 1, flags=conv_flags)['streamk'])
                 except RuntimeError:
                     ok = False
             self._chain_ok[key] = ok
@@ -236,11 +303,12 @@ class DarknetEngine(object):
     def _pooled_form(self, u, x, conv_flags):
         """Whether the library runs unit u on input x [B,H,W,C] with the 2x2 max-pool fused on the two-consumer tile (asked once per shape)."""
         b, h, w, _ = x.shape
-        key = (u.cin, u.cout, u.ksize, b, h, w, conv_flags)
+        key = (u.in_ch, u.out_ch, u.ksize, b, h, w, conv_flags)
         ok = self._pool_ok.get(key)
         if ok is None:
             try:
-                ok = ops.conv_choice(b, h, w, u.cin, u.cout, u.ksize, flags=conv_flags | ops.CONV_POOL2X2)['kernel'] == 'conv_wide_kernel'
+                ok = (u.in_ch % 32 == 0 and
+                      ops.conv_choice(b, h, w, u.in_ch, u.out_ch, u.ksize, flags=conv_flags | ops.CONV_POOL2X2)['kernel'] == 'conv_wide_kernel')
             except RuntimeError:
                 ok = False
             self._pool_ok[key] = ok
@@ -255,6 +323,10 @@ class DarknetEngine(object):
         (default STRICT_KEEP) -- inside the reference contract of 1e-3 at ~2.6x the tensor-core work."""
         if precision not in PRECISIONS:
             raise ValueError('precision must be one of %s' % (PRECISIONS,))
+        padded = self.padded_unit()
+        if precision == 'strict' and padded is not None:
+            raise ValueError("Darknet: precision 'strict' needs every width a multiple of 32 and layers1.0 at 32 filters; %s is pruned to "
+                             "another width" % padded)
         keep = STRICT_KEEP if keep is None else keep
         units = dict(zip(self.unit_keys(), self.all_units()))
         for key, u in units.items():
@@ -320,6 +392,10 @@ class DarknetEngine(object):
             return self._forward_strict(x, u8, p, conv_flags, collect)
 
         def conv(u, src, dst, **kw):
+            if u.in_ch % 32:
+                if ref:
+                    raise ValueError('Darknet: the CUDA-core reference conv has no channel-tail form')
+                return ops.conv_bn_act_tail(src, u.w16, u.scale, u.shift, u.slope, u.in_ch, out=dst, flags=conv_flags, **kw)
             return ops.conv_bn_act(src, u.w16, u.scale, u.shift, u.slope, out=dst, flags=conv_flags, ref=ref, workspace=p.workspace, **kw)
 
         u0 = self.units1[0]
@@ -350,7 +426,7 @@ class DarknetEngine(object):
             # 416x416); tests that inspect every layer (collect / ref) keep the two steps.  last1's full-resolution output feeds the
             # passthrough, so its pool stays a kernel of its own.
             fuse_pool = pooled is not None and u is not last1 and collect is None and not ref and (
-                (u.cin == 32 and u.ksize == 3 and u.cout <= 64 and (conv_flags & (ops.CONV_NO_SMALLK | ops.CONV_C32_IM2COL)) == 0
+                (u.in_ch == 32 and u.ksize == 3 and u.out_ch <= 64 and (conv_flags & (ops.CONV_NO_SMALLK | ops.CONV_C32_IM2COL)) == 0
                  and conv_flags < 256) or (self.fuse_wide_pool and self._pooled_form(u, cur, conv_flags)))
             if fuse_pool:
                 ops.conv_bn_act(cur, u.w16, u.scale, u.shift, u.slope, out=pooled, flags=conv_flags | ops.CONV_POOL2X2, workspace=p.workspace)
@@ -373,7 +449,7 @@ class DarknetEngine(object):
             if collect is not None:
                 collect[key] = out
             cur = out
-        conv(self.units2[-1], cur, p.cat, y_ch_off=self.unit_pt.cout * 4)
+        conv(self.units2[-1], cur, p.cat, y_ch_off=self.unit_pt.out_ch * 4)
         conv(self.units3[0], p.cat, p.l3)
         conv(self.units3[1], p.l3, p.feature, out_mode=ops.OUT_F32_NCHW)
         if collect is not None:

@@ -26,6 +26,8 @@ SIGNATURES = {
     'yb_conv_choice': [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_int * 6)],
     'yb_conv_bn_act_fwd_ws': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int, P,
                               c_longlong, P],
+    'yb_conv_bn_act_tail_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int,
+                                P],
     'yb_conv_bn_act_chain_fwd': [P, P, P, P, c_float, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong,
                                  c_int, c_int, P, c_longlong, P],
     'yb_conv_bn_act_split_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int,

@@ -209,6 +209,31 @@ def conv_bn_act(x, w, scale, shift, slope, out=None, out_mode=OUT_F16_NHWC, y_ch
     return out
 
 
+def round_up(n, m):
+    return (n + m - 1) // m * m
+
+
+def conv_bn_act_tail(x, w, scale, shift, slope, cin, out=None, out_mode=OUT_F16_NHWC, y_ch_off=0, flags=0):
+    """yb_conv_bn_act_tail_fwd: conv_bn_act on the first `cin` channels of x (cin % 8 == 0, not necessarily of 32).
+    x: fp16 [B,H,W,x_ld], x_ld >= cin; w: fp16 [Cout,k,k,round_up(cin, 32)], zero in channels >= cin (pack_weight_f16 of a weight
+    zero-padded on Cin).  out as conv_bn_act."""
+    _req(x, torch.float16, 'x'); _req(w, torch.float16, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    b, h, wd, x_ld = x.shape
+    cout, k, _, cin_pad = w.shape
+    if out is None:
+        out = (torch.empty(b, h, wd, cout, dtype=torch.float16, device=x.device) if out_mode == OUT_F16_NHWC
+               else torch.empty(b, cout, h, wd, dtype=torch.float32, device=x.device))
+    if out_mode == OUT_F16_NHWC:
+        _req(out, torch.float16, 'out')
+        y_ld = out.shape[-1]
+    else:
+        _req(out, torch.float32, 'out')
+        y_ld = 0
+    _ck(_l.load().yb_conv_bn_act_tail_fwd(_p(x), _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, cin, cin_pad, cout, k, x_ld, y_ld,
+                                          y_ch_off, out_mode, flags, _s()), 'yb_conv_bn_act_tail_fwd')
+    return out
+
+
 def _conv_chain(x, w, scale, shift, slope, chain, out, out_mode, y_ch_off, cin, flags, ref, workspace):
     w2, scale2, shift2, slope2 = chain
     _req(w2, torch.float16, 'w2'); _req(scale2, torch.float32, 'scale2'); _req(shift2, torch.float32, 'shift2')

@@ -138,6 +138,8 @@ int conv2d_choice(int, int, int, int, int, int, int, int, int, int, int, int, in
 int conv2d_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, int, int, int, int,
                    long long, int, int, int, void*, long long, double*, int, int, const float*, const float*, int, const ConvChain*, cudaStream_t);
 int pack_weight_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
+int conv_tail_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, int, long long, int,
+                      int, int, cudaStream_t);
 int stem3x3_s2(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
 int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
@@ -225,6 +227,13 @@ int yb_conv_bn_act_fwd_ws(const void* x, const void* w, const float* scale, cons
                           int flags, void* workspace, long long workspace_bytes, yb_stream_t stream) {
   return yb::conv_igemm_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cout, ksize, x_ld, y_ld, y_ch_off, out_mode,
                                 flags, workspace, workspace_bytes, nullptr, 0, -1, nullptr, nullptr, 0, S(stream));
+}
+
+int yb_conv_bn_act_tail_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
+                            int height, int width, int cin, int cin_pad, int cout, int ksize, int x_ld, long long y_ld, int y_ch_off,
+                            int out_mode, int flags, yb_stream_t stream) {
+  return yb::conv_tail_forward(x, w, scale, shift, slope, y, batch, height, width, cin, cin_pad, cout, ksize, x_ld, y_ld, y_ch_off, out_mode,
+                               flags, S(stream));
 }
 
 int yb_conv_bn_act_chain_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, const void* w2, const float* scale2,

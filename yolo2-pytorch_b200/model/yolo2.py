@@ -155,6 +155,14 @@ class Darknet(model.Backbone):
                 self._engine.set_precision(self._precision)
         return self._engine
 
+    @property
+    def trainer(self):
+        padded = self.engine.padded_unit()
+        if padded is not None:
+            raise ValueError('Darknet: training needs every width a multiple of 32 and layers1.0 at 32 filters; %s is pruned to another '
+                             'width (channel-pruned models run in eval mode)' % padded)
+        return model.Backbone.trainer.fget(self)
+
     def drop_operands(self):
         """The engine's per-unit operands (Darknet caches nothing on the module)."""
         if self._engine is not None:
@@ -206,7 +214,11 @@ class Tiny(model.Backbone):
     Kernel chain: the 3->16 first layer runs on the fused first-layer kernel with its 16 filters zero-padded to 32 (the
     extra channels come out as exact zeros and the next layer's weights are zero-padded on the input side to match), the
     two Cin = 32 layers on the halo-tile wgmma kernel with the 2x2 max-pool fused, the rest on the implicit-GEMM
-    kernel; `ConstantPad2d + MaxPool2d(2, stride=1)` is one HBM kernel."""
+    kernel; `ConstantPad2d + MaxPool2d(2, stride=1)` is one HBM kernel.
+
+    Channel-pruned checkpoints (model.ConfigChannels) run at their own widths in eval mode: every unit but the head stores
+    round_up(Cout, 8) channels (zero filters), the next unit's weight is zero-padded on the input side to that width, and a unit whose
+    input width is not a multiple of 32 runs on the channel-tail conv (yb_conv_bn_act_tail_fwd)."""
 
     TRAINER = _train.TinyTrainer
 
@@ -234,6 +246,21 @@ class Tiny(model.Backbone):
         """[(state_dict prefix 'layers.N', ConvUnit, followed_by)] in network order."""
         keys = ['layers.%d' % i for i, m in enumerate(self.layers) if not m.is_pool]
         return [(k, u, after) for k, (u, after) in zip(keys, self._plan())]
+
+    def padded_unit(self):
+        """The prefix of the first unit after layers.0 whose width is not a multiple of 32 (the head aside), or None."""
+        for key, u, _ in self.unit_keys()[1:-1]:
+            if u.cout % 32:
+                return key
+        return None
+
+    @property
+    def trainer(self):
+        padded = self.padded_unit()
+        if padded is not None:
+            raise ValueError('Tiny: training needs every width after layers.0 a multiple of 32; %s is pruned to another width '
+                             '(channel-pruned models run in eval mode)' % padded)
+        return model.Backbone.trainer.fget(self)
 
     def drop_operands(self):
         """The padded operands and the units' own (ConvUnit.refresh)."""
@@ -301,22 +328,30 @@ class Tiny(model.Backbone):
             raise RuntimeError('Tiny: the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
         w0, sc0, sh0 = self._padded('u0', u0, 32, 3, True)
         cur = _ops.conv0_bn_leaky_pool(x, w0, sc0, sh0, u0.slope)          # [B,H/2,W/2,32], channels >= cout are exact zeros
-        chan = 32
+        chan = 32                                                          # channels per pixel of `cur`
         for i, (u, after) in enumerate(plan[1:], 1):
             last = i == len(plan) - 1
-            if u.cin != chan:                                              # input side zero-padded to the producer's width
-                w_op, scale, shift = self._padded('u%d' % i, u, u.cout, chan, False)
+            cout_to = u.cout if last else _ops.round_up(u.cout, 8)          # stored width; the head writes fp32 NCHW at its own
+            cin_to = _ops.round_up(chan, 32)
+            if u.cin != cin_to or u.cout != cout_to:                       # zero-padded to the producer's width and the stored one
+                w_op, scale, shift = self._padded('u%d' % i, u, cout_to, cin_to, False)
             else:
                 w_op, scale, shift = u.w16, u.scale, u.shift
-            if last:
-                return _ops.conv_bn_act(cur, w_op, scale, shift, u.slope, out_mode=_ops.OUT_F32_NCHW)
-            fuse = after == 'pool' and chan == 32 and u.ksize == 3 and u.cout <= 64
-            if fuse:
-                cur = _ops.conv_bn_act(cur, w_op, scale, shift, u.slope, flags=_ops.CONV_POOL2X2)
+            if chan % 32:
+                def conv(**kw):
+                    return _ops.conv_bn_act_tail(cur, w_op, scale, shift, u.slope, chan, **kw)
             else:
-                cur = _ops.conv_bn_act(cur, w_op, scale, shift, u.slope)
+                def conv(**kw):
+                    return _ops.conv_bn_act(cur, w_op, scale, shift, u.slope, **kw)
+            if last:
+                return conv(out_mode=_ops.OUT_F32_NCHW)
+            fuse = after == 'pool' and chan == 32 and u.ksize == 3 and cout_to <= 64
+            if fuse:
+                cur = conv(flags=_ops.CONV_POOL2X2)
+            else:
+                cur = conv()
                 if after == 'pool':
                     cur = _ops.maxpool2x2(cur)
                 elif after == 'pool_s1':
                     cur = _ops.maxpool2x2_s1(cur)
-            chan = u.cout
+            chan = cout_to
