@@ -361,17 +361,23 @@ int yb_eval_match(const float* det_yx_min, const float* det_yx_max, const int* d
                   unsigned char* tp, yb_stream_t stream);
 
 /* ---- MobileNet plugin (model/mobilenet.py:25-85), inference ------------------------------------------------- */
-/* conv_bn(3,32,stride 2) + BN + ReLU: x fp32 NCHW [B,3,H,W] -> y fp16 NHWC [B,H/2,W/2,32] (model/mobilenet.py:25-30). */
+/* conv_bn(3,32,stride 2) + BN + ReLU: x fp32 NCHW [B,3,H,W] -> y fp16 NHWC [B,H/2,W/2,32] (model/mobilenet.py:25-30).  H and W even (odd is
+ * refused, output untouched); any H != W.  A 27-term fp32 fmaf chain per output, then one fp32 scale / shift and RN16. */
 int yb_mb_conv0_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch,
                             int height, int width, yb_stream_t stream);
-/* conv_dw: depthwise 3x3 (stride 1 or 2, pad 1) + BN + ReLU on fp16 NHWC; w fp32 [C][9] (model/mobilenet.py:33-38). */
+/* conv_dw: depthwise 3x3 (stride 1 or 2, pad 1) + BN + ReLU on fp16 NHWC; w fp32 [C][9] (model/mobilenet.py:33-38).  C % 8 == 0, H and W
+ * multiples of the stride, w / scale / shift 16 B aligned (otherwise refused, output untouched); any C/8 group count, any output width (8 output
+ * pixels per thread from ow = 52, 4 below, ragged last strips).  A 9-term fp32 fmaf chain per channel, then the epilogue. */
 int yb_dwconv3x3_bn_relu_fwd(const void* x, const float* w_c9, const float* scale, const float* shift, void* y, int batch, int height,
                              int width, int channels, int stride, yb_stream_t stream);
 
 /* ---- ResNet plugin (model/resnet.py:28-147), inference --------------------------------------------------------
  * stem: nn.Conv2d(3, 64, 7, stride 2, pad 3) + BatchNorm2d + ReLU (:107-109), x fp32 NCHW -> y fp16 NHWC [B,H/2,W/2,64]; nn.MaxPool2d(3, 2, 1) (:110);
  * x[:, ::2, ::2, :] -- a stride-2 "same" conv is its stride-1 form at the even pixels, so the stride-2 3x3 / 1x1 convs of the blocks (:33,:39,:65,:73)
- * run on yb_conv_bn_act_fwd + this selection; out = relu(a + b), the residual join (:58-59,:100-101). */
+ * run on yb_conv_bn_act_fwd + this selection; out = relu(a + b), the residual join (:58-59,:100-101).
+ * Limits: the stem needs even H and W (odd is refused, output untouched) and sums its 147 taps as one fp32 fmaf chain in (ci, r, s) order; the
+ * pool, subsample2 and add_relu need C % 8 == 0 (count % 8 == 0) and take any H, W >= 1.  The pool follows torch's max_pool2d: the first maximum
+ * in scan order, NaN if the window holds one.  subsample2 and add_relu are bit-exact restatements (add_relu may run in place). */
 int yb_stem7x7_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height, int width,
                            yb_stream_t stream);
 int yb_maxpool3x3_s2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
@@ -394,7 +400,8 @@ int yb_conv1x1_preact_fwd(const void* x, const void* w, const float* pre_scale, 
  * pooled tensor (pooling and a 1x1 conv commute in exact arithmetic).  H, W even, C and x_ld multiples of 8. */
 int yb_bn_relu_avgpool2x2_f16(const void* x, int x_ld, const float* scale, const float* shift, void* y, int batch, int height, int width,
                               int channels, yb_stream_t stream);
-/* yb_maxpool3x3_s2_f16 writing channels [y_ch_off, y_ch_off + C) of y [B,(H+1)/2,(W+1)/2,y_ld] (the stem pool into the first block's buffer). */
+/* yb_maxpool3x3_s2_f16 writing channels [y_ch_off, y_ch_off + C) of y [B,(H+1)/2,(W+1)/2,y_ld] (the stem pool into the first block's buffer);
+ * the same window, so also NaN for a window holding a NaN. */
 int yb_maxpool3x3_s2_ld_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
 
 /* ---- DenseNet plugin, training (b200.train_engine.DenseNetTrainer) ------------------------------------------------------------------
@@ -458,7 +465,7 @@ int yb_pack_weight_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, 
 int yb_stem3x3_s2_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height,
                               int width, int pad, yb_stream_t stream);
 /* F.max_pool2d(x, 3, stride=2) (no padding, floor): x [B,H,W,C] -> channels [y_ch_off, y_ch_off + C) of y [B,(H-3)/2+1,(W-3)/2+1,y_ld].
- * H, W >= 3; C, y_ld, y_ch_off multiples of 8. */
+ * H, W >= 3; C, y_ld, y_ch_off multiples of 8.  NaN for a window holding a NaN, as torch. */
 int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
 /* F.avg_pool2d(x, 3, stride=1, padding=1, count_include_pad=True): x, y [B,H,W,C]; y = fp16(fp32 sum of the in-range window / 9). */
 int yb_avgpool3x3_s1_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
@@ -517,12 +524,16 @@ int yb_pack_weights_khw_batch(const yb_pack_khw_unit* units_dev, int num_units, 
  * the activations are the generic train-mode kernels above (slope 0 = ReLU, slope 1 = identity); the 3x3 / 1x1 convs and their gradients are the
  * wgmma kernels, a stride-2 conv's backward being the stride-1 gradients of the zero-inserted dz (yb_upsample2_zero_f16).
  *   stem7x7_raw   the stem conv output z, fp16 NHWC [B,H/2,W/2,64], no BatchNorm, no ReLU;
- *   stem7x7_wgrad dw fp32 OIHW [64,3,7,7] (overwritten) from the fp32 NCHW image and dz fp16 NHWC [B,H/2,W/2,64];
+ *   stem7x7_wgrad dw fp32 OIHW [64,3,7,7] (overwritten) from the fp32 NCHW image and dz fp16 NHWC [B,H/2,W/2,64]; even H, W (odd: refused, dw
+ *                 untouched); each weight is an fp32 chain of 16 ceil(slabs / grid) products (16-pixel slabs, grid = min(ceil(pixels / 256),
+ *                 4 SMs): 5248 at 64 x 416^2 on 132 SMs), then grid fp32 atomics, in no fixed order;
  *   maxpool bwd   dx [B,H,W,C] from the pool's input x [B,H,W,C] and dy [B,(H+1)/2,(W+1)/2,C]: each output's gradient goes to the first maximum of
- *                 its window in scan order (torch's CPU rule); deterministic;
+ *                 its window in scan order, a NaN replacing it (torch's CPU rule); the at most 4 gradients of a pixel are added in fp32 in
+ *                 (oy, ox) order and rounded once; deterministic, bit-exact;
  *   upsample2_zero y [B,H,W,C] = x [B,(H+1)/2,(W+1)/2,C] at the even pixels, 0 elsewhere (the transpose of yb_subsample2_f16);
  *   residual_bwd  out [B,H,W,C] = (y > 0) ? g_a + S^T g_b : 0 with one rounding: y = the block input (NULL = no mask), g_a [B,H,W,C], g_b (NULL =
- *                 none) [B,H,W,C] for stride_b = 1 or [B,(H+1)/2,(W+1)/2,C] zero-inserted for stride_b = 2.  C % 8 == 0 for all four fp16 kernels. */
+ *                 none) [B,H,W,C] for stride_b = 1 or [B,(H+1)/2,(W+1)/2,C] zero-inserted for stride_b = 2, odd H and W included.  C % 8 == 0
+ *                 for all four fp16 kernels; they are bit-exact. */
 int yb_stem7x7_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, yb_stream_t stream);
 int yb_stem7x7_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream);
 int yb_maxpool3x3_s2_bwd_f16(const void* x, const void* dy, void* dx, int batch, int height, int width, int channels, yb_stream_t stream);
@@ -533,7 +544,11 @@ int yb_residual_bwd_f16(const void* y, const void* g_a, const void* g_b, int str
 /* Training of the MobileNet plugin: what torch autograd does for conv_bn / conv_dw (model/mobilenet.py:25-38).  The raw forms return the conv
  * output before BatchNorm / ReLU (train-mode statistics come from yb_bn_stats / yb_bn_finalize, the activation from yb_bn_act_apply with slope 0);
  * height / width are always those of the conv INPUT.  dgrad: da fp16 [B,H,W,C] from dz fp16 [B,H/stride,W/stride,C]; wgrad: dw fp32 [C][9]
- * (overwritten) from the input activation a and dz; first layer: dw fp32 OIHW [32,3,3,3] (overwritten) from the fp32 NCHW image and dz. */
+ * (overwritten) from the input activation a and dz; first layer: dw fp32 OIHW [32,3,3,3] (overwritten) from the fp32 NCHW image and dz.
+ * Limits: the first-layer forms need even H and W; the depthwise forms C % 8 == 0 and H, W multiples of the stride; the depthwise wgrad also
+ * C <= 1024 and 256 % (C / 8) == 0, i.e. C in {8, 16, ..., 1024} (otherwise refused, dw untouched).  The weight gradients are fp32 chains per
+ * thread (depthwise: ceil(pixels / (grid lanes)) products, lanes = 256 / (C / 8), grid = min(ceil(pixels / (16 lanes)), 4 SMs); first layer:
+ * lanes = 8, grid = min(ceil(pixels / 256), 6 SMs)), then lanes shared and grid global fp32 atomics, in no fixed order. */
 /* Strict-precision forms of the two MobileNet-specific layers (`[b200] precision = strict` on this plugin): activations are [hi | lo] fp16 pairs,
  * y_hi_lo = [B,H/2,W/2,64] for the first conv, x_hi_lo [B,H,W,2C] -> y_hi_lo [B,H/stride,W/stride,2C] for the depthwise conv (computed on hi + lo in
  * fp32); the pointwise convs and the head run yb_conv_bn_act_split_fwd. */

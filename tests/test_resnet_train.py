@@ -1,9 +1,9 @@
 """Training of the ResNet plugin (model.resnet in train() mode, b200.train_engine.ResNetTrainer).
 
 CPU: the train-mode restatement (tests/resnet_train_oracle.py) against one step executed with the reference's own modules
-(tests/golden/make_golden_resnet_train.py), and the trainer's gradient order.  GPU: the five training kernels against torch autograd, one step
-of resnet18 / resnet50 against the restatement with CPU autograd plus descent and the eval() hand-over, and the CUDA-graph step against the
-eager one."""
+(tests/golden/make_golden_resnet_train.py), and the trainer's gradient order.  GPU: one step of resnet18 / resnet50 against the restatement
+with CPU autograd plus descent and the eval() hand-over, and the CUDA-graph step against the eager one.  The training kernels themselves are
+checked element by element against float64 in test_plugin_ops_contract.py."""
 import configparser
 import os
 
@@ -144,73 +144,6 @@ def test_resnet_stride2_backward_is_transpose_of_subsample():
 # ------------------------------------------------------------------------------------------------
 # GPU
 # ------------------------------------------------------------------------------------------------
-def _nhwc16(t):
-    return t.permute(0, 2, 3, 1).contiguous().half().to(DEV)
-
-
-@pytest.mark.gpu
-def test_resnet_training_kernels_vs_torch():
-    """The five ResNet training kernels against torch on fp16-representable data: stem raw forward and weight gradient, max-pool backward
-    (with deliberate ties: a tied gradient lands on the element torch's CPU kernel picks), the zero-insert (bit-exact) and the block-boundary
-    gradient (one rounding, with and without mask and skip stride)."""
-    from b200 import ops
-    gen = torch.Generator().manual_seed(11)
-    # stem: raw forward and weight gradient
-    for (b, h, w) in ((2, 32, 48), (1, 64, 32)):
-        x = torch.rand(b, 3, h, w, generator=gen)
-        w7 = torch.randn(64, 3, 7, 7, generator=gen) * 0.1
-        z = torch.empty(b, h // 2, w // 2, 64, dtype=torch.float16, device=DEV)
-        ops.call('yb_stem7x7_raw_fwd', x.to(DEV), w7.to(DEV), z, b, h, w)
-        assert rel_err(z.permute(0, 3, 1, 2), F.conv2d(x, w7, None, 2, 3)) <= 1e-3, (b, h, w)
-        dz = torch.randn(b, 64, h // 2, w // 2, generator=gen).half().float()
-        wr = w7.clone().requires_grad_(True)
-        F.conv2d(x, wr, None, 2, 3).backward(dz)
-        dw = torch.full((64, 3, 7, 7), 3.0, dtype=torch.float32, device=DEV)
-        ops.call('yb_stem7x7_wgrad', x.to(DEV), _nhwc16(dz), dw, b, h, w)
-        assert rel_err(dw, wr.grad) <= 1e-4, (b, h, w)
-    # max-pool backward: a ReLU output (many exact zeros -> all-zero windows) plus repeated values
-    for (b, h, w, c) in ((2, 16, 16, 64), (1, 13, 10, 16)):
-        a = torch.relu(torch.randn(b, c, h, w, generator=gen)).half().float()
-        a[:, :, ::3, :] = 0.5                          # ties between non-zero values too
-        ar = a.clone().requires_grad_(True)
-        y = F.max_pool2d(ar, 3, 2, 1)
-        dy = torch.randn(y.shape, generator=gen).half().float()
-        y.backward(dy)
-        dx = torch.empty(b, h, w, c, dtype=torch.float16, device=DEV)
-        ops.call('yb_maxpool3x3_s2_bwd_f16', _nhwc16(a), _nhwc16(dy), dx, b, h, w, c)
-        got = dx.permute(0, 3, 1, 2).float().cpu()
-        assert rel_err(got, ar.grad) <= 2e-3, (b, h, w, c)
-        assert torch.equal(got != 0, ar.grad != 0), 'a tied gradient went to another element than torch picks'
-        # also the forward of the plugin agrees with the pooled values
-        yp = torch.empty(b, (h + 1) // 2, (w + 1) // 2, c, dtype=torch.float16, device=DEV)
-        ops.call('yb_maxpool3x3_s2_f16', _nhwc16(a), yp, b, h, w, c)
-        assert torch.equal(yp.permute(0, 3, 1, 2).float().cpu(), y.detach())
-    # zero insertion: bit-exact
-    for (b, h, w, c) in ((2, 14, 10, 64), (1, 7, 9, 8)):
-        xs = torch.randn(b, (h + 1) // 2, (w + 1) // 2, c, generator=gen).half()
-        ref = torch.zeros(b, h, w, c, dtype=torch.float16)
-        ref[:, ::2, ::2] = xs
-        out = torch.full((b, h, w, c), 9.0, dtype=torch.float16, device=DEV)
-        ops.call('yb_upsample2_zero_f16', xs.to(DEV), out, b, h, w, c)
-        assert torch.equal(out.cpu(), ref)
-    # block-boundary gradient: out = (y > 0) ? g_a + S^T g_b : 0, fp32 sum rounded once
-    b, h, w, c = 2, 10, 12, 32
-    y = torch.relu(torch.randn(b, h, w, c, generator=gen)).half()
-    ga = torch.randn(b, h, w, c, generator=gen).half()
-    for stride, with_b, with_mask in ((1, True, True), (2, True, True), (1, False, True), (2, True, False), (1, True, False)):
-        gb = torch.randn(b, h // stride, w // stride, c, generator=gen).half() if with_b else None
-        ref = ga.float()
-        if gb is not None:
-            up = torch.zeros(b, h, w, c)
-            up[:, ::stride, ::stride] = gb.float()
-            ref = ref + up
-        if with_mask:
-            ref = torch.where(y.float() > 0, ref, torch.zeros(()))
-        out = torch.empty(b, h, w, c, dtype=torch.float16, device=DEV)
-        ops.call('yb_residual_bwd_f16', y.to(DEV) if with_mask else None, ga.to(DEV), None if gb is None else gb.to(DEV), stride, out, b, h, w, c)
-        assert torch.equal(out.cpu(), ref.half()), (stride, with_b, with_mask)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('name', ['resnet18', 'resnet50'])
 def test_resnet_training_step_vs_oracle_and_descent(name):

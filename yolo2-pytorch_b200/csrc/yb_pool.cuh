@@ -1,5 +1,6 @@
 // nn.MaxPool2d(kernel_size=3, stride=2, padding=1) window on fp16 NHWC, shared by the ResNet pool (resnet_ops.cu) and the DenseNet stem
-// pool that writes into a channel slice of a wider buffer (densenet_ops.cu).
+// pool that writes into a channel slice of a wider buffer (densenet_ops.cu).  A window holding a NaN gives NaN (__hmax2_nan), as torch's
+// max_pool2d does and as the backward kernels' winner rule (a NaN replaces the running maximum) assumes.
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -12,7 +13,7 @@ __device__ __forceinline__ uint4 hmax8_(uint4 a, uint4 b) {
   const __half2* pb = reinterpret_cast<const __half2*>(&b);
   __half2* pr = reinterpret_cast<__half2*>(&r);
 #pragma unroll
-  for (int i = 0; i < 4; ++i) pr[i] = __hmax2(pa[i], pb[i]);
+  for (int i = 0; i < 4; ++i) pr[i] = __hmax2_nan(pa[i], pb[i]);
   return r;
 }
 
