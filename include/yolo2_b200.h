@@ -84,12 +84,20 @@ int yb_conv0_bn_leaky_pool_fwd(const float* x_nchw, const float* w_oihw, const f
  * transform/__init__.py) and cuts the host->device copy 4x. */
 int yb_conv0_u8_bn_leaky_pool_fwd(const unsigned char* x_nhwc_u8, const float* w_oihw, const float* scale, const float* shift,
                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream);
+/* Input transform forms of the first-layer entries (`_lut`): x uint8 NHWC [B,H,W,3] read through lut fp32 [3][256], the configured
+ * ToTensor + Normalize chain compiled by transform.TensorTransform (lut[c][v] = torchvision's value for byte v in channel c).  Each differs
+ * from its fp32 NCHW entry only in the load: padding stays 0 in the transformed domain, and the fp16 output equals that entry's output on
+ * the transformed fp32 image bit for bit.  Same limits as the fp32 entry; lut must not be NULL. */
+int yb_conv0_bn_leaky_pool_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream);
 /* VGG's features.0 (model/vgg.py:41-50, make_layers: Conv2d(3, v, 3, padding=1) -> [BatchNorm2d] -> ReLU [-> MaxPool2d(2, 2)]) with 64 filters:
  * x fp32 NCHW [B,3,H,W] -> y fp16 NHWC [B,H,W,64], or [B,H/2,W/2,64] with pool = 1 (the 2x2 max of the activated values).
  * w fp32 OIHW [64,3,3,3]; y = act(conv * scale + shift) with act(t) = t > 0 ? t : slope * t.  H % 32 == 0, W % 16 == 0.
  * A layer with fewer filters runs padded to 64 with zero weights, scale 1 and shift 0. */
 int yb_conv0_c64_bn_act_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, float slope, void* y_nhwc_f16,
                             int batch, int height, int width, int pool, yb_stream_t stream);
+int yb_conv0_c64_bn_act_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                float slope, void* y_nhwc_f16, int batch, int height, int width, int pool, yb_stream_t stream);
 /* k in {1,3}, stride 1, pad (k-1)/2 conv + per-channel scale/shift + leaky(slope) as a wgmma
  * implicit GEMM.  x: fp16 NHWC [B,H,W,Cin] with pixel pitch x_ld; w: fp16 [Cout][k][k][Cin];
  * y: fp16 NHWC (pixel pitch y_ld, first channel y_ch_off) or fp32 NCHW [B,Cout,H,W].
@@ -333,6 +341,9 @@ int yb_warp_affine_u8(const void* src, int src_h, int src_w, void* dst, int dst_
 /* torchvision ToTensor for a batch (the `transform_tensor` step, utils/data.py:120-121): uint8 NHWC [B,H,W,3] -> fp32 NCHW [B,3,H,W],
  * value / 255.  Only the training path needs the fp32 image (inference reads the uint8 frames in the first conv kernel). */
 int yb_totensor_u8(const void* src_nhwc_u8, float* dst_nchw_f32, int batch, int height, int width, yb_stream_t stream);
+/* The configured tensor transform (transform.TensorTransform: ToTensor, then per-channel Normalize) on a batch: uint8 NHWC [B,H,W,3] ->
+ * fp32 NCHW [B,3,H,W], dst = lut[c][src] with lut fp32 [3][256]. */
+int yb_totensor_lut_u8(const void* src_nhwc_u8, const float* lut, float* dst_nchw_f32, int batch, int height, int width, yb_stream_t stream);
 
 /* One segment of the photometric chain of transform/image.py (RandomBlur, BGR2HSV, RandomHue, RandomSaturation, RandomBrightness, HSV2RGB,
  * RandomGamma; config.ini `transform/image_train`) over a resized uint8 batch [B,H,W,3], out of place (dst != src), bit-exact with cv2 4.13.
@@ -365,6 +376,8 @@ int yb_eval_match(const float* det_yx_min, const float* det_yx_max, const int* d
  * refused, output untouched); any H != W.  A 27-term fp32 fmaf chain per output, then one fp32 scale / shift and RN16. */
 int yb_mb_conv0_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch,
                             int height, int width, yb_stream_t stream);
+int yb_mb_conv0_bn_relu_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                void* y_nhwc_f16, int batch, int height, int width, yb_stream_t stream);
 /* conv_dw: depthwise 3x3 (stride 1 or 2, pad 1) + BN + ReLU on fp16 NHWC; w fp32 [C][9] (model/mobilenet.py:33-38).  C % 8 == 0, H and W
  * multiples of the stride, w / scale / shift 16 B aligned (otherwise refused, output untouched); any C/8 group count, any output width (8 output
  * pixels per thread from ow = 52, 4 below, ragged last strips).  A 9-term fp32 fmaf chain per channel, then the epilogue. */
@@ -380,6 +393,8 @@ int yb_dwconv3x3_bn_relu_fwd(const void* x, const float* w_c9, const float* scal
  * in scan order, NaN if the window holds one.  subsample2 and add_relu are bit-exact restatements (add_relu may run in place). */
 int yb_stem7x7_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height, int width,
                            yb_stream_t stream);
+int yb_stem7x7_bn_relu_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                               void* y_nhwc_f16, int batch, int height, int width, yb_stream_t stream);
 int yb_maxpool3x3_s2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
 int yb_subsample2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream);
 int yb_add_relu_f16(const void* a, const void* b, void* out, long long count, yb_stream_t stream);
@@ -464,6 +479,8 @@ int yb_pack_weight_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, 
  * [B,(H+2pad-3)/2+1,(W+2pad-3)/2+1,32]; pad 0 (Inception) or 1 (the bits of yb_mb_conv0_bn_relu_fwd). */
 int yb_stem3x3_s2_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height,
                               int width, int pad, yb_stream_t stream);
+int yb_stem3x3_s2_bn_relu_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                  void* y_nhwc_f16, int batch, int height, int width, int pad, yb_stream_t stream);
 /* F.max_pool2d(x, 3, stride=2) (no padding, floor): x [B,H,W,C] -> channels [y_ch_off, y_ch_off + C) of y [B,(H-3)/2+1,(W-3)/2+1,y_ld].
  * H, W >= 3; C, y_ld, y_ch_off multiples of 8.  NaN for a window holding a NaN, as torch. */
 int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream);
@@ -554,6 +571,8 @@ int yb_residual_bwd_f16(const void* y, const void* g_a, const void* g_b, int str
  * fp32); the pointwise convs and the head run yb_conv_bn_act_split_fwd. */
 int yb_mb_conv0_split_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_hi_lo, int batch, int height, int width,
                           yb_stream_t stream);
+int yb_mb_conv0_split_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                              void* y_hi_lo, int batch, int height, int width, yb_stream_t stream);
 int yb_dwconv3x3_split_fwd(const void* x_hi_lo, const float* w_c9, const float* scale, const float* shift, void* y_hi_lo, int batch, int height, int width,
                            int channels, int stride, yb_stream_t stream);
 int yb_mb_conv0_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, yb_stream_t stream);

@@ -8,6 +8,7 @@ stream.  The 1280-channel concat buffer is written in place by the reorg kernel 
 and by layers2.7 (channels 256..1279), so torch.cat (model/yolo2.py:129) never runs.
 """
 import os
+import weakref
 
 import torch
 
@@ -231,6 +232,7 @@ class DarknetEngine(object):
         self._k2 = ['layers2.%d' % i for i, m in enumerate(dnn.layers2) if not m.is_pool]
         self.unit_pt = unit(dnn.passthrough)
         self.units3 = [unit(m) for m in dnn.layers3]
+        self._dnn = weakref.ref(dnn)        # its input_transform: the table uint8 frames go through
         self.plans = {}
         if not self.pools1[0]:
             raise RuntimeError('Darknet: layers1.0 must be followed by MaxPool2d (fused first-layer kernel)')
@@ -373,12 +375,13 @@ class DarknetEngine(object):
             u._bver = None
 
     def forward(self, x, conv_flags=0, ref=False, collect=None, plan_id=0):
-        """x: fp32 NCHW [B,3,H,W] on the GPU -> feature fp32 NCHW [B,A*(5+C),H/32,W/32]
-        (a plan-owned buffer, overwritten by the next call with the same shape).
+        """x: fp32 NCHW [B,3,H,W] on the GPU, or uint8 NHWC frames [B,H,W,3] -> feature fp32 NCHW [B,A*(5+C),H/32,W/32]
+        (a plan-owned buffer, overwritten by the next call with the same shape).  uint8 frames go through the Darknet's input_transform
+        table in the first-layer kernel, or without one through ToTensor's 1/255 scaling.
         `collect` (dict) receives references to every unit's fp16 NHWC output (tests)."""
         if not x.is_cuda:
             raise RuntimeError('Darknet: input must be a CUDA tensor; there is no CPU fallback')
-        u8 = x.dtype == torch.uint8          # raw RGB frames [B,H,W,3]: the kernel applies ToTensor's 1/255
+        u8 = x.dtype == torch.uint8          # raw RGB frames [B,H,W,3]: the kernel applies the input transform
         if u8:
             b, h, w, c = x.shape
         else:
@@ -398,9 +401,7 @@ class DarknetEngine(object):
                 return ops.conv_bn_act_tail(src, u.w16, u.scale, u.shift, u.slope, u.in_ch, out=dst, flags=conv_flags, **kw)
             return ops.conv_bn_act(src, u.w16, u.scale, u.shift, u.slope, out=dst, flags=conv_flags, ref=ref, workspace=p.workspace, **kw)
 
-        u0 = self.units1[0]
-        conv0 = ops.conv0_u8_bn_leaky_pool if u8 else ops.conv0_bn_leaky_pool
-        cur = conv0(x, u0.w16, u0.scale, u0.shift, u0.slope, out=p.a0)
+        cur = self._conv0(x, u8, p.a0)
         if collect is not None:
             collect['layers1.0(pooled)'] = cur
         x1 = None
@@ -457,6 +458,15 @@ class DarknetEngine(object):
             collect['layers3.0'] = p.l3
         return p.feature
 
+    def _conv0(self, x, u8, out):
+        """layers1.0 + its max-pool into `out`: fp32 image, or uint8 frames through the input transform's table (1/255 without one)."""
+        u0 = self.units1[0]
+        t = getattr(self._dnn(), 'input_transform', None) if u8 else None
+        if t is not None:
+            return ops.conv0_bn_leaky_pool(x, u0.w16, u0.scale, u0.shift, u0.slope, out=out, lut=t.lut(x.device))
+        conv0 = ops.conv0_u8_bn_leaky_pool if u8 else ops.conv0_bn_leaky_pool
+        return conv0(x, u0.w16, u0.scale, u0.shift, u0.slope, out=out)
+
     def _forward_strict(self, x, u8, p, conv_flags, collect):
         """Same chain with split-precision operands (see STRICT_KEEP).  Buffers of units with `out_lo` hold [hi | lo]."""
         def view(t, c, lo):
@@ -475,9 +485,7 @@ class DarknetEngine(object):
             return ops.conv_bn_act_split(src, u.w16, u.scale, u.shift, u.slope, dst, a_channels=src_c * (2 if split_a else 1), y_ch_off=y_ch_off,
                                          lo_ch_off=lo_ch_off, out_mode=out_mode, flags=conv_flags, workspace=p.workspace)
 
-        u0 = self.units1[0]
-        conv0 = ops.conv0_u8_bn_leaky_pool if u8 else ops.conv0_bn_leaky_pool
-        cur, cur_c, cur_lo = conv0(x, u0.w16, u0.scale, u0.shift, u0.slope, out=p.a0), u0.cout, False
+        cur, cur_c, cur_lo = self._conv0(x, u8, p.a0), self.units1[0].cout, False
         if collect is not None:
             collect['layers1.0(pooled)'] = cur
         x1 = None

@@ -20,6 +20,13 @@ SIGNATURES = {
     'yb_conv0_bn_leaky_pool_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
     'yb_conv0_u8_bn_leaky_pool_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
     'yb_conv0_c64_bn_act_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
+    'yb_conv0_bn_leaky_pool_lut_fwd': [P, P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
+    'yb_conv0_c64_bn_act_lut_fwd': [P, P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, P],
+    'yb_totensor_lut_u8': [P, P, P, c_int, c_int, c_int, P],
+    'yb_mb_conv0_bn_relu_lut_fwd': [P, P, P, P, P, P, c_int, c_int, c_int, P],
+    'yb_mb_conv0_split_lut_fwd': [P, P, P, P, P, P, c_int, c_int, c_int, P],
+    'yb_stem7x7_bn_relu_lut_fwd': [P, P, P, P, P, P, c_int, c_int, c_int, P],
+    'yb_stem3x3_s2_bn_relu_lut_fwd': [P, P, P, P, P, P, c_int, c_int, c_int, c_int, P],
     'yb_conv_bn_act_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, c_int, P],
     'yb_conv_bn_act_stats_fwd': [P, P, P, P, c_float, P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_longlong, c_int, c_int, P, P],
     'yb_conv_workspace_bytes': [],

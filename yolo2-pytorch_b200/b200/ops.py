@@ -91,18 +91,32 @@ def bn_fold(gamma, beta, mean, var, eps=1e-5):
     return scale, shift
 
 
-def conv0_bn_leaky_pool(x, w, scale, shift, slope, out=None):
-    """x fp32 NCHW [B,3,H,W] -> fp16 NHWC [B,H/2,W/2,32]."""
-    _req(x, torch.float32, 'x'); _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
-    b, c, h, wd = x.shape
+def _image(x, lut):
+    """The first-layer input's (b, c, h, w) and the pointer arguments that carry it: fp32 NCHW [B,3,H,W], or with a table (the `_lut`
+    entries) uint8 NHWC [B,H,W,3] and lut fp32 [3,256]."""
+    if lut is None:
+        _req(x, torch.float32, 'x')
+        return tuple(x.shape), (_p(x),)
+    _req(x, torch.uint8, 'x'); _req(lut, torch.float32, 'lut')
+    if tuple(lut.shape) != (3, 256):
+        raise ValueError('lut must be [3, 256], got %s' % (tuple(lut.shape),))
+    b, h, wd, c = x.shape
+    return (b, c, h, wd), (_p(x), _p(lut))
+
+
+def conv0_bn_leaky_pool(x, w, scale, shift, slope, out=None, lut=None):
+    """x fp32 NCHW [B,3,H,W] -> fp16 NHWC [B,H/2,W/2,32].  With `lut` (fp32 [3,256]): x uint8 NHWC [B,H,W,3] read through the table
+    (yb_conv0_bn_leaky_pool_lut_fwd)."""
+    _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    (b, c, h, wd), xa = _image(x, lut)
     if c != 3:
         raise ValueError('conv0 expects 3 input channels')
     cout = w.shape[0]
     if out is None:
         out = torch.empty(b, h // 2, wd // 2, cout, dtype=torch.float16, device=x.device)
     _req(out, torch.float16, 'out')
-    _ck(_l.load().yb_conv0_bn_leaky_pool_fwd(_p(x), _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, cout, _s()),
-             'yb_conv0_bn_leaky_pool_fwd')
+    name = 'yb_conv0_bn_leaky_pool_fwd' if lut is None else 'yb_conv0_bn_leaky_pool_lut_fwd'
+    _ck(getattr(_l.load(), name)(*xa, _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, cout, _s()), name)
     return out
 
 
@@ -121,11 +135,12 @@ def conv0_u8_bn_leaky_pool(x, w, scale, shift, slope, out=None):
     return out
 
 
-def conv0_c64_bn_act(x, w, scale, shift, slope, pool=False, out=None):
+def conv0_c64_bn_act(x, w, scale, shift, slope, pool=False, out=None, lut=None):
     """Conv2d(3, 64, 3, padding 1) + scale/shift + activation (+ 2x2 max-pool) of VGG's features.0 (yb_conv0_c64_bn_act_fwd):
-    x fp32 NCHW [B,3,H,W], w fp32 [64,3,3,3], scale / shift fp32 [64] -> fp16 NHWC [B,H,W,64], or [B,H/2,W/2,64] with `pool`."""
-    _req(x, torch.float32, 'x'); _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
-    b, c, h, wd = x.shape
+    x fp32 NCHW [B,3,H,W], w fp32 [64,3,3,3], scale / shift fp32 [64] -> fp16 NHWC [B,H,W,64], or [B,H/2,W/2,64] with `pool`.
+    With `lut` (fp32 [3,256]): x uint8 NHWC [B,H,W,3] read through the table (yb_conv0_c64_bn_act_lut_fwd)."""
+    _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    (b, c, h, wd), xa = _image(x, lut)
     if c != 3 or tuple(w.shape) != (64, 3, 3, 3) or scale.numel() != 64 or shift.numel() != 64:
         raise ValueError('conv0_c64: x [B,3,H,W], w [64,3,3,3] and 64 scales / shifts expected')
     oh, ow = (h // 2, wd // 2) if pool else (h, wd)
@@ -134,8 +149,8 @@ def conv0_c64_bn_act(x, w, scale, shift, slope, pool=False, out=None):
     _req(out, torch.float16, 'out')
     if tuple(out.shape) != (b, oh, ow, 64):
         raise ValueError('conv0_c64: out must be [%d,%d,%d,64]' % (b, oh, ow))
-    _ck(_l.load().yb_conv0_c64_bn_act_fwd(_p(x), _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, int(bool(pool)), _s()),
-        'yb_conv0_c64_bn_act_fwd')
+    name = 'yb_conv0_c64_bn_act_fwd' if lut is None else 'yb_conv0_c64_bn_act_lut_fwd'
+    _ck(getattr(_l.load(), name)(*xa, _p(w), _p(scale), _p(shift), float(slope), _p(out), b, h, wd, int(bool(pool)), _s()), name)
     return out
 
 
@@ -308,14 +323,16 @@ def pack_weight_khw_f16(w, cout_pad=None, cin_pad=None):
     return out
 
 
-def stem3x3_s2(x, w, scale, shift, pad=0):
-    """nn.Conv2d(3, 32, 3, stride 2, pad) + folded BatchNorm + ReLU: x fp32 NCHW [B,3,H,W] -> fp16 NHWC [B,OH,OW,32]."""
-    _req(x, torch.float32, 'x'); _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
-    b, c, h, wd = x.shape
+def stem3x3_s2(x, w, scale, shift, pad=0, lut=None):
+    """nn.Conv2d(3, 32, 3, stride 2, pad) + folded BatchNorm + ReLU: x fp32 NCHW [B,3,H,W] -> fp16 NHWC [B,OH,OW,32].  With `lut` (fp32
+    [3,256]): x uint8 NHWC [B,H,W,3] read through the table (yb_stem3x3_s2_bn_relu_lut_fwd)."""
+    _req(w, torch.float32, 'w'); _req(scale, torch.float32, 'scale'); _req(shift, torch.float32, 'shift')
+    (b, c, h, wd), xa = _image(x, lut)
     if c != 3 or tuple(w.shape) != (32, 3, 3, 3):
         raise ValueError('stem3x3_s2: x [B,3,H,W] and w [32,3,3,3] expected')
     out = torch.empty(b, conv2d_out_size(h, 3, 2, pad), conv2d_out_size(wd, 3, 2, pad), 32, dtype=torch.float16, device=x.device)
-    _ck(_l.load().yb_stem3x3_s2_bn_relu_fwd(_p(x), _p(w), _p(scale), _p(shift), _p(out), b, h, wd, pad, _s()), 'yb_stem3x3_s2_bn_relu_fwd')
+    name = 'yb_stem3x3_s2_bn_relu_fwd' if lut is None else 'yb_stem3x3_s2_bn_relu_lut_fwd'
+    _ck(getattr(_l.load(), name)(*xa, _p(w), _p(scale), _p(shift), _p(out), b, h, wd, pad, _s()), name)
     return out
 
 

@@ -74,8 +74,8 @@ int pack_weight(const float*, void*, int, int, int, int, int, cudaStream_t);
 int pack_weights_batch(const void*, int, int, cudaStream_t);
 void conv_set_trace(void*);
 int bn_fold(const float*, const float*, const float*, const float*, float, float*, float*, int, cudaStream_t);
-int conv0_tc_forward(const void*, int, const float*, const float*, const float*, float, void*, int, int, int, int, int, double*, cudaStream_t);
-int conv0_c64_forward(const float*, const float*, const float*, const float*, float, void*, int, int, int, int, cudaStream_t);
+int conv0_tc_forward(const void*, int, const float*, const float*, const float*, const float*, float, void*, int, int, int, int, int, double*, cudaStream_t);
+int conv0_c64_forward(const void*, const float*, const float*, const float*, const float*, float, void*, int, int, int, int, cudaStream_t);
 int conv0_c64_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
 int maxpool2x2(const void*, void*, int, int, int, int, int, cudaStream_t);
 int maxpool2x2_s1(const void*, void*, int, int, int, int, int, cudaStream_t);
@@ -104,6 +104,7 @@ int conv0_wgrad_bn(const float*, const void*, const void*, long long, int, const
                    cudaStream_t);
 int resize_batch_u8(const void*, const long long*, const int*, void*, int, int, int, int, float*, float*, int, cudaStream_t);
 int totensor_u8(const void*, float*, int, int, int, cudaStream_t);
+int totensor_lut_u8(const void*, const float*, float*, int, int, int, cudaStream_t);
 int photometric_batch_u8(const void*, void*, int, int, int, const void*, int, int, cudaStream_t);
 int warp_affine_u8(const void*, int, int, void*, int, int, const double*, const int*, cudaStream_t);
 int resize_aug_batch_u8(const void*, const long long*, const int*, const int*, const float*, const unsigned char*, void*, int, int, int, int, float*, float*,
@@ -114,7 +115,7 @@ int unpack_wgrad(const float*, float*, int, int, int, float, cudaStream_t);
 int grad_guard(float*, long long, float*, int, cudaStream_t);
 int grad_unscale_guard(float*, long long, float*, float*, int*, int, cudaStream_t);
 int conv_wgrad_forward(const void*, const void*, float*, int, int, int, int, int, int, int, int, cudaStream_t);
-int stem7x7(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
+int stem7x7(const void*, const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
 int stem7x7_wgrad(const float*, const void*, float*, int, int, int, cudaStream_t);
 int maxpool3x3_s2(const void*, void*, int, int, int, int, cudaStream_t);
 int maxpool3x3_s2_bwd(const void*, const void*, void*, int, int, int, int, cudaStream_t);
@@ -128,7 +129,7 @@ int comm_init(void**, int, const void*, int);
 int comm_destroy(void*);
 int allreduce_bucket(void*, void*, long long, int, cudaStream_t);
 int broadcast_buffer(void*, void*, long long, int, int, cudaStream_t);
-int mb_conv0(const float*, const float*, const float*, const float*, void*, int, int, int, int, int, cudaStream_t);
+int mb_conv0(const void*, const float*, const float*, const float*, const float*, void*, int, int, int, int, int, cudaStream_t);
 int dwconv3x3_split(const void*, const float*, const float*, const float*, void*, int, int, int, int, int, cudaStream_t);
 int dwconv3x3(const void*, const float*, const float*, const float*, void*, int, int, int, int, int, int, cudaStream_t);
 int dw_dgrad(const void*, const float*, void*, int, int, int, int, int, cudaStream_t);
@@ -140,7 +141,7 @@ int conv2d_forward(const void*, const void*, const float*, const float*, float, 
 int pack_weight_khw(const float*, void*, int, int, int, int, int, int, cudaStream_t);
 int conv_tail_forward(const void*, const void*, const float*, const float*, float, void*, int, int, int, int, int, int, int, int, long long, int,
                       int, int, cudaStream_t);
-int stem3x3_s2(const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
+int stem3x3_s2(const void*, const float*, const float*, const float*, const float*, void*, int, int, int, int, cudaStream_t);
 int maxpool3x3_s2_valid(const void*, void*, int, int, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1(const void*, void*, int, int, int, int, cudaStream_t);
 int avgpool3x3_s1_excl(const void*, void*, int, int, int, int, cudaStream_t);
@@ -189,17 +190,28 @@ int yb_bn_fold(const float* gamma, const float* beta, const float* running_mean,
 
 int yb_conv0_bn_leaky_pool_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, float slope,
                                void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream) {
-  return yb::conv0_tc_forward(x_nchw, 0, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, cout, 0, nullptr, S(stream));
+  return yb::conv0_tc_forward(x_nchw, 0, nullptr, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, cout, 0, nullptr, S(stream));
 }
 
 int yb_conv0_u8_bn_leaky_pool_fwd(const unsigned char* x_nhwc_u8, const float* w_oihw, const float* scale, const float* shift,
                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream) {
-  return yb::conv0_tc_forward(x_nhwc_u8, 1, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, cout, 0, nullptr, S(stream));
+  return yb::conv0_tc_forward(x_nhwc_u8, 1, nullptr, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, cout, 0, nullptr, S(stream));
+}
+
+int yb_conv0_bn_leaky_pool_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                   float slope, void* y_nhwc_f16, int batch, int height, int width, int cout, yb_stream_t stream) {
+  return yb::conv0_tc_forward(x_nhwc_u8, 2, lut, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, cout, 0, nullptr, S(stream));
 }
 
 int yb_conv0_c64_bn_act_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, float slope, void* y_nhwc_f16,
                             int batch, int height, int width, int pool, yb_stream_t stream) {
-  return yb::conv0_c64_forward(x_nchw, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, pool, S(stream));
+  return yb::conv0_c64_forward(x_nchw, nullptr, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, pool, S(stream));
+}
+
+int yb_conv0_c64_bn_act_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                float slope, void* y_nhwc_f16, int batch, int height, int width, int pool, yb_stream_t stream) {
+  if (!lut) return yb::fail(YB_ERR_BAD_ARG, "conv0_c64: null table");
+  return yb::conv0_c64_forward(x_nhwc_u8, lut, w_oihw, scale, shift, slope, y_nhwc_f16, batch, height, width, pool, S(stream));
 }
 
 int yb_conv_bn_act_fwd(const void* x, const void* w, const float* scale, const float* shift, float slope, void* y, int batch,
@@ -375,12 +387,12 @@ int yb_region_loss_bwd(const float* grad_terms, const float* grad_bg, const floa
 
 int yb_conv0_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, int cout,
                      yb_stream_t stream) {
-  return yb::conv0_tc_forward(x_nchw, 0, w_oihw, nullptr, nullptr, 1.f, z_nhwc_f16, batch, height, width, cout, 1, nullptr, S(stream));
+  return yb::conv0_tc_forward(x_nchw, 0, nullptr, w_oihw, nullptr, nullptr, 1.f, z_nhwc_f16, batch, height, width, cout, 1, nullptr, S(stream));
 }
 
 int yb_conv0_raw_stats_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, double* sums, int batch, int height, int width, int cout,
                            yb_stream_t stream) {
-  return yb::conv0_tc_forward(x_nchw, 0, w_oihw, nullptr, nullptr, 1.f, z_nhwc_f16, batch, height, width, cout, 1, sums, S(stream));
+  return yb::conv0_tc_forward(x_nchw, 0, nullptr, w_oihw, nullptr, nullptr, 1.f, z_nhwc_f16, batch, height, width, cout, 1, sums, S(stream));
 }
 
 int yb_pack_weights_batch(const yb_pack_unit* units_dev, int num_units, int total_blocks, yb_stream_t stream) {
@@ -478,6 +490,10 @@ int yb_totensor_u8(const void* src_nhwc_u8, float* dst_nchw_f32, int batch, int 
   return yb::totensor_u8(src_nhwc_u8, dst_nchw_f32, batch, height, width, S(stream));
 }
 
+int yb_totensor_lut_u8(const void* src_nhwc_u8, const float* lut, float* dst_nchw_f32, int batch, int height, int width, yb_stream_t stream) {
+  return yb::totensor_lut_u8(src_nhwc_u8, lut, dst_nchw_f32, batch, height, width, S(stream));
+}
+
 int yb_photometric_batch_u8(const void* src, void* dst, int batch, int height, int width, const void* params, int param_stride, int stages,
                             yb_stream_t stream) {
   return yb::photometric_batch_u8(src, dst, batch, height, width, params, param_stride, stages, S(stream));
@@ -492,12 +508,24 @@ int yb_eval_match(const float* det_yx_min, const float* det_yx_max, const int* d
 
 int yb_mb_conv0_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch,
                             int height, int width, yb_stream_t stream) {
-  return yb::mb_conv0(x_nchw, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, 0, S(stream));
+  return yb::mb_conv0(x_nchw, nullptr, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, 0, S(stream));
+}
+
+int yb_mb_conv0_bn_relu_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                void* y_nhwc_f16, int batch, int height, int width, yb_stream_t stream) {
+  if (!lut) return yb::fail(YB_ERR_BAD_ARG, "mb_conv0: null table");
+  return yb::mb_conv0(x_nhwc_u8, lut, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, 0, S(stream));
 }
 
 int yb_mb_conv0_split_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_hi_lo, int batch, int height, int width,
                           yb_stream_t stream) {
-  return yb::mb_conv0(x_nchw, w_oihw, scale, shift, y_hi_lo, batch, height, width, 0, 1, S(stream));
+  return yb::mb_conv0(x_nchw, nullptr, w_oihw, scale, shift, y_hi_lo, batch, height, width, 0, 1, S(stream));
+}
+
+int yb_mb_conv0_split_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                              void* y_hi_lo, int batch, int height, int width, yb_stream_t stream) {
+  if (!lut) return yb::fail(YB_ERR_BAD_ARG, "mb_conv0: null table");
+  return yb::mb_conv0(x_nhwc_u8, lut, w_oihw, scale, shift, y_hi_lo, batch, height, width, 0, 1, S(stream));
 }
 
 int yb_dwconv3x3_split_fwd(const void* x_hi_lo, const float* w_c9, const float* scale, const float* shift, void* y_hi_lo, int batch, int height, int width,
@@ -506,7 +534,7 @@ int yb_dwconv3x3_split_fwd(const void* x_hi_lo, const float* w_c9, const float* 
 }
 
 int yb_mb_conv0_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, yb_stream_t stream) {
-  return yb::mb_conv0(x_nchw, w_oihw, nullptr, nullptr, z_nhwc_f16, batch, height, width, 1, 0, S(stream));
+  return yb::mb_conv0(x_nchw, nullptr, w_oihw, nullptr, nullptr, z_nhwc_f16, batch, height, width, 1, 0, S(stream));
 }
 
 int yb_mb_conv0_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream) {
@@ -532,7 +560,13 @@ int yb_dwconv3x3_bn_relu_fwd(const void* x, const float* w_c9, const float* scal
 
 int yb_stem7x7_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height, int width,
                            yb_stream_t stream) {
-  return yb::stem7x7(x_nchw, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, S(stream));
+  return yb::stem7x7(x_nchw, nullptr, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, S(stream));
+}
+
+int yb_stem7x7_bn_relu_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                               void* y_nhwc_f16, int batch, int height, int width, yb_stream_t stream) {
+  if (!lut) return yb::fail(YB_ERR_BAD_ARG, "stem7x7: null table");
+  return yb::stem7x7(x_nhwc_u8, lut, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, 0, S(stream));
 }
 
 int yb_maxpool3x3_s2_f16(const void* x, void* y, int batch, int height, int width, int channels, yb_stream_t stream) {
@@ -546,7 +580,7 @@ int yb_subsample2_f16(const void* x, void* y, int batch, int height, int width, 
 int yb_add_relu_f16(const void* a, const void* b, void* out, long long count, yb_stream_t stream) { return yb::add_relu(a, b, out, count, S(stream)); }
 
 int yb_stem7x7_raw_fwd(const float* x_nchw, const float* w_oihw, void* z_nhwc_f16, int batch, int height, int width, yb_stream_t stream) {
-  return yb::stem7x7(x_nchw, w_oihw, nullptr, nullptr, z_nhwc_f16, batch, height, width, 1, S(stream));
+  return yb::stem7x7(x_nchw, nullptr, w_oihw, nullptr, nullptr, z_nhwc_f16, batch, height, width, 1, S(stream));
 }
 
 int yb_stem7x7_wgrad(const float* x_nchw, const void* dz_nhwc_f16, float* dw_oihw, int batch, int height, int width, yb_stream_t stream) {
@@ -584,7 +618,13 @@ int yb_pack_weight_khw_f16(const float* w_oihw, void* w_f16, int cout, int cin, 
 
 int yb_stem3x3_s2_bn_relu_fwd(const float* x_nchw, const float* w_oihw, const float* scale, const float* shift, void* y_nhwc_f16, int batch, int height,
                               int width, int pad, yb_stream_t stream) {
-  return yb::stem3x3_s2(x_nchw, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, pad, S(stream));
+  return yb::stem3x3_s2(x_nchw, nullptr, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, pad, S(stream));
+}
+
+int yb_stem3x3_s2_bn_relu_lut_fwd(const unsigned char* x_nhwc_u8, const float* lut, const float* w_oihw, const float* scale, const float* shift,
+                                  void* y_nhwc_f16, int batch, int height, int width, int pad, yb_stream_t stream) {
+  if (!lut) return yb::fail(YB_ERR_BAD_ARG, "stem3x3_s2: null table");
+  return yb::stem3x3_s2(x_nhwc_u8, lut, w_oihw, scale, shift, y_nhwc_f16, batch, height, width, pad, S(stream));
 }
 
 int yb_maxpool3x3_s2_valid_f16(const void* x, void* y, int y_ld, int y_ch_off, int batch, int height, int width, int channels, yb_stream_t stream) {

@@ -1,8 +1,9 @@
 // conv0 (layers1.0): 3x3 conv, Cin = 3 -> Cout = 32, + folded BN + leaky-ReLU + 2x2 max-pool, on the
 // tensor cores.  Replaces nn.Conv2d(3,32,3,pad 1) -> BatchNorm2d -> LeakyReLU -> MaxPool2d(2)
 // (reference model/yolo2.py:78-79) and doubles as the layout boundary: it reads the caller's
-// image batch (fp32 NCHW as the reference's ToTensor produces it, or raw uint8 NHWC frames scaled
-// by 1/255 == torchvision ToTensor) and writes the first fp16 NHWC activation.
+// image batch (fp32 NCHW as the reference's ToTensor produces it, raw uint8 NHWC frames scaled
+// by 1/255 == torchvision ToTensor, or uint8 NHWC frames through a ToTensor + Normalize table; yb_input.cuh) and writes the first fp16
+// NHWC activation.
 //
 // K = 27 is far too small for a TMA-fed pipeline (one pixel's im2col row is 54 bytes), so the CTA
 // builds the A operand itself: a 16x32-pixel conv tile (+1 halo) is staged in shared memory once,
@@ -15,6 +16,7 @@
 // channels.  Persistent CTAs (2 per SM), weights (B operand) built once per CTA.
 #include "yb_common.h"
 #include "yb_ptx.cuh"
+#include "yb_input.cuh"
 #include <stdlib.h>
 
 namespace yb {
@@ -32,7 +34,8 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 }
 
 struct Conv0Params {
-  const void* x;        // fp32 NCHW [B,3,H,W] or uint8 NHWC [B,H,W,3]
+  const void* x;        // fp32 NCHW [B,3,H,W] or uint8 NHWC [B,H,W,3] (InputMode)
+  const float* lut;     // kInLut: fp32 [3][256]
   const float* w;       // fp32 OIHW [32,3,3,3]
   const float* scale;
   const float* shift;
@@ -45,7 +48,7 @@ struct Conv0Params {
   int* dbg;
 };
 
-template <bool kU8>
+template <int kIn>
 __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_tc_kernel(const Conv0Params p) {
   __shared__ __align__(1024) uint8_t a_smem[4 * 128 * 64];          // 4 M-tiles x 128 rows x 64 B (SW64)
   __shared__ __align__(1024) uint8_t b_smem[kC0Out * 64];           // 32 rows (Cout) x 64 B (SW64)
@@ -94,7 +97,9 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_tc_kernel(const Conv0
       const int iy = y0 + r, ix = x0 + col;
       float val = 0.f;
       if (i < kPatchElems && iy >= 0 && iy < p.height && ix >= 0 && ix < p.width) {
-        if (kU8) {
+        if (kIn == kInLut) {
+          val = lut_pixel(p.x, p.lut, pimg, c, iy, ix, p.height, p.width);
+        } else if (kIn == kInU8) {
           val = static_cast<float>(__ldg(reinterpret_cast<const uint8_t*>(p.x) + ((static_cast<long long>(pimg) * p.height + iy) * p.width + ix) * 3 + c)) *
                 (1.f / 255.f);
         } else {
@@ -254,7 +259,7 @@ constexpr int kV2Iters = (kV2Pixels + 127) / 128;               // 5 pixels per 
 // roundings of sum |z| however many tiles a CTA runs: the variance var = sum z^2 / n - mean^2 amplifies that error by 1 + (mean / std)^2.
 constexpr int kV2StageBytes = kV2Rows * kV2Cols * kC0Out * 2;   // 32 KB
 
-template <bool kU8, bool kRaw>
+template <int kIn, bool kRaw>
 __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv0Params p) {
   __shared__ __align__(128) uint8_t stage[kRaw ? kV2StageBytes : 16];
   __shared__ double s_stats[2 * kC0Out];
@@ -306,7 +311,8 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv
       for (int ch = 0; ch < 3; ++ch) {
         float val = 0.f;
         if (ok) {
-          if (kU8) val = static_cast<float>(__ldg(reinterpret_cast<const uint8_t*>(p.x) + ((static_cast<long long>(pimg) * p.height + iy) * p.width + ix) * 3 + ch)) * (1.f / 255.f);
+          if (kIn == kInLut) val = lut_pixel(p.x, p.lut, pimg, ch, iy, ix, p.height, p.width);
+          else if (kIn == kInU8) val = static_cast<float>(__ldg(reinterpret_cast<const uint8_t*>(p.x) + ((static_cast<long long>(pimg) * p.height + iy) * p.width + ix) * 3 + ch)) * (1.f / 255.f);
           else val = __ldg(reinterpret_cast<const float*>(p.x) + ((static_cast<long long>(pimg) * 3 + ch) * p.height + iy) * p.width + ix);
         }
         v[k][ch] = val;
@@ -454,10 +460,13 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_k16_kernel(const Conv
   }
 }
 
-int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* scale, const float* shift, float slope, void* y, int batch,
+// in_mode: InputMode; lut is read in kInLut only
+int conv0_tc_forward(const void* x, int in_mode, const float* lut, const float* w, const float* scale, const float* shift, float slope, void* y, int batch,
                      int height, int width, int cout, int raw, double* stats, cudaStream_t stream) {
   YB_REQUIRE(x && w && y && (raw || (scale && shift)), "conv0: null pointer");
   YB_REQUIRE(cout == kC0Out, "conv0: Cout=%d unsupported (32)", cout);
+  YB_REQUIRE(in_mode == kInF32 || in_mode == kInU8 || (in_mode == kInLut && lut), "conv0: bad input mode %d (or a null table)", in_mode);
+  const bool x_is_u8 = in_mode != kInF32;
   // operands-in-place form when the shape tiles 32 x 16 (every multiple of 32, i.e. every Darknet input); YB_CONV0_V1=1 forces the first form
   static const int force_v1 = getenv("YB_CONV0_V1") ? atoi(getenv("YB_CONV0_V1")) : 0;
   const bool v2 = !force_v1 && batch > 0 && height > 0 && width > 0 && height % kV2Rows == 0 && width % kV2Cols == 0;
@@ -465,7 +474,7 @@ int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* sc
              "conv0: H must be a multiple of %d and W of %d, or H of %d and W of %d (got %dx%d)", kV2Rows, kV2Cols, kT0Rows, kT0Cols, height,
              width);
   Conv0Params p;
-  p.x = x; p.w = w; p.scale = scale; p.shift = shift; p.slope = slope; p.y = reinterpret_cast<__half*>(y);
+  p.x = x; p.lut = lut; p.w = w; p.scale = scale; p.shift = shift; p.slope = slope; p.y = reinterpret_cast<__half*>(y);
   p.batch = batch; p.height = height; p.width = width;
   p.tiles_x = v2 ? width / kV2Cols : width / kT0Cols;
   p.tiles_y = v2 ? height / kV2Rows : height / kT0Rows;
@@ -482,16 +491,18 @@ int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* sc
   if (v2) {
     if (x_is_u8) {
       YB_REQUIRE(!raw, "conv0: the uint8 input form has no raw output");
-      conv0_k16_kernel<true, false><<<grid, 128, 0, stream>>>(p);
+      if (in_mode == kInLut) conv0_k16_kernel<kInLut, false><<<grid, 128, 0, stream>>>(p);
+      else conv0_k16_kernel<kInU8, false><<<grid, 128, 0, stream>>>(p);
     } else if (raw) {
-      conv0_k16_kernel<false, true><<<grid, 128, 0, stream>>>(p);
+      conv0_k16_kernel<kInF32, true><<<grid, 128, 0, stream>>>(p);
     } else {
-      conv0_k16_kernel<false, false><<<grid, 128, 0, stream>>>(p);
+      conv0_k16_kernel<kInF32, false><<<grid, 128, 0, stream>>>(p);
     }
     return check_launch("conv0_k16_kernel");
   }
-  if (x_is_u8) conv0_tc_kernel<true><<<grid, 128, 0, stream>>>(p);
-  else conv0_tc_kernel<false><<<grid, 128, 0, stream>>>(p);
+  if (in_mode == kInLut) conv0_tc_kernel<kInLut><<<grid, 128, 0, stream>>>(p);
+  else if (in_mode == kInU8) conv0_tc_kernel<kInU8><<<grid, 128, 0, stream>>>(p);
+  else conv0_tc_kernel<kInF32><<<grid, 128, 0, stream>>>(p);
   return check_launch("conv0_tc_kernel");
 }
 
@@ -507,7 +518,7 @@ int conv0_tc_forward(const void* x, int x_is_u8, const float* w, const float* sc
 constexpr int kC64Out = 64;
 constexpr int kC64StageBytes = (kV2Rows / 2) * kV2Cols * kC64Out * 2;   // 32 KB
 
-template <bool kPool>
+template <int kIn, bool kPool>
 __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_c64_kernel(const Conv0Params p) {
   __shared__ __align__(128) uint8_t stage[kPool ? 16 : kC64StageBytes];
   __shared__ __align__(128) uint8_t patch_e[kV2Copy + 48];
@@ -552,8 +563,10 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_c64_kernel(const Conv
       const int iy = y0 + r, ix = x0 + c;
       const bool ok = i < kV2Pixels && iy >= 0 && iy < p.height && ix >= 0 && ix < p.width;
 #pragma unroll
-      for (int ch = 0; ch < 3; ++ch)
-        v[k][ch] = ok ? __ldg(reinterpret_cast<const float*>(p.x) + ((static_cast<long long>(pimg) * 3 + ch) * p.height + iy) * p.width + ix) : 0.f;
+      for (int ch = 0; ch < 3; ++ch) {
+        if (kIn == kInLut) v[k][ch] = ok ? lut_pixel(p.x, p.lut, pimg, ch, iy, ix, p.height, p.width) : 0.f;
+        else v[k][ch] = ok ? __ldg(reinterpret_cast<const float*>(p.x) + ((static_cast<long long>(pimg) * 3 + ch) * p.height + iy) * p.width + ix) : 0.f;
+      }
     }
   };
   float pre[kV2Iters][3];
@@ -646,13 +659,14 @@ __global__ void __launch_bounds__(128, kC0CtasPerSm) conv0_c64_kernel(const Conv
   }
 }
 
-int conv0_c64_forward(const float* x, const float* w, const float* scale, const float* shift, float slope, void* y, int batch, int height,
-                      int width, int pool, cudaStream_t stream) {
+// lut == nullptr: x is fp32 NCHW; otherwise uint8 NHWC read through lut[3][256]
+int conv0_c64_forward(const void* x, const float* lut, const float* w, const float* scale, const float* shift, float slope, void* y, int batch,
+                      int height, int width, int pool, cudaStream_t stream) {
   YB_REQUIRE(x && w && scale && shift && y, "conv0_c64: null pointer");
   YB_REQUIRE(batch > 0 && height > 0 && width > 0 && height % kV2Rows == 0 && width % kV2Cols == 0,
              "conv0_c64: H must be a multiple of %d and W of %d (got %dx%d)", kV2Rows, kV2Cols, height, width);
   Conv0Params p;
-  p.x = x; p.w = w; p.scale = scale; p.shift = shift; p.slope = slope; p.y = reinterpret_cast<__half*>(y);
+  p.x = x; p.lut = lut; p.w = w; p.scale = scale; p.shift = shift; p.slope = slope; p.y = reinterpret_cast<__half*>(y);
   p.batch = batch; p.height = height; p.width = width;
   p.tiles_x = width / kV2Cols;
   p.tiles_y = height / kV2Rows;
@@ -664,8 +678,13 @@ int conv0_c64_forward(const float* x, const float* w, const float* scale, const 
   p.dbg = debug_word_device();
   const int max_ctas = sm_count() * kC0CtasPerSm;
   const int grid = p.num_tiles < max_ctas ? p.num_tiles : max_ctas;
-  if (pool) conv0_c64_kernel<true><<<grid, 128, 0, stream>>>(p);
-  else conv0_c64_kernel<false><<<grid, 128, 0, stream>>>(p);
+  if (lut) {
+    if (pool) conv0_c64_kernel<kInLut, true><<<grid, 128, 0, stream>>>(p);
+    else conv0_c64_kernel<kInLut, false><<<grid, 128, 0, stream>>>(p);
+  } else {
+    if (pool) conv0_c64_kernel<kInF32, true><<<grid, 128, 0, stream>>>(p);
+    else conv0_c64_kernel<kInF32, false><<<grid, 128, 0, stream>>>(p);
+  }
   return check_launch("conv0_c64_kernel");
 }
 

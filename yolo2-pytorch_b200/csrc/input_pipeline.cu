@@ -96,6 +96,19 @@ __global__ void totensor_u8_kernel(const uint8_t* __restrict__ src, float* __res
   for (int c = 0; c < 3; ++c) d[static_cast<long long>(c) * hw] = __fdiv_rn(static_cast<float>(s[c]), 255.f);
 }
 
+// The configured tensor transform on a batch (transform.TensorTransform: ToTensor, then zero or more per-channel Normalize), compiled into
+// a table: uint8 NHWC [B,H,W,3] -> fp32 NCHW [B,3,H,W], dst = lut[c][src].  The table holds torchvision's own result for every byte value,
+// so the output is torchvision's bit for bit.
+__global__ void totensor_lut_u8_kernel(const uint8_t* __restrict__ src, const float* __restrict__ lut, float* __restrict__ dst, int batch, int hw) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;     // one thread per pixel
+  if (idx >= static_cast<long long>(batch) * hw) return;
+  const long long img = idx / hw, pix = idx - img * hw;
+  const uint8_t* s = src + idx * 3;
+  float* d = dst + img * 3 * hw + pix;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) d[static_cast<long long>(c) * hw] = __ldg(lut + c * 256 + s[c]);
+}
+
 // Augmented form (the default training resize `resize_train = transform.resize.label.RandomCrop`, config.ini:48, after the optional
 // `transform.augmentation.RandomFlipHorizontally`, config.ini:47): out = cv2.resize(crop(flip(image))).  Both are pure index transforms on
 // the SOURCE of the same bit-exact resize: a flipped image's column j is column (w - 1 - j) (cv2.flip(image, 1), augmentation.py:87-95),
@@ -412,6 +425,14 @@ int totensor_u8(const void* src, float* dst, int batch, int height, int width, c
   const long long total = static_cast<long long>(batch) * height * width;
   totensor_u8_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(static_cast<const uint8_t*>(src), dst, batch, height * width);
   return check_launch("totensor_u8_kernel");
+}
+
+int totensor_lut_u8(const void* src, const float* lut, float* dst, int batch, int height, int width, cudaStream_t stream) {
+  YB_REQUIRE(src && lut && dst && batch > 0 && height > 0 && width > 0, "totensor_lut_u8: bad argument");
+  const long long total = static_cast<long long>(batch) * height * width;
+  totensor_lut_u8_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(static_cast<const uint8_t*>(src), lut, dst, batch,
+                                                                                         height * width);
+  return check_launch("totensor_lut_u8_kernel");
 }
 
 int resize_batch_u8(const void* src, const long long* src_off, const int* src_hw, void* dst, int batch, int height, int width, int swap_rb,

@@ -6,15 +6,17 @@
 //              HBM-bound: one thread = 8 channels (16 B) of one output pixel, 9 vector loads, fp32 FMA, 16 B store.
 // The pointwise convs (conv_pw, :41-46) and the 1x1 head reuse the wgmma implicit-GEMM kernel (slope = 0 -> ReLU).
 #include "yb_common.h"
+#include "yb_input.cuh"
 #include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace yb {
 
-template <int kPad>
-__global__ void __launch_bounds__(256) mb_conv0_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ scale,
-                                                       const float* __restrict__ shift, __half* __restrict__ y, int batch, int height, int width, int raw,
-                                                       int split) {
+// kIn: kInF32 (x fp32 NCHW) or kInLut (x uint8 NHWC through lut[3][256]; yb_input.cuh)
+template <int kPad, int kIn>
+__global__ void __launch_bounds__(256) mb_conv0_kernel(const void* __restrict__ x, const float* __restrict__ lut, const float* __restrict__ w,
+                                                       const float* __restrict__ scale, const float* __restrict__ shift, __half* __restrict__ y, int batch,
+                                                       int height, int width, int raw, int split) {
   __shared__ __align__(16) float ws[27][32];
   __shared__ float sc[32], sh[32];
   for (int i = threadIdx.x; i < 27 * 32; i += blockDim.x) ws[i / 32][i % 32] = w[(i % 32) * 27 + i / 32];
@@ -39,7 +41,10 @@ __global__ void __launch_bounds__(256) mb_conv0_kernel(const float* __restrict__
 #pragma unroll
       for (int s = 0; s < 3; ++s) {
         const int ix = 2 * px - kPad + s;
-        const float v = (iy >= 0 && iy < height && ix >= 0 && ix < width) ? __ldg(x + ((static_cast<long long>(img) * 3 + c) * height + iy) * width + ix) : 0.f;
+        const bool in = iy >= 0 && iy < height && ix >= 0 && ix < width;
+        float v;
+        if (kIn == kInLut) v = in ? lut_pixel(x, lut, img, c, iy, ix, height, width) : 0.f;
+        else v = in ? __ldg(reinterpret_cast<const float*>(x) + ((static_cast<long long>(img) * 3 + c) * height + iy) * width + ix) : 0.f;
         const float4* wp = reinterpret_cast<const float4*>(&ws[c * 9 + r * 3 + s][0]);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
@@ -70,26 +75,39 @@ __global__ void __launch_bounds__(256) mb_conv0_kernel(const float* __restrict__
   }
 }
 
-int mb_conv0(const float* x, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width, int raw, int split,
-             cudaStream_t stream) {
-  YB_REQUIRE(x && w && (raw || (scale && shift)) && y && batch > 0 && height % 2 == 0 && width % 2 == 0 && !(raw && split), "mb_conv0: bad argument");
+// lut == nullptr: x is fp32 NCHW; otherwise uint8 NHWC read through lut[3][256] (not with raw)
+int mb_conv0(const void* x, const float* lut, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width, int raw,
+             int split, cudaStream_t stream) {
+  YB_REQUIRE(x && w && (raw || (scale && shift)) && y && batch > 0 && height % 2 == 0 && width % 2 == 0 && !(raw && split) && !(raw && lut),
+             "mb_conv0: bad argument");
   const long long total = static_cast<long long>(batch) * (height / 2) * (width / 2);
-  mb_conv0_kernel<1><<<static_cast<unsigned>((total + 255) / 256), 256, 0, stream>>>(x, w, raw ? w : scale, raw ? w : shift, reinterpret_cast<__half*>(y), batch, height, width,
-                                                                                    raw, split);
+  const unsigned grid = static_cast<unsigned>((total + 255) / 256);
+  if (lut)
+    mb_conv0_kernel<1, kInLut><<<grid, 256, 0, stream>>>(x, lut, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, 0, split);
+  else
+    mb_conv0_kernel<1, kInF32><<<grid, 256, 0, stream>>>(x, lut, w, raw ? w : scale, raw ? w : shift, reinterpret_cast<__half*>(y), batch, height, width,
+                                                         raw, split);
   return check_launch("mb_conv0_kernel");
 }
 
 // Inception-v3 Conv2d_1a_3x3: nn.Conv2d(3, 32, 3, stride 2, pad `pad`) + folded BatchNorm + ReLU, x fp32 NCHW [B,3,H,W] -> y fp16 NHWC
 // [B,(H+2pad-3)/2+1,(W+2pad-3)/2+1,32].  pad = 1 is the MobileNet instantiation (same bits as mb_conv0 at even H, W).
-int stem3x3_s2(const float* x, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width, int pad,
-               cudaStream_t stream) {
+// lut == nullptr: x is fp32 NCHW; otherwise uint8 NHWC read through lut[3][256]
+int stem3x3_s2(const void* x, const float* lut, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width,
+               int pad, cudaStream_t stream) {
   YB_REQUIRE(x && w && scale && shift && y && batch > 0 && (pad == 0 || pad == 1), "stem3x3_s2: bad argument (pad 0 or 1)");
   YB_REQUIRE(height + 2 * pad >= 3 && width + 2 * pad >= 3, "stem3x3_s2: %d x %d input gives an empty output", height, width);
   YB_REQUIRE((reinterpret_cast<uintptr_t>(y) & 15) == 0, "stem3x3_s2: y must be 16B aligned");
   const long long total = static_cast<long long>(batch) * ((height + 2 * pad - 3) / 2 + 1) * ((width + 2 * pad - 3) / 2 + 1);
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-  if (pad == 0) mb_conv0_kernel<0><<<grid, 256, 0, stream>>>(x, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, 0, 0);
-  else mb_conv0_kernel<1><<<grid, 256, 0, stream>>>(x, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, 0, 0);
+  __half* yh = reinterpret_cast<__half*>(y);
+  if (lut) {
+    if (pad == 0) mb_conv0_kernel<0, kInLut><<<grid, 256, 0, stream>>>(x, lut, w, scale, shift, yh, batch, height, width, 0, 0);
+    else mb_conv0_kernel<1, kInLut><<<grid, 256, 0, stream>>>(x, lut, w, scale, shift, yh, batch, height, width, 0, 0);
+  } else {
+    if (pad == 0) mb_conv0_kernel<0, kInF32><<<grid, 256, 0, stream>>>(x, lut, w, scale, shift, yh, batch, height, width, 0, 0);
+    else mb_conv0_kernel<1, kInF32><<<grid, 256, 0, stream>>>(x, lut, w, scale, shift, yh, batch, height, width, 0, 0);
+  }
   return check_launch("mb_conv0_kernel");
 }
 
@@ -477,8 +495,8 @@ int stem3x3_s2_raw(const float* x, const float* w, void* z, int batch, int heigh
   YB_REQUIRE((reinterpret_cast<uintptr_t>(z) & 15) == 0, "stem3x3_s2_raw: z must be 16B aligned");
   const long long total = static_cast<long long>(batch) * ((height + 2 * pad - 3) / 2 + 1) * ((width + 2 * pad - 3) / 2 + 1);
   const unsigned grid = static_cast<unsigned>((total + 255) / 256);
-  if (pad == 0) mb_conv0_kernel<0><<<grid, 256, 0, stream>>>(x, w, w, w, reinterpret_cast<__half*>(z), batch, height, width, 1, 0);
-  else mb_conv0_kernel<1><<<grid, 256, 0, stream>>>(x, w, w, w, reinterpret_cast<__half*>(z), batch, height, width, 1, 0);
+  if (pad == 0) mb_conv0_kernel<0, kInF32><<<grid, 256, 0, stream>>>(x, nullptr, w, w, w, reinterpret_cast<__half*>(z), batch, height, width, 1, 0);
+  else mb_conv0_kernel<1, kInF32><<<grid, 256, 0, stream>>>(x, nullptr, w, w, w, reinterpret_cast<__half*>(z), batch, height, width, 1, 0);
   return check_launch("mb_conv0_kernel");
 }
 

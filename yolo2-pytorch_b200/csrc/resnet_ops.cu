@@ -8,6 +8,7 @@
 //   add_relu    out += residual; relu (:58-59, :100-101); residual_bwd is the gradient at a block boundary.
 // The 3x3 / 1x1 convs themselves (with folded BN and ReLU or identity) are yb_conv_bn_act_fwd.
 #include "yb_common.h"
+#include "yb_input.cuh"
 #include "yb_pool.cuh"
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -18,9 +19,11 @@ constexpr int kStemOut = 64, kStemTaps = 147;
 
 // one thread per output pixel, all 64 channels in registers; weights [tap][64] in shared memory (tap = ci*49 + r*7 + s).
 // kRaw: the train-mode form, the conv output z itself (no BatchNorm, no ReLU; scale / shift unused).
-template <bool kRaw>
+// kIn: kInF32 (x fp32 NCHW) or kInLut (x_u8 uint8 NHWC through lut[3][256]; yb_input.cuh).
+template <bool kRaw, int kIn>
 __global__ void __launch_bounds__(128) stem7x7_kernel(const float* __restrict__ x, const float* __restrict__ w, const float* __restrict__ scale,
-                                                      const float* __restrict__ shift, __half* __restrict__ y, int batch, int height, int width) {
+                                                      const float* __restrict__ shift, __half* __restrict__ y, int batch, int height, int width,
+                                                      const uint8_t* __restrict__ x_u8, const float* __restrict__ lut) {
   extern __shared__ float ws[];            // [147][64]
   for (int i = threadIdx.x; i < kStemTaps * kStemOut; i += blockDim.x) ws[i] = w[(i % kStemOut) * kStemTaps + i / kStemOut];
   __syncthreads();
@@ -43,7 +46,9 @@ __global__ void __launch_bounds__(128) stem7x7_kernel(const float* __restrict__ 
 #pragma unroll
       for (int s = 0; s < 7; ++s) {
         const int ix = 2 * px - 3 + s;
-        const float v = (ix >= 0 && ix < width) ? __ldg(xp + static_cast<long long>(iy) * width + ix) : 0.f;
+        float v;
+        if (kIn == kInLut) v = (ix >= 0 && ix < width) ? lut_pixel(x_u8, lut, img, ci, iy, ix, height, width) : 0.f;
+        else v = (ix >= 0 && ix < width) ? __ldg(xp + static_cast<long long>(iy) * width + ix) : 0.f;
         const float4* wp = reinterpret_cast<const float4*>(ws + (ci * 49 + r * 7 + s) * kStemOut);
 #pragma unroll
         for (int q = 0; q < kStemOut / 4; ++q) {
@@ -71,21 +76,29 @@ __global__ void __launch_bounds__(128) stem7x7_kernel(const float* __restrict__ 
   }
 }
 
-// raw = 1: the train-mode form (scale / shift may be NULL)
-int stem7x7(const float* x, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width, int raw, cudaStream_t stream) {
-  YB_REQUIRE(x && w && (raw || (scale && shift)) && y && batch > 0 && height % 2 == 0 && width % 2 == 0, "stem7x7: bad argument");
+// raw = 1: the train-mode form (scale / shift may be NULL).  lut == nullptr: x is fp32 NCHW; otherwise uint8 NHWC read through lut[3][256] (not
+// with raw)
+int stem7x7(const void* x, const float* lut, const float* w, const float* scale, const float* shift, void* y, int batch, int height, int width, int raw,
+            cudaStream_t stream) {
+  YB_REQUIRE(x && w && (raw || (scale && shift)) && y && batch > 0 && height % 2 == 0 && width % 2 == 0 && !(raw && lut), "stem7x7: bad argument");
   const int smem = kStemTaps * kStemOut * static_cast<int>(sizeof(float));
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[raw ? 1 : 0]) {
-    YB_CUDA(cudaFuncSetAttribute(raw ? stem7x7_kernel<true> : stem7x7_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set[raw ? 1 : 0] = true;
+  const int form = lut ? 2 : raw ? 1 : 0;
+  static bool attr_set[3] = {false, false, false};
+  if (!attr_set[form]) {
+    YB_CUDA(cudaFuncSetAttribute(lut ? stem7x7_kernel<false, kInLut> : raw ? stem7x7_kernel<true, kInF32> : stem7x7_kernel<false, kInF32>,
+                                 cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set[form] = true;
   }
   const long long total = static_cast<long long>(batch) * (height / 2) * (width / 2);
   const unsigned grid = static_cast<unsigned>((total + 127) / 128);
-  if (raw)
-    stem7x7_kernel<true><<<grid, 128, smem, stream>>>(x, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width);
+  const float* xf = lut ? nullptr : static_cast<const float*>(x);
+  const uint8_t* xu = lut ? static_cast<const uint8_t*>(x) : nullptr;
+  if (lut)
+    stem7x7_kernel<false, kInLut><<<grid, 128, smem, stream>>>(xf, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, xu, lut);
+  else if (raw)
+    stem7x7_kernel<true, kInF32><<<grid, 128, smem, stream>>>(xf, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, xu, lut);
   else
-    stem7x7_kernel<false><<<grid, 128, smem, stream>>>(x, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width);
+    stem7x7_kernel<false, kInF32><<<grid, 128, smem, stream>>>(xf, w, scale, shift, reinterpret_cast<__half*>(y), batch, height, width, xu, lut);
   return check_launch("stem7x7_kernel");
 }
 

@@ -16,6 +16,7 @@ import torch.distributed as _dist
 from b200 import ddp as _ddp
 from b200 import engine as _engine
 from b200 import ops as _ops
+import transform as _transform
 
 
 class _TrainFunction(torch.autograd.Function):
@@ -46,8 +47,12 @@ class _TrainFunction(torch.autograd.Function):
 
 class Backbone(nn.Module):
     """Base of the backbone plugins.  Holds the kernel operands cached per parameter version (`_cache`), the lazily built trainer (an
-    instance of the b200.train_engine class `TRAINER`) and the train-mode entry through it."""
+    instance of the b200.train_engine class `TRAINER`) and the train-mode entry through it.
+
+    In eval mode every backbone takes either the fp32 NCHW image [B,3,H,W], taken as already transformed (as the reference's model takes
+    it), or a uint8 NHWC frame batch [B,H,W,3], which its first-layer kernel reads through `input_transform`'s table."""
     TRAINER = None
+    input_transform = None
 
     def __init__(self):
         nn.Module.__init__(self)
@@ -63,6 +68,30 @@ class Backbone(nn.Module):
     def drop_operands(self):
         """Forget every cached kernel operand."""
         self._cache.clear()
+
+    def set_input_transform(self, t):
+        """The tensor transform (transform.TensorTransform, e.g. the reference's `[transform] tensor` chain) that uint8 frame batches go
+        through: in the first-layer kernel in eval mode, and in train.iterate before a training step.  None (the default): ToTensor alone
+        (Darknet's uint8 path then scales by 1/255 in its kernel, as it always has).  Set it before capturing a CUDA graph.  Returns self."""
+        if t is not None and not isinstance(t, _transform.TensorTransform):
+            raise TypeError('set_input_transform expects a transform.TensorTransform or None, not %r' % (t,))
+        self.input_transform = t
+        return self
+
+    def input_lut(self, device):
+        """The table fp32 [3, 256] on `device` that a uint8 frame batch goes through: input_transform's, else ToTensor's."""
+        t = self.input_transform if self.input_transform is not None else _transform.to_tensor_transform()
+        return t.lut(device)
+
+    def eval_input(self, x):
+        """An eval-mode input -> (x, lut, (B, C, H, W)): a uint8 frame batch [B,H,W,C] with its table, or the fp32 image [B,C,H,W] with None."""
+        if x.dtype == torch.uint8:
+            if x.dim() != 4:
+                raise ValueError('%s expects uint8 frames [B,H,W,3], got %s' % (type(self).__name__, tuple(x.shape)))
+            b, h, w, c = x.shape
+            return x.contiguous(), self.input_lut(x.device), (b, c, h, w)
+        b, c, h, w = x.shape
+        return x.contiguous().float(), None, (b, c, h, w)
 
     def train(self, mode=True):
         """nn.Module.train + drop cached kernel operands on a mode switch: fused optimizers and CUDA-graph replays update parameters without

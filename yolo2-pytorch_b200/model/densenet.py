@@ -151,18 +151,21 @@ class DenseNet(model.Backbone):
         _ops.conv_bn_act(pooled, self._packed(key + '.conv', trans.conv.weight), self._const(1, co, buf.device), self._const(0, co, buf.device),
                          1.0, out=out, y_ch_off=0)
 
-    def stem(self, x, buf):
-        """conv0 + norm0 + relu0 + pool0 into channels [0, 64) of block 1's buffer."""
-        b, _, h, w = x.shape
+    def stem(self, x, buf, lut=None):
+        """conv0 + norm0 + relu0 + pool0 into channels [0, 64) of block 1's buffer; x fp32 NCHW, or uint8 NHWC read through `lut`."""
+        b, h, w = (x.shape[0], x.shape[2], x.shape[3]) if lut is None else x.shape[:3]
         f = self.features
         s, t = self._fold('norm0', f.norm0)
         stem = torch.empty(b, h // 2, w // 2, 64, dtype=torch.float16, device=x.device)
-        _ops.call('yb_stem7x7_bn_relu_fwd', x, f.conv0.weight.detach().float().contiguous(), s, t, stem, b, h, w)
+        if lut is None:
+            _ops.call('yb_stem7x7_bn_relu_fwd', x, f.conv0.weight.detach().float().contiguous(), s, t, stem, b, h, w)
+        else:
+            _ops.call('yb_stem7x7_bn_relu_lut_fwd', x, lut, f.conv0.weight.detach().float().contiguous(), s, t, stem, b, h, w)
         _ops.call('yb_maxpool3x3_s2_ld_f16', stem, buf, buf.shape[-1], 0, b, h // 2, w // 2, 64)
 
     def run(self, x, collect=None):
         """Forward on the kernels; `collect` (a dict) receives every dense block's and transition's output buffer (fp16 NHWC)."""
-        b, c, h, w = x.shape
+        x, lut, (b, c, h, w) = self.eval_input(x)
         if c != 3 or h % 32 or w % 32:
             raise ValueError('DenseNet expects [B,3,H,W] with H, W multiples of 32')
         why = self.unsupported()
@@ -170,11 +173,10 @@ class DenseNet(model.Backbone):
             raise NotImplementedError('DenseNet: no kernel path for %s' % why)
         if not x.is_cuda:
             raise RuntimeError('DenseNet: input must be a CUDA tensor; there is no CPU fallback')
-        x = x.contiguous().float()
         f = self.features
         hh, ww = h // 4, w // 4
         buf = torch.empty(b, hh, ww, self.block_channels[0][1], dtype=torch.float16, device=x.device)
-        self.stem(x, buf)
+        self.stem(x, buf, lut)
         for i, n in enumerate(self.block_config):
             name = 'denseblock%d' % (i + 1)
             block = getattr(f, name)

@@ -230,10 +230,10 @@ class Inception3(model.Backbone):
         fn = kind.get(tag) or kind[tag[0]]
         return fn(getattr(self, name), x)
 
-    def stem(self, x, collect=None):
-        """Conv2d_1a_3x3 .. the second max-pool: x fp32 NCHW -> Mixed_5b's input, fp16 NHWC [B,H5,W5,192]."""
+    def stem(self, x, collect=None, lut=None):
+        """Conv2d_1a_3x3 .. the second max-pool: x fp32 NCHW (or uint8 NHWC read through `lut`) -> Mixed_5b's input, fp16 NHWC [B,H5,W5,192]."""
         s, t = self._operands_stem()
-        a = _ops.stem3x3_s2(x, self.Conv2d_1a_3x3.conv.weight.detach().float().contiguous(), s, t, pad=0)
+        a = _ops.stem3x3_s2(x, self.Conv2d_1a_3x3.conv.weight.detach().float().contiguous(), s, t, pad=0, lut=lut)
         a = self.unit(self.Conv2d_2b_3x3, self.unit(self.Conv2d_2a_3x3, a))
         a = _ops.maxpool3x3_s2_valid(a)
         if collect is not None:
@@ -250,14 +250,14 @@ class Inception3(model.Backbone):
 
     def run(self, x, collect=None):
         """Forward on the kernels; `collect` (a dict) receives both stem pools and every Mixed_* output (fp16 NHWC)."""
-        b, c, h, w = x.shape
+        x, lut, (b, c, h, w) = self.eval_input(x)
         if c != 3:
             raise ValueError('Inception3 expects [B,3,H,W]')
         if h < MIN_SIZE or w < MIN_SIZE:
             raise ValueError('Inception3: a %d x %d input leaves a stage empty (H and W must be >= %d)' % (h, w, MIN_SIZE))
         if not x.is_cuda:
             raise RuntimeError('Inception3: input must be a CUDA tensor; there is no CPU fallback')
-        a = self.stem(x.contiguous().float(), collect)
+        a = self.stem(x, collect, lut)
         for name in BLOCKS:
             a = self.block(name, a)
             if collect is not None:

@@ -335,24 +335,24 @@ class Inception4(model.Backbone):
             self.unit(units[-1], t, out, off)
         return out
 
-    def stem(self, x):
-        """features.0 .. features.2: x fp32 NCHW -> Mixed_3a's input, fp16 NHWC."""
+    def stem(self, x, lut=None):
+        """features.0 .. features.2: x fp32 NCHW (or uint8 NHWC read through `lut`) -> Mixed_3a's input, fp16 NHWC."""
         f = self.features
         w32, s, t = self._operands(f[0])
-        a = _ops.stem3x3_s2(x, w32, s, t, pad=0)
+        a = _ops.stem3x3_s2(x, w32, s, t, pad=0, lut=lut)
         return self.unit(f[2], self.unit(f[1], a))
 
     def run(self, x, collect=None):
         """Forward on the kernels; `collect` (a dict) receives the stem output ('stem') and every block's buffer under its index (fp16 NHWC,
         padded layout: see `blocks`)."""
-        b, c, h, w = x.shape
+        x, lut, (b, c, h, w) = self.eval_input(x)
         if c != 3:
             raise ValueError('Inception4 expects [B,3,H,W]')
         if h < MIN_SIZE or w < MIN_SIZE:
             raise ValueError('Inception4: a %d x %d input leaves a stage empty (H and W must be >= %d)' % (h, w, MIN_SIZE))
         if not x.is_cuda:
             raise RuntimeError('Inception4: input must be a CUDA tensor; there is no CPU fallback')
-        a = self.stem(x.contiguous().float())
+        a = self.stem(x, lut)
         if collect is not None:
             collect['stem'] = a
         for i in range(3, 3 + len(self.blocks)):

@@ -102,14 +102,17 @@ class MobileNet(model.Backbone):
     def _packed_split(self, key, w):
         return self._cache.fetch(key, (w,), lambda: _ops.pack_weight_split_f16(w.detach().contiguous(), True, True))
 
-    def _forward_strict(self, x):
-        b, c, h, w = x.shape
+    def _forward_strict(self, x, lut, shape):
+        b, c, h, w = shape
         dev = x.device
         first = self.layers[0]
         scale, shift = self._fold('bn0', first.bn)
         ch = first.conv.weight.shape[0]
         cur = torch.empty(b, h // 2, w // 2, 2 * ch, dtype=torch.float16, device=dev)            # [hi | lo]
-        _ops.call('yb_mb_conv0_split_fwd', x, first.conv.weight.detach().contiguous(), scale, shift, cur, b, h, w)
+        if lut is None:
+            _ops.call('yb_mb_conv0_split_fwd', x, first.conv.weight.detach().contiguous(), scale, shift, cur, b, h, w)
+        else:
+            _ops.call('yb_mb_conv0_split_lut_fwd', x, lut, first.conv.weight.detach().contiguous(), scale, shift, cur, b, h, w)
         hh, ww = h // 2, w // 2
         for i, unit in enumerate(list(self.layers)[1:-1], 1):
             dw, pw = unit.dw, unit.pw
@@ -136,18 +139,21 @@ class MobileNet(model.Backbone):
             return self.train_forward(x)
         if not x.is_cuda:
             raise RuntimeError('MobileNet: input must be a CUDA tensor; there is no CPU fallback')
-        b, c, h, w = x.shape
+        x, lut, shape = self.eval_input(x)
+        b, c, h, w = shape
         if c != 3 or h % 32 or w % 32:
             raise ValueError('MobileNet expects [B,3,H,W] with H, W multiples of 32')
-        x = x.contiguous().float()
         first = self.layers[0]
         if first.conv.weight.shape[0] != 32:
             raise ValueError('MobileNet: the first layer must have 32 output channels')
         if self.precision == 'strict':
-            return self._forward_strict(x)
+            return self._forward_strict(x, lut, shape)
         scale, shift = self._fold('bn0', first.bn)
         cur = torch.empty(b, h // 2, w // 2, first.conv.weight.shape[0], dtype=torch.float16, device=x.device)
-        _ops.call('yb_mb_conv0_bn_relu_fwd', x, first.conv.weight.detach().contiguous(), scale, shift, cur, b, h, w)
+        if lut is None:
+            _ops.call('yb_mb_conv0_bn_relu_fwd', x, first.conv.weight.detach().contiguous(), scale, shift, cur, b, h, w)
+        else:
+            _ops.call('yb_mb_conv0_bn_relu_lut_fwd', x, lut, first.conv.weight.detach().contiguous(), scale, shift, cur, b, h, w)
         hh, ww = h // 2, w // 2
         for i, unit in enumerate(list(self.layers)[1:-1], 1):
             dw, pw = unit.dw, unit.pw

@@ -155,15 +155,17 @@ class ResNet(model.Backbone):
             return self.train_forward(x)
         if not x.is_cuda:
             raise RuntimeError('ResNet: input must be a CUDA tensor; there is no CPU fallback')
-        b, c, h, w = x.shape
+        x, lut, (b, c, h, w) = self.eval_input(x)
         if c != 3 or h % 32 or w % 32:
             raise ValueError('ResNet expects [B,3,H,W] with H, W multiples of 32')
         if self.conv1.weight.shape[0] != 64:
             raise ValueError('ResNet: the stem must have 64 output channels')
-        x = x.contiguous().float()
         scale, shift = self._fold('bn1', self.bn1)
         stem = torch.empty(b, h // 2, w // 2, 64, dtype=torch.float16, device=x.device)
-        _ops.call('yb_stem7x7_bn_relu_fwd', x, self.conv1.weight.detach().contiguous(), scale, shift, stem, b, h, w)
+        if lut is None:
+            _ops.call('yb_stem7x7_bn_relu_fwd', x, self.conv1.weight.detach().contiguous(), scale, shift, stem, b, h, w)
+        else:
+            _ops.call('yb_stem7x7_bn_relu_lut_fwd', x, lut, self.conv1.weight.detach().contiguous(), scale, shift, stem, b, h, w)
         cur = torch.empty(b, h // 4, w // 4, 64, dtype=torch.float16, device=x.device)
         _ops.call('yb_maxpool3x3_s2_f16', stem, cur, b, h // 2, w // 2, 64)
         for lname in ('layer1', 'layer2', 'layer3', 'layer4'):

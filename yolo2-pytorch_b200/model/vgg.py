@@ -149,17 +149,18 @@ class VGG(model.Backbone):
     # ---- forward ---------------------------------------------------------------------------------------
     def run(self, x, collect=None):
         """Forward on the kernels; `collect` (a dict) receives every MaxPool2d's output under its feature index (fp16 NHWC, padded layout)."""
-        if x.dim() != 4 or x.shape[1] != 3:
+        if x.dim() != 4:
             raise ValueError('VGG expects [B,3,H,W]')
-        b, _, h, w = x.shape
+        x, lut, (b, c, h, w) = self.eval_input(x)
+        if c != 3:
+            raise ValueError('VGG expects [B,3,H,W]')
         if h % 32 or w % 32 or h == 0 or w == 0:
             raise ValueError('VGG: H and W must be positive multiples of 32 (got %d x %d)' % (h, w))
         if not x.is_cuda:
             raise RuntimeError('VGG: input must be a CUDA tensor; there is no CPU fallback')
-        x = x.contiguous().float()
         u0 = self.units[0]
         w0, s, t = self._operands(0)
-        a = _ops.conv0_c64_bn_act(x, w0, s, t, 0.0, pool=u0.pool)
+        a = _ops.conv0_c64_bn_act(x, w0, s, t, 0.0, pool=u0.pool, lut=lut)
         if collect is not None and u0.pool:
             collect[u0.pool_index] = a
         for i in range(1, len(self.units)):

@@ -316,10 +316,9 @@ class Tiny(model.Backbone):
             return self.train_forward(x)
         if not x.is_cuda:
             raise RuntimeError('Tiny: input must be a CUDA tensor; there is no CPU fallback')
-        b, c, h, w = x.shape
+        x, lut, (b, c, h, w) = self.eval_input(x)
         if c != 3 or h % 32 or w % 32:
-            raise ValueError('Tiny expects fp32 [B,3,H,W] with H, W multiples of 32, got %s' % (tuple(x.shape),))
-        x = x.contiguous().float()
+            raise ValueError('Tiny expects fp32 [B,3,H,W] or uint8 [B,H,W,3] with H, W multiples of 32, got %s' % (tuple(x.shape),))
         plan = self._plan()
         for i, (u, _) in enumerate(plan):
             u.refresh(first_layer=(i == 0))
@@ -327,7 +326,7 @@ class Tiny(model.Backbone):
         if after0 != 'pool' or u0.cout > 32:
             raise RuntimeError('Tiny: the first unit must have <= 32 filters and be followed by MaxPool2d(2)')
         w0, sc0, sh0 = self._padded('u0', u0, 32, 3, True)
-        cur = _ops.conv0_bn_leaky_pool(x, w0, sc0, sh0, u0.slope)          # [B,H/2,W/2,32], channels >= cout are exact zeros
+        cur = _ops.conv0_bn_leaky_pool(x, w0, sc0, sh0, u0.slope, lut=lut)  # [B,H/2,W/2,32], channels >= cout are exact zeros
         chan = 32                                                          # channels per pixel of `cur`
         for i, (u, after) in enumerate(plan[1:], 1):
             last = i == len(plan) - 1

@@ -76,17 +76,20 @@ def loss_scale_config(config):
 
 
 def iterate(inference, optimizer, anchors, config, data, reducer=None):
-    """One training step (reference Train.iterate, train.py:338-362).  `data`: dict with `tensor` [B,3,H,W] fp32,
-    `yx_min`/`yx_max` [B,G,2] in pixels, `cls` [B,G].  Returns the same kind of dict as the reference; with `[train] loss_scale =
+    """One training step (reference Train.iterate, train.py:338-362).  `data`: dict with `tensor` [B,3,H,W] fp32 (or uint8 frames
+    [B,H,W,3], put through the backbone's input_transform, else ToTensor), `yx_min`/`yx_max` [B,G,2] in pixels, `cls` [B,G].  Returns the same kind of dict as the reference; with `[train] loss_scale =
     dynamic` it also holds `loss_scale`, the device scale (the trainer's static scale times its dynamic factor) the next step runs at."""
     dev = torch.device('cuda', torch.cuda.current_device())
     data = {k: (v.to(dev, non_blocking=True) if torch.is_tensor(v) else v) for k, v in data.items()}
     tensor = data['tensor']
-    if tensor.dtype == torch.uint8:                 # uint8 NHWC frames from utils.data.Collate: ToTensor on the device
-        import transform
-        tensor = transform.to_tensor(tensor)
-    height, width = tensor.shape[-2:]
     dnn = inference.dnn
+    if tensor.dtype == torch.uint8:                 # uint8 NHWC frames from utils.data.Collate: the input transform on the device
+        if getattr(dnn, 'input_transform', None) is not None:
+            tensor = dnn.input_transform(tensor)
+        else:
+            import transform
+            tensor = transform.to_tensor(tensor)
+    height, width = tensor.shape[-2:]
     if reducer is False:                           # this rank alone, no collective (compute-only timing of a data-parallel step)
         with _ddp.local_only():
             return iterate(inference, optimizer, anchors, config, data, None)

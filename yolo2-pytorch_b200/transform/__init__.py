@@ -6,7 +6,9 @@ frames in one launch -- optionally through the horizontal flip and the random-cr
 resize; `transform.augmentation.random_rotate` / `Rotator` and `transform.resize.image.fixed` (shrinking) run cv2.warpAffine's bilinear path in
 one kernel.  The photometric augmentations of `transform/image.py` (RandomBlur, BGR2HSV, RandomHue, RandomSaturation, RandomBrightness,
 HSV2RGB, RandomGamma) run bit-exactly with cv2 in one launch per chain segment over the resized batch (`transform.image.Compose`);
-`parse_transform` / `get_transform` build a configured sequence such as `transform/image_train` the way the reference does."""
+`parse_transform` / `get_transform` build a configured sequence such as `transform/image_train` the way the reference does.
+`TensorTransform` is the tensor chain that follows them (`[transform] tensor`: ToTensor, then per-channel Normalize), compiled into a
+per-channel table that the backbones' first-layer kernels read uint8 frames through."""
 import inspect
 
 import torch
@@ -30,6 +32,77 @@ def get_transform(config, sequence, compose=None):
     if compose is None:
         from transform.image import Compose as compose
     return compose([parse_transform(config, method) for method in sequence])
+
+
+class TensorTransform(object):
+    """The reference's `[transform] tensor` chain, built as `get_transform(config, config.get('transform', 'tensor').split(),
+    compose=TensorTransform)`: torchvision.transforms.ToTensor followed by zero or more 3-channel Normalizes (transform.image.Normalize or
+    torchvision's own).  Anything else raises ValueError naming the item.
+
+    The chain is compiled by running its own objects once on the CPU over a uint8 image that holds every byte value in every channel, so
+    `table[c][v]` (fp32 [3, 256]) is bit for bit what torchvision computes for byte v in channel c.  `lut(device)` is that table on a device
+    (cached; a backbone's first-layer `_lut` kernel reads through it), and calling the transform on a uint8 CUDA batch [B, H, W, 3] returns
+    the fp32 [B, 3, H, W] image in one launch."""
+
+    def __init__(self, sequence):
+        import torchvision
+        self.transforms = list(sequence)
+        for i, t in enumerate(self.transforms):
+            if i == 0:
+                if not isinstance(t, torchvision.transforms.ToTensor):
+                    raise ValueError('TensorTransform: the chain must start with torchvision.transforms.ToTensor, not %r' % (t,))
+            elif not isinstance(t, torchvision.transforms.Normalize):
+                raise ValueError('TensorTransform: only 3-channel Normalizes may follow ToTensor, not %r' % (t,))
+            elif torch.as_tensor(t.mean).numel() != 3 or torch.as_tensor(t.std).numel() != 3:
+                raise ValueError('TensorTransform: %r is not a 3-channel Normalize' % (t,))
+        if not self.transforms:
+            raise ValueError('TensorTransform: the chain must start with torchvision.transforms.ToTensor, not an empty chain')
+        image = torch.arange(256, dtype=torch.uint8).view(256, 1, 1).expand(256, 1, 3).numpy().copy()
+        x = image
+        for t in self.transforms:
+            x = t(x)
+        if x.dtype != torch.float32:
+            raise ValueError('TensorTransform: the chain yields %s, not float32' % (x.dtype,))
+        self.table = x[:, :, 0].contiguous()
+        self._luts = {}
+
+    def __repr__(self):
+        return 'TensorTransform(%r)' % (self.transforms,)
+
+    def lut(self, device):
+        """The table as a CUDA tensor fp32 [3, 256] on `device`, allocated once per device (never inside a CUDA-graph capture: call the
+        transform or an eager forward before capturing)."""
+        device = torch.device(device)
+        t = self._luts.get(device)
+        if t is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError('TensorTransform: the table for %s is first needed inside a CUDA-graph capture; run once eagerly before '
+                                   'capturing' % device)
+            t = self._luts[device] = self.table.to(device)
+        return t
+
+    def __call__(self, frames_u8):
+        """uint8 CUDA tensor [B, H, W, 3] -> float32 [B, 3, H, W], what the chain computes frame by frame (yb_totensor_lut_u8)."""
+        if not (isinstance(frames_u8, torch.Tensor) and frames_u8.is_cuda and frames_u8.dtype == torch.uint8 and frames_u8.dim() == 4
+                and frames_u8.shape[3] == 3):
+            raise RuntimeError('TensorTransform: expected a uint8 CUDA tensor [B, H, W, 3]')
+        frames_u8 = frames_u8.contiguous()
+        b, h, w, _ = frames_u8.shape
+        out = torch.empty(b, 3, h, w, dtype=torch.float32, device=frames_u8.device)
+        _ops.call('yb_totensor_lut_u8', frames_u8, self.lut(frames_u8.device), out, b, h, w)
+        return out
+
+
+_TO_TENSOR = None
+
+
+def to_tensor_transform():
+    """TensorTransform([ToTensor()]): the table a backbone reads uint8 frames through when no input transform is set."""
+    global _TO_TENSOR
+    if _TO_TENSOR is None:
+        import torchvision
+        _TO_TENSOR = TensorTransform([torchvision.transforms.ToTensor()])
+    return _TO_TENSOR
 
 
 def resize_batch(frames, height, width, bgr2rgb=True, yx_min=None, yx_max=None, flip=None, crop=None, margin=None):

@@ -16,6 +16,7 @@ import re
 
 import numpy as np
 import torch
+import torchvision
 
 from b200 import ops as _ops
 
@@ -31,6 +32,16 @@ def underscore(name):
 
 def _adjust(obj, config, cast):
     return tuple(map(cast, config.get('augmentation', underscore(type(obj).__name__)).split()))
+
+
+class Normalize(torchvision.transforms.Normalize):
+    """The reference's tensor transform (transform/image.py): `[transform] normalize = mean std`, each repeated over the 3 channels.  It
+    runs in a `transform.TensorTransform` chain after torchvision's ToTensor."""
+
+    def __init__(self, config):
+        name = underscore(type(self).__name__)
+        mean, std = tuple(map(float, config.get('transform', name).split()))
+        torchvision.transforms.Normalize.__init__(self, (mean, mean, mean), (std, std, std))
 
 
 class _Op(object):
